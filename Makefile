@@ -1,6 +1,6 @@
-# Builds libgf_b200.so (sm_100a only) in-tree.  `python -c "import __graft_entry__ as g; g.build()"` calls this.
+# Builds libgf_b200.so (sm_90a, H100) in-tree.  `python -c "import __graft_entry__ as g; g.build()"` calls this.
 NVCC ?= /usr/local/cuda/bin/nvcc
-ARCH := -gencode arch=compute_100a,code=sm_100a
+ARCH := -gencode arch=compute_90a,code=sm_90a
 CSRC := ground_fusion_b200/csrc
 OUT  := ground_fusion_b200/libgf_b200.so
 # -fmad=false: the front end is bit-exact with OpenCV's separately-rounded float ops (FMA only where written)

@@ -35,6 +35,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
+sys.dont_write_bytecode = True      # the tree may be read-only: nothing is written next to the sources
 
 FRAMES_PER_STEP = 100
 WORKLOADS = {
@@ -196,16 +197,20 @@ class Stream:
         p8 = [p8[0] * sc, p8[1] * sc, p8[2] * sc, p8[3] * sc] + p8[4:]
         self.tr = FeatureTracker(wl["w"], wl["h"], p8, wl["max_cnt"], wl["min_dist"], 1, 1, device=device)
         self.ring, self.k, self.dev_ms = ring, offset, 0.0
+        self.keep_last, self.last = False, None   # keep_last: the final step of run() also returns its per-frame results
 
     def run(self, n_steps, mode):
         """n_steps batches of FRAMES_PER_STEP frames; returns the device time of the run (CUDA events on the tracker's streams)."""
         g, d = self.ring.ptr[mode]
         n = self.ring.n
         self.tr.timer_start()
-        for _ in range(n_steps):
+        for step in range(n_steps):
             idx = [tri(self.k + j, n) for j in range(FRAMES_PER_STEP)]
             times = [(self.k + j) / 30.0 for j in range(FRAMES_PER_STEP)]
-            self.tr.trackBatch(times, [g[i] for i in idx], [d[i] for i in idx], on_device=(mode == "device"), want=False)
+            want = self.keep_last and step == n_steps - 1
+            res = self.tr.trackBatch(times, [g[i] for i in idx], [d[i] for i in idx], on_device=(mode == "device"), want=want)
+            if want:
+                self.last = res
             self.k += FRAMES_PER_STEP
         self.dev_ms = self.tr.timer_stop()
         return self.dev_ms
@@ -253,12 +258,15 @@ def timed(streams, n_steps, mode, barrier, sampler=None, threads=False):
     return el, max(s.dev_ms for s in streams)
 
 
-def fe_line(wl, rings, device, n_streams, steps, warmup, barrier, sampler, reduce_max, threads=False):
+def fe_line(wl, rings, device, n_streams, steps, warmup, barrier, sampler, reduce_max, threads=False, keep_last=False):
+    """keep_last: also return the per-frame results of the last timed device-resident step of stream 0 under "last"."""
     streams = [Stream(rings[0], wl, device, offset=17 * s) for s in range(n_streams)]
     from ground_fusion_b200 import _lib
     timed(streams, warmup, "device", barrier, threads=threads)
     l0 = _lib.lib().gf_kernel_launch_count()
+    streams[0].keep_last = keep_last
     el_dev, ms_dev = timed(streams, steps, "device", barrier, sampler, threads=threads)
+    streams[0].keep_last = False
     launches = _lib.lib().gf_kernel_launch_count() - l0
     timed(streams, max(1, warmup // 2), "host", barrier, threads=threads)
     el_e2e, ms_e2e = timed(streams, steps, "host", barrier, sampler, threads=threads)
@@ -269,7 +277,32 @@ def fe_line(wl, rings, device, n_streams, steps, warmup, barrier, sampler, reduc
     frames = n_streams * steps * FRAMES_PER_STEP
     return {"value": frames / el_dev, "e2e": frames / el_e2e, "ms_per_step": 1e3 * el_dev / steps, "ms_per_step_e2e": 1e3 * el_e2e / steps,
             "device_ms_per_step": ms_dev / steps, "device_ms_per_step_e2e": ms_e2e / steps, "streams_per_gpu": n_streams, "gpu_launches": int(launches),
-            "mean_features_tracked": float(np.mean([i["n_tracked"] for i in infos])), "mean_lk_iterations": float(np.mean([i["lk_iterations"] for i in infos]))}
+            "mean_features_tracked": float(np.mean([i["n_tracked"] for i in infos])), "mean_lk_iterations": float(np.mean([i["lk_iterations"] for i in infos])),
+            "last": streams[0].last}
+
+
+def dump_outputs(out_dir, last, max_cnt):
+    """Writes the per-frame results of one step (trackBatch's (obs, status, info) per frame) as float64 / float32 .npy files;
+    rows beyond a frame's count are NaN.  C2 at 100 frames per step: about 1.3 MB."""
+    from ground_fusion_b200._lib import TrackInfo
+    os.makedirs(out_dir, exist_ok=True)
+    n = len(last)
+    fields = [f for f, _ in TrackInfo._fields_]
+    ids = np.full((n, max_cnt), np.nan)
+    track_cnt = np.full((n, max_cnt), np.nan)
+    v = np.full((n, max_cnt, 8), np.nan)
+    status = np.full((n, max_cnt), np.nan, np.float32)
+    info = np.zeros((n, len(fields)))
+    for k, (obs, st, inf) in enumerate(last):
+        ids[k, :len(obs)] = obs["id"]
+        track_cnt[k, :len(obs)] = obs["track_cnt"]
+        v[k, :len(obs)] = obs["v"]
+        status[k, :len(st)] = st
+        info[k] = [inf[f] for f in fields]
+    arrays = {"fe_obs_id": ids, "fe_obs_track_cnt": track_cnt, "fe_obs_v": v, "fe_status": status, "fe_info": info}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+    return sorted(arrays)
 
 
 def ba_bench(device, clocks_mhz, n_windows=8, reps=200, cpu_seconds=8.0):
@@ -313,10 +346,11 @@ def ba_bench(device, clocks_mhz, n_windows=8, reps=200, cpu_seconds=8.0):
     L.gf_probe_fp64.argtypes = [ctypes.c_int, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)]
     L.gf_probe_fp64(device, ctypes.byref(dfma), ctypes.byref(dmma))
     fma = (nc + 1) ** 3 / 3.0 + nc * nc + 3.0 * n_lm * nc
-    mhz = clocks_mhz or 1965.0
+    mhz = clocks_mhz or 1980.0          # without an NVML clock sample: the maximum SM clock of an H100 SXM
     t_launch = (step_cycles / max(1, step_launches)) / (mhz * 1e6)
     ach = 2.0 * fma / t_launch / 1e9 if t_launch > 0 else None
-    n_sm = 148
+    import torch
+    n_sm = torch.cuda.get_device_properties(device).multi_processor_count
     out["roofline"] = {"kernel": "k_ba_step (one CTA: 8x8-tile left-looking Cholesky on DMMA.8x8x4, back substitution, dogleg, candidate)",
                        "bound": "tensor", "unit": "GFLOP/s (FP64)", "achieved": ach, "peak": dmma.value, "frac": ach / dmma.value if ach else None,
                        "peak_source": "gf_probe_fp64: DMMA.8x8x4 on all SMs, measured in this run (plain DFMA: %.0f GFLOP/s)" % dfma.value,
@@ -414,6 +448,9 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--cpu-seconds", type=float, default=8.0)
     ap.add_argument("--no-extras", action="store_true", help="only the headline C2 line (no stream sweep, C3/C4, BA)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step of the headline line returned (observations, status, info of its %d frames) "
+                         "as DIR/<name>.npy; the inputs depend only on the arguments" % FRAMES_PER_STEP)
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local = int(os.environ.get("LOCAL_RANK", "0"))
     wl = WORKLOADS["C2"]
@@ -473,8 +510,10 @@ def main():
     if rank == 0:
         sampler = ClockSampler(local); sampler.start()
     ring = Ring(rank, wl, torch)
-    head = fe_line(wl, [ring], local, 1, args.steps, args.warmup, barrier, sampler, reduce_max)
+    head = fe_line(wl, [ring], local, 1, args.steps, args.warmup, barrier, sampler, reduce_max, keep_last=args.dump_outputs is not None)
     clocks = sampler.summary() if sampler is not None else None
+    if args.dump_outputs is not None and rank == 0:
+        dump_outputs(args.dump_outputs, head["last"], wl["max_cnt"])
 
     extra = {}
     if world > 1 and not args.no_extras:
@@ -495,7 +534,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = peaks.get("hbm_gbs", 6650.0)
+    hbm = peaks.get("hbm_gbs", 3350.0)      # H100 SXM data sheet (HBM3) when no measured peak is at hand
     out = {"metric": "tracker_frames_per_sec", "value": world * head["value"], "unit": "frames/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
            "ms_per_step": head["ms_per_step"], "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
            "dtype": "u8/i32 fixed point + f32 (LK, min-eig), f64 (box sums, undistortion)", "data": "synthetic", "config": cfg,
@@ -531,8 +570,8 @@ def main():
         out["roofline"] = {"kernel": "k_track (fwd 4-level + reverse 2-level LK, one 8-warp CTA per feature)", "bound": "hbm",
                            "achieved": (lk_bytes / lk_s / 1e9) if lk_s > 0 else None, "peak": hbm, "unit": "GB/s",
                            "frac": (lk_bytes / lk_s / 1e9 / hbm) if lk_s > 0 else None,
-                           "traffic": 899072, "traffic_source": "dram__bytes_read+write of one k_track launch, profiles/r2_ncu_k_track_full.txt",
-                           "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 GB/s (of fallback)",
+                           "traffic": None,
+                           "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "H100 SXM data sheet, 3350 GB/s (not measured)",
                            "algorithmic_bytes_per_launch": lk_bytes, "kernel_ms": stage.get("lk"),
                            "note": "latency-bound by construction: per feature a chain of ~22 dependent LK iterations, each 105 dependent FADDs in OpenCV lane order; "
                                    "throughput comes from concurrent streams (see streams)"}
@@ -548,7 +587,7 @@ def main():
         r = fe_line(wl, [ring], local, 8, max(4, args.steps // 2), 2, barrier, None, reduce_max, threads=True)
         out["streams"] = {"unit": "frames/s", "per_streams_per_gpu": sweep,
                           "eight_streams_one_host_thread_each": {"value": r["value"], "e2e": r["e2e"]},
-                          "note": "independent trackers (gf_tracker handles) sharing one B200, all fed by ONE host thread through gf_tracker_track_batch_multi; eight_streams_one_host_thread_each = the same 8 trackers driven by 8 host threads calling gf_tracker_track_batch; e2e saturates on the host link (0.92 MB per frame: 31 k frames/s = 28.5 GB/s); C2 workload"}
+                          "note": "independent trackers (gf_tracker handles) sharing one GPU, all fed by ONE host thread through gf_tracker_track_batch_multi; eight_streams_one_host_thread_each = the same 8 trackers driven by 8 host threads calling gf_tracker_track_batch; e2e moves 0.92 MB per frame over the host link; C2 workload"}
         # ---- the other configurations ----
         cfgs = {}
         for name in ("C3", "C4"):

@@ -1,5 +1,5 @@
 // ba_chol.cuh -- dense FP64 linear algebra of the sliding-window solve on 8x8 tiles with FP64 tensor-core MMAs
-// (mma.sync m8n8k4 f64 = SASS DMMA.8x8x4; measured on B200: 64 FMA/clk/SM, 26 cycles dependent latency, tools/dmma_probe.cu).
+// (mma.sync m8n8k4 f64 = SASS DMMA.8x8x4; latency and rate per SM: tools/dmma_probe.cu).
 //
 // Replaces Ceres' DENSE_SCHUR linear solver (SchurEliminator + dense Cholesky; reference call site estimator.cpp:3303-3318):
 //   schur_tile      one 8x8 tile of the reduced camera system  S = H' + mu D^2 - W'^T C W'  (rank-L update on DMMA)

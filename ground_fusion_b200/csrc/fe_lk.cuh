@@ -52,9 +52,9 @@ static_assert((LK_IREG * LK_IPITCH) % 128 == 0 && (LK_MAXLEV * LK_IREG * LK_IPIT
 // ---- 2-D TMA staging of the LK windows --------------------------------------------------------------------------------
 // A window that lies inside its pyramid level is one cp.async.bulk.tensor.2d box: LK_IPITCH x LK_IREG bytes for a template
 // window, LK_JPITCH x LK_JR for a search region (the box is as wide as the staged row pitch, so the box IS the staging
-// layout).  The innermost box coordinate must put the box start on a 16-byte boundary -- measured on B200: an unaligned x
-// raises "illegal instruction" at the UTMALDG (tools/tma_probe.cu) -- so the box starts at x0 & ~15 and the first needed
-// column sits at byte x0 & 15 of every staged row.  Tensor maps: u8, rank 2, {w, h}, row stride = level pitch, no swizzle;
+// layout).  The innermost box coordinate is kept on a 16-byte boundary (an unaligned x has been seen to raise "illegal
+// instruction" at the UTMALDG), so the box starts at x0 & ~15 and the first needed column sits at byte x0 & 15 of every
+// staged row.  Tensor maps: u8, rank 2, {w, h}, row stride = level pitch, no swizzle;
 // columns beyond the image width are zero-filled and never read.  Windows that touch the border keep the REFLECT_101 gathers.
 struct LKMapSet {
     CUtensorMap prevI[LK_MAXLEV], curJ[LK_MAXLEV];   // forward pass: templates from the previous pyramid, search in the current one

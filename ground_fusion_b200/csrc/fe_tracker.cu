@@ -1,4 +1,4 @@
-// fe_tracker.cu -- gf_tracker_* and gf_stage_* (C ABI), the host side of the B200 front end.
+// fe_tracker.cu -- gf_tracker_* and gf_stage_* (C ABI), the host side of the front end.
 //
 // Mirrors FeatureTracker::trackImage (reference vins_estimator/src/featureTracker/feature_tracker.cpp:103-372).
 // One frame = fixed sequences of copies and kernels on three streams (no host round trip inside the frame; the only
@@ -98,7 +98,7 @@ __global__ void __launch_bounds__(LK_THREADS) k_lk_pred(Pyramid prev, Pyramid cu
 // Forward LK (3 levels) + reverse check (1 level, USE_INITIAL_FLOW) + inBorder + grey<=250
 // (feature_tracker.cpp:118-168).  One CTA of 4 warps per feature.
 #ifndef GF_TRACK_MIN_CTAS
-#define GF_TRACK_MIN_CTAS 3          // 79 registers: three features per SM when several streams share the GPU (2: 116 registers)
+#define GF_TRACK_MIN_CTAS 3          // 80 registers: three features per SM when several streams share the GPU (2: 110 registers)
 #endif
 __global__ void __launch_bounds__(LK_THREADS, GF_TRACK_MIN_CTAS) k_track(Pyramid prev, Pyramid cur, TrackScalars* sc, FeatArrays fa,
                                                       const FrameParams* fp, int flow_back, const __grid_constant__ LKMapSet M)
@@ -392,7 +392,7 @@ static int enqueue_pyramid(cudaStream_t s, const gf_tracker* t, int slot)
 extern "C" {
 
 const char* gf_last_error(void) { return g_err; }
-const char* gf_version(void) { return "gf_b200 0.1 sm_100a"; }
+const char* gf_version(void) { return "gf_b200 0.1 sm_90a"; }
 uint64_t gf_kernel_launch_count(void) { return g_launches.load(); }
 
 static int tracker_init(gf_tracker* t, int width, int height, const gf_tracker_cfg* cfg);
@@ -495,7 +495,7 @@ static int tracker_init(gf_tracker* t, int width, int height, const gf_tracker_c
     t->use_graph = getenv("GF_NO_GRAPH") == nullptr;
     t->batch_pipeline = getenv("GF_BATCH_PIPELINE") != nullptr;   // one graph per frame for batches (see gf_tracker_track_batch_multi)
     t->pdl_single_cta = getenv("GF_FE_PDL1") != nullptr && !t->profiling;   // PDL only into the two single-CTA kernels
-    t->use_pdl = getenv("GF_PDL") != nullptr;      // programmatic dependent launch inside dep(f): measured slower on B200 (DESIGN 1.3), off by default
+    t->use_pdl = getenv("GF_PDL") != nullptr;      // programmatic dependent launch inside dep(f): off by default (DESIGN 1.3)
     GF_CUDA(cudaDeviceSynchronize());
     return GF_OK;
 }
@@ -895,8 +895,8 @@ int gf_tracker_track_batch_multi(gf_tracker* const* trackers, int n_trackers, in
     if (n == 0) return GF_OK;
     int rc;
     // Default: every lane goes frame by frame through the five-stream submit / wait pipeline of gf_tracker_submit, lanes interleaved.
-    // GF_BATCH_PIPELINE=1 selects the one-graph-per-frame pipeline below instead; measured on one B200 box (C2, same run):
-    // single stream 10.89 k (default) vs 10.70 k frames/s, 8 streams 38.7 k vs 32.4 k -- joining prep(f+1) into the graph of
+    // GF_BATCH_PIPELINE=1 selects the one-graph-per-frame pipeline below instead; measured on one H100 SXM at 700 W (C2, same run):
+    // single stream 10.0 k (default) vs 9.6 k frames/s, 8 streams 26.6 k vs 23.0 k -- joining prep(f+1) into the graph of
     // dep(f) costs more overlap than the saved driver calls give back (DESIGN 1.3).
     bool any_pipeline = false;
     for (BatchLane& L : lanes) any_pipeline = any_pipeline || (L.t->use_graph && L.t->batch_pipeline);

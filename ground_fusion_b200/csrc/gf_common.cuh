@@ -1,4 +1,4 @@
-// gf_common.cuh -- shared helpers for libgf_b200.so (sm_100a only).
+// gf_common.cuh -- shared helpers for libgf_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,5 +1,5 @@
 /*
- * gf_b200.h -- C ABI of libgf_b200.so, the B200 (sm_100a) implementation of Ground-Fusion's two
+ * gf_b200.h -- C ABI of libgf_b200.so, the H100 (sm_90a) implementation of Ground-Fusion's two
  * data-parallel hot paths.  Plain pointers and sizes only; no exceptions cross this boundary.
  * Every entry point returns 0 on success or a negative gf_status.  Handles are thread-compatible:
  * one host thread per handle at a time (the reference runs FE on sync_thread and BA on processThread).
@@ -33,7 +33,7 @@ typedef enum gf_status {
 
 /* Text of the last error raised on the calling thread (never NULL). */
 const char* gf_last_error(void);
-/* Library version string, e.g. "gf_b200 0.1 sm_100a". */
+/* Library version string, e.g. "gf_b200 0.1 sm_90a". */
 const char* gf_version(void);
 /* Number of kernel launches issued by this library since load (all handles). */
 uint64_t gf_kernel_launch_count(void);
@@ -123,8 +123,8 @@ int gf_tracker_track_batch(gf_tracker* t, int n, const double* times, const void
 /* The same for several independent camera streams at once (a multi-camera rig, several robots served by one GPU): stream i
  * is trackers[i] with frames times / gray / depth [i*n + k] and results at out + (i*n + k)*max_cnt, n_out / info [i*n + k],
  * status_out + (i*n + k)*max_cnt.  One host thread feeds all streams round-robin (frame k of every stream is enqueued before
- * frame k-1 of any stream is collected), so a server does not need one thread per camera: measured on one B200, 8 streams reach
- * 35.6 k frames/s this way and 36.4 k with 8 threads calling gf_tracker_track_batch.  Results are identical to calling
+ * frame k-1 of any stream is collected), so a server does not need one thread per camera: measured on one H100 SXM at 700 W,
+ * 8 streams reach 26.6-27.0 k frames/s this way and 20.6-26.9 k with 8 threads calling gf_tracker_track_batch.  Results are identical to calling
  * gf_tracker_track_batch per stream. */
 int gf_tracker_track_batch_multi(gf_tracker* const* trackers, int n_trackers, int n, const double* times, const void* const* gray,
                                  size_t gray_pitch, const void* const* depth, size_t depth_pitch, int on_device,

@@ -1,4 +1,4 @@
-"""GPU parity tests of the front end (run with -m gpu on the B200 box).
+"""GPU parity tests of the front end (run with -m gpu on an H100).
 
 Every test calls the CUDA path through the C ABI (libgf_b200.so) and compares with the oracle:
 cv2 4.13.0 for the three OpenCV calls the reference makes (feature_tracker.cpp:118-153,198) and

@@ -1,5 +1,5 @@
 // Microbenchmark of the back end's tiled Cholesky (ba_chol.cuh) with per-warp, per-panel clock64() stamps.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/chol_bench tools/chol_bench.cu && tools/chol_bench [n]
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/chol_bench tools/chol_bench.cu && tools/chol_bench [n]
 #include <cstdio>
 #include <cstdlib>
 #include <vector>

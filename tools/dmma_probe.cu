@@ -1,4 +1,4 @@
-// DMMA (mma.sync m8n8k4 f64) latency / throughput probe for B200 (sm_100a), next to the DFMA rate of tools/fp64_probe.cu.
+// DMMA (mma.sync m8n8k4 f64) latency / throughput probe (sm_90a), next to the DFMA rate of tools/fp64_probe.cu.
 #include <cstdio>
 #include <cuda_runtime.h>
 __device__ __forceinline__ void dmma(double& c0, double& c1, double a, double b)
@@ -105,8 +105,10 @@ int main()
         k_tput<8><<<1, thr>>>(d, c, n); cudaMemcpy(hc, c, 8, cudaMemcpyDeviceToHost);
         printf("DMMA throughput 1 CTA x %4d thr, 8 acc: %.2f FMA/clk/SM\n", thr, 256.0 * 8 * n * (thr / 32) / (double)hc[0]);
     }
-    k_tput<8><<<148, 512>>>(d, c, n); cudaMemcpy(hc, c, 8, cudaMemcpyDeviceToHost);
-    printf("DMMA throughput 148 CTAs x 512 thr, 8 acc: %.2f FMA/clk/SM (CTA 0)\n", 256.0 * 8 * n * 16 / (double)hc[0]);
+    int n_sm = 0;
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, 0);
+    k_tput<8><<<n_sm, 512>>>(d, c, n); cudaMemcpy(hc, c, 8, cudaMemcpyDeviceToHost);
+    printf("DMMA throughput %d CTAs x 512 thr, 8 acc: %.2f FMA/clk/SM (CTA 0)\n", n_sm, 256.0 * 8 * n * 16 / (double)hc[0]);
     for (int thr : {64, 256, 512, 1024}) {
         k_bar<<<1, thr>>>(c, 2048); cudaMemcpy(hc, c, 16, cudaMemcpyDeviceToHost);
         printf("%4d thr: __syncthreads %.1f cycles\n", thr, hc[0] / 2048.0);

@@ -1,4 +1,4 @@
-// FP64 / shared-memory latency + throughput probe for B200 (sm_100a).
+// FP64 / shared-memory latency + throughput probe (sm_90a).
 #include <cstdio>
 #include <cuda_runtime.h>
 __global__ void k_lat(double* out, long long* cyc, int n) {

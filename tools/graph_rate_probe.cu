@@ -1,4 +1,4 @@
-// How many graph kernel nodes per second does one B200 retire when S host threads replay small graphs on S streams?
+// How many graph kernel nodes per second does one GPU retire when S host threads replay small graphs on S streams?
 // (Question behind it: is the front end with 8 trackers per GPU bound by node dispatch rather than by SM time?)
 #include <cuda_runtime.h>
 #include <chrono>
@@ -50,12 +50,14 @@ static double single_thread(int S, int nodes, int ctas, int threads, long long c
 int main()
 {
     cudaFree(0);
+    int n_sm = 0;
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, 0);
     struct Cfg { int nodes, ctas, threads; long long cycles; bool fork; const char* name; } cfgs[] = {
         {12, 1, 32, 0, false, "12 empty kernels, chain"},
         {12, 1, 32, 0, true, "12 empty kernels, two branches of 6"},
         {12, 1, 256, 10000, false, "12 x (1 CTA, 5 us), chain"},
         {12, 1, 256, 10000, true, "12 x (1 CTA, 5 us), two branches"},
-        {12, 148, 256, 10000, false, "12 x (148 CTAs, 5 us), chain"},
+        {12, n_sm, 256, 10000, false, "12 x (one CTA per SM, 5 us), chain"},
         {6, 1, 256, 20000, false, "6 x (1 CTA, 10 us), chain"},
     };
     for (auto& c : cfgs) {
