@@ -214,7 +214,10 @@ __device__ __forceinline__ void mask_tile_load(MaskTile& M, const TrackScalars* 
 }
 __device__ __forceinline__ bool mask_open(const MaskTile& M, const TrackScalars* sc, const float2* kept, int x, int y, int r2)
 {
-    if (M.overflow) {      // more neighbours than the list holds (cannot happen for features that are > r apart): exact slow path
+    // More neighbours than the list holds: exact slow path.  Kept features are > r apart, but at r = 5 about 75 of them fit a
+    // tile's 74x26 apron when packed on a lattice (gf_stage_gftt with such a kept list reaches this); the tracker's kept
+    // features on textured scenes put at most ~16 there at max_cnt 1000, min_dist 5.
+    if (M.overflow) {
         for (int i = 0; i < sc->n_kept; i++) {
             int dx = x - __float2int_rn(kept[i].x), dy = y - __float2int_rn(kept[i].y);
             if (dx * dx + dy * dy <= r2) return false;

@@ -105,13 +105,21 @@ class FeatureTracker:
         self.last_status = self._status[:info.n_prev].copy()
         return self._obs[:n.value].copy()
 
+    @staticmethod
+    def _rows(a, dtype):
+        """a itself when its rows are contiguous (any row pitch, e.g. a view into a wider buffer), else a contiguous copy."""
+        if isinstance(a, np.ndarray) and a.dtype == dtype and a.ndim == 2 and a.strides[1] == a.itemsize and a.strides[0] >= a.shape[1] * a.itemsize:
+            return a
+        return np.ascontiguousarray(a, dtype)
+
     def trackImageRaw(self, cur_time, img, depth=None):
-        """Returns the structured array of gf_obs in the tracker's internal (cur_pts) order."""
-        img = np.ascontiguousarray(img, np.uint8)
+        """Returns the structured array of gf_obs in the tracker's internal (cur_pts) order.  Row-padded views are passed
+        with their row pitch, as a cv::Mat with a larger step is in the reference."""
+        img = self._rows(img, np.uint8)
         assert img.shape == (self.height, self.width)
         dp, dpitch = None, 0
         if depth is not None:
-            depth = np.ascontiguousarray(depth, np.uint16)
+            depth = self._rows(depth, np.uint16)
             dp, dpitch = depth.ctypes.data, depth.strides[0]
         n, info = ctypes.c_int(0), TrackInfo()
         check(self.L.gf_tracker_track(self._h, float(cur_time), img.ctypes.data, img.strides[0], dp, dpitch,

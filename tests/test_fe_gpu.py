@@ -105,17 +105,31 @@ def test_gftt_matches_cv2(gf, seed, max_corners, min_dist, n_kept):
     assert got.shape == want.shape and np.array_equal(got, want), info
 
 
-def _run_sequence(gf, seed, n_frames, w=640, h=480, max_cnt=150, min_dist=30, noise=1.0):
+def _padded(a, pad):
+    """a as a view into a buffer `pad` elements wider per row; the padding holds the largest value of the type."""
+    buf = np.full((a.shape[0], a.shape[1] + pad), np.iinfo(a.dtype).max, a.dtype)
+    buf[:, :a.shape[1]] = a
+    return buf[:, :a.shape[1]]
+
+
+def _run_sequence(gf, seed, n_frames, w=640, h=480, max_cnt=150, min_dist=30, noise=1.0, pad=0, on_frame=None, cam=None):
+    """trackImage against the oracle frame by frame.  cam: the PinholeCamera (default: IDC_CAM scaled by w / 640).
+    pad > 0: gray and depth are passed as views into wider rows (row pitch > width).  on_frame(k, gpu, ref, got) runs
+    after the checks of frame k."""
     from ground_fusion_b200.synth import SyntheticStream
     from oracle.fe_oracle import IDC_CAM, FeatureTrackerOracle, PinholeCamera
-    sc = w / 640.0
-    cam = PinholeCamera(IDC_CAM["fx"] * sc, IDC_CAM["fy"] * sc, IDC_CAM["cx"] * sc, IDC_CAM["cy"] * sc,
-                        IDC_CAM["k1"], IDC_CAM["k2"], IDC_CAM["p1"], IDC_CAM["p2"])
+    if cam is None:
+        sc = w / 640.0
+        cam = PinholeCamera(IDC_CAM["fx"] * sc, IDC_CAM["fy"] * sc, IDC_CAM["cx"] * sc, IDC_CAM["cy"] * sc,
+                            IDC_CAM["k1"], IDC_CAM["k2"], IDC_CAM["p1"], IDC_CAM["p2"])
     stream = SyntheticStream(seed=seed, width=w, height=h, noise_sigma=noise)
     gpu = gf.FeatureTracker(w, h, cam.params8(), max_cnt, min_dist, 1, 1)
     ref = FeatureTrackerOracle(cam, max_cnt, min_dist, 1, 1)
     for k in range(n_frames):
         t, gray, depth = stream.frame(k)
+        if pad:
+            gray, depth = _padded(gray, pad), _padded(depth, pad)
+            assert gray.strides[0] > w and depth.strides[0] > 2 * w
         got = gpu.trackImageRaw(t, gray, depth)
         want = ref.trackImage(t, gray, depth)
         assert np.array_equal(gpu.last_status, ref.last_status), "frame %d: inlier mask differs" % k
@@ -124,6 +138,8 @@ def _run_sequence(gf, seed, n_frames, w=640, h=480, max_cnt=150, min_dist=30, no
         for o in got:
             assert np.array_equal(o["v"], want[int(o["id"])]), "frame %d id %d: %s vs %s" % (k, o["id"], o["v"], want[int(o["id"])])
         assert gpu.last_info["n_new"] == len(ref.last_n_pts)
+        if on_frame:
+            on_frame(k, gpu, ref, got)
     gpu.close()
 
 
