@@ -74,9 +74,9 @@ __global__ void __launch_bounds__(LK_THREADS) k_lk_stage(Pyramid I, Pyramid J, c
     lk_tma_init(sm, tid);
     LKTma T{M.prevI, M.curJ, 0u, M.enabled != 0};
     float2 p = prev_pts[i], init = use_init ? next_pts[i] : p, out;
-    int st, iters = 0;
+    int st, iters = 0, fallbacks = 0;
     long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    lk_track_point(sm, tid, I, J, p, init, use_init != 0, max_level, out, st, iters, pc, T);
+    lk_track_point(sm, tid, I, J, p, init, use_init != 0, max_level, out, st, iters, fallbacks, pc, T);
     if (tid == 0) { next_pts[i] = out; status[i] = (uint8_t)st; }
 }
 
@@ -89,9 +89,9 @@ __global__ void __launch_bounds__(LK_THREADS) k_lk_pred(Pyramid prev, Pyramid cu
     lk_tma_init(sm, tid);
     LKTma T{M.prevI, M.curJ, 0u, M.enabled != 0};
     float2 out;
-    int st, iters = 0;
+    int st, iters = 0, fallbacks = 0;
     long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    lk_track_point(sm, tid, prev, cur, fa.prev_pts[i], fa.pred_pts[i], true, 1, out, st, iters, pc, T);
+    lk_track_point(sm, tid, prev, cur, fa.prev_pts[i], fa.pred_pts[i], true, 1, out, st, iters, fallbacks, pc, T);
     if (tid == 0) { fa.cur_pts[i] = out; fa.status[i] = (uint8_t)st; if (st) atomicAdd(&sc->pred_succ, 1); atomicAdd(&sc->lk_iters, iters); }
 }
 
@@ -112,15 +112,15 @@ __global__ void __launch_bounds__(LK_THREADS, GF_TRACK_MIN_CTAS) k_track(Pyramid
     const float2 p = fa.prev_pts[i];
     const long long t0 = gf_clock();
     float2 q;
-    int st, iters = 0;
+    int st, iters = 0, fallbacks = 0;
     long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     if (fp->has_pred && sc->pred_succ >= 10) { q = fa.cur_pts[i]; st = fa.status[i]; }
-    else lk_track_point(sm, tid, prev, cur, p, p, false, 3, q, st, iters, pc, T);
+    else lk_track_point(sm, tid, prev, cur, p, p, false, 3, q, st, iters, fallbacks, pc, T);
     if (flow_back) {
         float2 r;
         int rst;
         T.mi = M.curI; T.mj = M.prevJ;          // roles swap for the reverse check
-        lk_track_point(sm, tid, cur, prev, q, p, true, 1, r, rst, iters, pc, T);
+        lk_track_point(sm, tid, cur, prev, q, p, true, 1, r, rst, iters, fallbacks, pc, T);
         double dx = (double)(p.x - r.x), dy = (double)(p.y - r.y);
         st = (st && rst && sqrt(dx * dx + dy * dy) <= 0.5) ? 1 : 0;
     }
@@ -137,7 +137,10 @@ __global__ void __launch_bounds__(LK_THREADS, GF_TRACK_MIN_CTAS) k_track(Pyramid
     if (tid == 0) {
         fa.cur_pts[i] = q; fa.status[i] = (uint8_t)st; atomicAdd(&sc->lk_iters, iters);
         if (fa.dbg && i < 4) for (int k = 0; k < 8; k++) fa.dbg[32 + 8 * i + k] = pc[k];
-        if (fa.dbg) { fa.dbg[64 + 8 * i] = gf_clock() - t0; fa.dbg[64 + 8 * i + 1] = iters; }
+        if (fa.dbg) {   // cycles, LK iterations, of which b sums from the integer partials / from the sequential chains
+            fa.dbg[64 + 8 * i] = gf_clock() - t0; fa.dbg[64 + 8 * i + 1] = iters;
+            fa.dbg[64 + 8 * i + 2] = iters - fallbacks; fa.dbg[64 + 8 * i + 3] = fallbacks;
+        }
     }
 }
 

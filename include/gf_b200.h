@@ -149,7 +149,9 @@ int gf_tracker_timer_stop(gf_tracker* t, float* ms);
 int gf_tracker_set_profiling(gf_tracker* t, int enable);
 int gf_tracker_last_stage_ms(gf_tracker* t, float* ms /* GF_FE_STAGES */);
 /* Development aid: clock64 phase counters of the single-CTA kernels ([0..63]) and per-feature LK cycles/iterations
- * ([64 + 8*i], [64 + 8*i + 1]).  n <= 64 + 8*1024. */
+ * ([64 + 8*i], [64 + 8*i + 1]); of those iterations, the ones whose mismatch vector came from exact integer sums and
+ * the ones that ran the sequential float chains ([64 + 8*i + 2], [64 + 8*i + 3]).  Rows past the frame's n_prev
+ * are stale.  n <= 64 + 8*1024. */
 int gf_tracker_debug_read(gf_tracker* t, long long* out, int n);
 
 /* ------------------------------------------------------------------------------------------------

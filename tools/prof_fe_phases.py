@@ -18,7 +18,10 @@ for k in range(n):
     a = np.array(buf[:], dtype=np.int64)
     lk = a[64:].reshape(-1, 8)
     cyc, it = lk[:, 0], lk[:, 1]
+    fast, slow = lk[:tr.last_info["n_prev"], 2:4].sum(0)      # rows past n_prev are stale
     print(f"frame {k}: dev {tr.last_device_ms():.3f} ms info {tr.last_info}")
+    print(f"   lk b sums: {fast} iterations from the integer partials, {slow} from the sequential chains"
+          f" ({100.0 * fast / max(fast + slow, 1):.1f} % fast)")
     print(f"   setmask cyc: compact {a[0]} sort {a[1]} greedy {a[2]} emit {a[3]}")
     print(f"   finalize cyc: nms {a[8]} topk {a[9]} emit {a[10]}  nacc {a[11]} ncand {a[12]}")
     print(f"   nms detail: setup {a[16]} A {a[13]} B {a[14]} C {a[15]} total {a[17]}")
