@@ -34,6 +34,9 @@ std::map<int, std::vector<std::pair<int, Eigen::Matrix<double, 8, 1>>>> FeatureT
         cfg_.max_cnt = MAX_CNT; cfg_.min_dist = MIN_DIST; cfg_.flow_back = FLOW_BACK; cfg_.depth_cam = depth_cam ? 1 : 0;
         row = _img.rows; col = _img.cols;
         if (gf_tracker_create(&gf_, device, col, row, &cfg_)) gf_fatal("gf_tracker_create");
+        // the reference equalises in getImageFromMsg before trackImage sees the frame; here the library does it on the GPU
+        // from the first frame on, which is the same image for every call (INTEGRATION.md)
+        if (EQUALIZE && gf_tracker_set_equalize(gf_, 40.0, 8, 8)) gf_fatal("gf_tracker_set_equalize");
         out_.resize(MAX_CNT > 0 ? MAX_CNT : 1);
     }
     prev_time = cur_time; cur_time = _cur_time;

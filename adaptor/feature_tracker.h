@@ -18,6 +18,8 @@
 extern int MAX_CNT;
 extern int MIN_DIST;
 extern int FLOW_BACK;
+// parameters.h:33: every image goes through cv::createCLAHE() (clip 40, 8 x 8 tiles) before trackImage (rosNodeTest.cpp:256-261)
+extern int EQUALIZE;
 
 class FeatureTracker
 {

@@ -1,14 +1,16 @@
 // Drives the adaptor classes from flat binary dumps written by tests/test_adaptor.py; the outputs go back as flat binaries.
 //   harness fe <in> <out>   frames through FeatureTracker::trackImage
+//   harness fe-eq <in> <out>  the same with EQUALIZE = 1
 //   harness ba <in> <out>   one window through Estimator::optimization()
 #include <cstdio>
 #include <cstdlib>
+#include <cstring>
 #include <vector>
 
 #include "estimator_ba.h"
 #include "feature_tracker.h"
 
-int MAX_CNT = 150, MIN_DIST = 30, FLOW_BACK = 1;
+int MAX_CNT = 150, MIN_DIST = 30, FLOW_BACK = 1, EQUALIZE = 0;
 int USE_IMU = 1, NUM_ITERATIONS = 8, ESTIMATE_TD = 0;
 double FOCAL_LENGTH = 600.0;
 Eigen::Vector3d G;
@@ -97,6 +99,7 @@ static int run_ba(const char *in, const char *out)
 
 int main(int argc, char **argv)
 {
-    if (argc != 4) { std::fprintf(stderr, "usage: harness fe|ba <in> <out>\n"); return 2; }
+    if (argc != 4) { std::fprintf(stderr, "usage: harness fe|fe-eq|ba <in> <out>\n"); return 2; }
+    if (!std::strcmp(argv[1], "fe-eq")) EQUALIZE = 1;
     return argv[1][0] == 'f' ? run_fe(argv[2], argv[3]) : run_ba(argv[2], argv[3]);
 }

@@ -63,12 +63,14 @@ def lib():
         L.gf_tracker_track_batch.argtypes = [vp, i, vp, vp, sz, vp, sz, i, vp, vp, vp, vp]
         L.gf_tracker_track_batch_multi.argtypes = [vp, i, i, vp, vp, sz, vp, sz, i, vp, vp, vp, vp]
         L.gf_tracker_set_prediction.argtypes = [vp, vp, vp, i]
+        L.gf_tracker_set_equalize.argtypes = [vp, d, i, i]
         L.gf_tracker_remove_ids.argtypes = [vp, vp, i]
         L.gf_tracker_last_device_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
         L.gf_tracker_set_profiling.argtypes = [vp, i]
         L.gf_tracker_last_stage_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
         L.gf_tracker_debug_read.argtypes = [vp, ctypes.POINTER(ctypes.c_longlong), ctypes.c_int]
         L.gf_stage_pyr_down.argtypes = [i, vp, i, i, vp]
+        L.gf_stage_clahe.argtypes = [i, vp, sz, i, i, d, i, i, vp]
         L.gf_stage_min_eig.argtypes = [i, vp, i, i, vp, ctypes.POINTER(i)]
         L.gf_stage_lk.argtypes = [i, vp, vp, i, i, vp, vp, i, i, i, vp]
         L.gf_stage_gftt.argtypes = [i, vp, i, i, vp, i, i, i, vp, ctypes.POINTER(i), ctypes.POINTER(TrackInfo)]

@@ -21,6 +21,7 @@
 #include <new>
 #include <vector>
 
+#include "fe_clahe.cuh"
 #include "fe_eig.cuh"
 #include "fe_lk.cuh"
 #include "fe_select.cuh"
@@ -40,14 +41,15 @@ struct FrameParams {
 // Frame intake of the batch pipeline: copies the frame named by *fp into pyramid level 0 and the depth slot (16 B per thread when
 // source and row pitch allow it).  A kernel instead of a memcpy node because the source address changes every frame while the
 // graph stays fixed.
+// row0 = h: depth only (with equalisation the CLAHE kernels write level 0 instead).
 __global__ void __launch_bounds__(256) k_copy_in(const FrameParams* __restrict__ fp, uint8_t* __restrict__ dst_gray, int gray_pitch,
-                                                 uint16_t* __restrict__ dst_depth, int depth_pitch_el, int w, int h)
+                                                 uint16_t* __restrict__ dst_depth, int depth_pitch_el, int w, int h, int row0)
 {
     const uint8_t* sg = fp->src_gray;
     const uint8_t* sd = (const uint8_t*)fp->src_depth;
     const long long gp = fp->src_gray_pitch, dp = fp->src_depth_pitch;
     const int depth_rows = (fp->depth_valid && sd) ? h : 0;
-    const int row = blockIdx.y;                       // rows 0..h-1: gray, h..2h-1: depth
+    const int row = blockIdx.y + row0;                // rows 0..h-1: gray, h..2h-1: depth
     const bool is_depth = row >= h;
     if (is_depth && row - h >= depth_rows) return;
     const uint8_t* src = is_depth ? sd + (long long)(row - h) * dp : sg + (long long)row * gp;
@@ -222,6 +224,14 @@ struct gf_tracker {
     int gbk_prep[6], gbk_dep[6], gbk_both[6];
     cudaEvent_t ev_fork, ev_fork2, ev_join[2];
     uint8_t* d_stage_gray[2]; uint16_t* d_stage_depth[2];   // H2D landing buffers of the batch pipeline (host frames)
+    // gf_tracker_set_equalize: CLAHE of every gray frame into pyramid level 0.  Frames land in d_raw first; the copy and both
+    // CLAHE kernels (a graph keyed by pyramid slot) run in order on s_up (batch pipeline: inside prep), so one raw buffer and
+    // one LUT block serve every frame in flight.
+    bool equalize;
+    ClaheGeom clahe;
+    cudaGraphExec_t g_clahe[3]; int gk_clahe[3];
+    uint8_t* d_raw; int raw_pitch;
+    uint8_t* d_lut;
     uint8_t* d_pyr[3][4];
     LKMapSet lk_maps[3];                   // [cur slot]: previous pyramid = slot (cur + 2) % 3
     int lw[4], lh[4], lp[4];
@@ -515,6 +525,7 @@ void gf_tracker_destroy(gf_tracker* t)
         for (cudaGraphExec_t g : {t->gb_prep[k], t->gb_dep[k], t->gb_both[k]}) if (g) cudaGraphExecDestroy(g);
         for (int p = 0; p < 2; p++) if (t->g_dep1[k][p]) cudaGraphExecDestroy(t->g_dep1[k][p]);
     }
+    for (int k = 0; k < 3; k++) if (t->g_clahe[k]) cudaGraphExecDestroy(t->g_clahe[k]);
     for (int s = 0; s < 3; s++) for (int l = 0; l < 4; l++) cudaFree(t->d_pyr[s][l]);
     for (int i = 0; i < 2; i++) {
         cudaFree(t->d_depth[i]); cudaFree(t->d_eig[i]); cudaFree(t->d_out[i]); cudaFree(t->d_fp[i]);
@@ -524,6 +535,7 @@ void gf_tracker_destroy(gf_tracker* t)
         for (cudaEvent_t e : {t->ev_up[i], t->ev_pyr[i], t->ev_eig[i], t->ev_dep[i], t->ev_t0[i], t->ev_out[i]}) if (e) cudaEventDestroy(e);
     }
     cudaFree(t->d_cov); cudaFree(t->d_box);
+    cudaFree(t->d_raw); cudaFree(t->d_lut);
     free_nms_grid(t->grid);
     cudaFree(t->d_sc);
     FeatArrays& fa = t->fa;
@@ -539,6 +551,27 @@ void gf_tracker_destroy(gf_tracker* t)
     if (t->ev_span1) cudaEventDestroy(t->ev_span1);
     cudaGetLastError();
     delete t;
+}
+
+int gf_tracker_set_equalize(gf_tracker* t, double clip_limit, int tiles_x, int tiles_y)
+{
+    if (!t) return set_err(GF_ERR_INVALID_ARG, "null tracker");
+    // accepted before the first frame only: no captured graph ever has to change
+    if (t->n_submitted > 0) return set_err(GF_ERR_INVALID_ARG, "gf_tracker_set_equalize must be called before the first frame");
+    if (tiles_x == 0) { t->equalize = false; return GF_OK; }
+    ClaheGeom g;
+    int rc = clahe_geometry(g, t->w, t->h, clip_limit, tiles_x, tiles_y);
+    if (rc) return rc;
+    GF_CUDA(cudaSetDevice(t->device));
+    rc = clahe_prepare(); if (rc) return rc;
+    if (!t->d_raw) {
+        t->raw_pitch = align_up(t->w, 16);
+        GF_CUDA(cudaMalloc(&t->d_raw, (size_t)t->raw_pitch * t->h));
+    }
+    if (!t->d_lut) GF_CUDA(cudaMalloc(&t->d_lut, (size_t)CLAHE_MAX_TILES * CLAHE_MAX_TILES * 256));
+    t->clahe = g;
+    t->equalize = true;
+    return GF_OK;
 }
 
 int gf_tracker_host_buffers(gf_tracker* t, uint8_t** gray, uint16_t** depth)
@@ -625,7 +658,8 @@ static int run_piece(gf_tracker* t, cudaStream_t s, cudaGraphExec_t* exec, int* 
     return GF_OK;
 }
 
-// Everything after the H2D (or D2D) copies of frame f have been enqueued on s_up.
+// Everything after the H2D (or D2D) copies of frame f have been enqueued on s_up.  With equalisation the gray frame is in
+// d_raw and CLAHE writes pyramid level 0 on s_up, ahead of ev_up (profiling: part of stage 1).
 static int enqueue_frame(gf_tracker* t, long long f, double time, bool depth_valid)
 {
     const int es = (int)(f % 2), key = (int)(f % 6), hp = t->has_pred ? 1 : 0;
@@ -633,6 +667,13 @@ static int enqueue_frame(gf_tracker* t, long long f, double time, bool depth_val
     t->h_fp[es]->has_pred = hp;
     t->h_fp[es]->depth_valid = depth_valid ? 1 : 0;
     GF_MARK(0, t->s_up);   // end of upload
+    if (t->equalize) {
+        const int slot = (int)(f % 3);
+        int rc = run_piece(t, t->s_up, &t->g_clahe[slot], &t->gk_clahe[slot], [&] {
+            return enqueue_clahe(t->s_up, ClaheSrc{t->d_raw, t->raw_pitch, nullptr, nullptr}, t->clahe, t->d_lut, t->d_pyr[slot][0], t->lp[0]);
+        });
+        if (rc) return rc;
+    }
     GF_CUDA(cudaEventRecord(t->ev_up[es], t->s_up));
     GF_CUDA(cudaStreamWaitEvent(t->s_pyr, t->ev_up[es], 0));
     GF_CUDA(cudaStreamWaitEvent(t->s_eig, t->ev_up[es], 0));
@@ -669,8 +710,15 @@ static int body_prep_b(gf_tracker* t, long long f, cudaStream_t m)
 {
     const int es = (int)(f % 2), slot = (int)(f % 3);
     GF_CUDA(cudaMemcpyAsync(t->d_fp[es], t->h_fp[es], sizeof(FrameParams), cudaMemcpyHostToDevice, m));
-    dim3 g((2 * t->w + 16 * 256 - 1) / (16 * 256), 2 * t->h);
-    k_copy_in<<<g, 256, 0, m>>>(t->d_fp[es], t->d_pyr[slot][0], t->lp[0], t->d_depth[es], t->depth_pitch_el, t->w, t->h); GF_LAUNCHED();
+    // with equalisation k_copy_in only takes the depth image, and CLAHE reads the gray frame at the address in FrameParams
+    const int row0 = t->equalize ? t->h : 0;
+    dim3 g((2 * t->w + 16 * 256 - 1) / (16 * 256), 2 * t->h - row0);
+    k_copy_in<<<g, 256, 0, m>>>(t->d_fp[es], t->d_pyr[slot][0], t->lp[0], t->d_depth[es], t->depth_pitch_el, t->w, t->h, row0); GF_LAUNCHED();
+    if (t->equalize) {
+        const ClaheSrc src{nullptr, 0, &t->d_fp[es]->src_gray, &t->d_fp[es]->src_gray_pitch};
+        int rc = enqueue_clahe(m, src, t->clahe, t->d_lut, t->d_pyr[slot][0], t->lp[0]);
+        if (rc) return rc;
+    }
     GF_CUDA(cudaEventRecord(t->ev_fork2, m));
     GF_CUDA(cudaStreamWaitEvent(t->s_eig, t->ev_fork2, 0));
     int rc = enqueue_pyramid(m, t, slot);
@@ -731,7 +779,8 @@ int gf_tracker_submit(gf_tracker* t, double time, const uint8_t* gray, size_t gr
     cudaStream_t s = t->s_up;
     GF_CUDA(cudaEventRecord(t->ev_t0[f % 2], s));
     t->t0_valid[f % 2] = true;
-    GF_CUDA(cudaMemcpy2DAsync(t->d_pyr[f % 3][0], t->lp[0], gray, gray_pitch, w, h, cudaMemcpyHostToDevice, s));
+    if (t->equalize) GF_CUDA(cudaMemcpy2DAsync(t->d_raw, t->raw_pitch, gray, gray_pitch, w, h, cudaMemcpyHostToDevice, s));
+    else GF_CUDA(cudaMemcpy2DAsync(t->d_pyr[f % 3][0], t->lp[0], gray, gray_pitch, w, h, cudaMemcpyHostToDevice, s));
     if (depth)
         GF_CUDA(cudaMemcpy2DAsync(t->d_depth[f % 2], (size_t)t->depth_pitch_el * 2, depth, depth_pitch, (size_t)w * 2, h, cudaMemcpyHostToDevice, s));
     return enqueue_frame(t, f, time, depth != nullptr);
@@ -748,7 +797,8 @@ int gf_tracker_submit_device(gf_tracker* t, double time, const void* d_gray, con
     cudaStream_t s = t->s_up;
     GF_CUDA(cudaEventRecord(t->ev_t0[f % 2], s));
     t->t0_valid[f % 2] = true;
-    GF_CUDA(cudaMemcpy2DAsync(t->d_pyr[f % 3][0], t->lp[0], d_gray, w, w, h, cudaMemcpyDeviceToDevice, s));
+    if (t->equalize) GF_CUDA(cudaMemcpy2DAsync(t->d_raw, t->raw_pitch, d_gray, w, w, h, cudaMemcpyDeviceToDevice, s));
+    else GF_CUDA(cudaMemcpy2DAsync(t->d_pyr[f % 3][0], t->lp[0], d_gray, w, w, h, cudaMemcpyDeviceToDevice, s));
     if (d_depth)
         GF_CUDA(cudaMemcpy2DAsync(t->d_depth[f % 2], (size_t)t->depth_pitch_el * 2, d_depth, (size_t)w * 2, (size_t)w * 2, h, cudaMemcpyDeviceToDevice, s));
     return enqueue_frame(t, f, time, d_depth != nullptr);
@@ -1075,6 +1125,24 @@ int gf_stage_pyr_down(int device, const uint8_t* src, int w, int h, uint8_t* dst
     k_pyr_down<<<g, b>>>(L, dd.as<uint8_t>(), dw, dh, dp); GF_LAUNCHED();
     GF_CUDA(cudaGetLastError());
     GF_CUDA(cudaMemcpy2D(dst, dw, dd.p, dp, dw, dh, cudaMemcpyDeviceToHost));
+    return GF_OK;
+}
+
+int gf_stage_clahe(int device, const uint8_t* src, size_t src_pitch, int w, int h, double clip_limit, int tiles_x, int tiles_y, uint8_t* dst)
+{
+    if (!src || !dst || src_pitch < (size_t)w) return set_err(GF_ERR_INVALID_ARG, "bad argument");
+    if (((w + 7) / 8) < 48 || ((h + 7) / 8) < 48 || w > 8192 || h > 8192)
+        return set_err(GF_ERR_UNSUPPORTED, "image must be at least 377x377 and at most 8192x8192");
+    ClaheGeom g;
+    int rc = clahe_geometry(g, w, h, clip_limit, tiles_x, tiles_y); if (rc) return rc;
+    rc = select_device(device); if (rc) return rc;
+    rc = clahe_prepare(); if (rc) return rc;
+    DevBuf ds, dd, dl;
+    const int pitch = align_up(w, 16);
+    if ((rc = ds.alloc((size_t)pitch * h)) || (rc = dd.alloc((size_t)pitch * h)) || (rc = dl.alloc(clahe_lut_bytes(g)))) return rc;
+    GF_CUDA(cudaMemcpy2D(ds.p, pitch, src, src_pitch, w, h, cudaMemcpyHostToDevice));
+    rc = enqueue_clahe(0, ClaheSrc{ds.as<uint8_t>(), pitch, nullptr, nullptr}, g, dl.as<uint8_t>(), dd.as<uint8_t>(), pitch); if (rc) return rc;
+    GF_CUDA(cudaMemcpy2D(dst, w, dd.p, pitch, w, h, cudaMemcpyDeviceToHost));
     return GF_OK;
 }
 

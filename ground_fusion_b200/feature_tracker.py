@@ -27,6 +27,17 @@ def pyr_down(img, device=0):
     return out
 
 
+def clahe(img, clip_limit=40.0, tile_grid=(8, 8), device=0):
+    """cv2.createCLAHE(clip_limit, tile_grid).apply(img) for u8 images (the kernels of the tracker's equalize option).
+    Row-padded views are passed with their row pitch."""
+    img = FeatureTracker._rows(img, np.uint8)
+    h, w = img.shape
+    out = np.empty((h, w), np.uint8)
+    check(_lib.lib().gf_stage_clahe(device, img.ctypes.data, img.strides[0], w, h, float(clip_limit), int(tile_grid[0]),
+                                    int(tile_grid[1]), out.ctypes.data))
+    return out
+
+
 def corner_min_eigen_val(img, device=0):
     img = _u8(img)
     h, w = img.shape
@@ -72,13 +83,21 @@ def setmask_order(track_cnt, device=0):
 class FeatureTracker:
     """trackImage / setPrediction / removeOutliers as in feature_tracker.h:47,70,72.
 
-    readIntrinsicParameter is folded into the constructor (pinhole = fx fy cx cy k1 k2 p1 p2)."""
+    readIntrinsicParameter is folded into the constructor (pinhole = fx fy cx cy k1 k2 p1 p2).  equalize: the config key
+    EQUALIZE -- every frame goes through cv::createCLAHE(clahe_clip, clahe_grid) first, as getImageFromMsg does."""
 
-    def __init__(self, width, height, pinhole, max_cnt=150, min_dist=30, flow_back=1, depth_cam=1, device=0):
+    def __init__(self, width, height, pinhole, max_cnt=150, min_dist=30, flow_back=1, depth_cam=1, device=0,
+                 equalize=False, clahe_clip=40.0, clahe_grid=(8, 8)):
         self.L = _lib.lib()
         cfg = TrackerCfg(int(max_cnt), int(min_dist), int(flow_back), int(depth_cam), (ctypes.c_double * 8)(*pinhole))
         self._h = ctypes.c_void_p()
         check(self.L.gf_tracker_create(ctypes.byref(self._h), int(device), int(width), int(height), ctypes.byref(cfg)))
+        if equalize:
+            try:
+                check(self.L.gf_tracker_set_equalize(self._h, float(clahe_clip), int(clahe_grid[0]), int(clahe_grid[1])))
+            except Exception:
+                self.close()
+                raise
         self.width, self.height, self.max_cnt = width, height, int(max_cnt)
         self._obs = np.zeros(self.max_cnt, OBS_DTYPE)
         self._status = np.zeros(self.max_cnt, np.uint8)
@@ -223,6 +242,10 @@ class FeatureTracker:
     def removeOutliers(self, removePtsIds):
         ids = np.array(sorted(removePtsIds), np.int32)
         check(self.L.gf_tracker_remove_ids(self._h, ids.ctypes.data if len(ids) else None, len(ids)))
+
+    def set_equalize(self, clip_limit=40.0, tile_grid=(8, 8)):
+        """gf_tracker_set_equalize: only before the first frame; tile_grid (0, 0) turns it off."""
+        check(self.L.gf_tracker_set_equalize(self._h, float(clip_limit), int(tile_grid[0]), int(tile_grid[1])))
 
     def set_profiling(self, on=True):
         check(self.L.gf_tracker_set_profiling(self._h, int(bool(on))))

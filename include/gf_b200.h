@@ -130,6 +130,14 @@ int gf_tracker_track_batch_multi(gf_tracker* const* trackers, int n_trackers, in
                                  size_t gray_pitch, const void* const* depth, size_t depth_pitch, int on_device,
                                  gf_obs* out, int* n_out, uint8_t* status_out, gf_track_info* info);
 
+/* The config key `equalize` (parameters.h:33): cv::createCLAHE(clip_limit, Size(tiles_x, tiles_y))->apply on every gray frame
+ * before it is tracked, as getImageFromMsg does (rosNodeTest.cpp:256-261; the reference's call is createCLAHE() with its
+ * defaults, clip_limit 40 and an 8 x 8 grid).  LK on both pyramids, goodFeaturesToTrack and the grey > 250 test then all see
+ * the equalised image, bit-exact with OpenCV 4.13.  Off by default; tiles_x = 0 turns it off.  1 <= tiles_x, tiles_y <= 16;
+ * clip_limit <= 0: no clipping.  Accepted only before the first frame is submitted (GF_ERR_INVALID_ARG afterwards).
+ * Covers every intake path: _track / _submit, _track_device / _submit_device and the batch calls. */
+int gf_tracker_set_equalize(gf_tracker* t, double clip_limit, int tiles_x, int tiles_y);
+
 /* FeatureTracker::setPrediction (feature_tracker.cpp:1006-1027): xyz are camera-frame 3-D points. */
 int gf_tracker_set_prediction(gf_tracker* t, const int32_t* ids, const double* xyz, int n);
 /* FeatureTracker::removeOutliers (feature_tracker.cpp:1029-1045). */
@@ -160,6 +168,10 @@ int gf_tracker_debug_read(gf_tracker* t, long long* out, int n);
  * ---------------------------------------------------------------------------------------------- */
 /* cv::pyrDown on u8 (LK pyramid level). dst is ((w+1)/2) x ((h+1)/2), tightly packed. */
 int gf_stage_pyr_down(int device, const uint8_t* src, int w, int h, uint8_t* dst);
+/* cv::createCLAHE(clip_limit, Size(tiles_x, tiles_y))->apply(src, dst) on u8 with the tracker's kernels (gf_tracker_set_equalize).
+ * src rows are src_pitch bytes apart; dst is w x h, tightly packed.  Same limits as the tracker's image and tile grid. */
+int gf_stage_clahe(int device, const uint8_t* src, size_t src_pitch, int w, int h, double clip_limit, int tiles_x, int tiles_y,
+                   uint8_t* dst);
 /* cv::cornerMinEigenVal(img, blockSize=3, ksize=3) as used by goodFeaturesToTrack. */
 int gf_stage_min_eig(int device, const uint8_t* img, int w, int h, float* eig, int* n_fixups);
 /* cv::calcOpticalFlowPyrLK(prev, next, prev_pts, next_pts, status, err, Size(21,21), max_level,
