@@ -9,6 +9,7 @@
 #include <utility>
 #include <vector>
 
+#include <darknet_ros_msgs/BoundingBoxes.h>
 #include <eigen3/Eigen/Dense>
 #include <opencv2/opencv.hpp>
 
@@ -30,6 +31,10 @@ class FeatureTracker
     FeatureTracker &operator=(const FeatureTracker &) = delete;
 
     std::map<int, std::vector<std::pair<int, Eigen::Matrix<double, 8, 1>>>> trackImage(double _cur_time, const cv::Mat &_img, const cv::Mat &_img1 = cv::Mat());
+    // USE_YOLO (Estimator::inputImagebox): trackImage, with the features strictly inside a detected box left out of the returned
+    // frame only; cur_pts / ids / track_cnt keep them, as the reference's do (feature_tracker.cpp:374-678)
+    std::map<int, std::vector<std::pair<int, Eigen::Matrix<double, 8, 1>>>> trackImagebox(double _cur_time, const darknet_ros_msgs::BoundingBoxesConstPtr &_boxes,
+                                                                                          const cv::Mat &_img, const cv::Mat &_img1 = cv::Mat());
     // readIntrinsicParameter(calib_file, depth) (feature_tracker.cpp:745-762) parses the camodocal YAML; the parsed PINHOLE
     // parameters are all this path needs.  With camodocal present: m_camera[0]->writeParameters(p) -> setPinhole(p[4..7], p[0..3]).
     void setPinhole(double fx, double fy, double cx, double cy, double k1, double k2, double p1, double p2, int depth);
@@ -47,7 +52,11 @@ class FeatureTracker
     int device = 0;          // CUDA device of this camera stream
 
   private:
+    void start(double _cur_time, const cv::Mat &_img);
+    std::map<int, std::vector<std::pair<int, Eigen::Matrix<double, 8, 1>>>> publish(int n, const uint8_t *in_box);
     gf_tracker *gf_ = nullptr;          // created on the first frame: needs its size
     gf_tracker_cfg cfg_{};
     std::vector<gf_obs> out_;
+    std::vector<uint8_t> in_box_;
+    std::vector<gf_box> boxes_;
 };

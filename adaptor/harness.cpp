@@ -1,10 +1,13 @@
 // Drives the adaptor classes from flat binary dumps written by tests/test_adaptor.py; the outputs go back as flat binaries.
 //   harness fe <in> <out>   frames through FeatureTracker::trackImage
 //   harness fe-eq <in> <out>  the same with EQUALIZE = 1
+//   harness fe-box <in> <out> frames and their detections (int m, m x 4 int64 after each frame) through
+//                             FeatureTracker::trackImagebox; after each featureFrame: cur_pts as (n, n x (id, x, y, track_cnt))
 //   harness ba <in> <out>   one window through Estimator::optimization()
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <vector>
 
 #include "estimator_ba.h"
@@ -18,7 +21,7 @@ Eigen::Vector3d G;
 static void rd(FILE *f, void *p, size_t n) { if (fread(p, 1, n, f) != n) { std::fprintf(stderr, "short read\n"); std::exit(2); } }
 template <class T> static T rd1(FILE *f) { T v; rd(f, &v, sizeof(T)); return v; }
 
-static int run_fe(const char *in, const char *out)
+static int run_fe(const char *in, const char *out, bool with_boxes)
 {
     FILE *f = fopen(in, "rb"), *o = fopen(out, "wb");
     if (!f || !o) return 2;
@@ -34,12 +37,28 @@ static int run_fe(const char *in, const char *out)
         if (with_depth) rd(f, depth.data(), depth.size() * 2);
         cv::Mat img(h, w, CV_8UC1, gray.data()), dimg;
         if (with_depth) dimg = cv::Mat(h, w, CV_16UC1, depth.data());
-        auto frame = tracker.trackImage(t, img, dimg);
+        std::map<int, std::vector<std::pair<int, Eigen::Matrix<double, 8, 1>>>> frame;
+        if (with_boxes) {
+            auto msg = std::make_shared<darknet_ros_msgs::BoundingBoxes>();
+            msg->bounding_boxes.resize(rd1<int>(f));
+            for (auto &b : msg->bounding_boxes) { b.xmin = rd1<int64_t>(f); b.ymin = rd1<int64_t>(f); b.xmax = rd1<int64_t>(f); b.ymax = rd1<int64_t>(f); }
+            frame = tracker.trackImagebox(t, msg, img, dimg);
+        } else {
+            frame = tracker.trackImage(t, img, dimg);
+        }
         const int m = (int)frame.size();
         fwrite(&m, 4, 1, o);
         for (auto &kv : frame) {                                   // std::map: ascending feature id, as featureBuf consumers see it
             fwrite(&kv.first, 4, 1, o);
             fwrite(kv.second[0].second.data(), 8, 8, o);
+        }
+        if (with_boxes) {
+            const int np = (int)tracker.cur_pts.size();
+            fwrite(&np, 4, 1, o);
+            for (int i = 0; i < np; i++) {
+                fwrite(&tracker.ids[i], 4, 1, o); fwrite(&tracker.cur_pts[i].x, 4, 1, o); fwrite(&tracker.cur_pts[i].y, 4, 1, o);
+                fwrite(&tracker.track_cnt[i], 4, 1, o);
+            }
         }
     }
     fclose(f); fclose(o);
@@ -99,7 +118,7 @@ static int run_ba(const char *in, const char *out)
 
 int main(int argc, char **argv)
 {
-    if (argc != 4) { std::fprintf(stderr, "usage: harness fe|fe-eq|ba <in> <out>\n"); return 2; }
+    if (argc != 4) { std::fprintf(stderr, "usage: harness fe|fe-eq|fe-box|ba <in> <out>\n"); return 2; }
     if (!std::strcmp(argv[1], "fe-eq")) EQUALIZE = 1;
-    return argv[1][0] == 'f' ? run_fe(argv[2], argv[3]) : run_ba(argv[2], argv[3]);
+    return argv[1][0] == 'f' ? run_fe(argv[2], argv[3], !std::strcmp(argv[1], "fe-box")) : run_ba(argv[2], argv[3]);
 }

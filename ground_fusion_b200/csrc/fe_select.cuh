@@ -494,6 +494,21 @@ __device__ __forceinline__ void cam_project(const CamParams& c, double X, double
 
 struct OutHeader { int n_out, n_prev, n_tracked, n_kept, n_new, n_cand, nms_rounds, eig_fixups, lk_iters, pad; };
 
+// The detections of one frame (trackImagebox, feature_tracker.cpp:374-678), converted on the host: box k is
+// b[k] = (lo_x, hi_x, lo_y, hi_y) with the corners as the reference has them, (float)(int)xmin etc.
+constexpr int GF_BOX_CAP = 100;      // GF_MAX_BOXES
+struct BoxSet { int n; int pad[3]; float4 b[GF_BOX_CAP]; };
+
+// pointPolygonTest(contour {xmin,ymin},{xmin,ymax},{xmax,ymax},{xmax,ymin}, pt, true) > 0 for any box: strictly inside.
+// For this axis-aligned contour the signed distance is positive exactly on the open rectangle between the float corners
+// (pinned against cv2 by tests/test_box_oracle.py), so the polygon test is four comparisons per box.
+__device__ __forceinline__ bool in_any_box(const float4* b, int n, float2 p)
+{
+    bool in = false;
+    for (int k = 0; k < n; k++) in |= (b[k].x < p.x) & (p.x < b[k].y) & (b[k].z < p.y) & (p.y < b[k].w);
+    return in;
+}
+
 // min-distance rounds, then top-K of the accepted corners, addPoints, undistortedPts, ptsVelocity, depth,
 // next-frame state.  Single CTA of 1024 threads; dynamic shared memory for the cell grid (see nms_cells).
 __global__ void __launch_bounds__(1024) k_select_finalize(TrackScalars* sc, FeatArrays fa, NmsGrid g, int w, int max_cnt, int min_dist,
@@ -502,12 +517,17 @@ __global__ void __launch_bounds__(1024) k_select_finalize(TrackScalars* sc, Feat
                                                           uint8_t* out_status /* may be null: copy of the LK status of the n_prev input features */,
                                                           uint4* host_mirror = nullptr /* batch pipeline: pinned host copy of the result block, written
                                                           by this kernel (16 B per thread, coalesced) instead of a D2H copy node on the dependent chain */,
-                                                          int mirror_obs_offset = 0 /* offsetof(OutBlock, obs) */)
+                                                          int mirror_obs_offset = 0 /* offsetof(OutBlock, obs) */,
+                                                          const BoxSet* boxes = nullptr /* the frame's detections, or null */,
+                                                          uint32_t* out_in_box = nullptr /* FE_CAP bits: output i lies inside a box */)
 {
     extern __shared__ __align__(16) unsigned char dyn_smem[];
     __shared__ unsigned long long keys[FE_SORT_CAP];
+    __shared__ float4 s_box[GF_BOX_CAP];
     const int tid = threadIdx.x;
     gf_pdl_wait();
+    const int n_box = boxes ? boxes->n : 0;
+    if (tid < n_box) s_box[tid] = boxes->b[tid];            // visible after the barriers of nms_cells
     const long long c0 = gf_clock();
     nms_cells(sc, g, w, min_dist, dyn_smem, fa.dbg);
     const long long c1 = gf_clock();
@@ -569,6 +589,7 @@ __global__ void __launch_bounds__(1024) k_select_finalize(TrackScalars* sc, Feat
     const int total = n_kept + n_new;
     const int n_id = sc->n_id;
     // addPoints + per-feature outputs; thread i <-> feature i of the new cur_pts order (kept..., new...)
+    bool boxed = false;
     if (tid < total) {
         float2 p, un_prev = make_float2(0.f, 0.f);
         int id, cnt;
@@ -600,6 +621,11 @@ __global__ void __launch_bounds__(1024) k_select_finalize(TrackScalars* sc, Feat
         out_obs[tid] = o;
         // state for the next frame (prev_pts = cur_pts; prev_un_pts_map = cur_un_pts_map)
         fa.prev_pts[tid] = p; fa.ids[tid] = id; fa.track_cnt[tid] = cnt; fa.prev_un[tid] = un;
+        boxed = in_any_box(s_box, n_box, p);
+    }
+    if (out_in_box) {       // a boxed feature stays in the state above; only featureFrame leaves it out
+        const unsigned bits = __ballot_sync(0xffffffffu, boxed);
+        if ((tid & 31) == 0) out_in_box[tid >> 5] = bits;
     }
     if (out_status && tid < sc->n_prev) out_status[tid] = fa.status[tid];
     __syncthreads();

@@ -11,7 +11,7 @@
 //   s_eig : (ev_up) k_cov_rows -> k_box_chain -> k_eig_from_box (ev_eig)
 //   s_main: (ev_pyr) [prediction LK] -> k_track (fwd LK 3 lvls + bwd LK 1 lvl + status rules) -> k_compact_setmask
 //           -> (ev_eig) masked max -> candidates -> k_select_finalize (min-distance rounds, top-K, addPoints,
-//           undistort, velocity, depth)  (ev_dep)
+//           undistort, velocity, depth; trackImagebox's in-box flags from the boxes in FrameParams)  (ev_dep)
 //   s_out : (ev_dep) D2H of the result block
 //
 // Buffers touched by more than one frame in flight are rotated: 3 pyramids (prev/cur/next), 2 depth images, 2 eig
@@ -36,7 +36,37 @@ struct FrameParams {
     double dt; int has_pred; int depth_valid;
     // batch pipeline only: where k_copy_in finds the frame (device pointers: the caller's, or the tracker's staging buffers)
     const uint8_t* src_gray; const uint16_t* src_depth; long long src_gray_pitch, src_depth_pitch;   // pitches in bytes
+    BoxSet boxes;            // trackImagebox's detections (n = 0: trackImage)
 };
+
+// The reference copies the int64 fields of darknet_ros_msgs/BoundingBox into `int` (a modular wrap) and those into the float
+// contour; the bounds of the open rectangle are kept ordered so that inverted boxes test as the contour does.
+static void put_boxes(BoxSet& s, const gf_box* b, int n)
+{
+    s.n = n;
+    for (int k = 0; k < n; k++) {
+        const float x0 = (float)(int32_t)(uint32_t)(uint64_t)b[k].xmin, y0 = (float)(int32_t)(uint32_t)(uint64_t)b[k].ymin;
+        const float x1 = (float)(int32_t)(uint32_t)(uint64_t)b[k].xmax, y1 = (float)(int32_t)(uint32_t)(uint64_t)b[k].ymax;
+        s.b[k] = make_float4(fminf(x0, x1), fmaxf(x0, x1), fminf(y0, y1), fmaxf(y0, y1));
+    }
+}
+static int check_boxes(const gf_box* b, int n)
+{
+    if (n < 0 || (n > 0 && !b)) return set_err(GF_ERR_INVALID_ARG, "bad box list");
+    if (n > GF_MAX_BOXES) return set_err(GF_ERR_CAPACITY, "more than GF_MAX_BOXES boxes in one frame");
+    return GF_OK;
+}
+
+// gf_stage_in_boxes: the test k_select_finalize applies to its outputs, on its own
+__global__ void __launch_bounds__(256) k_in_boxes_stage(const float2* pts, int n, const BoxSet* boxes, uint8_t* in_box)
+{
+    __shared__ float4 s_box[GF_BOX_CAP];
+    const int nb = boxes->n;
+    if ((int)threadIdx.x < nb) s_box[threadIdx.x] = boxes->b[threadIdx.x];
+    __syncthreads();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) in_box[i] = in_any_box(s_box, nb, pts[i]) ? 1 : 0;
+}
 
 // Frame intake of the batch pipeline: copies the frame named by *fp into pyramid level 0 and the depth slot (16 B per thread when
 // source and row pitch allow it).  A kernel instead of a memcpy node because the source address changes every frame while the
@@ -202,7 +232,8 @@ using namespace gf;
 
 // ------------------------------------------------------------------------------------------------
 constexpr int GF_PIPE = 2;           // frames in flight
-struct OutBlock { OutHeader hdr; uint8_t status[FE_CAP]; gf_obs obs[FE_CAP]; };   // one D2H copy per frame
+struct OutBlock { OutHeader hdr; uint8_t status[FE_CAP]; uint32_t in_box[FE_CAP / 32]; gf_obs obs[FE_CAP]; };   // one D2H copy per frame
+static_assert(GF_BOX_CAP == GF_MAX_BOXES, "BoxSet holds GF_MAX_BOXES boxes");
 
 struct gf_tracker {
     int device, w, h;
@@ -629,7 +660,8 @@ static int body_dep2(gf_tracker* t, long long f, bool mirror = false)
     GF_CUDA(launch_k(k_select_finalize, dim3(1), dim3(1024), t->grid_cells, s, pdl || (t->pdl_single_cta && !t->profiling), t->d_sc, t->fa, t->grid, t->w,
                      t->cfg.max_cnt, t->cfg.min_dist, t->cam, (const double*)&t->d_fp[es]->dt, (const uint16_t*)t->d_depth[es], t->depth_pitch_el, depth_mode,
                      (const int*)&t->d_fp[es]->depth_valid, t->h, &ob->hdr, ob->obs, ob->status,
-                     mirror ? reinterpret_cast<uint4*>(t->h_out[es]) : (uint4*)nullptr, (int)offsetof(OutBlock, obs))); GF_LAUNCHED();
+                     mirror ? reinterpret_cast<uint4*>(t->h_out[es]) : (uint4*)nullptr, (int)offsetof(OutBlock, obs),
+                     (const BoxSet*)&t->d_fp[es]->boxes, ob->in_box)); GF_LAUNCHED();
     GF_CUDA(cudaGetLastError());
     GF_MARK(5, s);
     return GF_OK;
@@ -660,12 +692,13 @@ static int run_piece(gf_tracker* t, cudaStream_t s, cudaGraphExec_t* exec, int* 
 
 // Everything after the H2D (or D2D) copies of frame f have been enqueued on s_up.  With equalisation the gray frame is in
 // d_raw and CLAHE writes pyramid level 0 on s_up, ahead of ev_up (profiling: part of stage 1).
-static int enqueue_frame(gf_tracker* t, long long f, double time, bool depth_valid)
+static int enqueue_frame(gf_tracker* t, long long f, double time, bool depth_valid, const gf_box* boxes, int n_boxes)
 {
     const int es = (int)(f % 2), key = (int)(f % 6), hp = t->has_pred ? 1 : 0;
     t->h_fp[es]->dt = time - t->prev_time;
     t->h_fp[es]->has_pred = hp;
     t->h_fp[es]->depth_valid = depth_valid ? 1 : 0;
+    put_boxes(t->h_fp[es]->boxes, boxes, n_boxes);
     GF_MARK(0, t->s_up);   // end of upload
     if (t->equalize) {
         const int slot = (int)(f % 3);
@@ -763,7 +796,8 @@ static int check_submit(gf_tracker* t)
     return GF_OK;
 }
 
-int gf_tracker_submit(gf_tracker* t, double time, const uint8_t* gray, size_t gray_pitch, const uint16_t* depth, size_t depth_pitch)
+static int submit_host(gf_tracker* t, double time, const uint8_t* gray, size_t gray_pitch, const uint16_t* depth, size_t depth_pitch,
+                       const gf_box* boxes, int n_boxes)
 {
     if (!t || !gray) return set_err(GF_ERR_INVALID_ARG, "null argument");
     int rc = check_submit(t);
@@ -783,10 +817,10 @@ int gf_tracker_submit(gf_tracker* t, double time, const uint8_t* gray, size_t gr
     else GF_CUDA(cudaMemcpy2DAsync(t->d_pyr[f % 3][0], t->lp[0], gray, gray_pitch, w, h, cudaMemcpyHostToDevice, s));
     if (depth)
         GF_CUDA(cudaMemcpy2DAsync(t->d_depth[f % 2], (size_t)t->depth_pitch_el * 2, depth, depth_pitch, (size_t)w * 2, h, cudaMemcpyHostToDevice, s));
-    return enqueue_frame(t, f, time, depth != nullptr);
+    return enqueue_frame(t, f, time, depth != nullptr, boxes, n_boxes);
 }
 
-int gf_tracker_submit_device(gf_tracker* t, double time, const void* d_gray, const void* d_depth)
+static int submit_dev(gf_tracker* t, double time, const void* d_gray, const void* d_depth, const gf_box* boxes, int n_boxes)
 {
     if (!t || !d_gray) return set_err(GF_ERR_INVALID_ARG, "null argument");
     int rc = check_submit(t);
@@ -801,10 +835,29 @@ int gf_tracker_submit_device(gf_tracker* t, double time, const void* d_gray, con
     else GF_CUDA(cudaMemcpy2DAsync(t->d_pyr[f % 3][0], t->lp[0], d_gray, w, w, h, cudaMemcpyDeviceToDevice, s));
     if (d_depth)
         GF_CUDA(cudaMemcpy2DAsync(t->d_depth[f % 2], (size_t)t->depth_pitch_el * 2, d_depth, (size_t)w * 2, (size_t)w * 2, h, cudaMemcpyDeviceToDevice, s));
-    return enqueue_frame(t, f, time, d_depth != nullptr);
+    return enqueue_frame(t, f, time, d_depth != nullptr, boxes, n_boxes);
 }
 
-int gf_tracker_wait(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* status_out, gf_track_info* info)
+int gf_tracker_submit(gf_tracker* t, double time, const uint8_t* gray, size_t gray_pitch, const uint16_t* depth, size_t depth_pitch)
+{
+    return submit_host(t, time, gray, gray_pitch, depth, depth_pitch, nullptr, 0);
+}
+
+int gf_tracker_submit_device(gf_tracker* t, double time, const void* d_gray, const void* d_depth)
+{
+    return submit_dev(t, time, d_gray, d_depth, nullptr, 0);
+}
+
+int gf_tracker_submit_boxes(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch,
+                            int on_device, const gf_box* boxes, int n_boxes)
+{
+    int rc = check_boxes(boxes, n_boxes);
+    if (rc) return rc;
+    return on_device ? submit_dev(t, time, gray, depth, boxes, n_boxes)
+                     : submit_host(t, time, (const uint8_t*)gray, gray_pitch, (const uint16_t*)depth, depth_pitch, boxes, n_boxes);
+}
+
+int gf_tracker_wait_boxes(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info)
 {
     if (!t) return set_err(GF_ERR_INVALID_ARG, "null tracker");
     if (in_flight(t) == 0) return set_err(GF_ERR_INVALID_ARG, "no frame in flight");
@@ -825,12 +878,18 @@ int gf_tracker_wait(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* status_out,
     if (t->cfg.depth_cam && !t->depth_valid[es]) n = 0;   // see body_dep2
     if (n_out) *n_out = n;
     if (out && n > 0) memcpy(out, ob.obs, (size_t)n * sizeof(gf_obs));
+    if (in_box) for (int i = 0; i < n; i++) in_box[i] = (uint8_t)((ob.in_box[i >> 5] >> (i & 31)) & 1u);
     if (status_out && hd.n_prev > 0) memcpy(status_out, ob.status, hd.n_prev);
     if (info) {
         info->n_prev = hd.n_prev; info->n_tracked = hd.n_tracked; info->n_kept = hd.n_kept; info->n_new = hd.n_new;
         info->n_candidates = hd.n_cand; info->nms_rounds = hd.nms_rounds; info->eig_fixups = hd.eig_fixups; info->lk_iterations = hd.lk_iters;
     }
     return GF_OK;
+}
+
+int gf_tracker_wait(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* status_out, gf_track_info* info)
+{
+    return gf_tracker_wait_boxes(t, out, n_out, nullptr, status_out, info);
 }
 
 int gf_tracker_track(gf_tracker* t, double time, const uint8_t* gray, size_t gray_pitch, const uint16_t* depth, size_t depth_pitch,
@@ -851,26 +910,40 @@ int gf_tracker_track_device(gf_tracker* t, double time, const void* d_gray, cons
     return gf_tracker_wait(t, out, n_out, status_out, info);
 }
 
+int gf_tracker_track_boxes(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch, int on_device,
+                           const gf_box* boxes, int n_boxes, gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info)
+{
+    if (t && in_flight(t) > 0) return set_err(GF_ERR_INVALID_ARG, "previous frame not collected: call gf_tracker_wait first");
+    int rc = gf_tracker_submit_boxes(t, time, gray, gray_pitch, depth, depth_pitch, on_device, boxes, n_boxes);
+    if (rc) return rc;
+    return gf_tracker_wait_boxes(t, out, n_out, in_box, status_out, info);
+}
+
 // One camera stream of a batch call: its frames, where its results go, and how far it has got.
 struct BatchLane {
     gf_tracker* t;
     const double* times; const void* const* gray; const void* const* depth;
     gf_obs* out; int* n_out; uint8_t* status_out; gf_track_info* info;
+    const gf_box* boxes; const int* box_start; uint8_t* in_box;     // frame k: boxes[box_start[k] .. box_start[k + 1]); nullable
     int collected, k0;
+    const gf_box* frame_boxes(int k) const { return box_start ? boxes + box_start[k] : nullptr; }
+    int n_boxes(int k) const { return box_start ? box_start[k + 1] - box_start[k] : 0; }
 };
 
 static int lane_collect(BatchLane& L)
 {
     const int k = L.collected++;
     const size_t cap = (size_t)L.t->cfg.max_cnt;
-    return gf_tracker_wait(L.t, L.out ? L.out + (size_t)k * cap : nullptr, L.n_out ? L.n_out + k : nullptr,
-                           L.status_out ? L.status_out + (size_t)k * cap : nullptr, L.info ? L.info + k : nullptr);
+    return gf_tracker_wait_boxes(L.t, L.out ? L.out + (size_t)k * cap : nullptr, L.n_out ? L.n_out + k : nullptr,
+                                 L.in_box ? L.in_box + (size_t)k * cap : nullptr, L.status_out ? L.status_out + (size_t)k * cap : nullptr,
+                                 L.info ? L.info + k : nullptr);
 }
 static int lane_submit_plain(BatchLane& L, int k, size_t gray_pitch, size_t depth_pitch, int on_device)
 {
     const void* dk = L.depth ? L.depth[k] : nullptr;
-    return on_device ? gf_tracker_submit_device(L.t, L.times[k], L.gray[k], dk)
-                     : gf_tracker_submit(L.t, L.times[k], (const uint8_t*)L.gray[k], gray_pitch, (const uint16_t*)dk, depth_pitch);
+    return on_device ? submit_dev(L.t, L.times[k], L.gray[k], dk, L.frame_boxes(k), L.n_boxes(k))
+                     : submit_host(L.t, L.times[k], (const uint8_t*)L.gray[k], gray_pitch, (const uint16_t*)dk, depth_pitch,
+                                   L.frame_boxes(k), L.n_boxes(k));
 }
 // Makes frame k reachable by its intake kernel: fills the pinned FrameParams slot the graph uploads and, for host frames,
 // copies them to the staging slot on s_up (s_main then waits for that copy before the graph that holds prep(k)).
@@ -883,6 +956,7 @@ static int lane_stage(BatchLane& L, int k, long long f, size_t gray_pitch, size_
     fp->dt = L.times[k] - (k > 0 ? L.times[k - 1] : t->prev_time);
     fp->has_pred = 0;
     fp->depth_valid = dk ? 1 : 0;
+    put_boxes(fp->boxes, L.frame_boxes(k), L.n_boxes(k));
     if (on_device) {
         fp->src_gray = (const uint8_t*)L.gray[k]; fp->src_gray_pitch = w;
         fp->src_depth = (const uint16_t*)dk; fp->src_depth_pitch = 2ll * w;
@@ -921,11 +995,19 @@ static int lane_issue(BatchLane& L, int k, int n, size_t gray_pitch, size_t dept
     return GF_OK;
 }
 
-int gf_tracker_track_batch_multi(gf_tracker* const* trackers, int n_trackers, int n, const double* times, const void* const* gray, size_t gray_pitch,
-                                 const void* const* depth, size_t depth_pitch, int on_device,
-                                 gf_obs* out, int* n_out, uint8_t* status_out, gf_track_info* info)
+int gf_tracker_track_batch_multi_boxes(gf_tracker* const* trackers, int n_trackers, int n, const double* times, const void* const* gray,
+                                       size_t gray_pitch, const void* const* depth, size_t depth_pitch, int on_device,
+                                       const gf_box* boxes, const int* box_start, gf_obs* out, int* n_out, uint8_t* in_box,
+                                       uint8_t* status_out, gf_track_info* info)
 {
     if (!trackers || n_trackers < 1 || n < 0 || (n > 0 && (!times || !gray))) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    if (box_start && n > 0) {            // every frame's list is checked before the first frame is submitted
+        for (long long k = 0; k < (long long)n_trackers * n; k++) {
+            if (box_start[k] < 0) return set_err(GF_ERR_INVALID_ARG, "bad box offsets");
+            int rc = check_boxes(boxes ? boxes + box_start[k] : nullptr, box_start[k + 1] - box_start[k]);
+            if (rc) return rc;
+        }
+    }
     std::vector<BatchLane> lanes((size_t)n_trackers);
     for (int i = 0; i < n_trackers; i++) {
         gf_tracker* t = trackers[i];
@@ -942,6 +1024,7 @@ int gf_tracker_track_batch_multi(gf_tracker* const* trackers, int n_trackers, in
         L.t = t; L.times = times + o; L.gray = gray + o; L.depth = depth ? depth + o : nullptr;
         L.out = out ? out + o * cap : nullptr; L.n_out = n_out ? n_out + o : nullptr;
         L.status_out = status_out ? status_out + o * cap : nullptr; L.info = info ? info + o : nullptr;
+        L.boxes = boxes; L.box_start = box_start ? box_start + o : nullptr; L.in_box = in_box ? in_box + o * cap : nullptr;
         L.collected = 0; L.k0 = 0;
         for (int k = 0; k < n; k++) if (!L.gray[k]) return set_err(GF_ERR_INVALID_ARG, "null frame pointer");
     }
@@ -995,11 +1078,27 @@ int gf_tracker_track_batch_multi(gf_tracker* const* trackers, int n_trackers, in
     return GF_OK;
 }
 
+int gf_tracker_track_batch_multi(gf_tracker* const* trackers, int n_trackers, int n, const double* times, const void* const* gray, size_t gray_pitch,
+                                 const void* const* depth, size_t depth_pitch, int on_device,
+                                 gf_obs* out, int* n_out, uint8_t* status_out, gf_track_info* info)
+{
+    return gf_tracker_track_batch_multi_boxes(trackers, n_trackers, n, times, gray, gray_pitch, depth, depth_pitch, on_device, nullptr, nullptr,
+                                              out, n_out, nullptr, status_out, info);
+}
+
 int gf_tracker_track_batch(gf_tracker* t, int n, const double* times, const void* const* gray, size_t gray_pitch,
                            const void* const* depth, size_t depth_pitch, int on_device,
                            gf_obs* out, int* n_out, uint8_t* status_out, gf_track_info* info)
 {
     return gf_tracker_track_batch_multi(&t, 1, n, times, gray, gray_pitch, depth, depth_pitch, on_device, out, n_out, status_out, info);
+}
+
+int gf_tracker_track_batch_boxes(gf_tracker* t, int n, const double* times, const void* const* gray, size_t gray_pitch,
+                                 const void* const* depth, size_t depth_pitch, int on_device, const gf_box* boxes, const int* box_start,
+                                 gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info)
+{
+    return gf_tracker_track_batch_multi_boxes(&t, 1, n, times, gray, gray_pitch, depth, depth_pitch, on_device, boxes, box_start,
+                                              out, n_out, in_box, status_out, info);
 }
 
 int gf_tracker_set_prediction(gf_tracker* t, const int32_t* ids, const double* xyz, int n)
@@ -1143,6 +1242,24 @@ int gf_stage_clahe(int device, const uint8_t* src, size_t src_pitch, int w, int 
     GF_CUDA(cudaMemcpy2D(ds.p, pitch, src, src_pitch, w, h, cudaMemcpyHostToDevice));
     rc = enqueue_clahe(0, ClaheSrc{ds.as<uint8_t>(), pitch, nullptr, nullptr}, g, dl.as<uint8_t>(), dd.as<uint8_t>(), pitch); if (rc) return rc;
     GF_CUDA(cudaMemcpy2D(dst, w, dd.p, pitch, w, h, cudaMemcpyDeviceToHost));
+    return GF_OK;
+}
+
+int gf_stage_in_boxes(int device, const float* pts, int n, const gf_box* boxes, int n_boxes, uint8_t* in_box)
+{
+    if (n < 0 || (n > 0 && (!pts || !in_box))) return set_err(GF_ERR_INVALID_ARG, "bad argument");
+    int rc = check_boxes(boxes, n_boxes); if (rc) return rc;
+    rc = select_device(device); if (rc) return rc;
+    if (n == 0) return GF_OK;
+    BoxSet bs;
+    put_boxes(bs, boxes, n_boxes);
+    DevBuf dp, db, dr;
+    if ((rc = dp.alloc((size_t)n * 8)) || (rc = db.alloc(sizeof(BoxSet))) || (rc = dr.alloc(n))) return rc;
+    GF_CUDA(cudaMemcpy(dp.p, pts, (size_t)n * 8, cudaMemcpyHostToDevice));
+    GF_CUDA(cudaMemcpy(db.p, &bs, sizeof(BoxSet), cudaMemcpyHostToDevice));
+    k_in_boxes_stage<<<(n + 255) / 256, 256>>>(dp.as<float2>(), n, db.as<BoxSet>(), dr.as<uint8_t>()); GF_LAUNCHED();
+    GF_CUDA(cudaGetLastError());
+    GF_CUDA(cudaMemcpy(in_box, dr.p, n, cudaMemcpyDeviceToHost));
     return GF_OK;
 }
 

@@ -70,6 +70,31 @@ def good_features_to_track(img, max_corners, min_dist, kept_pts=None, device=0):
     return out[:n.value].copy(), info.as_dict()
 
 
+def box_array(boxes):
+    """Detections as the (m, 4) int64 array of gf_box (xmin, ymin, xmax, ymax: the fields of darknet_ros_msgs/BoundingBox)."""
+    b = np.ascontiguousarray(np.zeros((0, 4)) if boxes is None or len(boxes) == 0 else boxes, np.int64).reshape(-1, 4)
+    return b
+
+
+def in_boxes(pts, boxes, device=0):
+    """trackImagebox's test on its own (gf_stage_in_boxes): 1 where pointPolygonTest(box contour, pt, true) > 0 for a box."""
+    p = np.ascontiguousarray(pts, np.float32).reshape(-1, 2)
+    b = box_array(boxes)
+    out = np.zeros(len(p), np.uint8)
+    check(_lib.lib().gf_stage_in_boxes(device, p.ctypes.data if len(p) else None, len(p), b.ctypes.data if len(b) else None, len(b),
+                                       out.ctypes.data if len(p) else None))
+    return out.view(np.bool_)
+
+
+def _box_csr(boxes):
+    """Per-frame box lists -> (gf_box array, n + 1 offsets)."""
+    arrs = [box_array(b) for b in boxes]
+    start = np.zeros(len(arrs) + 1, np.int32)
+    start[1:] = np.cumsum([len(a) for a in arrs])
+    flat = np.concatenate(arrs, 0) if arrs else np.zeros((0, 4), np.int64)
+    return np.ascontiguousarray(flat, np.int64), start
+
+
 def setmask_order(track_cnt, device=0):
     tc = np.ascontiguousarray(track_cnt, np.int32)
     perm = np.empty(len(tc), np.int32)
@@ -81,7 +106,7 @@ def setmask_order(track_cnt, device=0):
 
 
 class FeatureTracker:
-    """trackImage / setPrediction / removeOutliers as in feature_tracker.h:47,70,72.
+    """trackImage / trackImagebox / setPrediction / removeOutliers as in feature_tracker.h:47,48,70,72.
 
     readIntrinsicParameter is folded into the constructor (pinhole = fx fy cx cy k1 k2 p1 p2).  equalize: the config key
     EQUALIZE -- every frame goes through cv::createCLAHE(clahe_clip, clahe_grid) first, as getImageFromMsg does."""
@@ -150,6 +175,29 @@ class FeatureTracker:
         obs = self.trackImageRaw(cur_time, img, depth)
         return {int(o["id"]): o["v"].copy() for o in obs}
 
+    def trackImageboxRaw(self, cur_time, boxes, img, depth=None):
+        """trackImagebox (feature_tracker.cpp:374-678): (obs, in_box).  obs is exactly what trackImageRaw returns for the frame;
+        in_box[i] marks the features that trackImagebox leaves out of featureFrame because they lie strictly inside one of the
+        boxes ((m, 4) xmin, ymin, xmax, ymax).  Those features stay in the tracker and are tracked on the next frame."""
+        img = self._rows(img, np.uint8)
+        assert img.shape == (self.height, self.width)
+        dp, dpitch = None, 0
+        if depth is not None:
+            depth = self._rows(depth, np.uint16)
+            dp, dpitch = depth.ctypes.data, depth.strides[0]
+        b = box_array(boxes)
+        n, info = ctypes.c_int(0), TrackInfo()
+        in_box = np.zeros(self.max_cnt, np.uint8)
+        check(self.L.gf_tracker_track_boxes(self._h, float(cur_time), img.ctypes.data, img.strides[0], dp, dpitch, 0,
+                                            b.ctypes.data if len(b) else None, len(b), self._obs.ctypes.data, ctypes.byref(n),
+                                            in_box.ctypes.data, self._status.ctypes.data, ctypes.byref(info)))
+        return self._collect(n, info), in_box[:n.value].view(np.bool_)
+
+    def trackImagebox(self, cur_time, boxes, img, depth=None):
+        """{id: v[8]} of trackImage without the features strictly inside a box (Estimator::inputImagebox's front end)."""
+        obs, in_box = self.trackImageboxRaw(cur_time, boxes, img, depth)
+        return {int(o["id"]): o["v"].copy() for o in obs[~in_box]}
+
     def trackDevice(self, cur_time, d_gray_ptr, d_depth_ptr=None):
         n, info = ctypes.c_int(0), TrackInfo()
         check(self.L.gf_tracker_track_device(self._h, float(cur_time), d_gray_ptr, d_depth_ptr, self._obs.ctypes.data,
@@ -171,10 +219,16 @@ class FeatureTracker:
         dp, dpitch = (depth.ctypes.data, depth.strides[0]) if depth is not None else (None, 0)
         check(self.L.gf_tracker_submit(self._h, float(cur_time), img.ctypes.data, img.strides[0], dp, dpitch))
 
-    def trackBatch(self, times, gray_ptrs, depth_ptrs=None, on_device=False, gray_pitch=None, depth_pitch=None, want=True):
+    def trackBatch(self, times, gray_ptrs, depth_ptrs=None, on_device=False, gray_pitch=None, depth_pitch=None, want=True, boxes=None):
         """n consecutive trackImage calls in ONE library call (gf_tracker_track_batch: two frames in flight inside the
         library).  gray_ptrs / depth_ptrs: integer addresses of the frames (host, ideally pinned, or device).  Returns a
-        list of (obs, status, info) per frame when `want`, else None (bench loops that only need the work done)."""
+        list of (obs, status, info) per frame when `want`, else None (bench loops that only need the work done).
+        boxes: one (m, 4) box list per frame (empty: trackImage); the frames then go through trackImagebox
+        (gf_tracker_track_batch_boxes) and every result gains in_box: (obs, status, info, in_box)."""
+        if boxes is not None:
+            r = FeatureTracker.trackBatchMulti([self], [times], [gray_ptrs], None if depth_ptrs is None else [depth_ptrs], on_device,
+                                               gray_pitch, depth_pitch, want, boxes=[boxes])
+            return r[0] if want else None
         n = len(times)
         t = np.ascontiguousarray(times, np.float64)
         g = (ctypes.c_void_p * n)(*[int(a) for a in gray_ptrs])
@@ -193,9 +247,10 @@ class FeatureTracker:
         return [(obs[k, :cnt[k]].copy(), st[k, :info[k].n_prev].copy(), info[k].as_dict()) for k in range(n)]
 
     @staticmethod
-    def trackBatchMulti(trackers, times, gray_ptrs, depth_ptrs=None, on_device=False, gray_pitch=None, depth_pitch=None, want=True):
+    def trackBatchMulti(trackers, times, gray_ptrs, depth_ptrs=None, on_device=False, gray_pitch=None, depth_pitch=None, want=True, boxes=None):
         """gf_tracker_track_batch_multi: n frames on each of S independent trackers in one call, fed by one host thread.
-        times / gray_ptrs / depth_ptrs: per tracker lists of n entries.  Returns per tracker what trackBatch returns."""
+        times / gray_ptrs / depth_ptrs: per tracker lists of n entries.  Returns per tracker what trackBatch returns.
+        boxes: per tracker lists of n box lists (gf_tracker_track_batch_multi_boxes; results gain in_box as in trackBatch)."""
         S, n = len(trackers), len(times[0])
         a = trackers[0]
         assert all(len(x) == n for x in times) and all(tr.max_cnt == a.max_cnt and tr.width == a.width for tr in trackers)
@@ -207,14 +262,26 @@ class FeatureTracker:
         st = np.zeros((S, n, a.max_cnt), np.uint8) if want else None
         cnt = np.zeros((S, n), np.int32)
         info = (TrackInfo * (S * n))()
-        check(a.L.gf_tracker_track_batch_multi(h, S, n, t.ctypes.data, g, int(gray_pitch or a.width), d, int(depth_pitch or 2 * a.width),
-                                               int(bool(on_device)), obs.ctypes.data if want else None, cnt.ctypes.data,
-                                               st.ctypes.data if want else None, info))
+        if boxes is None:
+            check(a.L.gf_tracker_track_batch_multi(h, S, n, t.ctypes.data, g, int(gray_pitch or a.width), d, int(depth_pitch or 2 * a.width),
+                                                   int(bool(on_device)), obs.ctypes.data if want else None, cnt.ctypes.data,
+                                                   st.ctypes.data if want else None, info))
+        else:
+            assert len(boxes) == S and all(len(x) == n for x in boxes)
+            bx, start = _box_csr([b for row in boxes for b in row])
+            ib = np.zeros((S, n, a.max_cnt), np.uint8) if want else None
+            check(a.L.gf_tracker_track_batch_multi_boxes(h, S, n, t.ctypes.data, g, int(gray_pitch or a.width), d, int(depth_pitch or 2 * a.width),
+                                                         int(bool(on_device)), bx.ctypes.data if len(bx) else None, start.ctypes.data,
+                                                         obs.ctypes.data if want else None, cnt.ctypes.data, ib.ctypes.data if want else None,
+                                                         st.ctypes.data if want else None, info))
         for i, tr in enumerate(trackers):
             tr.batch_infos = [info[i * n + k].as_dict() for k in range(n)]
             tr.last_info = tr.batch_infos[-1] if n else {}
         if not want:
             return None
+        if boxes is not None:
+            return [[(obs[i, k, :cnt[i, k]].copy(), st[i, k, :info[i * n + k].n_prev].copy(), info[i * n + k].as_dict(),
+                      ib[i, k, :cnt[i, k]].view(np.bool_).copy()) for k in range(n)] for i in range(S)]
         return [[(obs[i, k, :cnt[i, k]].copy(), st[i, k, :info[i * n + k].n_prev].copy(), info[i * n + k].as_dict()) for k in range(n)] for i in range(S)]
 
     def submitDevice(self, cur_time, d_gray_ptr, d_depth_ptr=None):

@@ -181,10 +181,13 @@ class WindowEstimator:
             self.fm.removeFront(self.frame_count)                 # slideWindowNew (estimator.cpp:3839-3851)
 
 
-def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=True, max_iter=8, feedback=False, use_mcc=False):
+def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=True, max_iter=8, feedback=False, use_mcc=False, boxes=None):
     """Runs n_frames of `stream` through tracker -> fm -> ba.  Returns dict(t, P_est, P_gt, R_est, R_gt, keyframes, ...).
     tracker.trackImage(t, gray, depth) -> {id: v[8]};  fm / ba: see WindowEstimator.  feedback: the estimator calls the tracker's
-    removeOutliers / setPrediction after every optimisation (the reference with MULTIPLE_THREAD 0)."""
+    removeOutliers / setPrediction after every optimisation (the reference with MULTIPLE_THREAD 0).
+    boxes: USE_YOLO -- the detections of frame k in boxes[k] ((m, 4) xmin, ymin, xmax, ymax).  A frame with detections goes
+    through tracker.trackImagebox(t, boxes[k], gray, depth), one without through trackImage, as sync_process does
+    (rosNodeTest.cpp:433-439, 519-540)."""
     imu = ImuFromStream(stream)
     est = WindowEstimator(fm, ba, imu_propagate=imu_propagate, max_iter=max_iter, tracker=tracker if feedback else None, use_mcc=use_mcc)
     out_t, out_P, out_R, gt_P, gt_R, iters = [], [], [], [], [], []
@@ -198,7 +201,10 @@ def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=Tru
                 est.processIMU(dt, acc, gyr)
         else:
             acc, gyr = imu.sample(t); est.processIMU(0.0, acc, gyr)
-        image = tracker.trackImage(t, gray, depth)
+        if boxes is not None and len(boxes[k]) > 0:
+            image = tracker.trackImagebox(t, boxes[k], gray, depth)
+        else:
+            image = tracker.trackImage(t, gray, depth)
         if not est.nonlinear:                           # initialisation is out of scope: ground-truth states while the window fills
             R_wb, P = imu.pose_t(t)
             est.set_state(est.frame_count, R_wb, P, imu.velocity(t))

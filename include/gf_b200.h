@@ -138,6 +138,39 @@ int gf_tracker_track_batch_multi(gf_tracker* const* trackers, int n_trackers, in
  * Covers every intake path: _track / _submit, _track_device / _submit_device and the batch calls. */
 int gf_tracker_set_equalize(gf_tracker* t, double clip_limit, int tiles_x, int tiles_y);
 
+/* The config key `use_yolo` (parameters.cpp:159): FeatureTracker::trackImagebox (feature_tracker.cpp:374-678), which
+ * Estimator::inputImagebox (estimator.cpp:244-273) calls on every frame whose detection message has the frame's timestamp.  It is
+ * trackImage with one difference: a feature strictly inside a detected box, pointPolygonTest(contour of the box, pt, true) > 0, is
+ * left out of featureFrame.  It stays in the tracker (cur_pts / ids / track_cnt / velocity history): it is tracked on the next
+ * frame and counts against max_cnt.  The boxes are the fields of darknet_ros_msgs/BoundingBox; the reference copies them into
+ * `int`, and so does the library (a modular wrap of values outside int32).
+ *   _submit_boxes: gf_tracker_submit / gf_tracker_submit_device (on_device != 0: tightly packed device frames, pitches ignored)
+ *       with the frame's n_boxes boxes.  n_boxes == 0 is trackImage.  n_boxes > GF_MAX_BOXES (darknet_ros publishes at most 100,
+ *       YoloObjectDetector.cpp:559): GF_ERR_CAPACITY; n_boxes < 0 or boxes == NULL with n_boxes > 0: GF_ERR_INVALID_ARG; in both
+ *       cases no frame is consumed.  The boxes are copied before the call returns.
+ *   _wait_boxes: gf_tracker_wait plus in_box (nullable, capacity >= max_cnt): in_box[i] = 1 for the entries of out that
+ *       trackImagebox leaves out of featureFrame, 0 otherwise (all 0 for a frame submitted without boxes).  out / n_out /
+ *       status_out / info are exactly what trackImage returns for the frame.  Collects any frame.
+ *   _track_batch_boxes / _track_batch_multi_boxes: the batch calls with per-frame boxes: frame j (j = i*n + k for stream i) has
+ *       boxes[box_start[j] .. box_start[j + 1]) (box_start: n + 1, resp. n_trackers*n + 1 offsets; NULL: no boxes) and its flags at
+ *       in_box + j*max_cnt.  Every list is checked before the first frame is submitted.
+ * The box test runs on the device, inside the last kernel of the frame; the other entry points run the same kernels without boxes. */
+#define GF_MAX_BOXES 100
+typedef struct gf_box { int64_t xmin, ymin, xmax, ymax; } gf_box;
+int gf_tracker_submit_boxes(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch,
+                            int on_device, const gf_box* boxes, int n_boxes);
+int gf_tracker_wait_boxes(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info);
+/* Blocking form of _submit_boxes + _wait_boxes, the call trackImagebox makes (no frame may be in flight, as for gf_tracker_track). */
+int gf_tracker_track_boxes(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch, int on_device,
+                           const gf_box* boxes, int n_boxes, gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info);
+int gf_tracker_track_batch_boxes(gf_tracker* t, int n, const double* times, const void* const* gray, size_t gray_pitch,
+                                 const void* const* depth, size_t depth_pitch, int on_device, const gf_box* boxes, const int* box_start,
+                                 gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info);
+int gf_tracker_track_batch_multi_boxes(gf_tracker* const* trackers, int n_trackers, int n, const double* times, const void* const* gray,
+                                       size_t gray_pitch, const void* const* depth, size_t depth_pitch, int on_device,
+                                       const gf_box* boxes, const int* box_start, gf_obs* out, int* n_out, uint8_t* in_box,
+                                       uint8_t* status_out, gf_track_info* info);
+
 /* FeatureTracker::setPrediction (feature_tracker.cpp:1006-1027): xyz are camera-frame 3-D points. */
 int gf_tracker_set_prediction(gf_tracker* t, const int32_t* ids, const double* xyz, int n);
 /* FeatureTracker::removeOutliers (feature_tracker.cpp:1029-1045). */
@@ -172,6 +205,9 @@ int gf_stage_pyr_down(int device, const uint8_t* src, int w, int h, uint8_t* dst
  * src rows are src_pitch bytes apart; dst is w x h, tightly packed.  Same limits as the tracker's image and tile grid. */
 int gf_stage_clahe(int device, const uint8_t* src, size_t src_pitch, int w, int h, double clip_limit, int tiles_x, int tiles_y,
                    uint8_t* dst);
+/* trackImagebox's box test on its own (the device function of gf_tracker_submit_boxes): in_box[i] = 1 when point i
+ * (pts: n x,y float pairs) lies strictly inside one of the n_boxes boxes, as pointPolygonTest(contour, pt, true) > 0 decides. */
+int gf_stage_in_boxes(int device, const float* pts, int n, const gf_box* boxes, int n_boxes, uint8_t* in_box);
 /* cv::cornerMinEigenVal(img, blockSize=3, ksize=3) as used by goodFeaturesToTrack. */
 int gf_stage_min_eig(int device, const uint8_t* img, int w, int h, float* eig, int* n_fixups);
 /* cv::calcOpticalFlowPyrLK(prev, next, prev_pts, next_pts, status, err, Size(21,21), max_level,
