@@ -36,6 +36,8 @@ constexpr int X_POSE = 0, X_SB = 7 * MAXF, X_EX = X_SB + 9 * MAXF, X_TD = X_EX +
 constexpr int PAIR_THREADS = 256, PAIR_CHUNK = 64;   // factors staged per pass (2*64 rows x 20 cols in smem)
 constexpr int RB_THREADS = ST_THREADS;               // k_ba_step block size (ba_chol.cuh)
 constexpr int SCHUR_WARPS = 8;                       // k_ba_schur: one warp per 8x8 tile of the reduced system
+// k_ba_schur's dynamic shared memory at the largest window: cl[L] | ss[nc+1] | sv[nc] (above the 48 KB default from L ~ 5,800)
+constexpr size_t SCHUR_SMEM_MAX = sizeof(double) * (GF_BA_MAX_FREE_LANDMARKS + 2 * MAX_NC + 2);
 
 struct BaState {
     double x_cost, cand_cost, radius, mu, alpha, dogleg_norm, model_change, x_norm, step_norm, grad_max;
@@ -1378,6 +1380,7 @@ int gf_ba_create(gf_ba** out, int device)
     GF_CUDA(cudaFuncSetAttribute(k_ba_step<MAXR, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
     GF_CUDA(cudaFuncSetAttribute(k_jacobi_eig, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     GF_CUDA(cudaFuncSetAttribute(k_sym_eig_ql, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    GF_CUDA(cudaFuncSetAttribute(k_ba_schur, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCHUR_SMEM_MAX));
     *out = s;
     return GF_OK;
 }
@@ -1439,6 +1442,7 @@ int gf_ba_solve(gf_ba* s, const gf_ba_problem* p, gf_ba_summary* sum)
     for (int k = 0; k < nfeat; k++) if (col_feat[k] == -2) col_feat[k] = c++;
     d.L = c - d.nc; d.n = c;
     if (d.nc > MAX_NC) return set_err(GF_ERR_CAPACITY, "reduced system larger than 383 unknowns");
+    if (d.L > GF_BA_MAX_FREE_LANDMARKS) return set_err(GF_ERR_CAPACITY, "more than GF_BA_MAX_FREE_LANDMARKS (8192) free landmarks");
     // ---- sort visual factors by pose pair ----
     std::vector<int> pair_id(F * F, -1), pair_cnt;
     std::vector<int> pair_ij;

@@ -243,6 +243,10 @@ int gf_probe_fp64(int device, double* dfma_gflops, double* dmma_gflops);
  * ---------------------------------------------------------------------------------------------- */
 #define GF_BA_MAX_FRAMES 11          /* WINDOW_SIZE + 1 (parameters.h:24) */
 #define GF_BA_MAX_ITERATIONS 16
+/* Free landmarks (entries of para_feature that are not constant and have a visual factor) one gf_ba_solve accepts; more is
+ * GF_ERR_CAPACITY before anything is enqueued.  The Schur kernel stages 8 * (L + 2 nc + 2) bytes per CTA in shared memory
+ * (nc <= 383 reduced unknowns): 71 KB at this bound. */
+#define GF_BA_MAX_FREE_LANDMARKS 8192
 
 /* ProjectionTwoFrameOneCamFactor (factor/projectionTwoFrameOneCamFactor.h:21, .cpp:43-151) */
 typedef struct gf_ba_visual_factor {

@@ -30,15 +30,20 @@ def compare(ba, pb, max_iter, mid_rtol=1e-7, final_rtol=1e-9):
     b = pb.clone(); b.max_num_iterations = max_iter
     so = O.solve(a)
     sg = ba.optimization(b)
+    return assert_matches(sg, so, b, a, mid_rtol, final_rtol)
+
+
+def assert_matches(sg, so, b, a, mid_rtol=1e-7, final_rtol=1e-9, cost_atol=0.0):
+    """The parity bar between a GPU solve (summary sg, solved window b) and the oracle's (so, a)."""
     assert sg["iterations"] == so["iterations"], (sg, so)
     assert sg["num_successful_steps"] == so["num_successful_steps"]
     assert sg["termination"] == so["termination"]
     assert sg["reduced_dim"] == so["reduced_dim"] and sg["n_free_landmarks"] == so["n_free_landmarks"]
     # intermediate iterates of the steep phase (cost falling by 1e3 per step) amplify 1e-13 differences of the step
     # (atomic summation order, Schur vs dense elimination); the end points must agree to 1e-9
-    assert np.allclose(sg["cost"], so["cost"], rtol=mid_rtol, atol=0), (sg["cost"], so["cost"])
+    assert np.allclose(sg["cost"], so["cost"], rtol=mid_rtol, atol=cost_atol), (sg["cost"], so["cost"])
     assert np.isclose(sg["initial_cost"], so["initial_cost"], rtol=1e-12)
-    assert np.isclose(sg["final_cost"], so["final_cost"], rtol=final_rtol), (sg["final_cost"], so["final_cost"])
+    assert np.isclose(sg["final_cost"], so["final_cost"], rtol=final_rtol, atol=max(cost_atol, 1e-8)), (sg["final_cost"], so["final_cost"])
     assert np.allclose(sg["radius"], so["radius"], rtol=1e-6)
     assert np.abs(a.para_pose[:, :3] - b.para_pose[:, :3]).max() < 1e-6
     assert rot_err(a.para_pose[:, 3:], b.para_pose[:, 3:]).max() < 1e-6
