@@ -23,13 +23,6 @@ struct ClaheGeom {
     float lut_scale, inv_tw, inv_th;           // 255.f / (tw * th), 1.f / tw, 1.f / th
 };
 
-// The source of a frame: `ptr` / `pitch`, or, when `ind_ptr` is set, the address and pitch stored there (the batch pipeline's
-// FrameParams: the graph stays fixed while the frame's address changes)
-struct ClaheSrc {
-    const uint8_t* ptr; long long pitch;
-    const uint8_t* const* ind_ptr; const long long* ind_pitch;
-};
-
 inline int clahe_geometry(ClaheGeom& g, int w, int h, double clip_limit, int tiles_x, int tiles_y)
 {
     if (tiles_x < 1 || tiles_y < 1 || tiles_x > CLAHE_MAX_TILES || tiles_y > CLAHE_MAX_TILES)
@@ -52,14 +45,8 @@ inline int clahe_geometry(ClaheGeom& g, int w, int h, double clip_limit, int til
     return GF_OK;
 }
 
-__device__ __forceinline__ void clahe_src(const ClaheSrc& s, const uint8_t*& p, long long& pitch)
-{
-    if (s.ind_ptr) { p = *s.ind_ptr; pitch = *s.ind_pitch; }
-    else { p = s.ptr; pitch = s.pitch; }
-}
-
 // grid = tiles_x * tiles_y CTAs; lut: [tiles_y][tiles_x][256]
-__global__ void __launch_bounds__(CLAHE_LUT_THREADS) k_clahe_lut(ClaheSrc S, ClaheGeom g, uint8_t* __restrict__ lut)
+__global__ void __launch_bounds__(CLAHE_LUT_THREADS) k_clahe_lut(const uint8_t* src, long long pitch, ClaheGeom g, uint8_t* __restrict__ lut)
 {
     constexpr int NW = CLAHE_LUT_THREADS / 32;
     __shared__ int wh[NW][256];                // per-warp histograms
@@ -67,8 +54,6 @@ __global__ void __launch_bounds__(CLAHE_LUT_THREADS) k_clahe_lut(ClaheSrc S, Cla
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const int tx = blockIdx.x % g.tiles_x, ty = blockIdx.x / g.tiles_x;
     for (int i = tid; i < NW * 256; i += CLAHE_LUT_THREADS) (&wh[0][0])[i] = 0;
-    const uint8_t* src; long long pitch;
-    clahe_src(S, src, pitch);
     __syncthreads();
     const int area = g.tw * g.th, x0 = tx * g.tw, y0 = ty * g.th;
     // every lane of a warp runs the same trip count, so __match_any_sync sees the whole warp: lanes holding the same value
@@ -136,14 +121,12 @@ __global__ void __launch_bounds__(CLAHE_LUT_THREADS) k_clahe_lut(ClaheSrc S, Cla
 }
 
 // grid = ceil(h / CLAHE_APPLY_ROWS) CTAs, dynamic shared memory tiles_x * tiles_y * 256 bytes.
-__global__ void __launch_bounds__(CLAHE_APPLY_THREADS) k_clahe_apply(ClaheSrc S, ClaheGeom g, const uint8_t* __restrict__ lut,
-                                                                     uint8_t* __restrict__ dst, int dst_pitch)
+__global__ void __launch_bounds__(CLAHE_APPLY_THREADS) k_clahe_apply(const uint8_t* src, long long pitch, ClaheGeom g,
+                                                                     const uint8_t* __restrict__ lut, uint8_t* __restrict__ dst, int dst_pitch)
 {
     extern __shared__ __align__(16) uint8_t s_lut[];
     const int n16 = g.tiles_x * g.tiles_y * 16;
     for (int i = threadIdx.x; i < n16; i += CLAHE_APPLY_THREADS) ((uint4*)s_lut)[i] = __ldg((const uint4*)lut + i);
-    const uint8_t* src; long long pitch;
-    clahe_src(S, src, pitch);
     __syncthreads();
     const int chunks = (g.w + 15) >> 4, y_begin = blockIdx.x * CLAHE_APPLY_ROWS, y_end = min(y_begin + CLAHE_APPLY_ROWS, g.h);
     for (int item = threadIdx.x; item < (y_end - y_begin) * chunks; item += CLAHE_APPLY_THREADS) {
@@ -203,10 +186,10 @@ inline int clahe_prepare()
 }
 
 // Both kernels on s; lut: clahe_lut_bytes(g) bytes of device memory (16-byte aligned)
-inline int enqueue_clahe(cudaStream_t s, const ClaheSrc& src, const ClaheGeom& g, uint8_t* lut, uint8_t* dst, int dst_pitch)
+inline int enqueue_clahe(cudaStream_t s, const uint8_t* src, long long pitch, const ClaheGeom& g, uint8_t* lut, uint8_t* dst, int dst_pitch)
 {
-    k_clahe_lut<<<g.tiles_x * g.tiles_y, CLAHE_LUT_THREADS, 0, s>>>(src, g, lut); GF_LAUNCHED();
-    k_clahe_apply<<<(g.h + CLAHE_APPLY_ROWS - 1) / CLAHE_APPLY_ROWS, CLAHE_APPLY_THREADS, clahe_lut_bytes(g), s>>>(src, g, lut, dst, dst_pitch); GF_LAUNCHED();
+    k_clahe_lut<<<g.tiles_x * g.tiles_y, CLAHE_LUT_THREADS, 0, s>>>(src, pitch, g, lut); GF_LAUNCHED();
+    k_clahe_apply<<<(g.h + CLAHE_APPLY_ROWS - 1) / CLAHE_APPLY_ROWS, CLAHE_APPLY_THREADS, clahe_lut_bytes(g), s>>>(src, pitch, g, lut, dst, dst_pitch); GF_LAUNCHED();
     GF_CUDA(cudaGetLastError());
     return GF_OK;
 }

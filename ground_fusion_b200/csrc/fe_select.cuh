@@ -64,8 +64,6 @@ __global__ void __launch_bounds__(FE_CAP) k_compact_setmask(TrackScalars* sc, Fe
     __shared__ short cf[FE_CAP * SM_CF_MAX];
     __shared__ int ncf[FE_CAP];
     __shared__ uint8_t st[FE_CAP];
-    gf_pdl_trigger();
-    gf_pdl_wait();
     __shared__ int warp_sums[32];
     __shared__ int s_m;
     __shared__ SortWork swork;
@@ -238,8 +236,6 @@ __global__ void __launch_bounds__(256) k_eig_max(TrackScalars* sc, const float2*
     __shared__ MaskTile M;
     __shared__ unsigned int wb[8];
     const int x0 = blockIdx.x * MASK_TX, y0 = blockIdx.y * MASK_TY;
-    gf_pdl_trigger();
-    gf_pdl_wait();
     mask_tile_load(M, sc, kept, x0, y0, r);
     unsigned int best = 0;
     const int tx = threadIdx.x & 63, ty = threadIdx.x >> 6;
@@ -272,8 +268,6 @@ __global__ void __launch_bounds__(256) k_candidates(TrackScalars* sc, const floa
 {
     __shared__ MaskTile M;
     const int x0 = blockIdx.x * MASK_TX, y0 = blockIdx.y * MASK_TY;
-    gf_pdl_trigger();
-    gf_pdl_wait();
     mask_tile_load(M, sc, kept, x0, y0, r);
     const double maxVal = sc->max_key ? (double)float_from_order_key(sc->max_key) : 0.0;
     const float thr = (float)(maxVal * 0.01);
@@ -515,9 +509,6 @@ __global__ void __launch_bounds__(1024) k_select_finalize(TrackScalars* sc, Feat
                                                           CamParams cam, const double* dt_ptr, const uint16_t* depth, int dpitch /*elements*/,
                                                           int depth_cam_cfg, const int* depth_valid_ptr, int h, OutHeader* out_hdr, gf_obs* out_obs,
                                                           uint8_t* out_status /* may be null: copy of the LK status of the n_prev input features */,
-                                                          uint4* host_mirror = nullptr /* batch pipeline: pinned host copy of the result block, written
-                                                          by this kernel (16 B per thread, coalesced) instead of a D2H copy node on the dependent chain */,
-                                                          int mirror_obs_offset = 0 /* offsetof(OutBlock, obs) */,
                                                           const BoxSet* boxes = nullptr /* the frame's detections, or null */,
                                                           uint32_t* out_in_box = nullptr /* FE_CAP bits: output i lies inside a box */)
 {
@@ -525,7 +516,6 @@ __global__ void __launch_bounds__(1024) k_select_finalize(TrackScalars* sc, Feat
     __shared__ unsigned long long keys[FE_SORT_CAP];
     __shared__ float4 s_box[GF_BOX_CAP];
     const int tid = threadIdx.x;
-    gf_pdl_wait();
     const int n_box = boxes ? boxes->n : 0;
     if (tid < n_box) s_box[tid] = boxes->b[tid];            // visible after the barriers of nms_cells
     const long long c0 = gf_clock();
@@ -635,12 +625,6 @@ __global__ void __launch_bounds__(1024) k_select_finalize(TrackScalars* sc, Feat
         out_hdr->nms_rounds = sc->nms_rounds; out_hdr->eig_fixups = sc->eig_fixups; out_hdr->lk_iters = sc->lk_iters; sc->lk_iters = 0;
         sc->n_new = n_new; sc->n_out = total;
         sc->n_prev = total; sc->n_id = n_id + n_new; sc->eig_fixups = 0;
-    }
-    if (host_mirror) {      // the result block starts at out_hdr: header | status[FE_CAP] | obs[]
-        __syncthreads();
-        const uint4* src = reinterpret_cast<const uint4*>(out_hdr);
-        const int n16 = (mirror_obs_offset + total * (int)sizeof(gf_obs) + 15) / 16;
-        for (int i = tid; i < n16; i += 1024) host_mirror[i] = src[i];
     }
     GF_DBG(8, c1 - c0); GF_DBG(9, c2 - c1); GF_DBG(10, gf_clock() - c2); GF_DBG(11, nacc); GF_DBG(12, ncand);
 }

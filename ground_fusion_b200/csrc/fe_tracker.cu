@@ -34,8 +34,6 @@ std::atomic<uint64_t> g_launches{0};
 
 struct FrameParams {
     double dt; int has_pred; int depth_valid;
-    // batch pipeline only: where k_copy_in finds the frame (device pointers: the caller's, or the tracker's staging buffers)
-    const uint8_t* src_gray; const uint16_t* src_depth; long long src_gray_pitch, src_depth_pitch;   // pitches in bytes
     BoxSet boxes;            // trackImagebox's detections (n = 0: trackImage)
 };
 
@@ -66,32 +64,6 @@ __global__ void __launch_bounds__(256) k_in_boxes_stage(const float2* pts, int n
     __syncthreads();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) in_box[i] = in_any_box(s_box, nb, pts[i]) ? 1 : 0;
-}
-
-// Frame intake of the batch pipeline: copies the frame named by *fp into pyramid level 0 and the depth slot (16 B per thread when
-// source and row pitch allow it).  A kernel instead of a memcpy node because the source address changes every frame while the
-// graph stays fixed.
-// row0 = h: depth only (with equalisation the CLAHE kernels write level 0 instead).
-__global__ void __launch_bounds__(256) k_copy_in(const FrameParams* __restrict__ fp, uint8_t* __restrict__ dst_gray, int gray_pitch,
-                                                 uint16_t* __restrict__ dst_depth, int depth_pitch_el, int w, int h, int row0)
-{
-    const uint8_t* sg = fp->src_gray;
-    const uint8_t* sd = (const uint8_t*)fp->src_depth;
-    const long long gp = fp->src_gray_pitch, dp = fp->src_depth_pitch;
-    const int depth_rows = (fp->depth_valid && sd) ? h : 0;
-    const int row = blockIdx.y + row0;                // rows 0..h-1: gray, h..2h-1: depth
-    const bool is_depth = row >= h;
-    if (is_depth && row - h >= depth_rows) return;
-    const uint8_t* src = is_depth ? sd + (long long)(row - h) * dp : sg + (long long)row * gp;
-    uint8_t* dst = is_depth ? (uint8_t*)(dst_depth + (size_t)(row - h) * depth_pitch_el) : dst_gray + (size_t)row * gray_pitch;
-    const int nbytes = is_depth ? 2 * w : w;
-    const int x = (blockIdx.x * blockDim.x + threadIdx.x) * 16;
-    if (x >= nbytes) return;
-    if ((((uintptr_t)src | (uintptr_t)dst) & 15) == 0 && x + 16 <= nbytes) {
-        *(uint4*)(dst + x) = __ldg((const uint4*)(src + x));
-    } else {
-        for (int k = x; k < min(x + 16, nbytes); k++) dst[k] = __ldg(src + k);
-    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -138,7 +110,6 @@ __global__ void __launch_bounds__(LK_THREADS, GF_TRACK_MIN_CTAS) k_track(Pyramid
     __shared__ LKSmem sm;
     const int tid = threadIdx.x, i = blockIdx.x;
     if (i >= sc->n_prev) return;
-    gf_pdl_trigger();
     lk_tma_init(sm, tid);
     LKTma T{M.prevI, M.curJ, 0u, M.enabled != 0};
     const float2 p = fa.prev_pts[i];
@@ -248,16 +219,10 @@ struct gf_tracker {
     // CUDA graphs keyed by frame number mod 6 (= pyramid slot mod 3 x two-slot buffers)
     cudaGraphExec_t g_pyr[6], g_eig[6], g_dep1[6][2], g_dep2[6];
     int gk_pyr[6], gk_eig[6], gk_dep1[6][2], gk_dep2[6];
-    bool use_graph, use_pdl, pdl_single_cta, batch_pipeline;
-    // batch pipeline (gf_tracker_track_batch): one graph launch per frame on s_main = {track + select of frame f} || {intake,
-    // pyramid and min-eig map of frame f+1}; keyed by frame number mod 6 like the pieces above
-    cudaGraphExec_t gb_prep[6], gb_dep[6], gb_both[6];
-    int gbk_prep[6], gbk_dep[6], gbk_both[6];
-    cudaEvent_t ev_fork, ev_fork2, ev_join[2];
-    uint8_t* d_stage_gray[2]; uint16_t* d_stage_depth[2];   // H2D landing buffers of the batch pipeline (host frames)
+    bool use_graph;
     // gf_tracker_set_equalize: CLAHE of every gray frame into pyramid level 0.  Frames land in d_raw first; the copy and both
-    // CLAHE kernels (a graph keyed by pyramid slot) run in order on s_up (batch pipeline: inside prep), so one raw buffer and
-    // one LUT block serve every frame in flight.
+    // CLAHE kernels (a graph keyed by pyramid slot) run in order on s_up, so one raw buffer and one LUT block serve every frame
+    // in flight.
     bool equalize;
     ClaheGeom clahe;
     cudaGraphExec_t g_clahe[3]; int gk_clahe[3];
@@ -280,7 +245,7 @@ struct gf_tracker {
     int* h_tmp_ids; double* h_tmp_xyz;
     long long n_submitted, n_waited;     // frame counters; n_submitted - n_waited frames are in flight
     double prev_time;
-    bool has_pred, depth_valid[2], t0_valid[2];
+    bool has_pred, depth_valid[2];
     float last_ms;
 };
 
@@ -377,26 +342,13 @@ static void free_nms_grid(NmsGrid& g)
     cudaFree(g.cand_key); cudaFree(g.acc_key); cudaFree(g.dead);
 }
 
-// Launch with (pdl) or without a programmatic dependency on the previous kernel of the stream (gf_pdl_wait / gf_pdl_trigger).
-template <class... KArgs, class... Args>
-static cudaError_t launch_k(void (*k)(KArgs...), dim3 g, dim3 b, size_t smem, cudaStream_t s, bool pdl, Args... args)
-{
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = g; cfg.blockDim = b; cfg.dynamicSmemBytes = smem; cfg.stream = s;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, k, KArgs(args)...);
-}
-
 // GFTT tail shared by the tracker and gf_stage_gftt: mask -> max -> candidates -> NMS rounds
 static int enqueue_gftt_select(cudaStream_t s, TrackScalars* d_sc, const float2* kept_pts, const float* d_eig, int epitch, int w, int h,
-                               int min_dist, NmsGrid& grid, bool pdl = false)
+                               int min_dist, NmsGrid& grid)
 {
     dim3 tg((w + MASK_TX - 1) / MASK_TX, (h + MASK_TY - 1) / MASK_TY);
-    GF_CUDA(launch_k(k_eig_max, tg, dim3(256), 0, s, pdl, d_sc, kept_pts, d_eig, epitch, w, h, min_dist)); GF_LAUNCHED();
-    GF_CUDA(launch_k(k_candidates, tg, dim3(256), 0, s, pdl, d_sc, kept_pts, d_eig, epitch, w, h, min_dist, grid)); GF_LAUNCHED();
+    k_eig_max<<<tg, 256, 0, s>>>(d_sc, kept_pts, d_eig, epitch, w, h, min_dist); GF_LAUNCHED();
+    k_candidates<<<tg, 256, 0, s>>>(d_sc, kept_pts, d_eig, epitch, w, h, min_dist, grid); GF_LAUNCHED();
     GF_CUDA(cudaGetLastError());
     return GF_OK;
 }
@@ -486,8 +438,6 @@ static int tracker_init(gf_tracker* t, int width, int height, const gf_tracker_c
         GF_CUDA(cudaEventCreate(&t->ev_out[i]));
     }
     for (int i = 0; i < GF_FE_STAGES + 2; i++) GF_CUDA(cudaEventCreate(&t->ev_st[i]));
-    GF_CUDA(cudaEventCreateWithFlags(&t->ev_fork, cudaEventDisableTiming)); GF_CUDA(cudaEventCreateWithFlags(&t->ev_fork2, cudaEventDisableTiming));
-    for (int i = 0; i < 2; i++) GF_CUDA(cudaEventCreateWithFlags(&t->ev_join[i], cudaEventDisableTiming));
     GF_CUDA(cudaEventCreate(&t->ev_span0)); GF_CUDA(cudaEventCreate(&t->ev_span1));
     int lw = width, lh = height;
     for (int l = 0; l < 4; l++) {
@@ -509,8 +459,6 @@ static int tracker_init(gf_tracker* t, int width, int height, const gf_tracker_c
         GF_CUDA(cudaMalloc(&t->d_eig[i], (size_t)t->epitch * height * sizeof(float)));
         GF_CUDA(cudaMalloc(&t->d_out[i], sizeof(OutBlock)));
         GF_CUDA(cudaMalloc(&t->d_fp[i], sizeof(FrameParams)));
-        GF_CUDA(cudaMalloc(&t->d_stage_gray[i], (size_t)width * height));
-        GF_CUDA(cudaMalloc(&t->d_stage_depth[i], (size_t)width * height * sizeof(uint16_t)));
         GF_CUDA(cudaHostAlloc(&t->h_out[i], sizeof(OutBlock), cudaHostAllocDefault));
         GF_CUDA(cudaHostAlloc(&t->h_fp[i], sizeof(FrameParams), cudaHostAllocDefault));
     }
@@ -537,9 +485,6 @@ static int tracker_init(gf_tracker* t, int width, int height, const gf_tracker_c
     GF_CUDA(cudaHostAlloc(&t->h_tmp_ids, FE_CAP * sizeof(int), cudaHostAllocDefault));
     GF_CUDA(cudaHostAlloc(&t->h_tmp_xyz, FE_CAP * 3 * sizeof(double), cudaHostAllocDefault));
     t->use_graph = getenv("GF_NO_GRAPH") == nullptr;
-    t->batch_pipeline = getenv("GF_BATCH_PIPELINE") != nullptr;   // one graph per frame for batches (see gf_tracker_track_batch_multi)
-    t->pdl_single_cta = getenv("GF_FE_PDL1") != nullptr && !t->profiling;   // PDL only into the two single-CTA kernels
-    t->use_pdl = getenv("GF_PDL") != nullptr;      // programmatic dependent launch inside dep(f): off by default (DESIGN 1.3)
     GF_CUDA(cudaDeviceSynchronize());
     return GF_OK;
 }
@@ -553,15 +498,12 @@ void gf_tracker_destroy(gf_tracker* t)
         if (t->g_pyr[k]) cudaGraphExecDestroy(t->g_pyr[k]);
         if (t->g_eig[k]) cudaGraphExecDestroy(t->g_eig[k]);
         if (t->g_dep2[k]) cudaGraphExecDestroy(t->g_dep2[k]);
-        for (cudaGraphExec_t g : {t->gb_prep[k], t->gb_dep[k], t->gb_both[k]}) if (g) cudaGraphExecDestroy(g);
         for (int p = 0; p < 2; p++) if (t->g_dep1[k][p]) cudaGraphExecDestroy(t->g_dep1[k][p]);
     }
     for (int k = 0; k < 3; k++) if (t->g_clahe[k]) cudaGraphExecDestroy(t->g_clahe[k]);
     for (int s = 0; s < 3; s++) for (int l = 0; l < 4; l++) cudaFree(t->d_pyr[s][l]);
     for (int i = 0; i < 2; i++) {
         cudaFree(t->d_depth[i]); cudaFree(t->d_eig[i]); cudaFree(t->d_out[i]); cudaFree(t->d_fp[i]);
-        cudaFree(t->d_stage_gray[i]); cudaFree(t->d_stage_depth[i]);
-        if (t->ev_join[i]) cudaEventDestroy(t->ev_join[i]);
         cudaFreeHost(t->h_out[i]); cudaFreeHost(t->h_fp[i]);
         for (cudaEvent_t e : {t->ev_up[i], t->ev_pyr[i], t->ev_eig[i], t->ev_dep[i], t->ev_t0[i], t->ev_out[i]}) if (e) cudaEventDestroy(e);
     }
@@ -576,8 +518,6 @@ void gf_tracker_destroy(gf_tracker* t)
     cudaFreeHost(t->h_gray); cudaFreeHost(t->h_depth); cudaFreeHost(t->h_tmp_ids); cudaFreeHost(t->h_tmp_xyz);
     for (cudaStream_t st_ : {t->s_up, t->s_pyr, t->s_eig, t->s_main, t->s_out}) if (st_) cudaStreamDestroy(st_);
     for (int i = 0; i < GF_FE_STAGES + 2; i++) if (t->ev_st[i]) cudaEventDestroy(t->ev_st[i]);
-    if (t->ev_fork) cudaEventDestroy(t->ev_fork);
-    if (t->ev_fork2) cudaEventDestroy(t->ev_fork2);
     if (t->ev_span0) cudaEventDestroy(t->ev_span0);
     if (t->ev_span1) cudaEventDestroy(t->ev_span1);
     cudaGetLastError();
@@ -631,7 +571,7 @@ static int body_eig(gf_tracker* t, long long f)
     return enqueue_min_eig(t->s_eig, Pc.lv[0], t->d_eig[f % 2], t->epitch, t->d_cov, t->d_box);
 }
 
-static int body_dep1(gf_tracker* t, long long f, bool has_pred, bool pdl = false)
+static int body_dep1(gf_tracker* t, long long f, bool has_pred)
 {
     cudaStream_t s = t->s_main;
     Pyramid Pc = make_pyr(t, (int)(f % 3)), Pp = make_pyr(t, (int)((f + 2) % 3));
@@ -640,28 +580,25 @@ static int body_dep1(gf_tracker* t, long long f, bool has_pred, bool pdl = false
     if (has_pred) { k_lk_pred<<<lk_grid, LK_THREADS, 0, s>>>(Pp, Pc, t->d_sc, t->fa, M); GF_LAUNCHED(); }
     k_track<<<lk_grid, LK_THREADS, 0, s>>>(Pp, Pc, t->d_sc, t->fa, t->d_fp[f % 2], t->cfg.flow_back, M); GF_LAUNCHED();
     GF_MARK(2, s);
-    GF_CUDA(launch_k(k_compact_setmask, dim3(1), dim3(FE_CAP), 0, s, pdl || (t->pdl_single_cta && !t->profiling), t->d_sc, t->fa, t->cfg.min_dist)); GF_LAUNCHED();
+    k_compact_setmask<<<1, FE_CAP, 0, s>>>(t->d_sc, t->fa, t->cfg.min_dist); GF_LAUNCHED();
     GF_CUDA(cudaGetLastError());
     GF_MARK(3, s);
     return GF_OK;
 }
 
-static int body_dep2(gf_tracker* t, long long f, bool mirror = false)
+static int body_dep2(gf_tracker* t, long long f)
 {
-    const bool pdl = mirror && t->use_pdl;
     cudaStream_t s = t->s_main;
     const int es = (int)(f % 2);
-    int rc = enqueue_gftt_select(s, t->d_sc, t->fa.kept_pts, t->d_eig[es], t->epitch, t->w, t->h, t->cfg.min_dist, t->grid, pdl);
+    int rc = enqueue_gftt_select(s, t->d_sc, t->fa.kept_pts, t->d_eig[es], t->epitch, t->w, t->h, t->cfg.min_dist, t->grid);
     if (rc) return rc;
     GF_MARK(4, s);
     // reference quirk: depth_cam with an empty depth image produces an empty featureFrame (feature_tracker.cpp:342)
     const int depth_mode = t->cfg.depth_cam ? 1 : 0;
     OutBlock* ob = t->d_out[es];
-    GF_CUDA(launch_k(k_select_finalize, dim3(1), dim3(1024), t->grid_cells, s, pdl || (t->pdl_single_cta && !t->profiling), t->d_sc, t->fa, t->grid, t->w,
-                     t->cfg.max_cnt, t->cfg.min_dist, t->cam, (const double*)&t->d_fp[es]->dt, (const uint16_t*)t->d_depth[es], t->depth_pitch_el, depth_mode,
-                     (const int*)&t->d_fp[es]->depth_valid, t->h, &ob->hdr, ob->obs, ob->status,
-                     mirror ? reinterpret_cast<uint4*>(t->h_out[es]) : (uint4*)nullptr, (int)offsetof(OutBlock, obs),
-                     (const BoxSet*)&t->d_fp[es]->boxes, ob->in_box)); GF_LAUNCHED();
+    k_select_finalize<<<1, 1024, t->grid_cells, s>>>(t->d_sc, t->fa, t->grid, t->w, t->cfg.max_cnt, t->cfg.min_dist, t->cam, &t->d_fp[es]->dt,
+                                                     t->d_depth[es], t->depth_pitch_el, depth_mode, &t->d_fp[es]->depth_valid, t->h,
+                                                     &ob->hdr, ob->obs, ob->status, &t->d_fp[es]->boxes, ob->in_box); GF_LAUNCHED();
     GF_CUDA(cudaGetLastError());
     GF_MARK(5, s);
     return GF_OK;
@@ -703,7 +640,7 @@ static int enqueue_frame(gf_tracker* t, long long f, double time, bool depth_val
     if (t->equalize) {
         const int slot = (int)(f % 3);
         int rc = run_piece(t, t->s_up, &t->g_clahe[slot], &t->gk_clahe[slot], [&] {
-            return enqueue_clahe(t->s_up, ClaheSrc{t->d_raw, t->raw_pitch, nullptr, nullptr}, t->clahe, t->d_lut, t->d_pyr[slot][0], t->lp[0]);
+            return enqueue_clahe(t->s_up, t->d_raw, t->raw_pitch, t->clahe, t->d_lut, t->d_pyr[slot][0], t->lp[0]);
         });
         if (rc) return rc;
     }
@@ -737,56 +674,6 @@ static int enqueue_frame(gf_tracker* t, long long f, double time, bool depth_val
     return GF_OK;
 }
 
-// ---- batch pipeline: the bodies of gb_prep / gb_dep / gb_both (see gf_tracker) ----
-// Frame intake + pyramid + min-eig map of frame f, enqueued on m with the min-eig chain forked to s_eig and joined back.
-static int body_prep_b(gf_tracker* t, long long f, cudaStream_t m)
-{
-    const int es = (int)(f % 2), slot = (int)(f % 3);
-    GF_CUDA(cudaMemcpyAsync(t->d_fp[es], t->h_fp[es], sizeof(FrameParams), cudaMemcpyHostToDevice, m));
-    // with equalisation k_copy_in only takes the depth image, and CLAHE reads the gray frame at the address in FrameParams
-    const int row0 = t->equalize ? t->h : 0;
-    dim3 g((2 * t->w + 16 * 256 - 1) / (16 * 256), 2 * t->h - row0);
-    k_copy_in<<<g, 256, 0, m>>>(t->d_fp[es], t->d_pyr[slot][0], t->lp[0], t->d_depth[es], t->depth_pitch_el, t->w, t->h, row0); GF_LAUNCHED();
-    if (t->equalize) {
-        const ClaheSrc src{nullptr, 0, &t->d_fp[es]->src_gray, &t->d_fp[es]->src_gray_pitch};
-        int rc = enqueue_clahe(m, src, t->clahe, t->d_lut, t->d_pyr[slot][0], t->lp[0]);
-        if (rc) return rc;
-    }
-    GF_CUDA(cudaEventRecord(t->ev_fork2, m));
-    GF_CUDA(cudaStreamWaitEvent(t->s_eig, t->ev_fork2, 0));
-    int rc = enqueue_pyramid(m, t, slot);
-    if (rc) return rc;
-    Pyramid Pc = make_pyr(t, slot);
-    rc = enqueue_min_eig(t->s_eig, Pc.lv[0], t->d_eig[es], t->epitch, t->d_cov, t->d_box);
-    if (rc) return rc;
-    GF_CUDA(cudaEventRecord(t->ev_join[1], t->s_eig));
-    GF_CUDA(cudaStreamWaitEvent(m, t->ev_join[1], 0));
-    return GF_OK;
-}
-
-// Track + setMask + corner selection + observations of frame f (result block mirrored to pinned host memory), on s_main.
-static int body_dep_b(gf_tracker* t, long long f)
-{
-    int rc = body_dep1(t, f, false, t->use_pdl);
-    if (rc) return rc;
-    return body_dep2(t, f, true);      // the result block reaches the pinned host buffer from inside k_select_finalize
-}
-
-// dep(f) on s_main with prep(f + 1) as a parallel branch on s_pyr (+ s_eig): nothing in prep(f + 1) touches what dep(f) reads
-// (pyramid slots f % 3 and (f - 1) % 3, eig / depth / params / out slots f % 2).
-static int body_both_b(gf_tracker* t, long long f)
-{
-    GF_CUDA(cudaEventRecord(t->ev_fork, t->s_main));
-    GF_CUDA(cudaStreamWaitEvent(t->s_pyr, t->ev_fork, 0));
-    int rc = body_prep_b(t, f + 1, t->s_pyr);
-    if (rc) return rc;
-    rc = body_dep_b(t, f);
-    if (rc) return rc;
-    GF_CUDA(cudaEventRecord(t->ev_join[0], t->s_pyr));
-    GF_CUDA(cudaStreamWaitEvent(t->s_main, t->ev_join[0], 0));
-    return GF_OK;
-}
-
 extern "C" {
 
 static int check_submit(gf_tracker* t)
@@ -796,56 +683,43 @@ static int check_submit(gf_tracker* t)
     return GF_OK;
 }
 
-static int submit_host(gf_tracker* t, double time, const uint8_t* gray, size_t gray_pitch, const uint16_t* depth, size_t depth_pitch,
-                       const gf_box* boxes, int n_boxes)
+// Frame intake.  Host frames may have row pitches larger than the row; the caller's buffers are read by the copy engine
+// directly: truly asynchronous when they are pinned (gf_tracker_host_buffers or any cudaHostAlloc/cudaHostRegister memory:
+// keep them unchanged until the frame has been collected); for pageable memory CUDA stages the data before cudaMemcpy2DAsync
+// returns.  Device frames are tightly packed (the pitches are ignored).
+static int submit(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch, bool on_device,
+                  const gf_box* boxes, int n_boxes)
 {
     if (!t || !gray) return set_err(GF_ERR_INVALID_ARG, "null argument");
     int rc = check_submit(t);
     if (rc) return rc;
     GF_CUDA(cudaSetDevice(t->device));
     const int w = t->w, h = t->h;
-    if (gray_pitch < (size_t)w) return set_err(GF_ERR_INVALID_ARG, "gray_pitch smaller than width");
-    if (depth && depth_pitch < (size_t)w * 2) return set_err(GF_ERR_INVALID_ARG, "depth_pitch smaller than width*2");
-    // The caller's buffers are read by the copy engine directly: truly asynchronous when they are pinned
-    // (gf_tracker_host_buffers or any cudaHostAlloc/cudaHostRegister memory: keep them unchanged until the frame has
-    // been collected); for pageable memory CUDA stages the data before cudaMemcpy2DAsync returns.
+    if (on_device) {
+        gray_pitch = w; depth_pitch = (size_t)w * 2;
+    } else {
+        if (gray_pitch < (size_t)w) return set_err(GF_ERR_INVALID_ARG, "gray_pitch smaller than width");
+        if (depth && depth_pitch < (size_t)w * 2) return set_err(GF_ERR_INVALID_ARG, "depth_pitch smaller than width*2");
+    }
+    const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     const long long f = t->n_submitted;
     cudaStream_t s = t->s_up;
     GF_CUDA(cudaEventRecord(t->ev_t0[f % 2], s));
-    t->t0_valid[f % 2] = true;
-    if (t->equalize) GF_CUDA(cudaMemcpy2DAsync(t->d_raw, t->raw_pitch, gray, gray_pitch, w, h, cudaMemcpyHostToDevice, s));
-    else GF_CUDA(cudaMemcpy2DAsync(t->d_pyr[f % 3][0], t->lp[0], gray, gray_pitch, w, h, cudaMemcpyHostToDevice, s));
+    if (t->equalize) GF_CUDA(cudaMemcpy2DAsync(t->d_raw, t->raw_pitch, gray, gray_pitch, w, h, kind, s));
+    else GF_CUDA(cudaMemcpy2DAsync(t->d_pyr[f % 3][0], t->lp[0], gray, gray_pitch, w, h, kind, s));
     if (depth)
-        GF_CUDA(cudaMemcpy2DAsync(t->d_depth[f % 2], (size_t)t->depth_pitch_el * 2, depth, depth_pitch, (size_t)w * 2, h, cudaMemcpyHostToDevice, s));
+        GF_CUDA(cudaMemcpy2DAsync(t->d_depth[f % 2], (size_t)t->depth_pitch_el * 2, depth, depth_pitch, (size_t)w * 2, h, kind, s));
     return enqueue_frame(t, f, time, depth != nullptr, boxes, n_boxes);
-}
-
-static int submit_dev(gf_tracker* t, double time, const void* d_gray, const void* d_depth, const gf_box* boxes, int n_boxes)
-{
-    if (!t || !d_gray) return set_err(GF_ERR_INVALID_ARG, "null argument");
-    int rc = check_submit(t);
-    if (rc) return rc;
-    GF_CUDA(cudaSetDevice(t->device));
-    const int w = t->w, h = t->h;
-    const long long f = t->n_submitted;
-    cudaStream_t s = t->s_up;
-    GF_CUDA(cudaEventRecord(t->ev_t0[f % 2], s));
-    t->t0_valid[f % 2] = true;
-    if (t->equalize) GF_CUDA(cudaMemcpy2DAsync(t->d_raw, t->raw_pitch, d_gray, w, w, h, cudaMemcpyDeviceToDevice, s));
-    else GF_CUDA(cudaMemcpy2DAsync(t->d_pyr[f % 3][0], t->lp[0], d_gray, w, w, h, cudaMemcpyDeviceToDevice, s));
-    if (d_depth)
-        GF_CUDA(cudaMemcpy2DAsync(t->d_depth[f % 2], (size_t)t->depth_pitch_el * 2, d_depth, (size_t)w * 2, (size_t)w * 2, h, cudaMemcpyDeviceToDevice, s));
-    return enqueue_frame(t, f, time, d_depth != nullptr, boxes, n_boxes);
 }
 
 int gf_tracker_submit(gf_tracker* t, double time, const uint8_t* gray, size_t gray_pitch, const uint16_t* depth, size_t depth_pitch)
 {
-    return submit_host(t, time, gray, gray_pitch, depth, depth_pitch, nullptr, 0);
+    return submit(t, time, gray, gray_pitch, depth, depth_pitch, false, nullptr, 0);
 }
 
 int gf_tracker_submit_device(gf_tracker* t, double time, const void* d_gray, const void* d_depth)
 {
-    return submit_dev(t, time, d_gray, d_depth, nullptr, 0);
+    return submit(t, time, d_gray, 0, d_depth, 0, true, nullptr, 0);
 }
 
 int gf_tracker_submit_boxes(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch,
@@ -853,8 +727,7 @@ int gf_tracker_submit_boxes(gf_tracker* t, double time, const void* gray, size_t
 {
     int rc = check_boxes(boxes, n_boxes);
     if (rc) return rc;
-    return on_device ? submit_dev(t, time, gray, depth, boxes, n_boxes)
-                     : submit_host(t, time, (const uint8_t*)gray, gray_pitch, (const uint16_t*)depth, depth_pitch, boxes, n_boxes);
+    return submit(t, time, gray, gray_pitch, depth, depth_pitch, on_device != 0, boxes, n_boxes);
 }
 
 int gf_tracker_wait_boxes(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info)
@@ -865,8 +738,7 @@ int gf_tracker_wait_boxes(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* in_bo
     const int es = (int)(t->n_waited % 2);
     GF_CUDA(cudaEventSynchronize(t->ev_out[es]));
     t->n_waited++;
-    if (t->t0_valid[es]) GF_CUDA(cudaEventElapsedTime(&t->last_ms, t->ev_t0[es], t->ev_out[es]));
-    else t->last_ms = 0.f;          // batch pipeline: frames are not stamped individually
+    GF_CUDA(cudaEventElapsedTime(&t->last_ms, t->ev_t0[es], t->ev_out[es]));
     if (t->profiling) {
         cudaEvent_t b[8] = {t->ev_t0[es], t->ev_st[0], t->ev_st[1], t->ev_st[2], t->ev_st[3], t->ev_st[4], t->ev_st[5], t->ev_out[es]};
         for (int i = 0; i < 7; i++) GF_CUDA(cudaEventElapsedTime(&t->stage_ms[i], b[i], b[i + 1]));
@@ -925,7 +797,7 @@ struct BatchLane {
     const double* times; const void* const* gray; const void* const* depth;
     gf_obs* out; int* n_out; uint8_t* status_out; gf_track_info* info;
     const gf_box* boxes; const int* box_start; uint8_t* in_box;     // frame k: boxes[box_start[k] .. box_start[k + 1]); nullable
-    int collected, k0;
+    int collected;
     const gf_box* frame_boxes(int k) const { return box_start ? boxes + box_start[k] : nullptr; }
     int n_boxes(int k) const { return box_start ? box_start[k + 1] - box_start[k] : 0; }
 };
@@ -937,62 +809,6 @@ static int lane_collect(BatchLane& L)
     return gf_tracker_wait_boxes(L.t, L.out ? L.out + (size_t)k * cap : nullptr, L.n_out ? L.n_out + k : nullptr,
                                  L.in_box ? L.in_box + (size_t)k * cap : nullptr, L.status_out ? L.status_out + (size_t)k * cap : nullptr,
                                  L.info ? L.info + k : nullptr);
-}
-static int lane_submit_plain(BatchLane& L, int k, size_t gray_pitch, size_t depth_pitch, int on_device)
-{
-    const void* dk = L.depth ? L.depth[k] : nullptr;
-    return on_device ? submit_dev(L.t, L.times[k], L.gray[k], dk, L.frame_boxes(k), L.n_boxes(k))
-                     : submit_host(L.t, L.times[k], (const uint8_t*)L.gray[k], gray_pitch, (const uint16_t*)dk, depth_pitch,
-                                   L.frame_boxes(k), L.n_boxes(k));
-}
-// Makes frame k reachable by its intake kernel: fills the pinned FrameParams slot the graph uploads and, for host frames,
-// copies them to the staging slot on s_up (s_main then waits for that copy before the graph that holds prep(k)).
-static int lane_stage(BatchLane& L, int k, long long f, size_t gray_pitch, size_t depth_pitch, int on_device)
-{
-    gf_tracker* t = L.t;
-    const int es = (int)(f % 2), w = t->w, h = t->h;
-    const void* dk = L.depth ? L.depth[k] : nullptr;
-    FrameParams* fp = t->h_fp[es];
-    fp->dt = L.times[k] - (k > 0 ? L.times[k - 1] : t->prev_time);
-    fp->has_pred = 0;
-    fp->depth_valid = dk ? 1 : 0;
-    put_boxes(fp->boxes, L.frame_boxes(k), L.n_boxes(k));
-    if (on_device) {
-        fp->src_gray = (const uint8_t*)L.gray[k]; fp->src_gray_pitch = w;
-        fp->src_depth = (const uint16_t*)dk; fp->src_depth_pitch = 2ll * w;
-    } else {
-        GF_CUDA(cudaMemcpy2DAsync(t->d_stage_gray[es], w, L.gray[k], gray_pitch, w, h, cudaMemcpyHostToDevice, t->s_up));
-        if (dk) GF_CUDA(cudaMemcpy2DAsync(t->d_stage_depth[es], (size_t)w * 2, dk, depth_pitch, (size_t)w * 2, h, cudaMemcpyHostToDevice, t->s_up));
-        GF_CUDA(cudaEventRecord(t->ev_up[es], t->s_up));
-        GF_CUDA(cudaStreamWaitEvent(t->s_main, t->ev_up[es], 0));
-        fp->src_gray = t->d_stage_gray[es]; fp->src_gray_pitch = w;
-        fp->src_depth = dk ? t->d_stage_depth[es] : nullptr; fp->src_depth_pitch = 2ll * w;
-    }
-    return GF_OK;
-}
-// Launches the graph of frame k of the lane: dep(k) || prep(k + 1), or dep(k) alone for the last frame.
-static int lane_issue(BatchLane& L, int k, int n, size_t gray_pitch, size_t depth_pitch, int on_device)
-{
-    gf_tracker* t = L.t;
-    GF_CUDA(cudaSetDevice(t->device));
-    const long long f = t->n_submitted;
-    const int es = (int)(f % 2), key = (int)(f % 6);
-    int rc;
-    if (k + 1 < n) {
-        rc = lane_stage(L, k + 1, f + 1, gray_pitch, depth_pitch, on_device);
-        if (rc) return rc;
-        rc = run_piece(t, t->s_main, &t->gb_both[key], &t->gbk_both[key], [&] { return body_both_b(t, f); });
-    } else {
-        rc = run_piece(t, t->s_main, &t->gb_dep[key], &t->gbk_dep[key], [&] { return body_dep_b(t, f); });
-    }
-    if (rc) return rc;
-    GF_CUDA(cudaEventRecord(t->ev_out[es], t->s_main));
-    t->prev_time = L.times[k];
-    t->has_pred = false;
-    t->depth_valid[es] = L.depth && L.depth[k];
-    t->t0_valid[es] = false;
-    t->n_submitted = f + 1;
-    return GF_OK;
 }
 
 int gf_tracker_track_batch_multi_boxes(gf_tracker* const* trackers, int n_trackers, int n, const double* times, const void* const* gray,
@@ -1025,53 +841,19 @@ int gf_tracker_track_batch_multi_boxes(gf_tracker* const* trackers, int n_tracke
         L.out = out ? out + o * cap : nullptr; L.n_out = n_out ? n_out + o : nullptr;
         L.status_out = status_out ? status_out + o * cap : nullptr; L.info = info ? info + o : nullptr;
         L.boxes = boxes; L.box_start = box_start ? box_start + o : nullptr; L.in_box = in_box ? in_box + o * cap : nullptr;
-        L.collected = 0; L.k0 = 0;
+        L.collected = 0;
         for (int k = 0; k < n; k++) if (!L.gray[k]) return set_err(GF_ERR_INVALID_ARG, "null frame pointer");
     }
     if (n == 0) return GF_OK;
     int rc;
-    // Default: every lane goes frame by frame through the five-stream submit / wait pipeline of gf_tracker_submit, lanes interleaved.
-    // GF_BATCH_PIPELINE=1 selects the one-graph-per-frame pipeline below instead; measured on one H100 SXM at 700 W (C2, same run):
-    // single stream 10.0 k (default) vs 9.6 k frames/s, 8 streams 26.6 k vs 23.0 k -- joining prep(f+1) into the graph of
-    // dep(f) costs more overlap than the saved driver calls give back (DESIGN 1.3).
-    bool any_pipeline = false;
-    for (BatchLane& L : lanes) any_pipeline = any_pipeline || (L.t->use_graph && L.t->batch_pipeline);
-    if (!any_pipeline) {
-        for (int k = 0; k < n; k++) {
-            for (BatchLane& L : lanes) if ((rc = lane_submit_plain(L, k, gray_pitch, depth_pitch, on_device))) return rc;
-            for (BatchLane& L : lanes) if (in_flight(L.t) == GF_PIPE && (rc = lane_collect(L))) return rc;
-        }
-        for (BatchLane& L : lanes) while (in_flight(L.t) > 0) if ((rc = lane_collect(L))) return rc;
-        return GF_OK;
-    }
-    // lanes that cannot use the one-graph-per-frame pipeline for their first frame(s)
-    for (BatchLane& L : lanes) {
-        gf_tracker* t = L.t;
-        if (!t->use_graph || !t->batch_pipeline) {
-            for (int k = 0; k < n; k++) {
-                if ((rc = lane_submit_plain(L, k, gray_pitch, depth_pitch, on_device))) return rc;
-                if (in_flight(t) == GF_PIPE && (rc = lane_collect(L))) return rc;
-            }
-            while (in_flight(t) > 0) if ((rc = lane_collect(L))) return rc;
-            L.k0 = n;
-        } else if (t->has_pred) {                 // a pending setPrediction only concerns the first frame: it takes the other path
-            if ((rc = lane_submit_plain(L, 0, gray_pitch, depth_pitch, on_device)) || (rc = lane_collect(L))) return rc;
-            L.k0 = 1;
-        }
-    }
-    // one host thread feeds every lane round-robin: prep of the first frame, then one graph launch per lane and frame
-    // (tools/graph_rate_probe.cu: one thread replays small graphs into 8 streams at 114 k launches/s, 8 threads at 48-80 k)
-    for (BatchLane& L : lanes) {
-        if (L.k0 >= n) continue;
-        gf_tracker* t = L.t;
-        GF_CUDA(cudaSetDevice(t->device));
-        const long long f = t->n_submitted;
-        if ((rc = lane_stage(L, L.k0, f, gray_pitch, depth_pitch, on_device))) return rc;
-        const int key = (int)(f % 6);
-        if ((rc = run_piece(t, t->s_main, &t->gb_prep[key], &t->gbk_prep[key], [&] { return body_prep_b(t, f, t->s_main); }))) return rc;
-    }
+    // Every lane goes frame by frame through the five-stream submit / wait pipeline of gf_tracker_submit, lanes interleaved:
+    // one host thread keeps up to two frames in flight on each tracker.
     for (int k = 0; k < n; k++) {
-        for (BatchLane& L : lanes) if (k >= L.k0 && (rc = lane_issue(L, k, n, gray_pitch, depth_pitch, on_device))) return rc;
+        for (BatchLane& L : lanes) {
+            rc = submit(L.t, L.times[k], L.gray[k], gray_pitch, L.depth ? L.depth[k] : nullptr, depth_pitch, on_device != 0,
+                        L.frame_boxes(k), L.n_boxes(k));
+            if (rc) return rc;
+        }
         for (BatchLane& L : lanes) if (in_flight(L.t) == GF_PIPE && (rc = lane_collect(L))) return rc;
     }
     for (BatchLane& L : lanes) while (in_flight(L.t) > 0) if ((rc = lane_collect(L))) return rc;
@@ -1240,7 +1022,7 @@ int gf_stage_clahe(int device, const uint8_t* src, size_t src_pitch, int w, int 
     const int pitch = align_up(w, 16);
     if ((rc = ds.alloc((size_t)pitch * h)) || (rc = dd.alloc((size_t)pitch * h)) || (rc = dl.alloc(clahe_lut_bytes(g)))) return rc;
     GF_CUDA(cudaMemcpy2D(ds.p, pitch, src, src_pitch, w, h, cudaMemcpyHostToDevice));
-    rc = enqueue_clahe(0, ClaheSrc{ds.as<uint8_t>(), pitch, nullptr, nullptr}, g, dl.as<uint8_t>(), dd.as<uint8_t>(), pitch); if (rc) return rc;
+    rc = enqueue_clahe(0, ds.as<uint8_t>(), pitch, g, dl.as<uint8_t>(), dd.as<uint8_t>(), pitch); if (rc) return rc;
     GF_CUDA(cudaMemcpy2D(dst, w, dd.p, pitch, w, h, cudaMemcpyDeviceToHost));
     return GF_OK;
 }
@@ -1347,7 +1129,7 @@ int gf_stage_gftt(int device, const uint8_t* img, int w, int h, const float* kep
         fa.kept_pts = dk.as<float2>(); fa.kept_ids = dummy[4].as<int>(); fa.kept_cnt = dummy[5].as<int>(); fa.kept_un = dummy[6].as<float2>();
         CamParams cam; memset(&cam, 0, sizeof(cam)); cam.fx = cam.fy = 1.0; cam.no_distortion = 1;
         // max_cnt such that exactly max_corners new corners are requested
-        k_select_finalize<<<1, 1024, cells>>>(sc, fa, grid, w, n_kept + max_corners, min_dist, cam, nullptr, nullptr, 0, 0, nullptr, h, dhdr.as<OutHeader>(), dobs.as<gf_obs>(), nullptr); GF_LAUNCHED();
+        k_select_finalize<<<1, 1024, cells>>>(sc, fa, grid, w, n_kept + max_corners, min_dist, cam, nullptr, nullptr, 0, 0, nullptr, h, dhdr.as<OutHeader>(), dobs.as<gf_obs>(), nullptr, nullptr, nullptr); GF_LAUNCHED();
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) { snprintf(g_err, sizeof(g_err), "k_select_finalize launch: %s", cudaGetErrorString(e)); rc = GF_ERR_CUDA; }
     }

@@ -2,8 +2,8 @@
 
 gf_stage_in_boxes against cv2.pointPolygonTest on the probe sets of box_ref; tracker sequences on the synthetic stream with a moving
 object, fed its detections, 100-box lists with degenerate, inverted and out-of-image boxes, frames without boxes and a box over the
-whole image -- through every intake path (host / device frames, two frames in flight, both batch orchestrations, GF_NO_GRAPH,
-GF_PDL, profiling mode); the state invariant (boxes change in_box only); argument errors; the launch count; the C++ adaptor; and the
+whole image -- through every intake path (host / device frames, two frames in flight, batches, GF_NO_GRAPH, GF_LK_NO_TMA,
+profiling mode); the state invariant (boxes change in_box only); argument errors; the launch count; the C++ adaptor; and the
 replay loop with USE_YOLO."""
 import ctypes
 import os
@@ -201,23 +201,22 @@ def _ptrs(frames, on_device, keep):
     return [x.data_ptr() for x in gs], [x.data_ptr() for x in ds]
 
 
-@pytest.fixture(params=["streams", "one-graph-per-frame", "no-graph", "pdl"])
+@pytest.fixture(params=["streams", "no-graph", "no-tma", "no-graph-no-tma"])
 def orchestration(request, monkeypatch):
-    for v in ("GF_BATCH_PIPELINE", "GF_NO_GRAPH", "GF_PDL"):
-        monkeypatch.delenv(v, raising=False)
-    if request.param in ("one-graph-per-frame", "pdl"):
-        monkeypatch.setenv("GF_BATCH_PIPELINE", "1")
-    if request.param == "no-graph":
+    """The five-stream pipeline with CUDA graphs, GF_NO_GRAPH, GF_LK_NO_TMA and both; the tracker reads them when it is created."""
+    monkeypatch.delenv("GF_NO_GRAPH", raising=False)
+    monkeypatch.delenv("GF_LK_NO_TMA", raising=False)
+    if request.param in ("no-graph", "no-graph-no-tma"):
         monkeypatch.setenv("GF_NO_GRAPH", "1")
-    if request.param == "pdl":
-        monkeypatch.setenv("GF_PDL", "1")
+    if request.param in ("no-tma", "no-graph-no-tma"):
+        monkeypatch.setenv("GF_LK_NO_TMA", "1")
     return request.param
 
 
 @pytest.mark.parametrize("on_device", [False, True])
 def test_batch_matches_oracle(gf, orchestration, on_device):
-    if orchestration in ("no-graph", "pdl") and on_device:
-        pytest.skip("GF_NO_GRAPH / GF_PDL: once, host frames")
+    if orchestration == "no-graph" and on_device:
+        pytest.skip("GF_NO_GRAPH: once, host frames")
     frames = [(t, np.ascontiguousarray(g), np.ascontiguousarray(d), b) for t, g, d, b in dynamic_frames(10, 640, 480, 15)]
     want = _oracle(frames, 640)
     tr = gf.FeatureTracker(640, 480, _cam(640).params8(), 150, 30, 1, 1)
@@ -235,8 +234,8 @@ def test_batch_matches_oracle(gf, orchestration, on_device):
 @pytest.mark.parametrize("on_device", [False, True])
 def test_batch_multi_matches_oracle(gf, orchestration, on_device):
     from ground_fusion_b200.feature_tracker import FeatureTracker
-    if orchestration in ("no-graph", "pdl") and on_device:
-        pytest.skip("GF_NO_GRAPH / GF_PDL: once, host frames")
+    if orchestration == "no-graph" and on_device:
+        pytest.skip("GF_NO_GRAPH: once, host frames")
     S, n = 3, 9
     streams = [[(t, np.ascontiguousarray(g), np.ascontiguousarray(d), b) for t, g, d, b in dynamic_frames(40 + i, 640, 480, n)] for i in range(S)]
     streams[1] = [(t, g, d, np.zeros((0, 4), np.int64)) for t, g, d, _ in streams[1]]        # one stream without detections

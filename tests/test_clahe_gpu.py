@@ -2,8 +2,7 @@
 
 The CLAHE kernels against cv2.createCLAHE(clip, grid).apply, bit for bit; and whole tracker sequences with equalisation on
 against the cv2 oracle that equalises each frame before trackImage, as the reference does with `equalize` set -- through every
-intake path (host / device frames, the two-frames-in-flight pipeline, both batch orchestrations, GF_NO_GRAPH, GF_PDL,
-profiling mode).  The sequences are dark and low-contrast, derived from the synthetic stream by a gamma and a contrast squeeze."""
+intake path (host / device frames, the two-frames-in-flight pipeline, batches, GF_NO_GRAPH, GF_LK_NO_TMA, profiling mode).  The sequences are dark and low-contrast, derived from the synthetic stream by a gamma and a contrast squeeze."""
 import numpy as np
 import pytest
 
@@ -184,25 +183,23 @@ def _ptrs(frames, on_device, keep):
     return [x.data_ptr() for x in gs], [x.data_ptr() for x in ds]
 
 
-@pytest.fixture(params=["streams", "one-graph-per-frame", "no-graph", "pdl"])
+@pytest.fixture(params=["streams", "no-graph", "no-tma", "no-graph-no-tma"])
 def orchestration(request, monkeypatch):
-    """Both batch orchestrations (DESIGN 1.3), and GF_NO_GRAPH / GF_PDL once each; the tracker reads them when it is created."""
-    for v in ("GF_BATCH_PIPELINE", "GF_NO_GRAPH", "GF_PDL"):
-        monkeypatch.delenv(v, raising=False)
-    if request.param in ("one-graph-per-frame", "pdl"):
-        monkeypatch.setenv("GF_BATCH_PIPELINE", "1")
-    if request.param == "no-graph":
+    """The five-stream pipeline with CUDA graphs, GF_NO_GRAPH, GF_LK_NO_TMA and both; the tracker reads them when it is created."""
+    monkeypatch.delenv("GF_NO_GRAPH", raising=False)
+    monkeypatch.delenv("GF_LK_NO_TMA", raising=False)
+    if request.param in ("no-graph", "no-graph-no-tma"):
         monkeypatch.setenv("GF_NO_GRAPH", "1")
-    if request.param == "pdl":
-        monkeypatch.setenv("GF_PDL", "1")
+    if request.param in ("no-tma", "no-graph-no-tma"):
+        monkeypatch.setenv("GF_LK_NO_TMA", "1")
     return request.param
 
 
 @pytest.mark.parametrize("w,h", [(640, 480), (641, 481)])
 @pytest.mark.parametrize("on_device", [False, True])
 def test_equalized_batch_matches_oracle(gf, orchestration, on_device, w, h):
-    if orchestration in ("no-graph", "pdl") and (on_device or w != 640):
-        pytest.skip("GF_NO_GRAPH / GF_PDL: once, host frames at 640x480")
+    if orchestration == "no-graph" and (on_device or w != 640):
+        pytest.skip("GF_NO_GRAPH: once, host frames at 640x480")
     frames = [(t, np.ascontiguousarray(g), np.ascontiguousarray(d)) for t, g, d in dark_stream(seed=12, w=w, h=h, n=14)]
     want = _oracle_results(frames, w)
     tr = gf.FeatureTracker(w, h, _cam(w).params8(), 150, 30, 1, 1, equalize=True)
@@ -221,8 +218,8 @@ def test_equalized_batch_matches_oracle(gf, orchestration, on_device, w, h):
 @pytest.mark.parametrize("on_device", [False, True])
 def test_equalized_batch_multi_matches_oracle(gf, orchestration, on_device):
     from ground_fusion_b200.feature_tracker import FeatureTracker
-    if orchestration in ("no-graph", "pdl") and on_device:
-        pytest.skip("GF_NO_GRAPH / GF_PDL: once, host frames")
+    if orchestration == "no-graph" and on_device:
+        pytest.skip("GF_NO_GRAPH: once, host frames")
     S, n = 3, 8
     streams = [[(t, np.ascontiguousarray(g), np.ascontiguousarray(d)) for t, g, d in dark_stream(seed=30 + i, w=640, h=480, n=n)]
                for i in range(S)]

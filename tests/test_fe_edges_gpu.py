@@ -21,7 +21,7 @@ import numpy as np
 import pytest
 
 from conftest import make_texture_image, warp_image
-from test_fe_gpu import _padded, _run_sequence
+from test_fe_gpu import _padded, _run_sequence, lk_staging  # noqa: F401 (fixture)
 
 pytestmark = pytest.mark.gpu
 cv2 = pytest.importorskip("cv2")
@@ -73,16 +73,6 @@ def max_tile_apron(kept, w, h, r):
             m = (c[:, 0] >= x0 - r) & (c[:, 0] < x0 + 64 + r) & (c[:, 1] >= y0 - r) & (c[:, 1] < y0 + 16 + r)
             best = max(best, int(m.sum()))
     return best
-
-
-@pytest.fixture(params=["tma", "no-tma"])
-def lk_staging(request, monkeypatch):
-    """make_lk_maps reads GF_LK_NO_TMA on every call: with it the windows are staged by aligned 32-bit loads."""
-    if request.param == "no-tma":
-        monkeypatch.setenv("GF_LK_NO_TMA", "1")
-    else:
-        monkeypatch.delenv("GF_LK_NO_TMA", raising=False)
-    return request.param
 
 
 def check_lk(gf, a, b, pts, max_level, init=None):
@@ -372,15 +362,6 @@ def test_track_sequence_dense_1000_features(gf):
     assert max(aprons) > 8
 
 
-@pytest.fixture(params=["streams", "one-graph-per-frame"])
-def batch_mode(request, monkeypatch):
-    if request.param == "one-graph-per-frame":
-        monkeypatch.setenv("GF_BATCH_PIPELINE", "1")
-    else:
-        monkeypatch.delenv("GF_BATCH_PIPELINE", raising=False)
-    return request.param
-
-
 def _frame_ptrs(frames, on_device, pad, keep):
     """Frame addresses for trackBatch: host frames as views into rows `pad` elements wider, or packed device copies."""
     import torch
@@ -405,11 +386,11 @@ def _check_frames(want, got, base=0):
         assert o1.tobytes() == o2.tobytes(), "frame %d" % (base + k)
 
 
-@pytest.mark.parametrize("w,h", [(641, 481), (424, 400)])
+@pytest.mark.parametrize("w,h", [(641, 481), (424, 400), (752, 480), (480, 640)])
 @pytest.mark.parametrize("on_device", [False, True])
-def test_batch_odd_geometry_equals_track_image(gf, w, h, on_device, batch_mode):
-    """trackBatch at widths whose rows are not 16-byte aligned (k_copy_in falls back to byte copies), host frames with a
-    row pitch larger than the width, frames without a depth image in between; compared with trackImage."""
+def test_batch_odd_geometry_equals_track_image(gf, w, h, on_device):
+    """trackBatch at widths whose rows are not 16-byte aligned, at 752x480 and in portrait, host frames with a row pitch
+    larger than the width, frames without a depth image in between; compared with trackImage."""
     from ground_fusion_b200.synth import SyntheticStream
     from oracle.fe_oracle import IDC_CAM, PinholeCamera
     sc = w / 640.0
@@ -438,13 +419,13 @@ def test_batch_odd_geometry_equals_track_image(gf, w, h, on_device, batch_mode):
 
 # ---- D. orchestration switches ----------------------------------------------------------------------------------------
 
-@pytest.mark.parametrize("switch", ["GF_NO_GRAPH", "GF_PDL", "GF_FE_PDL1", "GF_LK_NO_TMA"])
-def test_tracker_switch_matches_oracle(gf, monkeypatch, switch):
+@pytest.mark.parametrize("switch", ["GF_NO_GRAPH", "GF_LK_NO_TMA"])
+@pytest.mark.parametrize("on_device", [False, True])
+def test_tracker_switch_matches_oracle(gf, monkeypatch, switch, on_device):
     """Each documented switch (read when the tracker is created): a 20-frame C2 sequence against the oracle, then the same
-    frames through trackBatch in both batch orchestrations (GF_PDL acts inside the one-graph-per-frame pipeline)."""
+    frames through trackBatch, from host or device memory."""
     from ground_fusion_b200.synth import SyntheticStream
     from oracle.fe_oracle import IDC_CAM, PinholeCamera
-    monkeypatch.delenv("GF_BATCH_PIPELINE", raising=False)
     monkeypatch.setenv(switch, "1")
     want = []
     _run_sequence(gf, seed=0, n_frames=20,
@@ -452,13 +433,12 @@ def test_tracker_switch_matches_oracle(gf, monkeypatch, switch):
     cam = PinholeCamera(**IDC_CAM)
     stream = SyntheticStream(seed=0)
     frames = [stream.frame(k) for k in range(20)]
-    for pipeline in (False, True):
-        if pipeline:
-            monkeypatch.setenv("GF_BATCH_PIPELINE", "1")
-        b = gf.FeatureTracker(640, 480, cam.params8(), 150, 30, 1, 1)
-        got = b.trackBatch([t for t, _, _ in frames], [g.ctypes.data for _, g, _ in frames], [d.ctypes.data for _, _, d in frames])
-        _check_frames(want, got)
-        b.close()
+    keep = []
+    gp, dp, gpitch, dpitch = _frame_ptrs(frames, on_device, 0, keep)
+    b = gf.FeatureTracker(640, 480, cam.params8(), 150, 30, 1, 1)
+    got = b.trackBatch([t for t, _, _ in frames], gp, dp, on_device=on_device, gray_pitch=gpitch, depth_pitch=dpitch)
+    _check_frames(want, got)
+    b.close()
 
 
 def test_ba_solve_without_pdl_matches_oracle():

@@ -105,6 +105,16 @@ def test_gftt_matches_cv2(gf, seed, max_corners, min_dist, n_kept):
     assert got.shape == want.shape and np.array_equal(got, want), info
 
 
+@pytest.fixture(params=["tma", "no-tma"])
+def lk_staging(request, monkeypatch):
+    """make_lk_maps reads GF_LK_NO_TMA on every call: with it the windows are staged by aligned 32-bit loads."""
+    if request.param == "no-tma":
+        monkeypatch.setenv("GF_LK_NO_TMA", "1")
+    else:
+        monkeypatch.delenv("GF_LK_NO_TMA", raising=False)
+    return request.param
+
+
 def _padded(a, pad):
     """a as a view into a buffer `pad` elements wider per row; the padding holds the largest value of the type."""
     buf = np.full((a.shape[0], a.shape[1] + pad), np.iinfo(a.dtype).max, a.dtype)
@@ -285,22 +295,12 @@ def test_prediction_and_remove_outliers(gf):
     gpu.close()
 
 
-@pytest.fixture(params=["streams", "one-graph-per-frame"])
-def batch_mode(request, monkeypatch):
-    """gf_tracker_track_batch(_multi) has two orchestrations (DESIGN 1.3); the tracker reads GF_BATCH_PIPELINE when it is created."""
-    if request.param == "one-graph-per-frame":
-        monkeypatch.setenv("GF_BATCH_PIPELINE", "1")
-    else:
-        monkeypatch.delenv("GF_BATCH_PIPELINE", raising=False)
-    return request.param
-
-
 @pytest.mark.parametrize("on_device", [False, True])
-def test_batch_pipeline_equals_blocking_calls(gf, on_device, batch_mode):
-    """gf_tracker_track_batch runs one graph per frame ({track + select of frame f} || {intake + pyramid + min-eig of f+1});
-    the frames must come out exactly as from trackImage: batches of 1, 2, 5, 7 and 10 frames back to back, frames without a
-    depth image in between, a setPrediction before a batch (first frame takes the other path), a removeOutliers and a
-    plain trackImage call between batches, host and device-resident frames."""
+def test_batch_pipeline_equals_blocking_calls(gf, on_device, lk_staging):
+    """gf_tracker_track_batch keeps two frames in flight through the five-stream pipeline; the frames must come out exactly as
+    from trackImage, with the LK windows staged by TMA and without: batches of 1, 2, 5, 7 and 10 frames back to back, frames without a depth image in between, a
+    setPrediction before a batch, a removeOutliers and a plain trackImage call between batches, host and device-resident
+    frames."""
     import torch
     from ground_fusion_b200.synth import SyntheticStream
     from oracle.fe_oracle import IDC_CAM, PinholeCamera
@@ -359,7 +359,7 @@ def test_batch_pipeline_equals_blocking_calls(gf, on_device, batch_mode):
 
 
 @pytest.mark.parametrize("on_device", [False, True])
-def test_multi_stream_batch_equals_single_stream_batches(gf, on_device, batch_mode):
+def test_multi_stream_batch_equals_single_stream_batches(gf, on_device, lk_staging):
     """gf_tracker_track_batch_multi: three independent streams (different scenes, one without depth images, one with a pending
     prediction) fed by one host thread come out exactly as from three gf_tracker_track_batch calls."""
     import torch
