@@ -926,20 +926,14 @@ __global__ void __launch_bounds__(RB_THREADS) k_ba_step(BaDev d)
 // as a similarity A <- J^T A J with J = product of the plane rotations: the matrix splits into disjoint 2x2 blocks
 // (row pair x column pair), each updated independently from the two rotations involved.  V accumulates the rotations
 // (columns = eigenvectors), w = diagonal at convergence (off-norm <= 1e-30 * diag-norm, like the oracle's sweep test).
-__global__ void __launch_bounds__(1024) k_jacobi_eig(double* Ag, double* Vg, double* w, int n, int* sweeps_out, int in_smem)
+__global__ void __launch_bounds__(1024) k_jacobi_eig(double* A, double* V, double* w, int n, int* sweeps_out)
 {
-    extern __shared__ double jsm[];           // c[np/2], s[np/2]; then int pr[np/2], qr[np/2]; then (in_smem) A[n*n], V[n*n]
+    extern __shared__ double jsm[];           // c[np/2], s[np/2]; then int pr[np/2], qr[np/2]
     __shared__ double sred[32];
     const int tid = threadIdx.x, nt = blockDim.x;
     const int np = (n + 1) & ~1, hp = np / 2;
     double* cs_c = jsm; double* cs_s = jsm + hp;
     int* pp = reinterpret_cast<int*>(jsm + 2 * hp); int* qq = pp + hp;
-    // small matrices (the reduced system of the marginalisation) live in shared memory for the whole decomposition
-    double* A = Ag; double* V = Vg;
-    if (in_smem) {
-        A = jsm + 2 * hp + ((2 * hp * (int)sizeof(int) + 7) / 8); V = A + (size_t)n * n;
-        for (int e = tid; e < n * n; e += nt) A[e] = Ag[e];
-    }
     for (int e = tid; e < n * n; e += nt) V[e] = (e / n == e % n) ? 1.0 : 0.0;
     __syncthreads();
     int sweep = 0;
@@ -950,13 +944,16 @@ __global__ void __launch_bounds__(1024) k_jacobi_eig(double* Ag, double* Vg, dou
         off = block_reduce_sum(off, sred); dg = block_reduce_sum(dg, sred);
         if (off <= 1e-30 * dg || off == 0.0) break;
         // rounding floor: with entries of 1e9 next to (numerically) zero eigenvalues the off-norm stalls around
-        // n * eps * |A| and never meets the test above; once it stops shrinking further sweeps only reshuffle noise
-        if (sweep >= 4 && off <= 1e-20 * dg && off >= 0.25 * prev_off) break;
+        // n * eps * |A| and never meets the test above; once it stops shrinking there further sweeps only reshuffle noise.
+        // The floor is (10 n eps)^2 of the squared diagonal norm: a fixed 1e-20 let a slow sweep among clustered small
+        // eigenvalues end the decomposition with off-diagonal entries of 1e-10 |A|, 400x double's accuracy at n = 198
+        const double floor_ = 10.0 * n * 2.220446049250313e-16;
+        if (sweep >= 4 && off <= floor_ * floor_ * dg && off >= 0.25 * prev_off) break;
         prev_off = off;
         for (int round = 0; round < np - 1; round++) {
-            if (tid < hp) {
-                int a = tid == 0 ? np - 1 : (round + tid) % (np - 1);
-                int b = tid == 0 ? round : (round + np - 1 - tid) % (np - 1);
+            for (int k = tid; k < hp; k += nt) {      // n > 2048: more pairs than threads
+                int a = k == 0 ? np - 1 : (round + k) % (np - 1);
+                int b = k == 0 ? round : (round + np - 1 - k) % (np - 1);
                 int p_ = min(a, b), q_ = max(a, b);
                 double c = 1.0, sn = 0.0;
                 if (q_ < n) {
@@ -967,7 +964,7 @@ __global__ void __launch_bounds__(1024) k_jacobi_eig(double* Ag, double* Vg, dou
                         c = 1.0 / sqrt(t * t + 1.0); sn = t * c;
                     }
                 }
-                cs_c[tid] = c; cs_s[tid] = sn; pp[tid] = p_; qq[tid] = q_;
+                cs_c[k] = c; cs_s[k] = sn; pp[k] = p_; qq[k] = q_;
             }
             __syncthreads();
             // A <- J^T A J on the 2x2 blocks (row pair r, column pair k).  The blocks are disjoint, so a thread first
@@ -1035,7 +1032,6 @@ __global__ void __launch_bounds__(1024) k_jacobi_eig(double* Ag, double* Vg, dou
         }
     }
     for (int i = tid; i < n; i += nt) w[i] = A[(size_t)i * n + i];
-    if (in_smem) for (int e = tid; e < n * n; e += nt) Vg[e] = V[e];
     if (tid == 0 && sweeps_out) *sweeps_out = sweep;
 }
 
@@ -1245,7 +1241,8 @@ __global__ void k_marg_reduce(MargDev q)   // A = Arr - Arm Amm_inv Amr, b = brr
 // When Amm - eps I is positive definite every eigenvalue passes the reference's eps test, the eigen-truncated inverse IS
 // the inverse, and Arr - Arm Amm^-1 Amr is the ordinary two-stage Schur complement: landmarks (1x1 pivots) first, then
 // the c x c block of pose0 / speedbias0.  Q is the (c+n) x (c+n) system left after the landmarks, order [c | kept].
-// flag[0] is set when the positive-definiteness test fails (the generic Jacobi path is run instead).
+// flag[0] is set when the positive-definiteness test fails (the generic Jacobi path is run instead).  Launched with at least
+// max(R^2, m) threads: thread e < R^2 forms Q[e], thread c <= e < m tests landmark pivot e.
 __global__ void k_marg_lm_elim(MargDev q, int c, double* Q, double* qb, double* Ceps, int* flag)
 {
     const int R = c + q.n, m = q.m, N = q.N;
@@ -1342,6 +1339,7 @@ struct gf_ba {
     void* hbuf; size_t hcap;     // pinned staging
     long long prof[32];
     int tile_cap;
+    int marg_info[3];            // last marginalisation: GF_MARG_PATH_* bits, Jacobi sweeps on Amm, on the reduced system
 };
 
 static int ensure(gf_ba* s, size_t dbytes)
@@ -1622,6 +1620,48 @@ int gf_ba_solve(gf_ba* s, const gf_ba_problem* p, gf_ba_summary* sum)
  * Returns n (> 0) or a negative error code. */
 }  // extern "C" (reopened below)
 
+// MarginalizationInfo::marginalize (marginalization_factor.cpp:272-302) on the dense system q.A, q.b already on the device,
+// columns [c dense | m - c diagonal landmarks | n kept]: the structured fast path when it applies, else the literal
+// eigen-truncated inverse of Amm; then the eigendecomposition of the reduced system and J0, r0.  d_sw: int[3] on the device
+// ([0], [1] Jacobi sweeps of Amm and of the reduced system, [2] the fast path's flag), h_flag: one host int (pinned in marg_run).  Host
+// synchronisation: one, to read the fast path's flag.  *path: GF_MARG_PATH_* bits.
+static int marg_schur_eig(const MargDev& q, int cdim, bool force_generic, double* Q, double* qb, double* Ceps, int* d_sw, int* h_flag,
+                          cudaStream_t st, int* path)
+{
+    const int m = q.m, n = q.n, Rdim = cdim + n;
+    const size_t mm = (size_t)m * m, nn = (size_t)n * n;
+    auto jac_smem = [](int nn_) { int hp = ((nn_ + 1) & ~1) / 2; return (size_t)hp * (2 * sizeof(double) + 2 * sizeof(int)) + 8; };
+    int* d_flag = d_sw + 2;
+    int p = n > 127 ? GF_MARG_PATH_GENERIC | GF_MARG_PATH_WIDE                 // k_marg_c_elim's shared buffer
+          : force_generic ? GF_MARG_PATH_GENERIC | GF_MARG_PATH_FORCED : 0;
+    if (!p) {
+        // regular case: Amm - eps I positive definite => eigen-truncated inverse == inverse => two-stage Schur complement
+        GF_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(int), st));
+        k_marg_lm_elim<<<(std::max(Rdim * Rdim, m) + 255) / 256, 256, 0, st>>>(q, cdim, Q, qb, Ceps, d_flag); GF_LAUNCHED();
+        k_marg_c_elim<<<1, 256, 0, st>>>(q, cdim, Q, qb, Ceps, d_flag); GF_LAUNCHED();
+        GF_CUDA(cudaMemcpyAsync(h_flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+        GF_CUDA(cudaStreamSynchronize(st));
+        if (*h_flag != 0) p = GF_MARG_PATH_GENERIC | GF_MARG_PATH_NOT_PD;
+    }
+    if (p & GF_MARG_PATH_GENERIC) {   // some eigenvalue of Amm may be below eps: the reference's eigen-truncated inverse, literally
+        k_marg_amm<<<(int)((mm + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
+        k_jacobi_eig<<<1, 1024, jac_smem(m), st>>>(q.Amm, q.Vm, q.wm, m, d_sw); GF_LAUNCHED();
+        k_marg_ainv<<<(int)((mm + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
+        k_marg_T<<<(int)(((size_t)n * m + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
+        k_marg_reduce<<<(int)((nn + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
+    }
+    if (n <= 128) {   // tridiagonalisation + implicit QL in shared memory (what the reference's Eigen solver does)
+        k_sym_eig_ql<<<1, QL_T, sizeof(double) * ((size_t)n * n + 4 * (size_t)n + 8), st>>>(q.Ar, q.Vr, q.wr, n); GF_LAUNCHED();
+    } else {
+        k_jacobi_eig<<<1, 1024, jac_smem(n), st>>>(q.Ar, q.Vr, q.wr, n, d_sw + 1); GF_LAUNCHED();
+        p |= GF_MARG_PATH_REDUCED_JACOBI;
+    }
+    k_marg_out<<<(int)((nn + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
+    GF_CUDA(cudaGetLastError());
+    *path = p;
+    return GF_OK;
+}
+
 enum { GF_MARG_OLD = 0, GF_MARG_SECOND_NEW = 1 };
 static int marg_run(gf_ba* s, const gf_ba_problem* p, int mode, gf_ba_prior* out, double* out_x0, double* out_J, double* out_r, float* device_ms)
 {
@@ -1806,40 +1846,19 @@ static int marg_run(gf_ba* s, const gf_ba_problem* p, int mode, gf_ba_prior* out
     const int eval_blocks = n_work + d.n_imu + d.n_wheel + d.n_plane + (pn ? 1 : 0);
     if (eval_blocks > 0) { k_ba_eval<<<eval_blocks, PAIR_THREADS, sizeof(double) * 2 * (size_t)pn, st>>>(d, 0); GF_LAUNCHED(); }
     k_marg_pack<<<(int)((NN + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
-    auto jac_smem = [](int nn_, bool in_smem) { int hp = ((nn_ + 1) & ~1) / 2; size_t b = (size_t)hp * (2 * sizeof(double) + 2 * sizeof(int)) + 8; return b + (in_smem ? 2 * sizeof(double) * (size_t)nn_ * nn_ : 0); };
-    const int cdim = (old_ && use_sb) ? 15 : 6, Rdim = cdim + n;
-    int* d_flag = (int*)(db + o_sw) + 2;
-    bool generic = n > 127;                                   // k_marg_c_elim's shared buffer
-    if (!generic) {
-        // regular case: Amm - eps I positive definite => eigen-truncated inverse == inverse => two-stage Schur complement
-        GF_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(int), st));
-        k_marg_lm_elim<<<(Rdim * Rdim + 255) / 256, 256, 0, st>>>(q, cdim, (double*)(db + o_Q), (double*)(db + o_qb), (double*)(db + o_ce), d_flag); GF_LAUNCHED();
-        k_marg_c_elim<<<1, 256, 0, st>>>(q, cdim, (const double*)(db + o_Q), (const double*)(db + o_qb), (const double*)(db + o_ce), d_flag); GF_LAUNCHED();
-        int* h_flag = (int*)(hb + o_sw);
-        GF_CUDA(cudaMemcpyAsync(h_flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
-        GF_CUDA(cudaStreamSynchronize(st));
-        generic = *h_flag != 0;
-    }
-    if (generic) {   // some eigenvalue of Amm may be below eps: the reference's eigen-truncated inverse, literally
-        k_marg_amm<<<(int)((mm + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
-        k_jacobi_eig<<<1, 1024, jac_smem(m, false), st>>>(q.Amm, q.Vm, q.wm, m, (int*)(db + o_sw), 0); GF_LAUNCHED();
-        k_marg_ainv<<<(int)((mm + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
-        k_marg_T<<<(int)(((size_t)n * m + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
-        k_marg_reduce<<<(int)((nn + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
-    }
-    if (n <= 128) {   // tridiagonalisation + implicit QL in shared memory (what the reference's Eigen solver does)
-        k_sym_eig_ql<<<1, QL_T, sizeof(double) * ((size_t)n * n + 4 * (size_t)n + 8), st>>>(q.Ar, q.Vr, q.wr, n); GF_LAUNCHED();
-    } else {
-        const bool r_in_smem = jac_smem(n, true) <= 200 * 1024;
-        k_jacobi_eig<<<1, 1024, jac_smem(n, r_in_smem), st>>>(q.Ar, q.Vr, q.wr, n, (int*)(db + o_sw) + 1, r_in_smem ? 1 : 0); GF_LAUNCHED();
-    }
-    k_marg_out<<<(int)((nn + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
-    GF_CUDA(cudaGetLastError());
+    const int cdim = (old_ && use_sb) ? 15 : 6;
+    int path = 0;
+    rc = marg_schur_eig(q, cdim, false, (double*)(db + o_Q), (double*)(db + o_qb), (double*)(db + o_ce), (int*)(db + o_sw), (int*)(hb + o_sw), st, &path);
+    if (rc) return rc;
     GF_CUDA(cudaMemcpyAsync(hb + o_J0, db + o_J0, sizeof(double) * nn, cudaMemcpyDeviceToHost, st));
     GF_CUDA(cudaMemcpyAsync(hb + o_r0, db + o_r0, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
     GF_CUDA(cudaMemcpyAsync(hb + o_st, db + o_st, sizeof(BaState), cudaMemcpyDeviceToHost, st));
     GF_CUDA(cudaEventRecord(s->e1, st));
+    GF_CUDA(cudaMemcpyAsync(hb + o_sw, db + o_sw, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));     // sweep counts (not timed)
     GF_CUDA(cudaStreamSynchronize(st));
+    s->marg_info[0] = path;
+    s->marg_info[1] = (path & GF_MARG_PATH_GENERIC) ? ((int*)(hb + o_sw))[0] : 0;
+    s->marg_info[2] = (path & GF_MARG_PATH_REDUCED_JACOBI) ? ((int*)(hb + o_sw))[1] : 0;
     if (((BaState*)(hb + o_st))->setup_failed) return set_err(GF_ERR_INVALID_ARG, "IMU covariance is not positive definite");
     if (device_ms) GF_CUDA(cudaEventElapsedTime(device_ms, s->e0, s->e1));
     memcpy(out_J, hb + o_J0, sizeof(double) * nn);
@@ -1928,6 +1947,13 @@ int gf_ba_double2vector(const gf_ba_problem* p, const double* R0_before, const d
     return GF_OK;
 }
 
+int gf_ba_last_marg_info(gf_ba* s, int* info3)
+{
+    if (!s || !info3) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    memcpy(info3, s->marg_info, sizeof(s->marg_info));
+    return GF_OK;
+}
+
 /* debug: clock64() cycles per phase of k_ba_step of the last solve (see PH() markers) */
 int gf_ba_debug_profile(gf_ba* s, long long* out32)
 {
@@ -2004,6 +2030,96 @@ extern "C" int gf_stage_spd_solve(int device, const double* A, const double* b, 
     cudaFree(dA); cudaFree(dL); cudaFree(dy); cudaFree(df);
     if (e != cudaSuccess) { snprintf(g_err, sizeof(g_err), "gf_stage_spd_solve: %s", cudaGetErrorString(e)); return GF_ERR_CUDA; }
     if (fail) return set_err(GF_ERR_INVALID_ARG, "matrix is not positive definite");
+    return GF_OK;
+}
+
+// Stage-level entry points (tests): the marginalisation's eigensolvers and its Schur complement on a given dense system.
+static int stage_device(int device)
+{
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return set_err(GF_ERR_NO_DEVICE, "no CUDA device visible; libgf_b200 has no CPU fallback");
+    if (device < 0 || device >= ndev) return set_err(GF_ERR_INVALID_ARG, "device index out of range");
+    GF_CUDA(cudaSetDevice(device));
+    return GF_OK;
+}
+
+// Largest Jacobi size the stage entry points take (gf_stage_sym_eig's n, gf_stage_marginalize's m): above 2048 the kernel's
+// 1024 threads each set up more than one rotation of a round, and the tests run this bound.
+constexpr int STAGE_JACOBI_MAX = 2304;
+
+extern "C" int gf_stage_sym_eig(int device, const double* A, int n, int method, double* w, double* V, int* sweeps)
+{
+    if (!A || !w || !V || n < 1 || (method == 0 && n > 128) || (method == 1 && n > STAGE_JACOBI_MAX) || (method != 0 && method != 1))
+        return set_err(GF_ERR_INVALID_ARG, "bad argument (method 0: 1 <= n <= 128, method 1: 1 <= n <= 2304)");
+    int rc = stage_device(device);
+    if (rc) return rc;
+    const size_t nn = (size_t)n * n;
+    std::vector<double> h(nn);
+    for (int i = 0; i < n; i++) for (int j = 0; j <= i; j++) h[(size_t)i * n + j] = h[(size_t)j * n + i] = A[(size_t)i * n + j];
+    double* dA = nullptr;
+    GF_CUDA(cudaMalloc(&dA, sizeof(double) * (3 * nn + n + 1)));           // A | V | w | sweep count
+    double* dV = dA + nn; double* dw = dV + nn; int* dsw = (int*)(dw + n);
+    cudaError_t e = cudaMemcpy(dA, h.data(), sizeof(double) * nn, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemset(dsw, 0, sizeof(int));
+    if (e == cudaSuccess && method == 0) {
+        e = cudaFuncSetAttribute(k_sym_eig_ql, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        if (e == cudaSuccess) { k_sym_eig_ql<<<1, QL_T, sizeof(double) * (nn + 4 * (size_t)n + 8)>>>(dA, dV, dw, n); GF_LAUNCHED(); }
+    } else if (e == cudaSuccess) {
+        const int hp = ((n + 1) & ~1) / 2;
+        e = cudaFuncSetAttribute(k_jacobi_eig, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        if (e == cudaSuccess) { k_jacobi_eig<<<1, 1024, (size_t)hp * (2 * sizeof(double) + 2 * sizeof(int)) + 8>>>(dA, dV, dw, n, dsw); GF_LAUNCHED(); }
+    }
+    if (e == cudaSuccess) e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpy(V, dV, sizeof(double) * nn, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(w, dw, sizeof(double) * n, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && sweeps) e = cudaMemcpy(sweeps, dsw, sizeof(int), cudaMemcpyDeviceToHost);
+    cudaFree(dA);
+    if (e != cudaSuccess) { snprintf(g_err, sizeof(g_err), "gf_stage_sym_eig: %s", cudaGetErrorString(e)); return GF_ERR_CUDA; }
+    return GF_OK;
+}
+
+extern "C" int gf_stage_marginalize(int device, const double* A, const double* b, int N, int c, int L, int force_generic,
+                                    double* J0, double* r0, int* path)
+{
+    const int m = c + L, n = N - m;
+    if (!A || !b || !J0 || !r0 || !path || c < 1 || c > 15 || L < 0 || m > STAGE_JACOBI_MAX || n < 1 || n > 16 * GF_BA_MAX_FRAMES + 22)
+        return set_err(GF_ERR_INVALID_ARG, "bad argument (1 <= c <= 15, L >= 0, c + L <= 2304, 1 <= N - c - L <= 198)");
+    for (int l = c; l < m; l++)
+        for (int k = c; k < m; k++)
+            if (k != l && A[(size_t)l * N + k] != 0.0) return set_err(GF_ERR_INVALID_ARG, "the landmark block is not diagonal");
+    int rc = stage_device(device);
+    if (rc) return rc;
+    const size_t NN = (size_t)N * N, mm = (size_t)m * m, nn = (size_t)n * n, R = (size_t)c + n;
+    const size_t nd = NN + N + 3 * mm + m + (size_t)n * m + 3 * nn + 3 * (size_t)n + R * R + R + 225;
+    double* d = nullptr;
+    GF_CUDA(cudaMalloc(&d, sizeof(double) * (nd + 2)));                       // ... | int[4] sweeps and flag
+    int* dsw = (int*)(d + nd);
+    MargDev q;
+    memset(&q, 0, sizeof(q));
+    q.N = N; q.m = m; q.n = n;
+    double* t = d;
+    auto take = [&](size_t k) { double* p = t; t += k; return p; };
+    q.A = take(NN); q.b = take(N); q.Amm = take(mm); q.Vm = take(mm); q.wm = take(m); q.Ainv = take(mm); q.T = take((size_t)n * m);
+    q.Ar = take(nn); q.Vr = take(nn); q.wr = take(n); q.br = take(n); q.J0 = take(nn); q.r0 = take(n);
+    double* dQ = take(R * R); double* dqb = take(R); double* dce = take(225);
+    int h_flag = 0, p = 0, hsw[2] = {0, 0};
+    cudaError_t e = cudaMemcpy(q.A, A, sizeof(double) * NN, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(q.b, b, sizeof(double) * N, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemset(dsw, 0, sizeof(int) * 4);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_sym_eig_ql, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_jacobi_eig, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (e == cudaSuccess) {
+        rc = marg_schur_eig(q, c, force_generic != 0, dQ, dqb, dce, dsw, &h_flag, 0, &p);
+        if (!rc) e = cudaMemcpy(J0, q.J0, sizeof(double) * nn, cudaMemcpyDeviceToHost);
+        if (!rc && e == cudaSuccess) e = cudaMemcpy(r0, q.r0, sizeof(double) * n, cudaMemcpyDeviceToHost);
+        if (!rc && e == cudaSuccess) e = cudaMemcpy(hsw, dsw, sizeof(int) * 2, cudaMemcpyDeviceToHost);
+    }
+    cudaFree(d);
+    if (rc) return rc;
+    if (e != cudaSuccess) { snprintf(g_err, sizeof(g_err), "gf_stage_marginalize: %s", cudaGetErrorString(e)); return GF_ERR_CUDA; }
+    path[0] = p;
+    path[1] = (p & GF_MARG_PATH_GENERIC) ? hsw[0] : 0;
+    path[2] = (p & GF_MARG_PATH_REDUCED_JACOBI) ? hsw[1] : 0;
     return GF_OK;
 }
 

@@ -37,6 +37,43 @@ def spd_solve(A, b, device=0, tile_cap=-1):
     return x
 
 
+SYM_EIG_METHODS = {"ql": 0, "jacobi": 1}
+
+
+def sym_eig(A, method, device=0):
+    """Eigendecomposition of a symmetric matrix (lower triangle read) by one of the marginalisation's eigensolvers
+    (gf_stage_sym_eig): "ql" = k_sym_eig_ql (n <= 128), "jacobi" = k_jacobi_eig.  Returns (w, V, sweeps): eigenvalues
+    unsorted, eigenvectors in the columns of V, Jacobi's sweep count (0 for QL)."""
+    L = _lib.lib()
+    dp = ctypes.POINTER(ctypes.c_double)
+    L.gf_stage_sym_eig.argtypes = [ctypes.c_int, dp, ctypes.c_int, ctypes.c_int, dp, dp, ctypes.POINTER(ctypes.c_int)]
+    A = np.ascontiguousarray(A, np.float64)
+    n = A.shape[0]
+    assert A.shape == (n, n)
+    w, V, sw = np.zeros(n), np.zeros((n, n)), ctypes.c_int(0)
+    check(L.gf_stage_sym_eig(int(device), A.ctypes.data_as(dp), n, SYM_EIG_METHODS[method], w.ctypes.data_as(dp), V.ctypes.data_as(dp),
+                             ctypes.byref(sw)))
+    return w, V, sw.value
+
+
+def marginalize_dense(A, b, c, L, force_generic=False, device=0):
+    """MarginalizationInfo::marginalize on a dense system (gf_stage_marginalize, the device code of the marginalisation):
+    columns [c dense | L landmarks (diagonal block) | n kept].  Returns (J0 n x n, r0 n, path) with
+    path = (GF_MARG_PATH_* bits, Jacobi sweeps on Amm, Jacobi sweeps on the reduced system)."""
+    lib = _lib.lib()
+    dp = ctypes.POINTER(ctypes.c_double)
+    lib.gf_stage_marginalize.argtypes = [ctypes.c_int, dp, dp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, dp, dp,
+                                         ctypes.POINTER(ctypes.c_int)]
+    A = np.ascontiguousarray(A, np.float64); b = np.ascontiguousarray(b, np.float64)
+    N = len(b)
+    assert A.shape == (N, N)
+    n = N - c - L
+    J0, r0, path = np.zeros((max(n, 0), max(n, 0))), np.zeros(max(n, 0)), (ctypes.c_int * 3)()
+    check(lib.gf_stage_marginalize(int(device), A.ctypes.data_as(dp), b.ctypes.data_as(dp), N, int(c), int(L), 1 if force_generic else 0,
+                                   J0.ctypes.data_as(dp), r0.ctypes.data_as(dp), path))
+    return J0, r0, tuple(path)
+
+
 class BundleAdjuster:
     """One solver workspace bound to one GPU (gf_ba).  optimization(problem) updates the para_* arrays of
     `problem` (ground_fusion_b200.ba_problem.Problem) in place, like Estimator::optimization() does with
@@ -85,6 +122,13 @@ class BundleAdjuster:
         """MARGIN_SECOND_NEW on the GPU (estimator.cpp:3536-3631): the last prior with para_Pose[WINDOW_SIZE - 1] marginalised;
         None when the prior does not hold that pose (the reference then keeps the prior as it is)."""
         return self._marginalize(problem, "gf_ba_marginalize_second_new")
+
+    def last_marg_info(self):
+        """(GF_MARG_PATH_* bits, Jacobi sweeps on Amm, Jacobi sweeps on the reduced system) of the last marginalisation."""
+        info = (ctypes.c_int * 3)()
+        self.L.gf_ba_last_marg_info.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int)]
+        check(self.L.gf_ba_last_marg_info(self._h, info))
+        return tuple(info)
 
     def solve_struct(self, p_struct):
         """Same, for a pre-built ctypes gf_ba_problem (avoids rebuilding it in timing loops)."""

@@ -230,6 +230,29 @@ int gf_stage_setmask_order(int device, const int32_t* track_cnt, int n, int32_t*
  * path (tests). */
 int gf_stage_spd_solve(int device, const double* A, const double* b, int n, double* x, int tile_cap);
 
+/* The marginalisation's symmetric eigensolvers on their own (A n x n row-major, lower triangle read; w[n], V n x n row-major
+ * with the eigenvectors in its columns, unsorted).  method 0: tridiagonalisation + implicit QL (k_sym_eig_ql, the reduced
+ * system when n <= 128), 1 <= n <= 128; method 1: parallel cyclic Jacobi in global memory (k_jacobi_eig, Amm of the literal
+ * path and reduced systems with n > 128), 1 <= n <= 2304.  sweeps: nullable, Jacobi's sweep count (cap 60; 0 for QL). */
+int gf_stage_sym_eig(int device, const double* A, int n, int method, double* w, double* V, int* sweeps);
+
+/* Which way a marginalisation went (bits of path[0] below and of gf_ba_last_marg_info). */
+#define GF_MARG_PATH_GENERIC 1         /* literal path: eigen-truncated inverse of the whole Amm (Jacobi); else structured fast path */
+#define GF_MARG_PATH_WIDE 2            /* ... because n > 127 (the fast path's c x (n + 1) buffer) */
+#define GF_MARG_PATH_NOT_PD 4          /* ... because Amm - 1e-8 I is not positive definite */
+#define GF_MARG_PATH_FORCED 8          /* ... because the caller asked for it */
+#define GF_MARG_PATH_REDUCED_JACOBI 16 /* reduced system decomposed by Jacobi (n > 128); else by QL */
+
+/* MarginalizationInfo::marginalize (marginalization_factor.cpp:272-302) on a given dense system, with the device code of
+ * gf_ba_marginalize_old: A (N x N row-major), b (N) in the column layout [c dense | L landmarks | n = N - c - L kept],
+ * 1 <= c <= 15, L >= 0, m = c + L <= 2304 (Jacobi size of the literal path), 1 <= n <= 16 * GF_BA_MAX_FRAMES + 22; the
+ * L x L landmark block must be diagonal (GF_ERR_INVALID_ARG otherwise).  force_generic: take the literal path even when the
+ * fast path applies.
+ * Out: J0 (n x n row-major) = sqrt(S) V^T, r0 (n) = sqrt(S^-1) V^T b; path[3] = GF_MARG_PATH_* bits, Jacobi sweeps on Amm
+ * (0 on the fast path), Jacobi sweeps on the reduced system (0 for QL). */
+int gf_stage_marginalize(int device, const double* A, const double* b, int N, int c, int L, int force_generic,
+                         double* J0, double* r0, int* path);
+
 /* Measured FP64 rates of the whole device (GFLOP/s, 2 flops per FMA): plain DFMA and tensor-core DMMA.8x8x4.  bench.py
  * quotes the back end's roofline fraction against these (MEASURED_PEAKS.json holds no FP64 figure). */
 int gf_probe_fp64(int device, double* dfma_gflops, double* dmma_gflops);
@@ -388,6 +411,9 @@ int gf_ba_marginalize_old(gf_ba* s, const gf_ba_problem* p, gf_ba_prior* out, do
  * unchanged: estimator.cpp:3538-3539), or a negative error code. */
 int gf_ba_marginalize_second_new(gf_ba* s, const gf_ba_problem* p, gf_ba_prior* out, double* out_x0, double* out_J, double* out_r,
                                  float* device_ms);
+/* The last marginalisation of this handle: info[0] = GF_MARG_PATH_* bits, info[1] = Jacobi sweeps on Amm (0 on the fast
+ * path), info[2] = Jacobi sweeps on the reduced system (0 for QL). */
+int gf_ba_last_marg_info(gf_ba* s, int* info3);
 
 /* Estimator::double2vector (estimator.cpp:2440-2494), the state part: host-only glue that maps the solved para_* arrays
  * back to Rs / Ps / Vs, rotating the window about z and shifting it so that frame 0 keeps the yaw and position it had
