@@ -1,5 +1,5 @@
 // Estimator::optimization() (vins_estimator/src/estimator/estimator.cpp:2884-3631) on libgf_b200.so: vector2double's arrays
-// are handed to gf_ba_solve as they are, the AddResidualBlock loops become descriptor rows, and the MARGIN_OLD /
+// are handed to gf_ba_solve (gf_ba_solve_multi for several estimators) as they are, the AddResidualBlock loops become descriptor rows, and the MARGIN_OLD /
 // MARGIN_SECOND_NEW branches become one call each.  Wheel, plane and GNSS blocks follow the same pattern (INTEGRATION.md);
 // this file carries the camera + IMU case the reference's default configs run.
 #include "estimator_ba.h"
@@ -32,10 +32,12 @@ Estimator::~Estimator()
     if (gf_ba_) gf_ba_destroy(gf_ba_);
 }
 
-void Estimator::optimization()
+// The ceres::Problem of estimator.cpp:2895-3300 as a gf_ba_problem; rows owns the factor tables P points into
+void Estimator::buildProblem(BaRows &rows)
 {
     if (!gf_ba_ && gf_ba_create(&gf_ba_, device)) gf_fatal("gf_ba_create");
-    gf_ba_problem P{};
+    gf_ba_problem &P = rows.P;
+    P = gf_ba_problem{};
     P.n_frames = frame_count + 1;
     P.max_num_iterations = NUM_ITERATIONS;                                   // estimator.cpp:3308
     P.para_pose = &para_Pose[0][0]; P.para_speed_bias = &para_SpeedBias[0][0];
@@ -49,7 +51,8 @@ void Estimator::optimization()
     copy3(G, P.gravity);
     P.visual_sqrt_info = FOCAL_LENGTH / 1.5;                                 // :193
 
-    std::vector<gf_ba_imu_factor> imu;
+    std::vector<gf_ba_imu_factor> &imu = rows.imu;
+    imu.clear();
     if (USE_IMU)
         for (int i = 0; i < frame_count; i++) {                              // :3104-3113
             const int j = i + 1;
@@ -63,8 +66,9 @@ void Estimator::optimization()
             to_row_major(pre->jacobian, f.jacobian); to_row_major(pre->covariance, f.covariance);
             imu.push_back(f);
         }
-    std::vector<gf_ba_visual_factor> vis;
-    std::vector<uint8_t> feature_const;
+    std::vector<gf_ba_visual_factor> &vis = rows.vis;
+    std::vector<uint8_t> &feature_const = rows.feature_const;
+    vis.clear(); feature_const.clear();
     int feature_index = -1;
     for (auto &it_per_id : f_manager.feature) {                              // :3268-3296
         it_per_id.used_num = (int)it_per_id.feature_per_frame.size();
@@ -90,9 +94,39 @@ void Estimator::optimization()
     P.imu = imu.data(); P.n_imu = (int)imu.size();
     P.feature_const = feature_const.data();
     P.prior = have_prior_ ? &prior_ : nullptr;                               // :2895-2903
+}
 
-    if (gf_ba_solve(gf_ba_, &P, &last_summary)) gf_fatal("gf_ba_solve");     // ceres::Solve, :3318
+void Estimator::optimization()
+{
+    BaRows rows;
+    buildProblem(rows);
+    if (gf_ba_solve(gf_ba_, &rows.P, &last_summary)) gf_fatal("gf_ba_solve");     // ceres::Solve, :3318
+    marginalize(rows.P);
+}
 
+// Several estimators (one per robot / camera rig served by this GPU) at the same point of their processImage: every window is
+// built as optimization() builds it, all are solved by one gf_ba_solve_multi call from this thread, then each estimator runs its
+// own marginalisation.  The same blocks and priors as calling optimization() on each in turn.
+void Estimator::optimizationMulti(Estimator *const *est, int n)
+{
+    std::vector<BaRows> rows(n);
+    std::vector<gf_ba *> handles(n);
+    std::vector<gf_ba_problem> P(n);
+    std::vector<gf_ba_summary> S(n);
+    for (int k = 0; k < n; k++) {
+        est[k]->buildProblem(rows[k]);
+        P[k] = rows[k].P; handles[k] = est[k]->gf_ba_;
+    }
+    if (gf_ba_solve_multi(handles.data(), n, P.data(), S.data(), nullptr)) gf_fatal("gf_ba_solve_multi");
+    for (int k = 0; k < n; k++) {
+        est[k]->last_summary = S[k];
+        est[k]->marginalize(P[k]);
+    }
+}
+
+// MARGIN_OLD / MARGIN_SECOND_NEW at the end of optimization(): the prior of the next window
+void Estimator::marginalize(const gf_ba_problem &P)
+{
     const size_t cap = 16 * (size_t)P.n_frames + 24;
     std::vector<double> x0(cap), J(cap * cap), r(cap);
     gf_ba_prior next{};

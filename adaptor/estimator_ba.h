@@ -45,6 +45,7 @@ class Estimator
     Estimator();
     ~Estimator();
     void optimization();
+    static void optimizationMulti(Estimator *const *est, int n);
 
     int frame_count = WINDOW_SIZE;
     MarginalizationFlag marginalization_flag = MARGIN_OLD;
@@ -61,8 +62,17 @@ class Estimator
     gf_ba_summary last_summary{};
     int device = 0;
     int prior_dim() const { return have_prior_ ? prior_.n : 0; }
+    const gf_ba_prior &prior() const { return prior_; }
 
   private:
+    struct BaRows {                  // one window's gf_ba_problem and the factor tables it points into
+        gf_ba_problem P{};
+        std::vector<gf_ba_imu_factor> imu;
+        std::vector<gf_ba_visual_factor> vis;
+        std::vector<uint8_t> feature_const;
+    };
+    void buildProblem(BaRows &rows);
+    void marginalize(const gf_ba_problem &P);
     gf_ba *gf_ba_ = nullptr;
     // last_marginalization_info + last_marginalization_parameter_blocks (estimator.h:318-319)
     bool have_prior_ = false;

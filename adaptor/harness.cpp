@@ -4,6 +4,8 @@
 //   harness fe-box <in> <out> frames and their detections (int m, m x 4 int64 after each frame) through
 //                             FeatureTracker::trackImagebox; after each featureFrame: cur_pts as (n, n x (id, x, y, track_cnt))
 //   harness ba <in> <out>   one window through Estimator::optimization()
+//   harness ba-multi <in> <out>  several estimators' windows, each round through one Estimator::optimizationMulti call
+//   harness ba-seq <in> <out>    the same input through each estimator's optimization() in turn
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -65,6 +67,56 @@ static int run_fe(const char *in, const char *out, bool with_boxes)
     return 0;
 }
 
+// one window of the input (the Estimator members optimization() reads) into est
+static void read_window(FILE *f, Estimator &est, int n_frames)
+{
+    est.marginalization_flag = rd1<int>(f) ? Estimator::MARGIN_SECOND_NEW : Estimator::MARGIN_OLD;
+    const int n_feat = rd1<int>(f);
+    rd(f, est.para_Pose, sizeof(double) * 7 * n_frames);
+    rd(f, est.para_SpeedBias, sizeof(double) * 9 * n_frames);
+    rd(f, est.para_Ex_Pose[0], 56);
+    for (int k = 0; k < n_frames; k++) for (int c = 0; c < 3; c++) est.Vs[k](c) = est.para_SpeedBias[k][c];
+    for (int j = 1; j < n_frames; j++) {
+        delete est.pre_integrations[j];
+        IntegrationBase *b = est.pre_integrations[j] = new IntegrationBase;
+        b->sum_dt = rd1<double>(f);
+        rd(f, b->delta_p.data(), 24); rd(f, b->delta_q.coeffs().data(), 32); rd(f, b->delta_v.data(), 24);
+        rd(f, b->linearized_ba.data(), 24); rd(f, b->linearized_bg.data(), 24);
+        double m[225];
+        rd(f, m, sizeof(m)); for (int i = 0; i < 15; i++) for (int c = 0; c < 15; c++) b->jacobian(i, c) = m[i * 15 + c];
+        rd(f, m, sizeof(m)); for (int i = 0; i < 15; i++) for (int c = 0; c < 15; c++) b->covariance(i, c) = m[i * 15 + c];
+    }
+    est.f_manager.feature.clear();
+    for (int k = 0; k < n_feat; k++) {
+        FeaturePerId it;
+        it.feature_id = k; it.start_frame = rd1<int>(f);
+        const int n_obs = rd1<int>(f);
+        it.estimate_flag = rd1<int>(f);
+        est.para_Feature[k][0] = rd1<double>(f);
+        for (int q = 0; q < n_obs; q++) {
+            FeaturePerFrame fr;
+            rd(f, fr.point.data(), 24); rd(f, fr.velocity.data(), 16); fr.cur_td = rd1<double>(f);
+            it.feature_per_frame.push_back(fr);
+        }
+        est.f_manager.feature.push_back(it);
+    }
+}
+
+// the solved window: blocks, then iterations, final cost, prior dimension, termination; with_prior: the next prior's r0 and J0
+static void write_window(FILE *o, const Estimator &est, int n_frames, bool with_prior)
+{
+    fwrite(est.para_Pose, sizeof(double) * 7, n_frames, o);
+    fwrite(est.para_SpeedBias, sizeof(double) * 9, n_frames, o);
+    fwrite(&est.para_Feature[0][0], sizeof(double), est.f_manager.feature.size(), o);
+    const double tail[4] = {(double)est.last_summary.iterations, est.last_summary.final_cost, (double)est.prior_dim(), (double)est.last_summary.termination};
+    fwrite(tail, 8, 4, o);
+    if (with_prior && est.prior_dim() > 0) {
+        const int n = est.prior_dim();
+        fwrite(est.prior().linearized_residuals, sizeof(double), n, o);
+        fwrite(est.prior().linearized_jacobians, sizeof(double), (size_t)n * n, o);
+    }
+}
+
 static int run_ba(const char *in, const char *out)
 {
     FILE *f = fopen(in, "rb"), *o = fopen(out, "wb");
@@ -75,42 +127,32 @@ static int run_ba(const char *in, const char *out)
     NUM_ITERATIONS = rd1<int>(f);
     rd(f, G.data(), 24);
     for (int w = 0; w < n_windows; w++) {
-        est.marginalization_flag = rd1<int>(f) ? Estimator::MARGIN_SECOND_NEW : Estimator::MARGIN_OLD;
-        const int n_feat = rd1<int>(f);
-        rd(f, est.para_Pose, sizeof(double) * 7 * n_frames);
-        rd(f, est.para_SpeedBias, sizeof(double) * 9 * n_frames);
-        rd(f, est.para_Ex_Pose[0], 56);
-        for (int k = 0; k < n_frames; k++) for (int c = 0; c < 3; c++) est.Vs[k](c) = est.para_SpeedBias[k][c];
-        for (int j = 1; j < n_frames; j++) {
-            delete est.pre_integrations[j];
-            IntegrationBase *b = est.pre_integrations[j] = new IntegrationBase;
-            b->sum_dt = rd1<double>(f);
-            rd(f, b->delta_p.data(), 24); rd(f, b->delta_q.coeffs().data(), 32); rd(f, b->delta_v.data(), 24);
-            rd(f, b->linearized_ba.data(), 24); rd(f, b->linearized_bg.data(), 24);
-            double m[225];
-            rd(f, m, sizeof(m)); for (int i = 0; i < 15; i++) for (int c = 0; c < 15; c++) b->jacobian(i, c) = m[i * 15 + c];
-            rd(f, m, sizeof(m)); for (int i = 0; i < 15; i++) for (int c = 0; c < 15; c++) b->covariance(i, c) = m[i * 15 + c];
-        }
-        est.f_manager.feature.clear();
-        for (int k = 0; k < n_feat; k++) {
-            FeaturePerId it;
-            it.feature_id = k; it.start_frame = rd1<int>(f);
-            const int n_obs = rd1<int>(f);
-            it.estimate_flag = rd1<int>(f);
-            est.para_Feature[k][0] = rd1<double>(f);
-            for (int q = 0; q < n_obs; q++) {
-                FeaturePerFrame fr;
-                rd(f, fr.point.data(), 24); rd(f, fr.velocity.data(), 16); fr.cur_td = rd1<double>(f);
-                it.feature_per_frame.push_back(fr);
-            }
-            est.f_manager.feature.push_back(it);
-        }
+        read_window(f, est, n_frames);
         est.optimization();
-        fwrite(est.para_Pose, sizeof(double) * 7, n_frames, o);
-        fwrite(est.para_SpeedBias, sizeof(double) * 9, n_frames, o);
-        fwrite(&est.para_Feature[0][0], sizeof(double), n_feat, o);
-        const double tail[4] = {(double)est.last_summary.iterations, est.last_summary.final_cost, (double)est.prior_dim(), (double)est.last_summary.termination};
-        fwrite(tail, 8, 4, o);
+        write_window(o, est, n_frames, false);
+    }
+    fclose(f); fclose(o);
+    return 0;
+}
+
+// n_est estimators, each with its own chain of windows: int n_est, then the `ba` input with n_windows = n_est * rounds windows in
+// round-major order (window r * n_est + e belongs to estimator e).  batched: each round is one Estimator::optimizationMulti call;
+// else every estimator's optimization() in turn.  Output: the windows in input order, each followed by the prior it left.
+static int run_ba_multi(const char *in, const char *out, bool batched)
+{
+    FILE *f = fopen(in, "rb"), *o = fopen(out, "wb");
+    if (!f || !o) return 2;
+    const int n_est = rd1<int>(f), n_frames = rd1<int>(f), n_windows = rd1<int>(f);
+    NUM_ITERATIONS = rd1<int>(f);
+    rd(f, G.data(), 24);
+    std::vector<std::unique_ptr<Estimator>> est;
+    std::vector<Estimator *> ptr;
+    for (int e = 0; e < n_est; e++) { est.emplace_back(new Estimator); est.back()->frame_count = n_frames - 1; ptr.push_back(est.back().get()); }
+    for (int r = 0; r < n_windows / n_est; r++) {
+        for (int e = 0; e < n_est; e++) read_window(f, *est[e], n_frames);
+        if (batched) Estimator::optimizationMulti(ptr.data(), n_est);
+        else for (int e = 0; e < n_est; e++) est[e]->optimization();
+        for (int e = 0; e < n_est; e++) write_window(o, *est[e], n_frames, true);
     }
     fclose(f); fclose(o);
     return 0;
@@ -118,7 +160,8 @@ static int run_ba(const char *in, const char *out)
 
 int main(int argc, char **argv)
 {
-    if (argc != 4) { std::fprintf(stderr, "usage: harness fe|fe-eq|fe-box|ba <in> <out>\n"); return 2; }
+    if (argc != 4) { std::fprintf(stderr, "usage: harness fe|fe-eq|fe-box|ba|ba-multi|ba-seq <in> <out>\n"); return 2; }
     if (!std::strcmp(argv[1], "fe-eq")) EQUALIZE = 1;
+    if (!std::strcmp(argv[1], "ba-multi") || !std::strcmp(argv[1], "ba-seq")) return run_ba_multi(argv[2], argv[3], argv[1][3] == 'm');
     return argv[1][0] == 'f' ? run_fe(argv[2], argv[3], !std::strcmp(argv[1], "fe-box")) : run_ba(argv[2], argv[3]);
 }

@@ -38,6 +38,9 @@ constexpr int RB_THREADS = ST_THREADS;               // k_ba_step block size (ba
 constexpr int SCHUR_WARPS = 8;                       // k_ba_schur: one warp per 8x8 tile of the reduced system
 // k_ba_schur's dynamic shared memory at the largest window: cl[L] | ss[nc+1] | sv[nc] (above the 48 KB default from L ~ 5,800)
 constexpr size_t SCHUR_SMEM_MAX = sizeof(double) * (GF_BA_MAX_FREE_LANDMARKS + 2 * MAX_NC + 2);
+// k_ba_step's dynamic shared memory at nc = MAX_NC (factor tiles | diagonal inverses | 3 tiles | y, z), 219.5 KB: with the
+// kernel's static shared memory (the window descriptor among it) within the 227 KB a CTA may have
+constexpr size_t STEP_SMEM_MAX = sizeof(double) * (64 * TILE_CAP + 64 * MAX_N8 + 192 + 2 * 8 * MAX_N8);
 
 struct BaState {
     double x_cost, cand_cost, radius, mu, alpha, dogleg_norm, model_change, x_norm, step_norm, grad_max;
@@ -77,7 +80,20 @@ struct BaDev {
     int tile_cap;             // factor tiles kept in shared memory (TILE_CAP; smaller only when GF_BA_TILE_CAP is set, to test the spill path)
     double gravity[3], vis_sqrt_info;
     BaState* st;
+    int eval_grid, schur_grid;   // this window's own CTA counts of k_ba_eval / k_ba_schur (a batch launches the largest; the rest exit)
 };
+static_assert(sizeof(BaDev) % 8 == 0, "BaDev is copied to shared memory in 8-byte words");
+
+// Every kernel of a solve serves a batch of windows (gf_ba_solve_multi; gf_ba_solve is the batch of one): blockIdx.y picks the
+// window and its descriptor is copied to shared memory at kernel entry.  The descriptors travel with the upload that precedes the
+// whole launch chain, so the copy may run before gf_pdl_wait and overlaps the tail of the predecessor; a __syncthreads must
+// follow before the descriptor is read.
+__device__ __forceinline__ void load_window(BaDev& sd, const BaDev* __restrict__ src)
+{
+    const unsigned long long* s = reinterpret_cast<const unsigned long long*>(src);
+    unsigned long long* t = reinterpret_cast<unsigned long long*>(&sd);
+    for (int e = threadIdx.x; e < (int)(sizeof(BaDev) / 8); e += blockDim.x) t[e] = s[e];
+}
 
 __device__ __forceinline__ double* acc_H(const BaDev& d, int b) { return d.acc[b]; }
 __device__ __forceinline__ double* acc_g(const BaDev& d, int b) { return d.acc[b] + (size_t)d.nc * d.nc; }
@@ -164,8 +180,12 @@ __device__ __forceinline__ bool imu_sqrt_info_warp(const double* __restrict__ co
     }
     return ok;
 }
-__global__ void k_ba_prior_hessian(BaDev d)
+__global__ void k_ba_prior_hessian(const BaDev* __restrict__ wins)
 {
+    __shared__ BaDev sd;
+    load_window(sd, wins + blockIdx.y);
+    __syncthreads();
+    const BaDev& d = sd;
     const int nc = d.nc, pn = d.pn;
     int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= pn * pn) return;
@@ -445,19 +465,24 @@ __device__ __forceinline__ void ba_eval_body(const BaDev& d, int mode)
     }
 }
 
-__global__ void __launch_bounds__(PAIR_THREADS) k_ba_eval(BaDev d, int mode)
+__global__ void __launch_bounds__(PAIR_THREADS) k_ba_eval(const BaDev* __restrict__ wins, int mode)
 {
+    __shared__ BaDev sd;
     gf::gf_pdl_trigger();      // no-ops unless launched with a programmatic dependency (gf_ba_solve)
+    load_window(sd, wins + blockIdx.y);
     gf::gf_pdl_wait();
+    __syncthreads();
+    const BaDev& d = sd;
+    if ((int)blockIdx.x >= d.eval_grid) return;
     ba_eval_body(d, mode);
     if (mode == 1) {
-        // the last CTA to finish takes the decision (accept / reject, radius, mu, convergence): no separate launch
+        // the last of the window's CTAs to finish takes the decision (accept / reject, radius, mu, convergence): no separate launch
         __shared__ int s_last;
         __syncthreads();
         if (threadIdx.x == 0) {
             __threadfence();
             const unsigned int t = atomicAdd(&d.st->eval_ticket, 1u);
-            s_last = (t == gridDim.x - 1);
+            s_last = (t == (unsigned)d.eval_grid - 1);
         }
         __syncthreads();
         if (s_last) {
@@ -615,12 +640,18 @@ __device__ __forceinline__ void schur_tile(const BaDev& d, const double* __restr
     *reinterpret_cast<double2*>(d.Sg + (size_t)tix(I, J) * 64 + (lane >> 2) * 8 + 2 * (lane & 3)) = make_double2(out[0], out[1]);
 }
 
-__global__ void __launch_bounds__(SCHUR_WARPS * 32) k_ba_schur(BaDev d)
+__global__ void __launch_bounds__(SCHUR_WARPS * 32) k_ba_schur(const BaDev* __restrict__ wins)
 {
     extern __shared__ double ssm[];                // tile CTAs: cl[L] | ss[nc+1] | sv[nc];  last CTA: delta[n]
     __shared__ double sred2[2 * SCHUR_WARPS];
+    __shared__ BaDev sd;
     gf::gf_pdl_trigger();
+    load_window(sd, wins + blockIdx.y);
     gf::gf_pdl_wait();
+    __syncthreads();
+    const BaDev& d = sd;
+    const int grid = d.schur_grid;                 // this window's CTAs: the tile CTAs, then the one that prepares the vectors
+    if ((int)blockIdx.x >= grid) return;
     const BaState& st = *d.st;
     if (st.done || st.setup_failed) return;
     const bool fresh = st.need_linearize != 0;
@@ -628,7 +659,7 @@ __global__ void __launch_bounds__(SCHUR_WARPS * 32) k_ba_schur(BaDev d)
     {   // clear the accumulator that is free during this iteration: k_ba_eval(1) linearises the candidate into it
         const int freeb = fresh ? st.cur : (st.cur ^ 1);
         const size_t tot = acc_size(d.nc, d.L);
-        const size_t nthr = (size_t)gridDim.x * blockDim.x;
+        const size_t nthr = (size_t)grid * blockDim.x;
         const size_t me = (size_t)blockIdx.x * blockDim.x + tid;
         for (size_t e = me; e < tot; e += nthr) d.acc[freeb][e] = 0.0;
         if (me == 0) d.st->acc_cost[freeb] = 0.0;
@@ -642,7 +673,7 @@ __global__ void __launch_bounds__(SCHUR_WARPS * 32) k_ba_schur(BaDev d)
     const double mu = st.mu;
     // everything (scale, D, c_l) is recomputed locally from the accumulators so that this kernel can run before k_ba_step adopts them
     auto scale_of = [&](int c) { return first ? 1.0 / (1.0 + sqrt(c < nc ? H[(size_t)c * nc + c] + Hp[(size_t)c * nc + c] : hll[c - nc])) : d.scale[c]; };
-    if (blockIdx.x == gridDim.x - 1) {
+    if ((int)blockIdx.x == grid - 1) {
         // ---- the last CTA prepares what k_ba_step needs before it can factor: D, gs = g'/D, e_l = 1 / (h'_ll + mu D_l^2), the
         // Jacobi scale (iteration 0) and, for a fresh linearisation, |x| and the gradient max-norm |x - Plus(x, -g)|_inf
         // (TrustRegionMinimizer's gradient tolerance test) -- off the single-CTA critical path of k_ba_step ----
@@ -687,7 +718,7 @@ __global__ void __launch_bounds__(SCHUR_WARPS * 32) k_ba_schur(BaDev d)
     __syncthreads();
     const int n8 = (nc + 8) >> 3, ntiles = n8 * (n8 + 1) / 2;
     double num = 0, den = 0;
-    const int gw = blockIdx.x * SCHUR_WARPS + warp, nw = (gridDim.x - 1) * SCHUR_WARPS;
+    const int gw = blockIdx.x * SCHUR_WARPS + warp, nw = (grid - 1) * SCHUR_WARPS;
     for (int t = gw; t < ntiles; t += nw) {
         int I = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
         while (tix(I + 1, 0) <= t) I++;
@@ -728,15 +759,20 @@ __global__ void __launch_bounds__(SCHUR_WARPS * 32) k_ba_schur(BaDev d)
 // DoglegStrategy::ComputeStep + TrustRegionMinimizer::ComputeTrustRegionStep + candidate point, one CTA.
 // Dynamic shared memory: factor tiles (<= tile_cap; first filled with the reduced system by a TMA bulk copy) | inverses of the
 // diagonal tiles | 2 scratch tiles | last diagonal tile | y.  After the back substitution the tile area is dead and holds delta.
+// One CTA per window of `list` (the windows of a batch that take this instantiation).
 template <int R, bool SPILL>
-__global__ void __launch_bounds__(RB_THREADS) k_ba_step(BaDev d)
+__global__ void __launch_bounds__(RB_THREADS) k_ba_step(const BaDev* __restrict__ wins, const int* __restrict__ list)
 {
     extern __shared__ __align__(128) double S[];
     __shared__ double sred[64];
     __shared__ __align__(8) unsigned long long mbar;
     __shared__ int s_fail, s_go;
+    __shared__ BaDev sd;
     gf::gf_pdl_trigger();
+    load_window(sd, wins + list[blockIdx.y]);
     gf::gf_pdl_wait();
+    __syncthreads();
+    const BaDev& d = sd;
     BaState& st = *d.st;
     if (st.done || st.setup_failed) return;
     const int tid = threadIdx.x, nt = blockDim.x, warp = tid >> 5, lane = tid & 31, nwarp = nt >> 5;
@@ -1374,8 +1410,8 @@ int gf_ba_create(gf_ba** out, int device)
     GF_CUDA(cudaEventCreate(&s->e0)); GF_CUDA(cudaEventCreate(&s->e1));
     s->tile_cap = TILE_CAP;
     if (const char* e_ = getenv("GF_BA_TILE_CAP")) { const int v = atoi(e_); if (v >= 0 && v < TILE_CAP) s->tile_cap = v; }
-    GF_CUDA(cudaFuncSetAttribute(k_ba_step<MAXR / 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    GF_CUDA(cudaFuncSetAttribute(k_ba_step<MAXR, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+    GF_CUDA(cudaFuncSetAttribute(k_ba_step<MAXR / 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)STEP_SMEM_MAX));
+    GF_CUDA(cudaFuncSetAttribute(k_ba_step<MAXR, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)STEP_SMEM_MAX));
     GF_CUDA(cudaFuncSetAttribute(k_jacobi_eig, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     GF_CUDA(cudaFuncSetAttribute(k_sym_eig_ql, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     GF_CUDA(cudaFuncSetAttribute(k_ba_schur, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCHUR_SMEM_MAX));
@@ -1395,9 +1431,31 @@ void gf_ba_destroy(gf_ba* s)
     delete s;
 }
 
-int gf_ba_solve(gf_ba* s, const gf_ba_problem* p, gf_ba_summary* sum)
+}  // extern "C" (reopened below)
+
+// ------------------------------------------------------------------------------------------------
+// One solve in four parts, shared by gf_ba_solve (the batch of one) and gf_ba_solve_multi:
+//   ba_layout   argument checks and the column layout of one window (host only: nothing is written anywhere)
+//   ba_pack     the window's upload image in its handle's pinned buffer, and its descriptor
+//   ba_batch    the uploads, the launch chain of the whole batch on the first handle's stream, the downloads
+//   ba_finish   write-back of one window's blocks and summary
+struct BaWindow {
+    BaDev d;                                   // device pointers are set by ba_pack
+    std::vector<int> col_feat, pair_id, pair_start, work_start, work_ij, pcol;
+    size_t px0_len;
+    int n_work, pn, n8, ntiles, eval_blocks;
+    bool spill;                                // k_ba_step<MAXR, true>: the factor does not fit the shared-memory tiles
+    size_t prior_smem, step_smem, schur_smem;
+    size_t o_X, o_vis, o_imu, o_whl, o_plf, o_ps, o_pij, o_cf, o_pJ, o_pr0, o_px0, o_pcol, o_Xc, o_st, upload_bytes;
+    size_t o_sq, o_Hp, o_a0, o_a1, o_vec, o_Sg, o_Lg, bytes;
+    size_t base;                               // offset of the window in its handle's buffers (the batch table comes first in the lead handle's)
+};
+
+static size_t al16(size_t v) { return (v + 15) / 16 * 16; }
+
+static int ba_layout(const gf_ba* s, const gf_ba_problem* p, BaWindow& w)
 {
-    if (!s || !p || !sum) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    if (!p) return set_err(GF_ERR_INVALID_ARG, "null argument");
     if (p->n_frames < 1 || p->n_frames > GF_BA_MAX_FRAMES) return set_err(GF_ERR_INVALID_ARG, "n_frames out of range");
     if (p->n_visual < 0 || p->n_imu < 0 || p->n_features < 0) return set_err(GF_ERR_INVALID_ARG, "negative factor / feature count");
     if (!p->para_pose || !p->para_ex_pose || !p->para_td) return set_err(GF_ERR_INVALID_ARG, "null parameter block");
@@ -1406,11 +1464,9 @@ int gf_ba_solve(gf_ba* s, const gf_ba_problem* p, gf_ba_summary* sum)
     if (p->n_wheel < 0 || (p->n_wheel > 0 && (!p->wheel || !p->para_ex_wheel || !p->para_ix_wheel || !p->para_td_wheel))) return set_err(GF_ERR_INVALID_ARG, "wheel factors without their parameter blocks");
     if (p->n_plane < 0 || p->n_plane > PAIR_THREADS || (p->n_plane > 0 && (!p->plane_frames || !p->para_ex_wheel || !p->para_plane_R || !p->para_plane_Z))) return set_err(GF_ERR_INVALID_ARG, "plane factors without their parameter blocks");
     if (p->max_num_iterations < 0 || p->max_num_iterations > GF_BA_MAX_ITERATIONS) return set_err(GF_ERR_INVALID_ARG, "max_num_iterations out of range");
-    GF_CUDA(cudaSetDevice(s->device));
-    memset(sum, 0, sizeof(*sum));
     const int F = p->n_frames, nfeat = p->n_features;
     // ---- layout (same rules as ceres::Problem construction, estimator.cpp:2950-3100, 3233-3246, 3291) ----
-    BaDev d; memset(&d, 0, sizeof(d));
+    BaDev& d = w.d; memset(&d, 0, sizeof(d));
     d.F = F; d.nfeat = nfeat; d.n_vis = p->n_visual; d.n_imu = p->n_imu; d.n_wheel = p->n_wheel; d.n_plane = p->n_plane;
     d.pr_mask = p->plane_r_subset_mask; for (int k = 0; k < 3; k++) d.plane_sinfo[k] = p->plane_sqrt_info[k];
     const bool use_sb = p->para_speed_bias && !p->pose0_const;
@@ -1430,7 +1486,8 @@ int gf_ba_solve(gf_ba* s, const gf_ba_problem* p, gf_ba_summary* sum)
     if (p->n_plane > 0 && !p->plane_const) { d.col_pr = c; c += 3; d.col_pz = c++; }
     for (int k = 0; k < p->n_plane; k++) if (p->plane_frames[k] < 0 || p->plane_frames[k] >= F) return set_err(GF_ERR_INVALID_ARG, "plane factor frame out of range");
     d.nc = c;
-    std::vector<int> col_feat(nfeat > 0 ? nfeat : 1, -1);
+    std::vector<int>& col_feat = w.col_feat;
+    col_feat.assign(nfeat > 0 ? nfeat : 1, -1);
     for (int v = 0; v < p->n_visual; v++) {
         int k = p->visual[v].feature;
         if (k < 0 || k >= nfeat || p->visual[v].imu_i < 0 || p->visual[v].imu_i >= F || p->visual[v].imu_j < 0 || p->visual[v].imu_j >= F)
@@ -1442,28 +1499,32 @@ int gf_ba_solve(gf_ba* s, const gf_ba_problem* p, gf_ba_summary* sum)
     if (d.nc > MAX_NC) return set_err(GF_ERR_CAPACITY, "reduced system larger than 383 unknowns");
     if (d.L > GF_BA_MAX_FREE_LANDMARKS) return set_err(GF_ERR_CAPACITY, "more than GF_BA_MAX_FREE_LANDMARKS (8192) free landmarks");
     // ---- sort visual factors by pose pair ----
-    std::vector<int> pair_id(F * F, -1), pair_cnt;
-    std::vector<int> pair_ij;
+    std::vector<int>& pair_id = w.pair_id;
+    pair_id.assign(F * F, -1);
+    std::vector<int> pair_cnt, pair_ij;
     for (int v = 0; v < p->n_visual; v++) {
         int key = p->visual[v].imu_i * F + p->visual[v].imu_j;
         if (pair_id[key] < 0) { pair_id[key] = (int)pair_cnt.size(); pair_cnt.push_back(0); pair_ij.push_back(p->visual[v].imu_i); pair_ij.push_back(p->visual[v].imu_j); }
         pair_cnt[pair_id[key]]++;
     }
     const int n_pairs = (int)pair_cnt.size();
-    std::vector<int> pair_start(n_pairs + 1, 0);
+    std::vector<int>& pair_start = w.pair_start;
+    pair_start.assign(n_pairs + 1, 0);
     for (int k = 0; k < n_pairs; k++) pair_start[k + 1] = pair_start[k] + pair_cnt[k];
     // one CTA of k_ba_eval per (pair, chunk of <= PAIR_CHUNK factors): long pairs are cut so that the CTAs are balanced
-    std::vector<int> work_start(1, 0), work_ij;
+    w.work_start.assign(1, 0); w.work_ij.clear();
     for (int k = 0; k < n_pairs; k++)
         for (int c0 = pair_start[k]; c0 < pair_start[k + 1]; c0 += PAIR_CHUNK) {
-            work_ij.push_back(pair_ij[2 * k]); work_ij.push_back(pair_ij[2 * k + 1]);
-            work_start.push_back(std::min(c0 + PAIR_CHUNK, pair_start[k + 1]));
+            w.work_ij.push_back(pair_ij[2 * k]); w.work_ij.push_back(pair_ij[2 * k + 1]);
+            w.work_start.push_back(std::min(c0 + PAIR_CHUNK, pair_start[k + 1]));
         }
-    const int n_work = (int)work_ij.size() / 2;
+    const int n_work = (int)w.work_ij.size() / 2;
+    w.n_work = n_work;
     d.n_pairs = n_work;
     const gf_ba_prior* pr = (p->prior && p->prior->n > 0) ? p->prior : nullptr;
     const int pn = pr ? pr->n : 0;
-    std::vector<int> pcol(pn > 0 ? pn : 1, -1);
+    w.pn = pn;
+    w.pcol.assign(pn > 0 ? pn : 1, -1);
     size_t px0_len = 0;
     if (pr) {
         if (pr->n_blocks > 64) return set_err(GF_ERR_CAPACITY, "more than 64 prior blocks");
@@ -1478,30 +1539,50 @@ int gf_ba_solve(gf_ba* s, const gf_ba_problem* p, gf_ba_summary* sum)
             int lc = kind == GF_BA_BLOCK_POSE ? d.col_pose[idx] : kind == GF_BA_BLOCK_SPEEDBIAS ? d.col_sb[idx] : kind == GF_BA_BLOCK_EX_POSE ? d.col_ex : kind == GF_BA_BLOCK_TD ? d.col_td
                      : kind == GF_BA_BLOCK_EX_WHEEL ? d.col_exw : kind == GF_BA_BLOCK_SX ? d.col_ix[0] : kind == GF_BA_BLOCK_SY ? d.col_ix[1] : kind == GF_BA_BLOCK_SW ? d.col_ix[2]
                      : kind == GF_BA_BLOCK_TD_WHEEL ? d.col_tdw : kind == GF_BA_BLOCK_PLANE_R ? d.col_pr : d.col_pz;
-            if (lc >= 0) for (int k = 0; k < ls; k++) pcol[pr->block_idx[b] + k] = lc + k;
+            if (lc >= 0) for (int k = 0; k < ls; k++) w.pcol[pr->block_idx[b] + k] = lc + k;
             px0_len += gs;
         }
     }
-    // ---- pack one upload buffer ----
+    w.px0_len = px0_len;
+    for (int k = 0; k < p->n_wheel; k++) if (p->wheel[k].i < 0 || p->wheel[k].i >= F || p->wheel[k].j < 0 || p->wheel[k].j >= F) return set_err(GF_ERR_INVALID_ARG, "wheel factor index out of range");
+    for (int k = 0; k < p->n_imu; k++) if (p->imu[k].i < 0 || p->imu[k].i >= F || p->imu[k].j < 0 || p->imu[k].j >= F) return set_err(GF_ERR_INVALID_ARG, "imu factor index out of range");
+    // ---- offsets in the handle's buffers (relative to w.base) ----
     const int nc = d.nc, L = d.L, n = d.n;
     const int n8 = (nc + 8) / 8, ntiles = n8 * (n8 + 1) / 2;      // 8x8 tiles of the (nc+1)-row augmented reduced system
-    auto al = [](size_t v) { return (v + 15) / 16 * 16; };
+    w.n8 = n8; w.ntiles = ntiles;
     size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += al(bytes); return o; };
-    const size_t o_X = take(sizeof(double) * (X_FEAT + nfeat)), o_vis = take(sizeof(gf_ba_visual_factor) * (size_t)p->n_visual),
-                 o_imu = take(sizeof(gf_ba_imu_factor) * (size_t)p->n_imu), o_whl = take(sizeof(gf_ba_wheel_factor) * (size_t)p->n_wheel), o_plf = take(sizeof(int) * (size_t)(p->n_plane > 0 ? p->n_plane : 1)), o_ps = take(sizeof(int) * (n_work + 1)), o_pij = take(sizeof(int) * 2 * (size_t)(n_work > 0 ? n_work : 1)),
-                 o_cf = take(sizeof(int) * (size_t)(nfeat > 0 ? nfeat : 1)), o_pJ = take(sizeof(double) * (size_t)pn * pn), o_pr0 = take(sizeof(double) * pn),
-                 o_px0 = take(sizeof(double) * px0_len), o_pcol = take(sizeof(int) * (size_t)(pn > 0 ? pn : 1));
-    const size_t o_Xc = take(sizeof(double) * (X_FEAT + nfeat)), o_st = take(sizeof(BaState));     // uploaded too: candidate := x, initial solver state
-    const size_t upload_bytes = off;
-    const size_t o_sq = take(sizeof(double) * 225 * (size_t)(p->n_imu > 0 ? p->n_imu : 1)),
-                 o_Hp = take(sizeof(double) * (size_t)nc * nc), o_a0 = take(sizeof(double) * acc_size(nc, L)), o_a1 = take(sizeof(double) * acc_size(nc, L)),
-                 o_vec = take(sizeof(double) * 6 * (size_t)(n > 0 ? n : 1)), o_Sg = take(sizeof(double) * 64 * (size_t)ntiles),
-                 o_Lg = take(sizeof(double) * 64 * (size_t)(ntiles > s->tile_cap ? ntiles - s->tile_cap : 1));
-    int rc = ensure(s, off);
-    if (rc) return rc;
-    char* hb = (char*)s->hbuf; char* db = (char*)s->dbuf;
-    double* hX = (double*)(hb + o_X);
+    auto take = [&](size_t bytes) { size_t o = off; off += al16(bytes); return o; };
+    w.o_X = take(sizeof(double) * (X_FEAT + nfeat)); w.o_vis = take(sizeof(gf_ba_visual_factor) * (size_t)p->n_visual);
+    w.o_imu = take(sizeof(gf_ba_imu_factor) * (size_t)p->n_imu); w.o_whl = take(sizeof(gf_ba_wheel_factor) * (size_t)p->n_wheel);
+    w.o_plf = take(sizeof(int) * (size_t)(p->n_plane > 0 ? p->n_plane : 1)); w.o_ps = take(sizeof(int) * (n_work + 1));
+    w.o_pij = take(sizeof(int) * 2 * (size_t)(n_work > 0 ? n_work : 1)); w.o_cf = take(sizeof(int) * (size_t)(nfeat > 0 ? nfeat : 1));
+    w.o_pJ = take(sizeof(double) * (size_t)pn * pn); w.o_pr0 = take(sizeof(double) * pn);
+    w.o_px0 = take(sizeof(double) * px0_len); w.o_pcol = take(sizeof(int) * (size_t)(pn > 0 ? pn : 1));
+    w.o_Xc = take(sizeof(double) * (X_FEAT + nfeat)); w.o_st = take(sizeof(BaState));     // uploaded too: candidate := x, initial solver state
+    w.upload_bytes = off;
+    w.o_sq = take(sizeof(double) * 225 * (size_t)(p->n_imu > 0 ? p->n_imu : 1));
+    w.o_Hp = take(sizeof(double) * (size_t)nc * nc); w.o_a0 = take(sizeof(double) * acc_size(nc, L)); w.o_a1 = take(sizeof(double) * acc_size(nc, L));
+    w.o_vec = take(sizeof(double) * 6 * (size_t)(n > 0 ? n : 1)); w.o_Sg = take(sizeof(double) * 64 * (size_t)ntiles);
+    w.o_Lg = take(sizeof(double) * 64 * (size_t)(ntiles > s->tile_cap ? ntiles - s->tile_cap : 1));
+    w.bytes = off;
+    // ---- launch shapes ----
+    w.eval_blocks = n_work + p->n_imu + p->n_wheel + (p->n_plane > 0 ? 1 : 0) + (pn ? 1 : 0);
+    d.eval_grid = w.eval_blocks > 0 ? w.eval_blocks : 1;
+    d.schur_grid = (ntiles + SCHUR_WARPS - 1) / SCHUR_WARPS + 1;      // + the CTA that prepares k_ba_step's vectors and norms
+    d.tile_cap = s->tile_cap;
+    w.spill = !(ntiles <= s->tile_cap && n8 <= (MAXR / 2) * CH_BULK);
+    w.prior_smem = sizeof(double) * 2 * (size_t)pn;
+    w.step_smem = sizeof(double) * (64 * (size_t)std::min(ntiles, s->tile_cap) + 64 * (size_t)n8 + 192 + 2 * (size_t)((nc + 8) & ~7));
+    w.schur_smem = sizeof(double) * (size_t)std::max(L + 2 * nc + 2, n + 1);
+    return GF_OK;
+}
+
+static void ba_pack(gf_ba* s, const gf_ba_problem* p, BaWindow& w)
+{
+    const int F = p->n_frames, nfeat = p->n_features, n = w.d.n, pn = w.pn;
+    const gf_ba_prior* pr = pn ? p->prior : nullptr;
+    char* hb = (char*)s->hbuf + w.base; char* db = (char*)s->dbuf + w.base;
+    double* hX = (double*)(hb + w.o_X);
     memset(hX, 0, sizeof(double) * (X_FEAT + nfeat));
     memcpy(hX + X_POSE, p->para_pose, sizeof(double) * 7 * F);
     if (p->para_speed_bias) memcpy(hX + X_SB, p->para_speed_bias, sizeof(double) * 9 * F);
@@ -1510,102 +1591,185 @@ int gf_ba_solve(gf_ba* s, const gf_ba_problem* p, gf_ba_summary* sum)
     hX[X_EXW + 6] = 1.0; hX[X_IX] = hX[X_IX + 1] = hX[X_IX + 2] = 1.0;
     if (p->n_wheel > 0) { memcpy(hX + X_EXW, p->para_ex_wheel, sizeof(double) * 7); memcpy(hX + X_IX, p->para_ix_wheel, sizeof(double) * 3); hX[X_TDW] = p->para_td_wheel[0]; }
     hX[X_PR + 3] = 1.0;
-    if (p->n_plane > 0) { memcpy(hX + X_EXW, p->para_ex_wheel, sizeof(double) * 7); memcpy(hX + X_PR, p->para_plane_R, sizeof(double) * 4); hX[X_PZ] = p->para_plane_Z[0]; memcpy(hb + o_plf, p->plane_frames, sizeof(int) * p->n_plane); }
+    if (p->n_plane > 0) { memcpy(hX + X_EXW, p->para_ex_wheel, sizeof(double) * 7); memcpy(hX + X_PR, p->para_plane_R, sizeof(double) * 4); hX[X_PZ] = p->para_plane_Z[0]; memcpy(hb + w.o_plf, p->plane_frames, sizeof(int) * p->n_plane); }
     memcpy(hX + X_FEAT, p->para_feature, sizeof(double) * nfeat);
-    memcpy(hb + o_Xc, hX, sizeof(double) * (X_FEAT + nfeat));           // the candidate starts as a copy: its constant blocks never change
+    memcpy(hb + w.o_Xc, hX, sizeof(double) * (X_FEAT + nfeat));           // the candidate starts as a copy: its constant blocks never change
     {   // TrustRegionMinimizer / DoglegStrategy initial state; the first linearisation goes to buffer 0
-        BaState* h0 = (BaState*)(hb + o_st);
+        BaState* h0 = (BaState*)(hb + w.o_st);
         memset(h0, 0, sizeof(BaState));
         h0->radius = 1e4; h0->mu = 1e-8; h0->need_linearize = 1; h0->cur = 1; h0->first = 1; h0->max_iter = p->max_num_iterations;
     }
     {   // factors sorted by pair
-        gf_ba_visual_factor* hv = (gf_ba_visual_factor*)(hb + o_vis);
-        std::vector<int> fill(pair_start.begin(), pair_start.end() - 1);
-        for (int v = 0; v < p->n_visual; v++) { int k = pair_id[p->visual[v].imu_i * F + p->visual[v].imu_j]; hv[fill[k]++] = p->visual[v]; }
+        gf_ba_visual_factor* hv = (gf_ba_visual_factor*)(hb + w.o_vis);
+        std::vector<int> fill(w.pair_start.begin(), w.pair_start.end() - 1);
+        for (int v = 0; v < p->n_visual; v++) { int k = w.pair_id[p->visual[v].imu_i * F + p->visual[v].imu_j]; hv[fill[k]++] = p->visual[v]; }
     }
-    if (p->n_imu) memcpy(hb + o_imu, p->imu, sizeof(gf_ba_imu_factor) * (size_t)p->n_imu);
-    if (p->n_wheel) memcpy(hb + o_whl, p->wheel, sizeof(gf_ba_wheel_factor) * (size_t)p->n_wheel);
-    for (int k = 0; k < p->n_wheel; k++) if (p->wheel[k].i < 0 || p->wheel[k].i >= F || p->wheel[k].j < 0 || p->wheel[k].j >= F) return set_err(GF_ERR_INVALID_ARG, "wheel factor index out of range");
-    for (int k = 0; k < p->n_imu; k++) if (p->imu[k].i < 0 || p->imu[k].i >= F || p->imu[k].j < 0 || p->imu[k].j >= F) return set_err(GF_ERR_INVALID_ARG, "imu factor index out of range");
-    memcpy(hb + o_ps, work_start.data(), sizeof(int) * (n_work + 1));
-    if (n_work) memcpy(hb + o_pij, work_ij.data(), sizeof(int) * 2 * n_work);
-    memcpy(hb + o_cf, col_feat.data(), sizeof(int) * (size_t)(nfeat > 0 ? nfeat : 1));
+    if (p->n_imu) memcpy(hb + w.o_imu, p->imu, sizeof(gf_ba_imu_factor) * (size_t)p->n_imu);
+    if (p->n_wheel) memcpy(hb + w.o_whl, p->wheel, sizeof(gf_ba_wheel_factor) * (size_t)p->n_wheel);
+    memcpy(hb + w.o_ps, w.work_start.data(), sizeof(int) * (w.n_work + 1));
+    if (w.n_work) memcpy(hb + w.o_pij, w.work_ij.data(), sizeof(int) * 2 * w.n_work);
+    memcpy(hb + w.o_cf, w.col_feat.data(), sizeof(int) * (size_t)(nfeat > 0 ? nfeat : 1));
     if (pr) {
-        memcpy(hb + o_pJ, pr->linearized_jacobians, sizeof(double) * (size_t)pn * pn);
-        memcpy(hb + o_pr0, pr->linearized_residuals, sizeof(double) * pn);
-        memcpy(hb + o_px0, pr->x0, sizeof(double) * px0_len);
-        memcpy(hb + o_pcol, pcol.data(), sizeof(int) * pn);
+        memcpy(hb + w.o_pJ, pr->linearized_jacobians, sizeof(double) * (size_t)pn * pn);
+        memcpy(hb + w.o_pr0, pr->linearized_residuals, sizeof(double) * pn);
+        memcpy(hb + w.o_px0, pr->x0, sizeof(double) * w.px0_len);
+        memcpy(hb + w.o_pcol, w.pcol.data(), sizeof(int) * pn);
     }
-    d.col_feat = (const int*)(db + o_cf); d.X = (double*)(db + o_X); d.Xc = (double*)(db + o_Xc);
-    d.vis = (const gf_ba_visual_factor*)(db + o_vis); d.pair_start = (const int*)(db + o_ps); d.pair_ij = (const int*)(db + o_pij);
-    d.imu = (const gf_ba_imu_factor*)(db + o_imu); d.imu_sqrt = (double*)(db + o_sq);
-    d.wheel = (const gf_ba_wheel_factor*)(db + o_whl); d.plane_frames = (const int*)(db + o_plf);
-    d.pJ = (const double*)(db + o_pJ); d.pr0 = (const double*)(db + o_pr0); d.px0 = (const double*)(db + o_px0); d.pcol = (const int*)(db + o_pcol);
-    d.Hp = (double*)(db + o_Hp); d.acc[0] = (double*)(db + o_a0); d.acc[1] = (double*)(db + o_a1);
-    double* vec = (double*)(db + o_vec);
+    BaDev& d = w.d;
+    d.col_feat = (const int*)(db + w.o_cf); d.X = (double*)(db + w.o_X); d.Xc = (double*)(db + w.o_Xc);
+    d.vis = (const gf_ba_visual_factor*)(db + w.o_vis); d.pair_start = (const int*)(db + w.o_ps); d.pair_ij = (const int*)(db + w.o_pij);
+    d.imu = (const gf_ba_imu_factor*)(db + w.o_imu); d.imu_sqrt = (double*)(db + w.o_sq);
+    d.wheel = (const gf_ba_wheel_factor*)(db + w.o_whl); d.plane_frames = (const int*)(db + w.o_plf);
+    d.pJ = (const double*)(db + w.o_pJ); d.pr0 = (const double*)(db + w.o_pr0); d.px0 = (const double*)(db + w.o_px0); d.pcol = (const int*)(db + w.o_pcol);
+    d.Hp = (double*)(db + w.o_Hp); d.acc[0] = (double*)(db + w.o_a0); d.acc[1] = (double*)(db + w.o_a1);
+    double* vec = (double*)(db + w.o_vec);
     const size_t nn = (size_t)(n > 0 ? n : 1);
     d.scale = vec; d.diag = vec + nn; d.gs = vec + 2 * nn; d.gn = vec + 3 * nn; d.step = vec + 4 * nn; d.delta = vec + 5 * nn;
-    d.Sg = (double*)(db + o_Sg); d.Lg = (double*)(db + o_Lg); d.tile_cap = s->tile_cap;
-    d.st = (BaState*)(db + o_st);
+    d.Sg = (double*)(db + w.o_Sg); d.Lg = (double*)(db + w.o_Lg);
+    d.st = (BaState*)(db + w.o_st);
     for (int k = 0; k < 3; k++) d.gravity[k] = p->gravity[k];
     d.vis_sqrt_info = p->visual_sqrt_info;
+}
 
-    cudaStream_t st = s->s;
-    GF_CUDA(cudaEventRecord(s->e0, st));
-    GF_CUDA(cudaMemcpyAsync(db, hb, upload_bytes, cudaMemcpyHostToDevice, st));
-    GF_CUDA(cudaMemsetAsync(db + o_Hp, 0, al(sizeof(double) * (size_t)nc * nc) + al(sizeof(double) * acc_size(nc, L)) * 2, st));   // H_prior, both accumulators
-    if (pn) { k_ba_prior_hessian<<<(pn * pn + 255) / 256, 256, 0, st>>>(d); GF_LAUNCHED(); }
-    const int eval_blocks = n_work + p->n_imu + p->n_wheel + (p->n_plane > 0 ? 1 : 0) + (pn ? 1 : 0);
-    const size_t prior_smem = sizeof(double) * 2 * (size_t)pn;
-    const size_t step_smem = sizeof(double) * (64 * (size_t)std::min(ntiles, s->tile_cap) + 64 * (size_t)n8 + 192 + 2 * (size_t)((nc + 8) & ~7));
-    const size_t schur_smem = sizeof(double) * (size_t)std::max(L + 2 * nc + 2, n + 1);
-    const int schur_grid = (ntiles + SCHUR_WARPS - 1) / SCHUR_WARPS + 1;      // + the CTA that prepares k_ba_step's vectors and norms
-    const int iters = p->max_num_iterations;
-    if (eval_blocks > 0) { k_ba_eval<<<eval_blocks, PAIR_THREADS, prior_smem, st>>>(d, 0); GF_LAUNCHED(); }
-    // Every kernel of the loop is launched with a programmatic dependency on its predecessor: its CTAs become resident while the
-    // predecessor still runs and sit in griddepcontrol.wait, which hides the launch latency at the 26 kernel boundaries of a solve
-    // (measured on one H100 SXM at 700 W, C2 window: 0.79-0.80 -> 0.77 ms per solve; GF_BA_NO_PDL=1 restores plain stream order for A/B runs)
-    static const bool pdl = getenv("GF_BA_NO_PDL") == nullptr;
-    auto launch = [&](auto kern, int grid, int block, size_t smem, auto... args) -> cudaError_t {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(block); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
-        return cudaLaunchKernelEx(&cfg, kern, args...);
-    };
-    for (int it = 0; it <= iters; it++) {
-        GF_CUDA(launch(k_ba_schur, schur_grid, SCHUR_WARPS * 32, schur_smem, d)); GF_LAUNCHED();      // (the closing launch only prepares the norms)
-        if (ntiles <= s->tile_cap && n8 <= (MAXR / 2) * CH_BULK) GF_CUDA(launch(k_ba_step<MAXR / 2, false>, 1, RB_THREADS, step_smem, d));
-        else GF_CUDA(launch(k_ba_step<MAXR, true>, 1, RB_THREADS, step_smem, d));
-        GF_LAUNCHED();
-        if (it == iters) break;                  // the extra k_ba_step adopts the last linearisation and closes the run
-        GF_CUDA(launch(k_ba_eval, eval_blocks > 0 ? eval_blocks : 1, PAIR_THREADS, prior_smem, d, 1)); GF_LAUNCHED();   // + decision (last CTA)
-    }
-    GF_CUDA(cudaGetLastError());
-    GF_CUDA(cudaMemcpyAsync(hb + o_X, db + o_X, sizeof(double) * (X_FEAT + nfeat), cudaMemcpyDeviceToHost, st));
-    GF_CUDA(cudaMemcpyAsync(hb + o_st, db + o_st, sizeof(BaState), cudaMemcpyDeviceToHost, st));
-    GF_CUDA(cudaEventRecord(s->e1, st));
-    GF_CUDA(cudaStreamSynchronize(st));
-    float ms = 0;
-    GF_CUDA(cudaEventElapsedTime(&ms, s->e0, s->e1));
-    const BaState* hs = (const BaState*)(hb + o_st);
-    if (hs->setup_failed) return set_err(GF_ERR_INVALID_ARG, "an IMU covariance is singular or not positive definite; parameter blocks left untouched");
+static void ba_finish(gf_ba* s, const gf_ba_problem* p, const BaWindow& w, gf_ba_summary* sum, float ms)
+{
+    const char* hb = (const char*)s->hbuf + w.base;
+    const double* hX = (const double*)(hb + w.o_X);
+    const BaState* hs = (const BaState*)(hb + w.o_st);
+    const int F = p->n_frames;
     memcpy(p->para_pose, hX + X_POSE, sizeof(double) * 7 * F);
     if (p->para_speed_bias) memcpy(p->para_speed_bias, hX + X_SB, sizeof(double) * 9 * F);
     memcpy(p->para_ex_pose, hX + X_EX, sizeof(double) * 7);
     p->para_td[0] = hX[X_TD];
     if (p->n_wheel > 0) { memcpy(p->para_ex_wheel, hX + X_EXW, sizeof(double) * 7); memcpy(p->para_ix_wheel, hX + X_IX, sizeof(double) * 3); p->para_td_wheel[0] = hX[X_TDW]; }
     if (p->n_plane > 0) { memcpy(p->para_ex_wheel, hX + X_EXW, sizeof(double) * 7); memcpy(p->para_plane_R, hX + X_PR, sizeof(double) * 4); p->para_plane_Z[0] = hX[X_PZ]; }
-    memcpy(p->para_feature, hX + X_FEAT, sizeof(double) * nfeat);
+    memcpy(p->para_feature, hX + X_FEAT, sizeof(double) * p->n_features);
     sum->iterations = hs->it; sum->num_successful_steps = hs->n_success; sum->termination = hs->termination;
-    sum->reduced_dim = nc; sum->n_free_landmarks = L; sum->n_residuals = pn + 15 * p->n_imu + 6 * p->n_wheel + 3 * p->n_plane + 2 * p->n_visual;
+    sum->reduced_dim = w.d.nc; sum->n_free_landmarks = w.d.L; sum->n_residuals = w.pn + 15 * p->n_imu + 6 * p->n_wheel + 3 * p->n_plane + 2 * p->n_visual;
     sum->initial_cost = hs->cost_hist[0]; sum->final_cost = hs->x_cost;
     for (int k = 0; k <= GF_BA_MAX_ITERATIONS; k++) { sum->cost[k] = hs->cost_hist[k]; sum->radius[k] = hs->radius_hist[k]; }
     sum->device_ms = ms;
     memcpy(s->prof, hs->prof, sizeof(s->prof));
-    return GF_OK;
+}
+
+// prefixes the error text with the window it belongs to (gf_ba_solve_multi)
+static int window_err(int k, int rc)
+{
+    char t[sizeof(g_err)];
+    snprintf(t, sizeof(t), "window %d: %s", k, g_err);
+    memcpy(g_err, t, sizeof(t));
+    return rc;
+}
+
+// Windows k = 0..n-1 (problem ps[k] on handle hs[k]), every one validated before anything is written or enqueued.  All work goes to
+// hs[0]'s stream; hs[0]'s buffers also hold the batch table: the n descriptors and the two lists of windows per k_ba_step
+// instantiation.  Launch count: that of the window with the most iterations, plus one k_ba_step per iteration when both
+// instantiations are needed.
+static int ba_batch(gf_ba* const* hs, int n, const gf_ba_problem* ps, gf_ba_summary* sums, int32_t* status, bool multi)
+{
+    std::vector<BaWindow> W(n);
+    for (int k = 0; k < n; k++) { const int rc = ba_layout(hs[k], &ps[k], W[k]); if (rc) return multi ? window_err(k, rc) : rc; }
+    gf_ba* lead = hs[0];
+    GF_CUDA(cudaSetDevice(lead->device));
+    const size_t table = al16((sizeof(BaDev) + 2 * sizeof(int)) * (size_t)n);
+    for (int k = 0; k < n; k++) {
+        W[k].base = k == 0 ? table : 0;
+        const int rc = ensure(hs[k], W[k].base + W[k].bytes);
+        if (rc) return rc;
+    }
+    for (int k = 0; k < n; k++) { memset(&sums[k], 0, sizeof(sums[k])); if (status) status[k] = GF_OK; ba_pack(hs[k], &ps[k], W[k]); }
+    BaDev* hdesc = (BaDev*)lead->hbuf;
+    int* hlist = (int*)(hdesc + n);                 // [0, n_small): k_ba_step<MAXR / 2, false>;  [n, n + n_spill): k_ba_step<MAXR, true>
+    int n_small = 0, n_spill = 0, iters = 0, eval_grid = 1, schur_grid = 1, prior_grid = 0;
+    bool any_eval = false;
+    size_t prior_smem = 0, schur_smem = 0, step_smem[2] = {0, 0};
+    for (int k = 0; k < n; k++) {
+        const BaWindow& w = W[k];
+        hdesc[k] = w.d;
+        if (w.spill) hlist[n + n_spill++] = k; else hlist[n_small++] = k;
+        iters = std::max(iters, ps[k].max_num_iterations);
+        eval_grid = std::max(eval_grid, w.d.eval_grid); schur_grid = std::max(schur_grid, w.d.schur_grid);
+        if (w.pn) prior_grid = std::max(prior_grid, (w.pn * w.pn + 255) / 256);
+        any_eval = any_eval || w.eval_blocks > 0;
+        prior_smem = std::max(prior_smem, w.prior_smem); schur_smem = std::max(schur_smem, w.schur_smem);
+        step_smem[w.spill] = std::max(step_smem[w.spill], w.step_smem);
+    }
+    const BaDev* wins = (const BaDev*)lead->dbuf;
+    const int* dlist = (const int*)(wins + n);
+    cudaStream_t st = lead->s;
+    GF_CUDA(cudaEventRecord(lead->e0, st));
+    for (int k = 0; k < n; k++) {     // the first handle's upload carries the batch table in front of its window
+        char* db = (char*)hs[k]->dbuf;
+        GF_CUDA(cudaMemcpyAsync(db, hs[k]->hbuf, W[k].base + W[k].upload_bytes, cudaMemcpyHostToDevice, st));
+        GF_CUDA(cudaMemsetAsync(db + W[k].base + W[k].o_Hp, 0, al16(sizeof(double) * (size_t)W[k].d.nc * W[k].d.nc) + al16(sizeof(double) * acc_size(W[k].d.nc, W[k].d.L)) * 2, st));   // H_prior, both accumulators
+    }
+    if (prior_grid) { k_ba_prior_hessian<<<dim3(prior_grid, n), 256, 0, st>>>(wins); GF_LAUNCHED(); }
+    if (any_eval) { k_ba_eval<<<dim3(eval_grid, n), PAIR_THREADS, prior_smem, st>>>(wins, 0); GF_LAUNCHED(); }
+    // Every kernel of the loop is launched with a programmatic dependency on its predecessor: its CTAs become resident while the
+    // predecessor still runs and sit in griddepcontrol.wait, which hides the launch latency at the 26 kernel boundaries of a solve
+    // (measured on one H100 SXM at 700 W, C2 window: 0.79-0.80 -> 0.77 ms per solve; GF_BA_NO_PDL=1 restores plain stream order for A/B runs)
+    static const bool pdl = getenv("GF_BA_NO_PDL") == nullptr;
+    auto launch = [&](auto kern, dim3 grid, int block, size_t smem, auto... args) -> cudaError_t {
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = grid; cfg.blockDim = dim3(block); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        at[0].val.programmaticStreamSerializationAllowed = 1;
+        cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
+        return cudaLaunchKernelEx(&cfg, kern, args...);
+    };
+    // Windows with a smaller max_num_iterations are stopped by their own state (BaState::max_iter): their kernels return at once
+    for (int it = 0; it <= iters; it++) {
+        GF_CUDA(launch(k_ba_schur, dim3(schur_grid, n), SCHUR_WARPS * 32, schur_smem, wins)); GF_LAUNCHED();      // (the closing launch only prepares the norms)
+        if (n_small) { GF_CUDA(launch(k_ba_step<MAXR / 2, false>, dim3(1, n_small), RB_THREADS, step_smem[0], wins, dlist)); GF_LAUNCHED(); }
+        if (n_spill) { GF_CUDA(launch(k_ba_step<MAXR, true>, dim3(1, n_spill), RB_THREADS, step_smem[1], wins, dlist + n)); GF_LAUNCHED(); }
+        if (it == iters) break;                  // the extra k_ba_step adopts the last linearisation and closes the run
+        GF_CUDA(launch(k_ba_eval, dim3(eval_grid, n), PAIR_THREADS, prior_smem, wins, 1)); GF_LAUNCHED();   // + decision (last CTA of each window)
+    }
+    GF_CUDA(cudaGetLastError());
+    for (int k = 0; k < n; k++) {
+        char* hb = (char*)hs[k]->hbuf + W[k].base; char* db = (char*)hs[k]->dbuf + W[k].base;
+        GF_CUDA(cudaMemcpyAsync(hb + W[k].o_X, db + W[k].o_X, sizeof(double) * (X_FEAT + ps[k].n_features), cudaMemcpyDeviceToHost, st));
+        GF_CUDA(cudaMemcpyAsync(hb + W[k].o_st, db + W[k].o_st, sizeof(BaState), cudaMemcpyDeviceToHost, st));
+    }
+    GF_CUDA(cudaEventRecord(lead->e1, st));
+    GF_CUDA(cudaStreamSynchronize(st));
+    float ms = 0;
+    GF_CUDA(cudaEventElapsedTime(&ms, lead->e0, lead->e1));
+    int rc = GF_OK;
+    for (int k = n - 1; k >= 0; k--) {           // backwards: the error text names the first failing window
+        const BaState* h = (const BaState*)((const char*)hs[k]->hbuf + W[k].base + W[k].o_st);
+        if (h->setup_failed) {
+            rc = set_err(GF_ERR_INVALID_ARG, "an IMU covariance is singular or not positive definite; parameter blocks left untouched");
+            if (multi) window_err(k, rc);
+            if (status) status[k] = GF_ERR_INVALID_ARG;
+            continue;
+        }
+        ba_finish(hs[k], &ps[k], W[k], &sums[k], ms);
+    }
+    return rc;
+}
+
+extern "C" {
+
+int gf_ba_solve(gf_ba* s, const gf_ba_problem* p, gf_ba_summary* sum)
+{
+    if (!s || !p || !sum) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    return ba_batch(&s, 1, p, sum, nullptr, false);
+}
+
+int gf_ba_solve_multi(gf_ba* const* solvers, int n, const gf_ba_problem* problems, gf_ba_summary* summaries, int32_t* status)
+{
+    if (!solvers || !problems || !summaries) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    if (n < 1) return set_err(GF_ERR_INVALID_ARG, "n must be at least 1");
+    if (n > GF_BA_MAX_MULTI) return set_err(GF_ERR_CAPACITY, "more than GF_BA_MAX_MULTI (256) windows");
+    for (int k = 0; k < n; k++) {
+        if (!solvers[k]) return window_err(k, set_err(GF_ERR_INVALID_ARG, "null handle"));
+        if (solvers[k]->device != solvers[0]->device) return window_err(k, set_err(GF_ERR_INVALID_ARG, "handle bound to another device than window 0's"));
+        for (int j = 0; j < k; j++)
+            if (solvers[j] == solvers[k]) { snprintf(g_err, sizeof(g_err), "window %d: handle already used by window %d", k, j); return GF_ERR_INVALID_ARG; }
+    }
+    return ba_batch(solvers, n, problems, summaries, status, true);
 }
 
 /* MARGIN_OLD (estimator.cpp:3334-3535) + MarginalizationInfo::{preMarginalize, marginalize}
@@ -1778,7 +1942,7 @@ static int marg_run(gf_ba* s, const gf_ba_problem* p, int mode, gf_ba_prior* out
     const size_t o_X = take(sizeof(double) * (X_FEAT + nfeat)), o_vis = take(sizeof(gf_ba_visual_factor) * (nv ? nv : 1)), o_imu = take(sizeof(gf_ba_imu_factor)), o_whl = take(sizeof(gf_ba_wheel_factor)), o_plf = take(sizeof(int) * 4),
                  o_ps = take(sizeof(int) * (n_work + 1)), o_pij = take(sizeof(int) * 2 * (size_t)(n_work > 0 ? n_work : 1)), o_cf = take(sizeof(int) * (size_t)(nfeat > 0 ? nfeat : 1)),
                  o_pJ = take(sizeof(double) * (size_t)pn * pn), o_pr0 = take(sizeof(double) * pn), o_px0 = take(sizeof(double) * px0_len), o_pcol = take(sizeof(int) * (size_t)(pn > 0 ? pn : 1));
-    const size_t o_st = take(sizeof(BaState));
+    const size_t o_st = take(sizeof(BaState)), o_dev = take(sizeof(BaDev));
     const size_t upload_bytes = off;
     const size_t NN = (size_t)N * N, mm = (size_t)m * m, nn = (size_t)n * n;
     const size_t o_sq = take(sizeof(double) * 225), o_Hp = take(sizeof(double) * NN), o_a0 = take(sizeof(double) * acc_size(N, 0)),
@@ -1832,7 +1996,10 @@ static int marg_run(gf_ba* s, const gf_ba_problem* p, int mode, gf_ba_prior* out
     d.Hp = (double*)(db + o_Hp); d.acc[0] = (double*)(db + o_a0); d.acc[1] = d.acc[0];
     d.st = (BaState*)(db + o_st);
     memcpy(d.gravity, p->gravity, sizeof(d.gravity)); d.vis_sqrt_info = p->visual_sqrt_info;
-    const size_t NN_ = (size_t)N * N; (void)NN_;
+    const int eval_blocks = n_work + d.n_imu + d.n_wheel + d.n_plane + (pn ? 1 : 0);
+    d.eval_grid = eval_blocks;
+    memcpy(hb + o_dev, &d, sizeof(d));                         // the kernels read the descriptor from the device (a batch of one window)
+    const BaDev* dd = (const BaDev*)(db + o_dev);
     MargDev q;
     q.N = N; q.m = m; q.n = n; q.H = d.acc[0]; q.Hp = d.Hp; q.g = d.acc[0] + NN;      // acc layout: [H N*N | g N | ...]
     q.A = (double*)(db + o_A); q.b = (double*)(db + o_b); q.Amm = (double*)(db + o_Amm); q.Vm = (double*)(db + o_Vm); q.wm = (double*)(db + o_wm);
@@ -1842,9 +2009,8 @@ static int marg_run(gf_ba* s, const gf_ba_problem* p, int mode, gf_ba_prior* out
     GF_CUDA(cudaEventRecord(s->e0, st));
     GF_CUDA(cudaMemcpyAsync(db, hb, upload_bytes, cudaMemcpyHostToDevice, st));
     GF_CUDA(cudaMemsetAsync(db + o_Hp, 0, al(sizeof(double) * NN) + al(sizeof(double) * acc_size(N, 0)), st));     // H_prior and the accumulator
-    if (pn) { k_ba_prior_hessian<<<(pn * pn + 255) / 256, 256, 0, st>>>(d); GF_LAUNCHED(); }
-    const int eval_blocks = n_work + d.n_imu + d.n_wheel + d.n_plane + (pn ? 1 : 0);
-    if (eval_blocks > 0) { k_ba_eval<<<eval_blocks, PAIR_THREADS, sizeof(double) * 2 * (size_t)pn, st>>>(d, 0); GF_LAUNCHED(); }
+    if (pn) { k_ba_prior_hessian<<<(pn * pn + 255) / 256, 256, 0, st>>>(dd); GF_LAUNCHED(); }
+    if (eval_blocks > 0) { k_ba_eval<<<eval_blocks, PAIR_THREADS, sizeof(double) * 2 * (size_t)pn, st>>>(dd, 0); GF_LAUNCHED(); }
     k_marg_pack<<<(int)((NN + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
     const int cdim = (old_ && use_sb) ? 15 : 6;
     int path = 0;

@@ -74,6 +74,36 @@ def marginalize_dense(A, b, c, L, force_generic=False, device=0):
     return J0, r0, tuple(path)
 
 
+def _solve_multi_fn():
+    L = _lib.lib()
+    L.gf_ba_solve_multi.argtypes = [ctypes.POINTER(ctypes.c_void_p), ctypes.c_int, ctypes.POINTER(BaProblem), ctypes.POINTER(BaSummary),
+                                    ctypes.POINTER(ctypes.c_int32)]
+    return L.gf_ba_solve_multi
+
+
+def solve_multi_structs(adjusters, p_array):
+    """gf_ba_solve_multi for a pre-built ctypes array of gf_ba_problem (BaProblem * n), e.g. in timing loops: window k is
+    p_array[k] on adjusters[k] (distinct BundleAdjusters on one device).  Returns (BaSummary * n, status int32 array): status[k]
+    < 0 marks a window whose IMU covariance is singular (its blocks are left untouched); argument errors raise GfError."""
+    n = len(adjusters)
+    handles = (ctypes.c_void_p * n)(*[a._h.value for a in adjusters])
+    sums, status = (BaSummary * n)(), np.zeros(n, np.int32)
+    rc = _solve_multi_fn()(handles, n, p_array, sums, status.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)))
+    if rc != 0 and not (status < 0).any():
+        check(rc)
+    return sums, status
+
+
+def solve_multi(adjusters, problems):
+    """Estimator::optimization() of several windows in one batched call (gf_ba_solve_multi): problems[k]
+    (ground_fusion_b200.ba_problem.Problem) is solved on adjusters[k] and updated in place.  Returns (summary dicts, statuses);
+    status k < 0: window k's IMU covariance is singular and its blocks are untouched.  device_ms is the time of the whole batch."""
+    assert len(adjusters) == len(problems)
+    p_array = (BaProblem * len(problems))(*[p.struct() for p in problems])
+    sums, status = solve_multi_structs(adjusters, p_array)
+    return [s.as_dict() for s in sums], [int(v) for v in status]
+
+
 class BundleAdjuster:
     """One solver workspace bound to one GPU (gf_ba).  optimization(problem) updates the para_* arrays of
     `problem` (ground_fusion_b200.ba_problem.Problem) in place, like Estimator::optimization() does with

@@ -384,6 +384,23 @@ int gf_ba_create(gf_ba** out, int device);
 void gf_ba_destroy(gf_ba* s);
 /* ceres::Solve + double2vector's input: optimises the blocks of `p` in place. */
 int gf_ba_solve(gf_ba* s, const gf_ba_problem* p, gf_ba_summary* summary);
+/* The sliding windows of several estimators in one call (several robots or camera rigs served by one GPU): one window cannot
+ * fill the device (its trust-region loop is a chain of small latency-bound launches), a batch runs every kernel of that chain
+ * once for all windows (window = blockIdx.y), so the launch count does not grow with n.  Window k is problems[k], solved with
+ * solvers[k]'s workspace and tile cap; its blocks are updated in place and summaries[k] filled exactly as
+ * gf_ba_solve(solvers[k], &problems[k], &summaries[k]) would (same kernels, same arithmetic; like two gf_ba_solve calls of one
+ * window, results may differ in the last bits because the Hessian is summed with atomics).  The exception is device_ms: the
+ * CUDA-event time of the whole batch, the same in every summary.  max_num_iterations may differ between windows.
+ *   1 <= n <= GF_BA_MAX_MULTI (more: GF_ERR_CAPACITY); the handles must be distinct and bound to the same device.  Every
+ *   window is checked as gf_ba_solve checks it before anything is enqueued; on an argument error nothing is modified and
+ *   gf_last_error() starts with "window k: ".
+ *   status (nullable, n): 0, or GF_ERR_INVALID_ARG for a window whose IMU covariance turned out singular on the device: its
+ *   blocks and summary are left untouched (summary zeroed), the other windows are written back, and the call returns
+ *   GF_ERR_INVALID_ARG.
+ * All work runs on solvers[0]'s stream, driven by the calling thread; no handle of the batch may be used by another thread
+ * during the call. */
+#define GF_BA_MAX_MULTI 256
+int gf_ba_solve_multi(gf_ba* const* solvers, int n, const gf_ba_problem* problems, gf_ba_summary* summaries, int32_t* status);
 /* Counters of the last solve (32 slots).  [30] = SM cycles (clock64) spent inside the k_ba_step launches that took a
  * trust-region step, [31] = their number: bench.py derives the step kernel's achieved FP64 rate from them.  Slots 0..15 are
  * per-phase cycles and only filled in a -DGF_PROFILE build. */
