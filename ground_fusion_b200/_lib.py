@@ -143,6 +143,20 @@ class BaSummary(ctypes.Structure):
                 "radius": list(self.radius)[:n + 1], "device_ms": self.device_ms}
 
 
+_MAXF = 11          # GF_BA_MAX_FRAMES
+
+
+class BaStepCapture(ctypes.Structure):
+    """gf_ba_step_capture: what the solve computes inside its first iteration (gf_ba_first_step)."""
+    ARRAYS = ("imu_sqrt", "H", "Hp", "g", "W", "hll", "scale", "D", "gs", "e_l", "S", "gn", "delta", "Xc")
+    _fields_ = ([(n, _i) for n in ("nc", "L", "n", "spill")] + [("col_pose", _i * _MAXF), ("col_sb", _i * _MAXF)]
+                + [(n, _i) for n in ("col_ex", "col_td", "col_exw")] + [("col_ix", _i * 3)] + [(n, _i) for n in ("col_tdw", "col_pr", "col_pz")]
+                + [(n, _i) for n in ("solver_failed", "step_valid", "done", "termination", "iterations")]
+                + [(n, _d) for n in ("initial_cost", "cauchy_num", "cauchy_den", "alpha", "dogleg_a", "dogleg_b", "dogleg_norm",
+                                     "model_change", "step_norm", "grad_max", "x_norm", "mu", "radius")]
+                + [("col_feat", ctypes.POINTER(_i))] + [(n, _dp) for n in ARRAYS])
+
+
 BLOCK_POSE, BLOCK_SPEEDBIAS, BLOCK_EX_POSE, BLOCK_TD = 0, 1, 2, 3
 BLOCK_EX_WHEEL, BLOCK_SX, BLOCK_SY, BLOCK_SW, BLOCK_TD_WHEEL = 4, 5, 6, 7, 8
 BLOCK_PLANE_R, BLOCK_PLANE_Z = 10, 11

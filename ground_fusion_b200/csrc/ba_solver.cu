@@ -47,6 +47,7 @@ struct BaState {
     double cost_hist[GF_BA_MAX_ITERATIONS + 1], radius_hist[GF_BA_MAX_ITERATIONS + 1];
     double acc_cost[2];          // cost accumulated by k_ba_eval into buffer 0/1
     double cauchy_num, cauchy_den;   // |gs|^2 and v^T H' v accumulated by k_ba_schur
+    double dl_a, dl_b;           // the last dogleg step in D-space: dl_a * gs + dl_b * gn
     int it, reuse, done, termination, n_success, invalid_streak, need_linearize, step_valid, cur, first, max_iter, solver_failed;
     unsigned int eval_ticket;    // CTAs of the current k_ba_eval(1) that have finished: the last one runs the decision
     int setup_failed;            // sticky: an IMU covariance was singular / not positive definite (first k_ba_eval); nothing is solved
@@ -943,7 +944,7 @@ __global__ void __launch_bounds__(RB_THREADS) k_ba_step(const BaDev* __restrict_
         plus_free(d, d.X, dl, d.Xc, tid, nt, s2, mx);
         s2 = block_reduce_sum(s2, sred);
         if (tid == 0) {
-            st.dogleg_norm = dn; st.model_change = model_change; st.step_norm = sqrt(s2);
+            st.dogleg_norm = dn; st.model_change = model_change; st.step_norm = sqrt(s2); st.dl_a = ca; st.dl_b = cb;
             st.step_valid = model_change > 0.0 ? 1 : 0;
             st.cand_cost = 0.0;
         }
@@ -1492,6 +1493,7 @@ static int ba_layout(const gf_ba* s, const gf_ba_problem* p, BaWindow& w)
         int k = p->visual[v].feature;
         if (k < 0 || k >= nfeat || p->visual[v].imu_i < 0 || p->visual[v].imu_i >= F || p->visual[v].imu_j < 0 || p->visual[v].imu_j >= F)
             return set_err(GF_ERR_INVALID_ARG, "visual factor index out of range");
+        if (p->visual[v].imu_i == p->visual[v].imu_j) return set_err(GF_ERR_INVALID_ARG, "visual factor with imu_i == imu_j");
         if (!p->feature_const[k] && col_feat[k] == -1) col_feat[k] = -2;
     }
     for (int k = 0; k < nfeat; k++) if (col_feat[k] == -2) col_feat[k] = c++;
@@ -1577,7 +1579,8 @@ static int ba_layout(const gf_ba* s, const gf_ba_problem* p, BaWindow& w)
     return GF_OK;
 }
 
-static void ba_pack(gf_ba* s, const gf_ba_problem* p, BaWindow& w)
+// radius, mu: the initial trust-region state (Ceres' defaults 1e4, 1e-8 for a solve); max_iter: BaState::max_iter
+static void ba_pack(gf_ba* s, const gf_ba_problem* p, BaWindow& w, double radius, double mu, int max_iter)
 {
     const int F = p->n_frames, nfeat = p->n_features, n = w.d.n, pn = w.pn;
     const gf_ba_prior* pr = pn ? p->prior : nullptr;
@@ -1597,7 +1600,7 @@ static void ba_pack(gf_ba* s, const gf_ba_problem* p, BaWindow& w)
     {   // TrustRegionMinimizer / DoglegStrategy initial state; the first linearisation goes to buffer 0
         BaState* h0 = (BaState*)(hb + w.o_st);
         memset(h0, 0, sizeof(BaState));
-        h0->radius = 1e4; h0->mu = 1e-8; h0->need_linearize = 1; h0->cur = 1; h0->first = 1; h0->max_iter = p->max_num_iterations;
+        h0->radius = radius; h0->mu = mu; h0->need_linearize = 1; h0->cur = 1; h0->first = 1; h0->max_iter = max_iter;
     }
     {   // factors sorted by pair
         gf_ba_visual_factor* hv = (gf_ba_visual_factor*)(hb + w.o_vis);
@@ -1661,11 +1664,21 @@ static int window_err(int k, int rc)
     return rc;
 }
 
+static void capture_window(const gf_ba* s, const gf_ba_problem* p, const BaWindow& w, gf_ba_step_capture* c);
+
+// gf_ba_first_step: the solve's chain stopped after the first k_ba_step, with every intermediate downloaded
+struct BaCapture {
+    double radius, mu;
+    gf_ba_step_capture* out;      // one per window
+};
+
 // Windows k = 0..n-1 (problem ps[k] on handle hs[k]), every one validated before anything is written or enqueued.  All work goes to
 // hs[0]'s stream; hs[0]'s buffers also hold the batch table: the n descriptors and the two lists of windows per k_ba_step
 // instantiation.  Launch count: that of the window with the most iterations, plus one k_ba_step per iteration when both
-// instantiations are needed.
-static int ba_batch(gf_ba* const* hs, int n, const gf_ba_problem* ps, gf_ba_summary* sums, int32_t* status, bool multi)
+// instantiations are needed.  cap (non-null): the same chain up to the first k_ba_step (k_ba_prior_hessian, k_ba_eval(0),
+// k_ba_schur, k_ba_step), the window's whole device image copied back after k_ba_schur and after k_ba_step, nothing written back.
+static int ba_batch(gf_ba* const* hs, int n, const gf_ba_problem* ps, gf_ba_summary* sums, int32_t* status, bool multi,
+                    const BaCapture* cap = nullptr)
 {
     std::vector<BaWindow> W(n);
     for (int k = 0; k < n; k++) { const int rc = ba_layout(hs[k], &ps[k], W[k]); if (rc) return multi ? window_err(k, rc) : rc; }
@@ -1674,10 +1687,15 @@ static int ba_batch(gf_ba* const* hs, int n, const gf_ba_problem* ps, gf_ba_summ
     const size_t table = al16((sizeof(BaDev) + 2 * sizeof(int)) * (size_t)n);
     for (int k = 0; k < n; k++) {
         W[k].base = k == 0 ? table : 0;
-        const int rc = ensure(hs[k], W[k].base + W[k].bytes);
+        const int rc = ensure(hs[k], W[k].base + W[k].bytes * (cap ? 2 : 1));      // a capture stages two images of the window
         if (rc) return rc;
     }
-    for (int k = 0; k < n; k++) { memset(&sums[k], 0, sizeof(sums[k])); if (status) status[k] = GF_OK; ba_pack(hs[k], &ps[k], W[k]); }
+    for (int k = 0; k < n; k++) {
+        if (sums) memset(&sums[k], 0, sizeof(sums[k]));
+        if (status) status[k] = GF_OK;
+        if (cap) ba_pack(hs[k], &ps[k], W[k], cap->radius, cap->mu, 1);
+        else ba_pack(hs[k], &ps[k], W[k], 1e4, 1e-8, ps[k].max_num_iterations);
+    }
     BaDev* hdesc = (BaDev*)lead->hbuf;
     int* hlist = (int*)(hdesc + n);                 // [0, n_small): k_ba_step<MAXR / 2, false>;  [n, n + n_spill): k_ba_step<MAXR, true>
     int n_small = 0, n_spill = 0, iters = 0, eval_grid = 1, schur_grid = 1, prior_grid = 0;
@@ -1687,7 +1705,7 @@ static int ba_batch(gf_ba* const* hs, int n, const gf_ba_problem* ps, gf_ba_summ
         const BaWindow& w = W[k];
         hdesc[k] = w.d;
         if (w.spill) hlist[n + n_spill++] = k; else hlist[n_small++] = k;
-        iters = std::max(iters, ps[k].max_num_iterations);
+        iters = cap ? 0 : std::max(iters, ps[k].max_num_iterations);
         eval_grid = std::max(eval_grid, w.d.eval_grid); schur_grid = std::max(schur_grid, w.d.schur_grid);
         if (w.pn) prior_grid = std::max(prior_grid, (w.pn * w.pn + 255) / 256);
         any_eval = any_eval || w.eval_blocks > 0;
@@ -1721,14 +1739,19 @@ static int ba_batch(gf_ba* const* hs, int n, const gf_ba_problem* ps, gf_ba_summ
     // Windows with a smaller max_num_iterations are stopped by their own state (BaState::max_iter): their kernels return at once
     for (int it = 0; it <= iters; it++) {
         GF_CUDA(launch(k_ba_schur, dim3(schur_grid, n), SCHUR_WARPS * 32, schur_smem, wins)); GF_LAUNCHED();      // (the closing launch only prepares the norms)
+        for (int k = 0; cap && k < n; k++) {      // the reduced system, e_l and the Cauchy sums before k_ba_step consumes them
+            const size_t o = W[k].base;
+            GF_CUDA(cudaMemcpyAsync((char*)hs[k]->hbuf + o + W[k].bytes, (char*)hs[k]->dbuf + o, W[k].bytes, cudaMemcpyDeviceToHost, st));
+        }
         if (n_small) { GF_CUDA(launch(k_ba_step<MAXR / 2, false>, dim3(1, n_small), RB_THREADS, step_smem[0], wins, dlist)); GF_LAUNCHED(); }
         if (n_spill) { GF_CUDA(launch(k_ba_step<MAXR, true>, dim3(1, n_spill), RB_THREADS, step_smem[1], wins, dlist + n)); GF_LAUNCHED(); }
-        if (it == iters) break;                  // the extra k_ba_step adopts the last linearisation and closes the run
+        if (it == iters) break;                  // the extra k_ba_step adopts the last linearisation and closes the run (a capture: the first step)
         GF_CUDA(launch(k_ba_eval, dim3(eval_grid, n), PAIR_THREADS, prior_smem, wins, 1)); GF_LAUNCHED();   // + decision (last CTA of each window)
     }
     GF_CUDA(cudaGetLastError());
     for (int k = 0; k < n; k++) {
         char* hb = (char*)hs[k]->hbuf + W[k].base; char* db = (char*)hs[k]->dbuf + W[k].base;
+        if (cap) { GF_CUDA(cudaMemcpyAsync(hb, db, W[k].bytes, cudaMemcpyDeviceToHost, st)); continue; }
         GF_CUDA(cudaMemcpyAsync(hb + W[k].o_X, db + W[k].o_X, sizeof(double) * (X_FEAT + ps[k].n_features), cudaMemcpyDeviceToHost, st));
         GF_CUDA(cudaMemcpyAsync(hb + W[k].o_st, db + W[k].o_st, sizeof(BaState), cudaMemcpyDeviceToHost, st));
     }
@@ -1745,12 +1768,101 @@ static int ba_batch(gf_ba* const* hs, int n, const gf_ba_problem* ps, gf_ba_summ
             if (status) status[k] = GF_ERR_INVALID_ARG;
             continue;
         }
-        ba_finish(hs[k], &ps[k], W[k], &sums[k], ms);
+        if (cap) capture_window(hs[k], &ps[k], W[k], &cap->out[k]);
+        else ba_finish(hs[k], &ps[k], W[k], &sums[k], ms);
     }
     return rc;
 }
 
+// 1 <= n <= GF_BA_MAX_MULTI distinct handles on one device
+static int check_batch(gf_ba* const* solvers, int n)
+{
+    if (n < 1) return set_err(GF_ERR_INVALID_ARG, "n must be at least 1");
+    if (n > GF_BA_MAX_MULTI) return set_err(GF_ERR_CAPACITY, "more than GF_BA_MAX_MULTI (256) windows");
+    for (int k = 0; k < n; k++) {
+        if (!solvers[k]) return window_err(k, set_err(GF_ERR_INVALID_ARG, "null handle"));
+        if (solvers[k]->device != solvers[0]->device) return window_err(k, set_err(GF_ERR_INVALID_ARG, "handle bound to another device than window 0's"));
+        for (int j = 0; j < k; j++)
+            if (solvers[j] == solvers[k]) { snprintf(g_err, sizeof(g_err), "window %d: handle already used by window %d", k, j); return GF_ERR_INVALID_ARG; }
+    }
+    return GF_OK;
+}
+
+// Unpacks one window's two device images (after k_ba_schur: hbuf + base + bytes; after k_ba_step: hbuf + base) into *c
+static void capture_window(const gf_ba* s, const gf_ba_problem* p, const BaWindow& w, gf_ba_step_capture* c)
+{
+    const char* hb = (const char*)s->hbuf + w.base;          // after k_ba_step
+    const char* ha = hb + w.bytes;                           // after k_ba_schur
+    const BaDev& d = w.d;
+    const int nc = d.nc, L = d.L, n = d.n, F = p->n_frames;
+    const size_t nn = (size_t)(n > 0 ? n : 1);
+    const BaState* sa = (const BaState*)(ha + w.o_st);
+    const BaState* sb = (const BaState*)(hb + w.o_st);
+    c->nc = nc; c->L = L; c->n = n; c->spill = w.spill ? 1 : 0;
+    for (int f = 0; f < GF_BA_MAX_FRAMES; f++) { c->col_pose[f] = d.col_pose[f]; c->col_sb[f] = d.col_sb[f]; }
+    c->col_ex = d.col_ex; c->col_td = d.col_td; c->col_exw = d.col_exw; c->col_tdw = d.col_tdw; c->col_pr = d.col_pr; c->col_pz = d.col_pz;
+    for (int k = 0; k < 3; k++) c->col_ix[k] = d.col_ix[k];
+    c->initial_cost = sb->x_cost; c->cauchy_num = sa->cauchy_num; c->cauchy_den = sa->cauchy_den; c->alpha = sb->alpha;
+    c->dogleg_a = sb->dl_a; c->dogleg_b = sb->dl_b; c->dogleg_norm = sb->dogleg_norm; c->model_change = sb->model_change;
+    c->step_norm = sb->step_norm; c->grad_max = sb->grad_max; c->x_norm = sb->x_norm; c->mu = sb->mu; c->radius = sb->radius;
+    c->solver_failed = sb->solver_failed; c->step_valid = sb->step_valid; c->done = sb->done; c->termination = sb->termination;
+    c->iterations = sb->it;
+    // the first linearisation went to accumulator 0 (the host uploads cur = 1)
+    const double* acc = (const double*)(hb + w.o_a0);
+    const double* vb = (const double*)(hb + w.o_vec);        // scale | D | gs | gn | step | delta
+    const double* va = (const double*)(ha + w.o_vec);
+    if (c->col_feat) memcpy(c->col_feat, w.col_feat.data(), sizeof(int) * (size_t)p->n_features);
+    if (c->imu_sqrt) memcpy(c->imu_sqrt, hb + w.o_sq, sizeof(double) * 225 * (size_t)p->n_imu);
+    if (c->H) memcpy(c->H, acc, sizeof(double) * (size_t)nc * nc);
+    if (c->Hp) memcpy(c->Hp, hb + w.o_Hp, sizeof(double) * (size_t)nc * nc);
+    if (c->g) memcpy(c->g, acc + (size_t)nc * nc, sizeof(double) * n);
+    if (c->W) memcpy(c->W, acc + (size_t)nc * nc + n, sizeof(double) * (size_t)L * nc);
+    if (c->hll) memcpy(c->hll, acc + (size_t)nc * nc + n + (size_t)L * nc, sizeof(double) * L);
+    if (c->scale) memcpy(c->scale, vb, sizeof(double) * n);
+    if (c->D) memcpy(c->D, vb + nn, sizeof(double) * n);
+    if (c->gs) memcpy(c->gs, vb + 2 * nn, sizeof(double) * n);
+    if (c->e_l) memcpy(c->e_l, va + 3 * nn + nc, sizeof(double) * L);      // gn[nc + l] holds e_l until k_ba_step overwrites it
+    if (c->gn) memcpy(c->gn, vb + 3 * nn, sizeof(double) * n);
+    if (c->S) {          // tiles tix(I, J) (row-major 8x8) of the (nc+1)-row augmented system -> dense lower triangle
+        const double* Sg = (const double*)(ha + w.o_Sg);
+        const int m = nc + 1;
+        for (int a = 0; a < m; a++)
+            for (int b = 0; b < m; b++)
+                c->S[(size_t)a * m + b] = b > a ? 0.0 : Sg[(size_t)tix(a >> 3, b >> 3) * 64 + (a & 7) * 8 + (b & 7)];
+    }
+    if (c->delta)        // k_ba_step's own formula on the vectors it used (delta itself may live in shared memory only)
+        for (int k = 0; k < n; k++) c->delta[k] = (sb->dl_a * vb[2 * nn + k] + sb->dl_b * vb[3 * nn + k]) / vb[nn + k] * vb[k];
+    if (c->Xc) {         // pose | speed-bias | ex | td | ex_wheel | sx sy sw | td_wheel | plane R | plane Z | features
+        const double* X = (const double*)(hb + w.o_Xc);
+        double* o = c->Xc;
+        memcpy(o, X + X_POSE, sizeof(double) * 7 * F); o += 7 * F;
+        memcpy(o, X + X_SB, sizeof(double) * 9 * F); o += 9 * F;
+        memcpy(o, X + X_EX, sizeof(double) * (X_FEAT - X_EX)); o += X_FEAT - X_EX;
+        memcpy(o, X + X_FEAT, sizeof(double) * (size_t)p->n_features);
+    }
+}
+
 extern "C" {
+
+int gf_ba_step_dims(gf_ba* s, const gf_ba_problem* p, int* dims3)
+{
+    if (!s || !p || !dims3) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    BaWindow w;
+    const int rc = ba_layout(s, p, w);
+    if (rc) return rc;
+    dims3[0] = w.d.nc; dims3[1] = w.d.L; dims3[2] = w.d.n;
+    return GF_OK;
+}
+
+int gf_ba_first_step(gf_ba* const* solvers, int n, const gf_ba_problem* problems, double radius, double mu, gf_ba_step_capture* out)
+{
+    if (!solvers || !problems || !out) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    if (const int rc = check_batch(solvers, n)) return rc;
+    // mu >= 1 skips the Gauss-Newton solve and mu = 0 would never leave k_ba_step's retry loop
+    if (!(radius > 0.0) || !(mu > 0.0 && mu < 1.0)) return set_err(GF_ERR_INVALID_ARG, "radius must be > 0 and mu in (0, 1)");
+    const BaCapture cap = {radius, mu, out};
+    return ba_batch(solvers, n, problems, nullptr, nullptr, n > 1, &cap);
+}
 
 int gf_ba_solve(gf_ba* s, const gf_ba_problem* p, gf_ba_summary* sum)
 {
@@ -1761,14 +1873,7 @@ int gf_ba_solve(gf_ba* s, const gf_ba_problem* p, gf_ba_summary* sum)
 int gf_ba_solve_multi(gf_ba* const* solvers, int n, const gf_ba_problem* problems, gf_ba_summary* summaries, int32_t* status)
 {
     if (!solvers || !problems || !summaries) return set_err(GF_ERR_INVALID_ARG, "null argument");
-    if (n < 1) return set_err(GF_ERR_INVALID_ARG, "n must be at least 1");
-    if (n > GF_BA_MAX_MULTI) return set_err(GF_ERR_CAPACITY, "more than GF_BA_MAX_MULTI (256) windows");
-    for (int k = 0; k < n; k++) {
-        if (!solvers[k]) return window_err(k, set_err(GF_ERR_INVALID_ARG, "null handle"));
-        if (solvers[k]->device != solvers[0]->device) return window_err(k, set_err(GF_ERR_INVALID_ARG, "handle bound to another device than window 0's"));
-        for (int j = 0; j < k; j++)
-            if (solvers[j] == solvers[k]) { snprintf(g_err, sizeof(g_err), "window %d: handle already used by window %d", k, j); return GF_ERR_INVALID_ARG; }
-    }
+    if (const int rc = check_batch(solvers, n)) return rc;
     return ba_batch(solvers, n, problems, summaries, status, true);
 }
 
@@ -1834,6 +1939,8 @@ static int marg_run(gf_ba* s, const gf_ba_problem* p, int mode, gf_ba_prior* out
     GF_CUDA(cudaSetDevice(s->device));
     const int F = p->n_frames, nfeat = p->n_features;
     const bool use_sb = p->para_speed_bias && !p->pose0_const;
+    // a residual block may not list one parameter block twice (ceres::Problem refuses it; the reference never builds one)
+    for (int v = 0; v < p->n_visual; v++) if (p->visual[v].imu_i == p->visual[v].imu_j) return set_err(GF_ERR_INVALID_ARG, "visual factor with imu_i == imu_j");
     // ---- the marginalised and the kept blocks (same rules as the oracle) ----
     std::vector<int> lm_col(nfeat > 0 ? nfeat : 1, -1);
     int pos = 0;

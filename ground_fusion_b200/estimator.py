@@ -104,6 +104,54 @@ def solve_multi(adjusters, problems):
     return [s.as_dict() for s in sums], [int(v) for v in status]
 
 
+def _capture_buffers(adjuster, problem):
+    """A gf_ba_step_capture whose arrays are numpy buffers sized for `problem` (gf_ba_step_dims), and those buffers."""
+    L = _lib.lib()
+    L.gf_ba_step_dims.argtypes = [ctypes.c_void_p, ctypes.POINTER(BaProblem), ctypes.POINTER(ctypes.c_int)]
+    dims = (ctypes.c_int * 3)()
+    p = problem.struct()
+    check(L.gf_ba_step_dims(adjuster._h, ctypes.byref(p), dims))
+    nc, nl, n = dims
+    shapes = {"imu_sqrt": (problem.n_imu, 15, 15), "H": (nc, nc), "Hp": (nc, nc), "g": (n,), "W": (nl, nc), "hll": (nl,), "scale": (n,),
+              "D": (n,), "gs": (n,), "e_l": (nl,), "S": (nc + 1, nc + 1), "gn": (n,), "delta": (n,),
+              "Xc": (16 * problem.n_frames + 24 + problem.n_features,)}
+    bufs = {k: np.zeros(v) for k, v in shapes.items()}
+    bufs["col_feat"] = np.zeros(max(problem.n_features, 1), np.int32)
+    c = _lib.BaStepCapture()
+    for k in _lib.BaStepCapture.ARRAYS:
+        setattr(c, k, bufs[k].ctypes.data_as(ctypes.POINTER(ctypes.c_double)) if bufs[k].size else None)
+    c.col_feat = bufs["col_feat"].ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
+    return c, bufs
+
+
+def _capture_dict(c, bufs, problem):
+    out = {k: getattr(c, k) for k, _ in c._fields_ if k not in _lib.BaStepCapture.ARRAYS and k != "col_feat"}
+    for k in ("col_pose", "col_sb", "col_ix"):
+        out[k] = list(out[k])
+    out["col_pose"], out["col_sb"] = out["col_pose"][:problem.n_frames], out["col_sb"][:problem.n_frames]
+    out.update({k: v for k, v in bufs.items() if k != "col_feat"})
+    out["col_feat"] = bufs["col_feat"][:problem.n_features].copy()
+    return out
+
+
+def first_step_multi(adjusters, problems, radius=1e4, mu=1e-8):
+    """gf_ba_first_step: the chain of solve_multi from the trust-region state (radius, mu), stopped after the first dogleg step.
+    Returns one dict per window with the linearisation (H, Hp, g, W, hll, imu_sqrt), the scaling (scale, D, gs, e_l), the
+    reduced system S (lower triangle, rhs in row nc), the Cauchy terms, the Gauss-Newton and dogleg step (gn, dogleg_a/b,
+    delta, model_change) and the candidate Xc.  No parameter block is modified."""
+    assert len(adjusters) == len(problems)
+    n = len(adjusters)
+    caps = [_capture_buffers(a, p) for a, p in zip(adjusters, problems)]
+    L = _lib.lib()
+    L.gf_ba_first_step.argtypes = [ctypes.POINTER(ctypes.c_void_p), ctypes.c_int, ctypes.POINTER(BaProblem), ctypes.c_double,
+                                   ctypes.c_double, ctypes.POINTER(_lib.BaStepCapture)]
+    handles = (ctypes.c_void_p * n)(*[a._h.value for a in adjusters])
+    p_array = (BaProblem * n)(*[p.struct() for p in problems])
+    out = (_lib.BaStepCapture * n)(*[c for c, _ in caps])
+    check(L.gf_ba_first_step(handles, n, p_array, float(radius), float(mu), out))
+    return [_capture_dict(out[k], caps[k][1], problems[k]) for k in range(n)]
+
+
 class BundleAdjuster:
     """One solver workspace bound to one GPU (gf_ba).  optimization(problem) updates the para_* arrays of
     `problem` (ground_fusion_b200.ba_problem.Problem) in place, like Estimator::optimization() does with
@@ -159,6 +207,10 @@ class BundleAdjuster:
         self.L.gf_ba_last_marg_info.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int)]
         check(self.L.gf_ba_last_marg_info(self._h, info))
         return tuple(info)
+
+    def first_step(self, problem, radius=1e4, mu=1e-8):
+        """The solve's first iteration on this handle, captured stage by stage (see first_step_multi)."""
+        return first_step_multi([self], [problem], radius, mu)[0]
 
     def solve_struct(self, p_struct):
         """Same, for a pre-built ctypes gf_ba_problem (avoids rebuilding it in timing loops)."""

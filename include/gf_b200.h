@@ -401,6 +401,44 @@ int gf_ba_solve(gf_ba* s, const gf_ba_problem* p, gf_ba_summary* summary);
  * during the call. */
 #define GF_BA_MAX_MULTI 256
 int gf_ba_solve_multi(gf_ba* const* solvers, int n, const gf_ba_problem* problems, gf_ba_summary* summaries, int32_t* status);
+
+/* What the solve computes inside its first iteration, for testing the kernels stage by stage (gf_ba_first_step).  Columns
+ * follow the solve's layout: nc camera columns (col_* below, -1 = constant or absent), then the L free landmarks (col_feat).
+ * The int / double scalars are filled by the call; every pointer is a caller buffer sized from gf_ba_step_dims, or NULL to
+ * skip that array. */
+typedef struct gf_ba_step_capture {
+    int32_t nc, L, n, spill;          /* reduced dimension, free landmarks, nc + L; 1 = the factor spilled out of shared memory */
+    int32_t col_pose[GF_BA_MAX_FRAMES], col_sb[GF_BA_MAX_FRAMES], col_ex, col_td, col_exw, col_ix[3], col_tdw, col_pr, col_pz;
+    int32_t solver_failed, step_valid, done, termination, iterations;   /* BaState after the step (done: stopped before stepping) */
+    double initial_cost;              /* cost at x                                                                           */
+    double cauchy_num, cauchy_den, alpha;   /* |gs|^2, v^T H' v (v = gs / D), alpha = num / den                              */
+    double dogleg_a, dogleg_b;        /* the D-space step dogleg_a * gs + dogleg_b * gn                                        */
+    double dogleg_norm, model_change, step_norm, grad_max, x_norm;
+    double mu, radius;                /* mu after k_ba_step (larger than the given one only if the Cholesky had to be retried) */
+    int32_t* col_feat;                /* [n_features] column of each landmark, -1 = constant or unobserved                   */
+    double* imu_sqrt;                 /* [n_imu][15][15] sqrt-information LLT(cov^-1).L^T of every IMU factor                */
+    double* H;                        /* [nc][nc] camera block of J^T J without the prior                                    */
+    double* Hp;                       /* [nc][nc] J0^T J0 of the marginalisation prior                                       */
+    double* g;                        /* [n] J^T r (prior included)                                                          */
+    double* W;                        /* [L][nc] landmark-camera block of J^T J                                              */
+    double* hll;                      /* [L] landmark diagonal of J^T J                                                      */
+    double *scale, *D, *gs;           /* [n] Jacobi scale, D = sqrt(clamp(diag(H') , 1e-6, 1e32)), gs = g' / D               */
+    double* e_l;                      /* [L] 1 / (h'_ll + mu D_l^2)                                                          */
+    double* S;                        /* [nc+1][nc+1] reduced system (H' + mu D^2 with the landmarks eliminated), lower
+                                       * triangle; row nc holds the right-hand side, S[nc][nc] = 1                             */
+    double* gn;                       /* [n] Gauss-Newton step in D-space                                                    */
+    double* delta;                    /* [n] ambient step (dogleg_a gs + dogleg_b gn) / D * scale                            */
+    double* Xc;                       /* [16 n_frames + 24 + n_features] candidate x (+) delta: pose[7F] | speed-bias[9F] | ex
+                                       * pose[7] | td | wheel extrinsic[7] | sx sy sw | wheel td | plane R[4] | plane Z | features */
+} gf_ba_step_capture;
+/* dims3 = {nc, L, n} of the window as gf_ba_solve would lay it out; argument errors as gf_ba_solve. */
+int gf_ba_step_dims(gf_ba* s, const gf_ba_problem* p, int* dims3);
+/* The chain of gf_ba_solve_multi (same layout, packing, kernels, grids and launch attributes), started from the trust-region
+ * radius `radius` and LM damping `mu` and stopped after the first k_ba_step: the initial linearisation, the reduced system, the
+ * dogleg step and the candidate point of every window go to out[k].  No parameter block is written.  radius must be > 0 and mu
+ * in (0, 1) (GF_ERR_INVALID_ARG).  A window whose IMU covariance is singular or indefinite fails the call with
+ * GF_ERR_INVALID_ARG (error text "window k: ..." when n > 1). */
+int gf_ba_first_step(gf_ba* const* solvers, int n, const gf_ba_problem* problems, double radius, double mu, gf_ba_step_capture* out);
 /* Counters of the last solve (32 slots).  [30] = SM cycles (clock64) spent inside the k_ba_step launches that took a
  * trust-region step, [31] = their number: bench.py derives the step kernel's achieved FP64 rate from them.  Slots 0..15 are
  * per-phase cycles and only filled in a -DGF_PROFILE build. */

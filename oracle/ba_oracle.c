@@ -740,6 +740,14 @@ static void state_store(const gf_ba_problem* p, const state_t* s)
     memcpy(p->para_feature, s->feat, sizeof(double) * p->n_features);
 }
 
+/* A residual block may not list one parameter block twice (ceres::Problem refuses it; the reference builds the visual factor
+ * only for imu_i != imu_j): such a window is an argument error. */
+static int same_frame_visual(const gf_ba_problem* p)
+{
+    for (int v = 0; v < p->n_visual; v++) if (p->visual[v].imu_i == p->visual[v].imu_j) return 1;
+    return 0;
+}
+
 static void make_layout(const gf_ba_problem* p, layout_t* L)
 {
     int c = 0;
@@ -1028,7 +1036,6 @@ static double linearize_blocks(const gf_ba_problem* p, const layout_t* L, const 
         for (int k = 0; k < 2; k++) { Jf[k] *= sc; Jtd[k] *= sc; res[k] *= sc; }
         int cols[5] = {L->col_pose[f->imu_i], L->col_pose[f->imu_j], L->col_ex, L->col_feat[f->feature], L->col_td}, sizes[5] = {6, 6, 6, 1, 1}, lds[5] = {7, 7, 7, 1, 1};
         double* Js[5] = {Ji, Jj, Jex, Jf, Jtd};
-        if (f->imu_i == f->imu_j) cols[1] = -1;
         add_blocks(H, g, n, 2, res, 5, cols, sizes, lds, Js);
     }
     return cost;
@@ -1166,6 +1173,7 @@ GFO void gfo_ba_set_tolerances(double f, double g, double x) { g_func_tol = f; g
 
 GFO int gfo_ba_solve(const gf_ba_problem* p, gf_ba_summary* sum)
 {
+    if (same_frame_visual(p)) return GF_ERR_INVALID_ARG;
     layout_t L; make_layout(p, &L);
     const int n = L.n_cols, m = L.n_rows;
     memset(sum, 0, sizeof(*sum));
@@ -1298,6 +1306,7 @@ done:
 /* cost at the current parameter values (1/2 sum rho) -- test aid */
 GFO double gfo_ba_cost(const gf_ba_problem* p)
 {
+    if (same_frame_visual(p)) return NAN;
     layout_t L; make_layout(p, &L);
     double* imu_sqrt = (double*)malloc(sizeof(double) * 225 * (p->n_imu > 0 ? p->n_imu : 1));
     for (int k = 0; k < p->n_imu; k++) gfo_sqrt_info(p->imu[k].covariance, 15, imu_sqrt + 225 * k);
@@ -1312,9 +1321,10 @@ GFO double gfo_ba_cost(const gf_ba_problem* p)
  * (finite differences, SciPy cross-check).  Returns rows; cols via *n_cols. */
 GFO int gfo_ba_linearize(const gf_ba_problem* p, double* r_out, double* J_out, int* n_cols, int cap_rows, int cap_cols)
 {
+    if (same_frame_visual(p)) return GF_ERR_INVALID_ARG;
     layout_t L; make_layout(p, &L);
     *n_cols = L.n_cols;
-    if (L.n_rows > cap_rows || L.n_cols > cap_cols) { free(L.col_feat); return -1; }
+    if (L.n_rows > cap_rows || L.n_cols > cap_cols) { free(L.col_feat); return GF_ERR_CAPACITY; }
     double* imu_sqrt = (double*)malloc(sizeof(double) * 225 * (p->n_imu > 0 ? p->n_imu : 1));
     for (int k = 0; k < p->n_imu; k++) gfo_sqrt_info(p->imu[k].covariance, 15, imu_sqrt + 225 * k);
     state_t x; state_load(p, &x);
@@ -1343,6 +1353,7 @@ GFO void gfo_ba_plus(const gf_ba_problem* p, const double* delta)
  * sw and the wheel time offset follow as kept blocks.  out_x0 / out_J / out_r must hold 16F+19, n*n, n doubles. */
 static int marg_run(const gf_ba_problem* p, int second_new, gf_ba_prior* out, double* out_x0, double* out_J, double* out_r)
 {
+    if (same_frame_visual(p)) return GF_ERR_INVALID_ARG;
     const int F = p->n_frames;
     const int use_sb = (p->para_speed_bias != NULL) && !p->pose0_const;
     state_t s; state_load(p, &s);

@@ -63,7 +63,7 @@ def linearize(pb, cap_rows=6000, cap_cols=600):
     nc = ctypes.c_int(0)
     rows = lib().gfo_ba_linearize(ctypes.byref(p), r.ctypes.data_as(_dp), J.ctypes.data_as(_dp), ctypes.byref(nc), cap_rows, cap_cols)
     if rows < 0:
-        raise RuntimeError("capacity")
+        raise RuntimeError("oracle linearisation failed: %d (-1: invalid window, -4: capacity)" % rows)
     n = nc.value
     return r[:rows].copy(), J[:rows * n].reshape(rows, n).copy()
 
