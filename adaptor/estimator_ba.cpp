@@ -1,6 +1,6 @@
 // Estimator::optimization() (vins_estimator/src/estimator/estimator.cpp:2884-3631) on libgf_b200.so: vector2double's arrays
 // are handed to gf_ba_solve (gf_ba_solve_multi for several estimators) as they are, the AddResidualBlock loops become descriptor rows, and the MARGIN_OLD /
-// MARGIN_SECOND_NEW branches become one call each.  Wheel, plane and GNSS blocks follow the same pattern (INTEGRATION.md);
+// MARGIN_SECOND_NEW branches become one call each (one gf_ba_marginalize_multi call for several estimators).  Wheel, plane and GNSS blocks follow the same pattern (INTEGRATION.md);
 // this file carries the camera + IMU case the reference's default configs run.
 #include "estimator_ba.h"
 
@@ -105,8 +105,9 @@ void Estimator::optimization()
 }
 
 // Several estimators (one per robot / camera rig served by this GPU) at the same point of their processImage: every window is
-// built as optimization() builds it, all are solved by one gf_ba_solve_multi call from this thread, then each estimator runs its
-// own marginalisation.  The same blocks and priors as calling optimization() on each in turn.
+// built as optimization() builds it, all are solved by one gf_ba_solve_multi call from this thread, then all are marginalised
+// by one gf_ba_marginalize_multi call, each as its own marginalization_flag says.  The same blocks and priors as calling
+// optimization() on each in turn.
 void Estimator::optimizationMulti(Estimator *const *est, int n)
 {
     std::vector<BaRows> rows(n);
@@ -118,10 +119,20 @@ void Estimator::optimizationMulti(Estimator *const *est, int n)
         P[k] = rows[k].P; handles[k] = est[k]->gf_ba_;
     }
     if (gf_ba_solve_multi(handles.data(), n, P.data(), S.data(), nullptr)) gf_fatal("gf_ba_solve_multi");
+    std::vector<int32_t> modes(n), kept(n);
+    std::vector<gf_ba_prior> next(n);
+    std::vector<std::vector<double>> x0(n), J(n), r(n);
+    std::vector<double *> px0(n), pJ(n), pr(n);
     for (int k = 0; k < n; k++) {
         est[k]->last_summary = S[k];
-        est[k]->marginalize(P[k]);
+        modes[k] = est[k]->marginalization_flag == MARGIN_OLD ? GF_BA_MARGIN_OLD : GF_BA_MARGIN_SECOND_NEW;
+        const size_t cap = 16 * (size_t)P[k].n_frames + 24;
+        x0[k].resize(cap); J[k].resize(cap * cap); r[k].resize(cap);
+        px0[k] = x0[k].data(); pJ[k] = J[k].data(); pr[k] = r[k].data();
     }
+    if (gf_ba_marginalize_multi(handles.data(), n, P.data(), modes.data(), next.data(), px0.data(), pJ.data(), pr.data(), kept.data(), nullptr))
+        gf_fatal("gf_ba_marginalize_multi");
+    for (int k = 0; k < n; k++) est[k]->adoptPrior(kept[k], next[k], x0[k], J[k], r[k]);
 }
 
 // MARGIN_OLD / MARGIN_SECOND_NEW at the end of optimization(): the prior of the next window
@@ -136,10 +147,16 @@ void Estimator::marginalize(const gf_ba_problem &P)
     else                                                                     // :3536-3631
         n = gf_ba_marginalize_second_new(gf_ba_, &P, &next, x0.data(), J.data(), r.data(), nullptr);
     if (n < 0) gf_fatal("marginalisation");
-    if (n > 0) {                                   // n == 0: MARGIN_SECOND_NEW with a prior that does not hold the pose -> keep it
-        prior_x0_.swap(x0); prior_J_.swap(J); prior_r_.swap(r);
-        prior_ = next;
-        prior_.x0 = prior_x0_.data(); prior_.linearized_jacobians = prior_J_.data(); prior_.linearized_residuals = prior_r_.data();
-        have_prior_ = true;
-    }
+    adoptPrior(n, next, x0, J, r);
+}
+
+// The marginalisation's result (n = its return value) becomes the prior of the next window; x0, J, r are the buffers `next`
+// points into and are taken over
+void Estimator::adoptPrior(int n, const gf_ba_prior &next, std::vector<double> &x0, std::vector<double> &J, std::vector<double> &r)
+{
+    if (n == 0) return;                            // MARGIN_SECOND_NEW with a prior that does not hold the pose -> keep it
+    prior_x0_.swap(x0); prior_J_.swap(J); prior_r_.swap(r);
+    prior_ = next;
+    prior_.x0 = prior_x0_.data(); prior_.linearized_jacobians = prior_J_.data(); prior_.linearized_residuals = prior_r_.data();
+    have_prior_ = true;
 }

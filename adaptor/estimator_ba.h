@@ -73,6 +73,7 @@ class Estimator
     };
     void buildProblem(BaRows &rows);
     void marginalize(const gf_ba_problem &P);
+    void adoptPrior(int n, const gf_ba_prior &next, std::vector<double> &x0, std::vector<double> &J, std::vector<double> &r);
     gf_ba *gf_ba_ = nullptr;
     // last_marginalization_info + last_marginalization_parameter_blocks (estimator.h:318-319)
     bool have_prior_ = false;

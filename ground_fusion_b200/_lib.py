@@ -162,3 +162,5 @@ BLOCK_EX_WHEEL, BLOCK_SX, BLOCK_SY, BLOCK_SW, BLOCK_TD_WHEEL = 4, 5, 6, 7, 8
 BLOCK_PLANE_R, BLOCK_PLANE_Z = 10, 11
 # GF_MARG_PATH_* bits (which way a marginalisation went)
 MARG_PATH_GENERIC, MARG_PATH_WIDE, MARG_PATH_NOT_PD, MARG_PATH_FORCED, MARG_PATH_REDUCED_JACOBI = 1, 2, 4, 8, 16
+# GF_BA_MARGIN_* (gf_ba_marginalize_multi's modes; Estimator::marginalization_flag)
+MARGIN_OLD, MARGIN_SECOND_NEW = 0, 1

@@ -963,10 +963,26 @@ __global__ void __launch_bounds__(RB_THREADS) k_ba_step(const BaDev* __restrict_
 // as a similarity A <- J^T A J with J = product of the plane rotations: the matrix splits into disjoint 2x2 blocks
 // (row pair x column pair), each updated independently from the two rotations involved.  V accumulates the rotations
 // (columns = eigenvectors), w = diagonal at convergence (off-norm <= 1e-30 * diag-norm, like the oracle's sweep test).
-__global__ void __launch_bounds__(1024) k_jacobi_eig(double* A, double* V, double* w, int n, int* sweeps_out)
+// One CTA per listed window (MargDev table below): which = 0 decomposes its Amm (m x m), 1 its reduced system (n x n).
+struct MargDev {
+    int N, m, n, c;               // c: the dense block of the fast path (pose0 [+ speedbias0])
+    const double *H, *Hp, *g;     // accumulated by k_ba_eval (N x N, N)
+    double *A, *b;                // N x N, N
+    double *Amm, *Vm, *wm, *Ainv; // m x m ...
+    double *T;                    // n x m
+    double *Ar, *Vr, *wr, *br;    // n x n ...
+    double *J0, *r0;
+    double *Q, *qb, *Ceps;        // fast path: (c+n)^2 system left after the landmarks, its rhs, the eps-shifted c x c block
+    int* sw;                      // [0], [1] Jacobi sweeps on Amm / on the reduced system, [2] the fast path's not-PD flag
+};
+
+__global__ void __launch_bounds__(1024) k_jacobi_eig(const MargDev* __restrict__ tab, const int* __restrict__ list, int which)
 {
     extern __shared__ double jsm[];           // c[np/2], s[np/2]; then int pr[np/2], qr[np/2]
     __shared__ double sred[32];
+    const MargDev q = tab[list[blockIdx.x]];
+    double* A = which ? q.Ar : q.Amm; double* V = which ? q.Vr : q.Vm; double* w = which ? q.wr : q.wm;
+    const int n = which ? q.n : q.m;
     const int tid = threadIdx.x, nt = blockDim.x;
     const int np = (n + 1) & ~1, hp = np / 2;
     double* cs_c = jsm; double* cs_s = jsm + hp;
@@ -1069,21 +1085,26 @@ __global__ void __launch_bounds__(1024) k_jacobi_eig(double* A, double* V, doubl
         }
     }
     for (int i = tid; i < n; i += nt) w[i] = A[(size_t)i * n + i];
-    if (tid == 0 && sweeps_out) *sweeps_out = sweep;
+    if (tid == 0) q.sw[which] = sweep;
 }
 
 // Symmetric eigendecomposition for the reduced system of the marginalisation (n <= 128): Householder tridiagonalisation +
 // implicit-shift QL (EISPACK tred2 / tql2, the algorithm family of Eigen's SelfAdjointEigenSolver; same restatement as
 // oracle/ba_oracle.c sym_eig_ql).  One CTA of 128 threads, V column-major in shared memory.  The Householder steps are
 // thread-parallel over rows/columns; in the QL phase thread 0 runs the scalar recurrence of a sweep and publishes the plane
-// rotations, then every thread applies them to its own row of V.
+// rotations, then every thread applies them to its own row of V.  One CTA per listed window, on its reduced system.
 constexpr int QL_T = 128;
-__global__ void __launch_bounds__(QL_T) k_sym_eig_ql(const double* __restrict__ Ag, double* __restrict__ Vg, double* __restrict__ wg, int n)
+__global__ void __launch_bounds__(QL_T) k_sym_eig_ql(const MargDev* __restrict__ tab, const int* __restrict__ list)
 {
     extern __shared__ double qsm[];          // V[n*n] | d[n] | e[n+1] | rc[n] | rs[n]
     __shared__ double sred[32];
     __shared__ double sh_h, sh_scale, sh_hh;
     __shared__ int sh_m, sh_more;
+    const MargDev q = tab[list[blockIdx.x]];
+    const double* __restrict__ Ag = q.Ar;
+    double* __restrict__ Vg = q.Vr;
+    double* __restrict__ wg = q.wr;
+    const int n = q.n;
     double* V = qsm; double* d = V + (size_t)n * n; double* e = d + n; double* rc = e + n + 1; double* rs = rc + n;
     const int tid = threadIdx.x;
 #define VV(i, j) V[(size_t)(j) * n + (i)]
@@ -1220,50 +1241,49 @@ __global__ void __launch_bounds__(QL_T) k_sym_eig_ql(const double* __restrict__ 
 #undef VV
 }
 
-struct MargDev {
-    int N, m, n;
-    const double *H, *Hp, *g;     // accumulated by k_ba_eval (N x N, N)
-    double *A, *b;                // N x N, N
-    double *Amm, *Vm, *wm, *Ainv; // m x m ...
-    double *T;                    // n x m
-    double *Ar, *Vr, *wr, *br;    // n x n ...
-    double *J0, *r0;
-};
-
-__global__ void k_marg_pack(MargDev q)
+// The k_marg_* kernels serve a batch of windows (gf_ba_marginalize_multi; the single calls are the batch of one): tab holds
+// every window's descriptor, list the windows a launch serves (window = list[blockIdx.y]).  The grid is the largest over the
+// listed windows and each thread exits against its own window's sizes.
+#define MARG_WINDOW() const MargDev q = tab[list[blockIdx.y]]; const int e = blockIdx.x * blockDim.x + threadIdx.x
+__global__ void k_marg_pack(const MargDev* __restrict__ tab, const int* __restrict__ list)
 {
-    const int e = blockIdx.x * blockDim.x + threadIdx.x, N = q.N;
+    MARG_WINDOW();
+    const int N = q.N;
     if (e < N * N) q.A[e] = q.H[e] + q.Hp[e];
     if (e < N) q.b[e] = q.g[e];
 }
-__global__ void k_marg_amm(MargDev q)      // Amm = 0.5 (Amm + Amm^T)   (marginalization_factor.cpp:278)
+__global__ void k_marg_amm(const MargDev* __restrict__ tab, const int* __restrict__ list)      // Amm = 0.5 (Amm + Amm^T)   (marginalization_factor.cpp:278)
 {
-    const int e = blockIdx.x * blockDim.x + threadIdx.x, m = q.m, N = q.N;
+    MARG_WINDOW();
+    const int m = q.m, N = q.N;
     if (e >= m * m) return;
     const int i = e / m, j = e - i * m;
     q.Amm[e] = 0.5 * (q.A[(size_t)i * N + j] + q.A[(size_t)j * N + i]);
 }
-__global__ void k_marg_ainv(MargDev q)     // Amm_inv = V diag(w > eps ? 1/w : 0) V^T     (:279-283)
+__global__ void k_marg_ainv(const MargDev* __restrict__ tab, const int* __restrict__ list)     // Amm_inv = V diag(w > eps ? 1/w : 0) V^T     (:279-283)
 {
-    const int e = blockIdx.x * blockDim.x + threadIdx.x, m = q.m;
+    MARG_WINDOW();
+    const int m = q.m;
     if (e >= m * m) return;
     const int i = e / m, j = e - i * m;
     double v = 0;
     for (int k = 0; k < m; k++) { const double wk = q.wm[k]; if (wk > 1e-8) v += q.Vm[(size_t)i * m + k] * (1.0 / wk) * q.Vm[(size_t)j * m + k]; }
     q.Ainv[e] = v;
 }
-__global__ void k_marg_T(MargDev q)        // T = Arm Amm_inv
+__global__ void k_marg_T(const MargDev* __restrict__ tab, const int* __restrict__ list)        // T = Arm Amm_inv
 {
-    const int e = blockIdx.x * blockDim.x + threadIdx.x, m = q.m, n = q.n, N = q.N;
+    MARG_WINDOW();
+    const int m = q.m, n = q.n, N = q.N;
     if (e >= n * m) return;
     const int i = e / m, j = e - i * m;
     double v = 0;
     for (int k = 0; k < m; k++) v += q.A[(size_t)(m + i) * N + k] * q.Ainv[(size_t)k * m + j];
     q.T[e] = v;
 }
-__global__ void k_marg_reduce(MargDev q)   // A = Arr - Arm Amm_inv Amr, b = brr - Arm Amm_inv bmm   (:286-292); lower triangle mirrored
+__global__ void k_marg_reduce(const MargDev* __restrict__ tab, const int* __restrict__ list)   // A = Arr - Arm Amm_inv Amr, b = brr - Arm Amm_inv bmm   (:286-292); lower triangle mirrored
 {
-    const int e = blockIdx.x * blockDim.x + threadIdx.x, m = q.m, n = q.n, N = q.N;
+    MARG_WINDOW();
+    const int m = q.m, n = q.n, N = q.N;
     if (e < n * n) {
         const int i = e / n, j = e - i * n;
         if (j <= i) {
@@ -1278,12 +1298,13 @@ __global__ void k_marg_reduce(MargDev q)   // A = Arr - Arm Amm_inv Amr, b = brr
 // When Amm - eps I is positive definite every eigenvalue passes the reference's eps test, the eigen-truncated inverse IS
 // the inverse, and Arr - Arm Amm^-1 Amr is the ordinary two-stage Schur complement: landmarks (1x1 pivots) first, then
 // the c x c block of pose0 / speedbias0.  Q is the (c+n) x (c+n) system left after the landmarks, order [c | kept].
-// flag[0] is set when the positive-definiteness test fails (the generic Jacobi path is run instead).  Launched with at least
-// max(R^2, m) threads: thread e < R^2 forms Q[e], thread c <= e < m tests landmark pivot e.
-__global__ void k_marg_lm_elim(MargDev q, int c, double* Q, double* qb, double* Ceps, int* flag)
+// sw[2] is set when the positive-definiteness test fails (the generic Jacobi path is run instead).  Launched with at least
+// max(R^2, m) threads per window: thread e < R^2 forms Q[e], thread c <= e < m tests landmark pivot e.
+__global__ void k_marg_lm_elim(const MargDev* __restrict__ tab, const int* __restrict__ list)
 {
-    const int R = c + q.n, m = q.m, N = q.N;
-    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    MARG_WINDOW();
+    const int c = q.c, R = c + q.n, m = q.m, N = q.N;
+    double *Q = q.Q, *qb = q.qb, *Ceps = q.Ceps;
     auto gi = [&](int i) { return i < c ? i : m + (i - c); };       // compact index -> column of A
     if (e < R * R) {
         const int i = e / R, j = e - i * R, ai = gi(i), aj = gi(j);
@@ -1303,14 +1324,17 @@ __global__ void k_marg_lm_elim(MargDev q, int c, double* Q, double* qb, double* 
         for (int l = c; l < m; l++) v -= 0.5 * (q.A[(size_t)ai * N + l] + q.A[(size_t)l * N + ai]) * q.b[l] / q.A[(size_t)l * N + l];
         qb[e] = v;
     }
-    if (e >= c && e < m && !(q.A[(size_t)e * N + e] - 1e-8 > 0.0)) atomicExch(flag, 1);
+    if (e >= c && e < m && !(q.A[(size_t)e * N + e] - 1e-8 > 0.0)) atomicExch(q.sw + 2, 1);
 }
-// single CTA: Cholesky of the c x c block (and of its eps-shifted twin for the test), X = S^-1 [Q_cr | q_c], reduced system
-__global__ void __launch_bounds__(256) k_marg_c_elim(MargDev q, int c, const double* Q, const double* qb, const double* Ceps, int* flag)
+// one CTA per window: Cholesky of the c x c block (and of its eps-shifted twin for the test), X = S^-1 [Q_cr | q_c], reduced system
+__global__ void __launch_bounds__(256) k_marg_c_elim(const MargDev* __restrict__ tab, const int* __restrict__ list)
 {
     __shared__ double Lc[15 * 15], Le[15 * 15];
     __shared__ double X[15 * 128];            // c x (n + 1), n <= 127
-    const int tid = threadIdx.x, n = q.n, R = c + n;
+    const MargDev q = tab[list[blockIdx.y]];
+    const int tid = threadIdx.x, n = q.n, c = q.c, R = c + n;
+    const double *Q = q.Q, *qb = q.qb, *Ceps = q.Ceps;
+    int* flag = q.sw + 2;
     if (tid == 0) {
         bool ok = true;
         for (int pass = 0; pass < 2 && ok; pass++) {
@@ -1349,9 +1373,10 @@ __global__ void __launch_bounds__(256) k_marg_c_elim(MargDev q, int c, const dou
     }
 }
 
-__global__ void k_marg_out(MargDev q)      // J0 = sqrt(S) V^T, r0 = sqrt(S^-1) V^T b     (:294-302)
+__global__ void k_marg_out(const MargDev* __restrict__ tab, const int* __restrict__ list)      // J0 = sqrt(S) V^T, r0 = sqrt(S^-1) V^T b     (:294-302)
 {
-    const int e = blockIdx.x * blockDim.x + threadIdx.x, n = q.n;
+    MARG_WINDOW();
+    const int n = q.n;
     if (e < n * n) {
         const int k = e / n, i = e - k * n;
         const double S = q.wr[k] > 1e-8 ? q.wr[k] : 0.0;
@@ -1363,6 +1388,7 @@ __global__ void k_marg_out(MargDev q)      // J0 = sqrt(S) V^T, r0 = sqrt(S^-1) 
         q.r0[e] = sqrt(Si) * vb;
     }
 }
+#undef MARG_WINDOW
 
 }  // namespace gfba
 
@@ -1889,77 +1915,145 @@ int gf_ba_solve_multi(gf_ba* const* solvers, int n, const gf_ba_problem* problem
  * Returns n (> 0) or a negative error code. */
 }  // extern "C" (reopened below)
 
-// MarginalizationInfo::marginalize (marginalization_factor.cpp:272-302) on the dense system q.A, q.b already on the device,
-// columns [c dense | m - c diagonal landmarks | n kept]: the structured fast path when it applies, else the literal
-// eigen-truncated inverse of Amm; then the eigendecomposition of the reduced system and J0, r0.  d_sw: int[3] on the device
-// ([0], [1] Jacobi sweeps of Amm and of the reduced system, [2] the fast path's flag), h_flag: one host int (pinned in marg_run).  Host
-// synchronisation: one, to read the fast path's flag.  *path: GF_MARG_PATH_* bits.
-static int marg_schur_eig(const MargDev& q, int cdim, bool force_generic, double* Q, double* qb, double* Ceps, int* d_sw, int* h_flag,
-                          cudaStream_t st, int* path)
+// MarginalizationInfo::marginalize (marginalization_factor.cpp:272-302) on the dense systems of a batch of windows already on
+// the device (q.A, q.b; columns [c dense | m - c diagonal landmarks | n kept]): the structured fast path on the windows it
+// applies to, the literal eigen-truncated inverse of Amm on the others, then the eigendecomposition of every reduced system
+// and J0, r0.  Each kernel is launched once for the windows of its list, so the launch count depends on which paths occur and
+// not on the number of windows.  Host synchronisation: one when some window tries the fast path, to read every flag at once.
+enum { MARG_ALL, MARG_FAST, MARG_LITERAL, MARG_QL, MARG_JACOBI, MARG_LISTS };
+struct MargBatch {
+    int n;                        // windows
+    const MargDev* hq;            // their descriptors (host) ...
+    const MargDev* dq;            // ... and the same table on the device
+    int* hl; const int* dl;       // MARG_LISTS lists of n window indices each: host staging (uploaded before the chain), device
+    int cnt[MARG_LISTS];
+    int* hsw; const int* dsw;     // int[4] per window (MargDev::sw), zero before the chain: host staging, device
+};
+
+// The window lists and each window's path bits before anything runs; the literal list grows once the fast path's flags are read
+static void marg_plan(MargBatch& b, bool force_generic, int* paths)
 {
-    const int m = q.m, n = q.n, Rdim = cdim + n;
-    const size_t mm = (size_t)m * m, nn = (size_t)n * n;
+    const int n = b.n;
+    for (int s = 0; s < MARG_LISTS; s++) b.cnt[s] = 0;
+    auto put = [&](int s, int k) { b.hl[s * n + b.cnt[s]++] = k; };
+    for (int k = 0; k < n; k++) {
+        const int nk = b.hq[k].n;
+        int p = nk > 127 ? GF_MARG_PATH_GENERIC | GF_MARG_PATH_WIDE                // k_marg_c_elim's shared buffer
+              : force_generic ? GF_MARG_PATH_GENERIC | GF_MARG_PATH_FORCED : 0;
+        put(MARG_ALL, k);
+        put(p ? MARG_LITERAL : MARG_FAST, k);
+        if (nk <= 128) put(MARG_QL, k);   // tridiagonalisation + implicit QL in shared memory (what the reference's Eigen solver does)
+        else { put(MARG_JACOBI, k); p |= GF_MARG_PATH_REDUCED_JACOBI; }
+        paths[k] = p;
+    }
+}
+
+static int marg_schur_eig(MargBatch& b, cudaStream_t st, int* paths)
+{
+    const int n = b.n;
+    const MargDev* dq = b.dq;
+    auto dlist = [&](int s) { return b.dl + (size_t)s * n; };
+    // 256-thread CTAs for the largest work(window) of list s, one grid row per listed window
+    auto grid = [&](int s, auto work) {
+        size_t mx = 1;
+        for (int i = 0; i < b.cnt[s]; i++) mx = std::max(mx, (size_t)work(b.hq[b.hl[s * n + i]]));
+        return dim3((unsigned)((mx + 255) / 256), (unsigned)b.cnt[s]);
+    };
+    auto smem = [&](int s, auto bytes) {
+        size_t mx = 0;
+        for (int i = 0; i < b.cnt[s]; i++) mx = std::max(mx, (size_t)bytes(b.hq[b.hl[s * n + i]]));
+        return mx;
+    };
     auto jac_smem = [](int nn_) { int hp = ((nn_ + 1) & ~1) / 2; return (size_t)hp * (2 * sizeof(double) + 2 * sizeof(int)) + 8; };
-    int* d_flag = d_sw + 2;
-    int p = n > 127 ? GF_MARG_PATH_GENERIC | GF_MARG_PATH_WIDE                 // k_marg_c_elim's shared buffer
-          : force_generic ? GF_MARG_PATH_GENERIC | GF_MARG_PATH_FORCED : 0;
-    if (!p) {
+    if (b.cnt[MARG_FAST]) {
         // regular case: Amm - eps I positive definite => eigen-truncated inverse == inverse => two-stage Schur complement
-        GF_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(int), st));
-        k_marg_lm_elim<<<(std::max(Rdim * Rdim, m) + 255) / 256, 256, 0, st>>>(q, cdim, Q, qb, Ceps, d_flag); GF_LAUNCHED();
-        k_marg_c_elim<<<1, 256, 0, st>>>(q, cdim, Q, qb, Ceps, d_flag); GF_LAUNCHED();
-        GF_CUDA(cudaMemcpyAsync(h_flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+        const int* l = dlist(MARG_FAST);
+        k_marg_lm_elim<<<grid(MARG_FAST, [](const MargDev& q) { return std::max((q.c + q.n) * (q.c + q.n), q.m); }), 256, 0, st>>>(dq, l); GF_LAUNCHED();
+        k_marg_c_elim<<<dim3(1, b.cnt[MARG_FAST]), 256, 0, st>>>(dq, l); GF_LAUNCHED();
+        GF_CUDA(cudaMemcpyAsync(b.hsw, b.dsw, sizeof(int) * 4 * (size_t)n, cudaMemcpyDeviceToHost, st));
         GF_CUDA(cudaStreamSynchronize(st));
-        if (*h_flag != 0) p = GF_MARG_PATH_GENERIC | GF_MARG_PATH_NOT_PD;
+        const int lit0 = b.cnt[MARG_LITERAL];
+        for (int i = 0; i < b.cnt[MARG_FAST]; i++) {
+            const int k = b.hl[MARG_FAST * n + i];
+            if (b.hsw[4 * k + 2] != 0) { paths[k] |= GF_MARG_PATH_GENERIC | GF_MARG_PATH_NOT_PD; b.hl[MARG_LITERAL * n + b.cnt[MARG_LITERAL]++] = k; }
+        }
+        if (b.cnt[MARG_LITERAL] > lit0)
+            GF_CUDA(cudaMemcpyAsync((int*)dlist(MARG_LITERAL) + lit0, b.hl + MARG_LITERAL * n + lit0, sizeof(int) * (b.cnt[MARG_LITERAL] - lit0),
+                                    cudaMemcpyHostToDevice, st));
     }
-    if (p & GF_MARG_PATH_GENERIC) {   // some eigenvalue of Amm may be below eps: the reference's eigen-truncated inverse, literally
-        k_marg_amm<<<(int)((mm + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
-        k_jacobi_eig<<<1, 1024, jac_smem(m), st>>>(q.Amm, q.Vm, q.wm, m, d_sw); GF_LAUNCHED();
-        k_marg_ainv<<<(int)((mm + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
-        k_marg_T<<<(int)(((size_t)n * m + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
-        k_marg_reduce<<<(int)((nn + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
+    if (b.cnt[MARG_LITERAL]) {   // some eigenvalue of Amm may be below eps: the reference's eigen-truncated inverse, literally
+        const int* l = dlist(MARG_LITERAL);
+        k_marg_amm<<<grid(MARG_LITERAL, [](const MargDev& q) { return q.m * q.m; }), 256, 0, st>>>(dq, l); GF_LAUNCHED();
+        k_jacobi_eig<<<b.cnt[MARG_LITERAL], 1024, smem(MARG_LITERAL, [&](const MargDev& q) { return jac_smem(q.m); }), st>>>(dq, l, 0); GF_LAUNCHED();
+        k_marg_ainv<<<grid(MARG_LITERAL, [](const MargDev& q) { return q.m * q.m; }), 256, 0, st>>>(dq, l); GF_LAUNCHED();
+        k_marg_T<<<grid(MARG_LITERAL, [](const MargDev& q) { return q.n * q.m; }), 256, 0, st>>>(dq, l); GF_LAUNCHED();
+        k_marg_reduce<<<grid(MARG_LITERAL, [](const MargDev& q) { return q.n * q.n; }), 256, 0, st>>>(dq, l); GF_LAUNCHED();
     }
-    if (n <= 128) {   // tridiagonalisation + implicit QL in shared memory (what the reference's Eigen solver does)
-        k_sym_eig_ql<<<1, QL_T, sizeof(double) * ((size_t)n * n + 4 * (size_t)n + 8), st>>>(q.Ar, q.Vr, q.wr, n); GF_LAUNCHED();
-    } else {
-        k_jacobi_eig<<<1, 1024, jac_smem(n), st>>>(q.Ar, q.Vr, q.wr, n, d_sw + 1); GF_LAUNCHED();
-        p |= GF_MARG_PATH_REDUCED_JACOBI;
+    if (b.cnt[MARG_QL]) {
+        k_sym_eig_ql<<<b.cnt[MARG_QL], QL_T, smem(MARG_QL, [](const MargDev& q) { return sizeof(double) * ((size_t)q.n * q.n + 4 * (size_t)q.n + 8); }), st>>>(dq, dlist(MARG_QL));
+        GF_LAUNCHED();
     }
-    k_marg_out<<<(int)((nn + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
+    if (b.cnt[MARG_JACOBI]) {
+        k_jacobi_eig<<<b.cnt[MARG_JACOBI], 1024, smem(MARG_JACOBI, [&](const MargDev& q) { return jac_smem(q.n); }), st>>>(dq, dlist(MARG_JACOBI), 1);
+        GF_LAUNCHED();
+    }
+    k_marg_out<<<grid(MARG_ALL, [](const MargDev& q) { return q.n * q.n; }), 256, 0, st>>>(dq, dlist(MARG_ALL)); GF_LAUNCHED();
     GF_CUDA(cudaGetLastError());
-    *path = p;
     return GF_OK;
 }
 
-enum { GF_MARG_OLD = 0, GF_MARG_SECOND_NEW = 1 };
-static int marg_run(gf_ba* s, const gf_ba_problem* p, int mode, gf_ba_prior* out, double* out_x0, double* out_J, double* out_r, float* device_ms)
+// ------------------------------------------------------------------------------------------------
+// One marginalisation in three parts, shared by the single calls (the batch of one) and gf_ba_marginalize_multi:
+//   marg_layout   argument checks, the marginalised and kept blocks and the buffer layout of one window (host only)
+//   marg_pack     the window's upload image in its handle's pinned buffer, and its BaDev / MargDev descriptors
+//   marg_finish   the prior for the next window (kept blocks after addr_shift, J0, r0) from the downloaded image
+enum { GF_MARG_OLD = GF_BA_MARGIN_OLD, GF_MARG_SECOND_NEW = GF_BA_MARGIN_SECOND_NEW };
+struct MargWindow {
+    BaDev d;                                   // device pointers are set by marg_pack
+    MargDev q;
+    bool old_, skip;                           // skip: MARGIN_SECOND_NEW and the prior does not hold the pose (the call returns 0)
+    int F, fdrop, m, n, N, cdim, pn, n_work;
+    std::vector<int> lm_col, start, work_start, work_ij, pcol;
+    std::vector<gf_ba_visual_factor> vis0;
+    const gf_ba_imu_factor* imu01;
+    const gf_ba_wheel_factor* wheel01;
+    size_t px0_len;
+    size_t o_X, o_vis, o_imu, o_whl, o_plf, o_ps, o_pij, o_cf, o_pJ, o_pr0, o_px0, o_pcol, o_st, upload_bytes;
+    size_t o_J0, o_r0, o_sq, o_Hp, o_a0, o_A, o_b, o_Amm, o_Vm, o_wm, o_Ainv, o_T, o_Ar, o_Vr, o_wr, o_br, o_sw, o_Q, o_qb, o_ce, bytes;
+    size_t base;                               // offset of the window in its handle's buffers (the batch table comes first in the lead handle's)
+};
+
+static int marg_layout(const gf_ba_problem* p, int mode, MargWindow& w)
 {
-    if (!s || !p || !out || !out_x0 || !out_J || !out_r) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    if (!p) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    if (mode != GF_MARG_OLD && mode != GF_MARG_SECOND_NEW) return set_err(GF_ERR_INVALID_ARG, "unknown marginalisation mode");
     if (p->n_frames < 2 || p->n_frames > GF_BA_MAX_FRAMES) return set_err(GF_ERR_INVALID_ARG, "n_frames out of range");
-    GF_CUDA(cudaSetDevice(s->device));
     const int F = p->n_frames, nfeat = p->n_features;
     const bool use_sb = p->para_speed_bias && !p->pose0_const;
     // a residual block may not list one parameter block twice (ceres::Problem refuses it; the reference never builds one)
     for (int v = 0; v < p->n_visual; v++) if (p->visual[v].imu_i == p->visual[v].imu_j) return set_err(GF_ERR_INVALID_ARG, "visual factor with imu_i == imu_j");
     // ---- the marginalised and the kept blocks (same rules as the oracle) ----
-    std::vector<int> lm_col(nfeat > 0 ? nfeat : 1, -1);
+    std::vector<int>& lm_col = w.lm_col;
+    lm_col.assign(nfeat > 0 ? nfeat : 1, -1);
     int pos = 0;
-    BaDev d; memset(&d, 0, sizeof(d));
+    BaDev& d = w.d; memset(&d, 0, sizeof(d));
     d.F = F; d.nfeat = nfeat; d.lm_dense = 1;
     for (int f = 0; f < MAXF; f++) { d.col_pose[f] = -1; d.col_sb[f] = -1; }
     d.col_ex = d.col_td = d.col_exw = d.col_tdw = -1; d.col_ix[0] = d.col_ix[1] = d.col_ix[2] = -1; d.col_pr = d.col_pz = -1; d.n_plane = 0;
     const bool old_ = mode == GF_MARG_OLD;
     const int fdrop = old_ ? 0 : F - 2;                        // MARGIN_OLD drops frame 0, MARGIN_SECOND_NEW para_Pose[WINDOW_SIZE - 1]
+    w.old_ = old_; w.F = F; w.fdrop = fdrop; w.skip = false;
     const gf_ba_prior* pr = (p->prior && p->prior->n > 0) ? p->prior : nullptr;
     if (!old_) {
         // estimator.cpp:3538-3539: only when the last prior holds para_Pose[WINDOW_SIZE - 1]; otherwise the prior stays as it is
         bool has = false;
         if (pr) for (int b = 0; b < pr->n_blocks; b++) if (pr->block_kind[b] == GF_BA_BLOCK_POSE && pr->block_index[b] == fdrop) has = true;
-        if (!has) return 0;
+        if (!has) { w.skip = true; return GF_OK; }
     }
     d.col_pose[fdrop] = pos; pos += 6;
     if (old_ && use_sb) { d.col_sb[0] = pos; pos += 9; }
-    std::vector<gf_ba_visual_factor> vis0;
+    std::vector<gf_ba_visual_factor>& vis0 = w.vis0;
+    vis0.clear();
     for (int v = 0; old_ && v < p->n_visual; v++) {
         const gf_ba_visual_factor& f = p->visual[v];
         if (f.feature < 0 || f.feature >= nfeat || f.imu_i < 0 || f.imu_i >= F || f.imu_j < 0 || f.imu_j >= F) return set_err(GF_ERR_INVALID_ARG, "visual factor index out of range");
@@ -1984,13 +2078,13 @@ static int marg_run(gf_ba* s, const gf_ba_problem* p, int mode, gf_ba_prior* out
             else return set_err(GF_ERR_INVALID_ARG, "unknown prior block kind");
         }
     }
-    const gf_ba_imu_factor* imu01 = nullptr;
-    for (int k = 0; old_ && k < p->n_imu; k++) if (p->imu[k].i == 0 && p->imu[k].j == 1 && p->imu[k].sum_dt < 10.0) { imu01 = &p->imu[k]; used_pose[1] = true; used_sb[1] = true; }
+    w.imu01 = nullptr;
+    for (int k = 0; old_ && k < p->n_imu; k++) if (p->imu[k].i == 0 && p->imu[k].j == 1 && p->imu[k].sum_dt < 10.0) { w.imu01 = &p->imu[k]; used_pose[1] = true; used_sb[1] = true; }
     for (const auto& f : vis0) { used_pose[f.imu_j] = true; used_ex = true; used_td = true; }
     // WheelFactor(pre_integrations_wheel[1]) with para_Pose[0] dropped (estimator.cpp:3367-3377)
-    const gf_ba_wheel_factor* wheel01 = nullptr;
+    w.wheel01 = nullptr;
     if (p->n_wheel > 0 && (!p->wheel || !p->para_ex_wheel || !p->para_ix_wheel || !p->para_td_wheel)) return set_err(GF_ERR_INVALID_ARG, "wheel factors without their parameter blocks");
-    for (int k = 0; old_ && k < p->n_wheel; k++) if (p->wheel[k].i == 0 && p->wheel[k].j == 1 && p->wheel[k].sum_dt < 10.0) { wheel01 = &p->wheel[k]; used_pose[1] = true; used_exw = true; used_ix[0] = used_ix[1] = used_ix[2] = true; used_tdw = true; }
+    for (int k = 0; old_ && k < p->n_wheel; k++) if (p->wheel[k].i == 0 && p->wheel[k].j == 1 && p->wheel[k].sum_dt < 10.0) { w.wheel01 = &p->wheel[k]; used_pose[1] = true; used_exw = true; used_ix[0] = used_ix[1] = used_ix[2] = true; used_tdw = true; }
     // PlaneFactor(para_Pose[0], para_Ex_Pose_wheel, para_plane_R, para_plane_Z) with para_Pose[0] dropped (estimator.cpp:3379-3390)
     bool plane0 = false;
     for (int k = 0; old_ && k < p->n_plane; k++) if (p->plane_frames && p->plane_frames[k] == 0) plane0 = true;
@@ -2014,19 +2108,23 @@ static int marg_run(gf_ba* s, const gf_ba_problem* p, int mode, gf_ba_prior* out
     if (used_pz) d.col_pz = pos++;
     const int N = pos, n = N - m;
     if (n <= 0) return set_err(GF_ERR_INVALID_ARG, "nothing is kept by the marginalisation");
-    d.nc = N; d.L = 0; d.n = N; d.n_vis = (int)vis0.size(); d.n_imu = imu01 ? 1 : 0; d.n_wheel = wheel01 ? 1 : 0; d.n_plane = plane0 ? 1 : 0;
+    w.m = m; w.n = n; w.N = N; w.cdim = (old_ && use_sb) ? 15 : 6;
+    d.nc = N; d.L = 0; d.n = N; d.n_vis = (int)vis0.size(); d.n_imu = w.imu01 ? 1 : 0; d.n_wheel = w.wheel01 ? 1 : 0; d.n_plane = plane0 ? 1 : 0;
     d.pr_mask = 0; for (int k = 0; k < 3; k++) d.plane_sinfo[k] = p->plane_sqrt_info[k];
     // ---- visual factors by pose pair (0, j), cut into chunks ----
-    std::vector<int> cnt(F, 0), start(F + 1, 0);
+    std::vector<int> cnt(F, 0);
+    w.start.assign(F + 1, 0);
     for (const auto& f : vis0) cnt[f.imu_j]++;
-    for (int j = 0; j < F; j++) start[j + 1] = start[j] + cnt[j];
-    std::vector<int> work_start(1, 0), work_ij;
+    for (int j = 0; j < F; j++) w.start[j + 1] = w.start[j] + cnt[j];
+    w.work_start.assign(1, 0); w.work_ij.clear();
     for (int j = 0; j < F; j++)
-        for (int c0 = start[j]; c0 < start[j + 1]; c0 += PAIR_CHUNK) { work_ij.push_back(0); work_ij.push_back(j); work_start.push_back(std::min(c0 + PAIR_CHUNK, start[j + 1])); }
-    const int n_work = (int)work_ij.size() / 2;
+        for (int c0 = w.start[j]; c0 < w.start[j + 1]; c0 += PAIR_CHUNK) { w.work_ij.push_back(0); w.work_ij.push_back(j); w.work_start.push_back(std::min(c0 + PAIR_CHUNK, w.start[j + 1])); }
+    const int n_work = (int)w.work_ij.size() / 2;
+    w.n_work = n_work;
     d.n_pairs = n_work;
     const int pn = pr ? pr->n : 0;
-    std::vector<int> pcol(pn > 0 ? pn : 1, -1);
+    w.pn = pn;
+    w.pcol.assign(pn > 0 ? pn : 1, -1);
     size_t px0_len = 0;
     if (pr) {
         d.pn = pn; d.pnb = pr->n_blocks;
@@ -2037,30 +2135,41 @@ static int marg_run(gf_ba* s, const gf_ba_problem* p, int mode, gf_ba_prior* out
             const int lc = kind == GF_BA_BLOCK_POSE ? d.col_pose[idx] : kind == GF_BA_BLOCK_SPEEDBIAS ? d.col_sb[idx] : kind == GF_BA_BLOCK_EX_POSE ? d.col_ex : kind == GF_BA_BLOCK_TD ? d.col_td
                            : kind == GF_BA_BLOCK_EX_WHEEL ? d.col_exw : kind == GF_BA_BLOCK_TD_WHEEL ? d.col_tdw : kind == GF_BA_BLOCK_PLANE_R ? d.col_pr : kind == GF_BA_BLOCK_PLANE_Z ? d.col_pz
                            : d.col_ix[kind - GF_BA_BLOCK_SX];
-            if (lc >= 0) for (int k = 0; k < ls; k++) pcol[pr->block_idx[b] + k] = lc + k;
+            if (lc >= 0) for (int k = 0; k < ls; k++) w.pcol[pr->block_idx[b] + k] = lc + k;
             px0_len += gs;
         }
     }
-    // ---- one upload buffer + work space ----
-    auto al = [](size_t v) { return (v + 15) / 16 * 16; };
+    w.px0_len = px0_len;
+    d.eval_grid = n_work + d.n_imu + d.n_wheel + d.n_plane + (pn ? 1 : 0);
+    // ---- offsets in the handle's buffers (relative to w.base): the upload, then the work space.  The solver state ends the
+    // upload and J0, r0 follow it, so that one download brings back everything the host reads ----
     size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += al(bytes); return o; };
+    auto take = [&](size_t bytes) { size_t o = off; off += al16(bytes); return o; };
     const size_t nv = vis0.size();
-    const size_t o_X = take(sizeof(double) * (X_FEAT + nfeat)), o_vis = take(sizeof(gf_ba_visual_factor) * (nv ? nv : 1)), o_imu = take(sizeof(gf_ba_imu_factor)), o_whl = take(sizeof(gf_ba_wheel_factor)), o_plf = take(sizeof(int) * 4),
-                 o_ps = take(sizeof(int) * (n_work + 1)), o_pij = take(sizeof(int) * 2 * (size_t)(n_work > 0 ? n_work : 1)), o_cf = take(sizeof(int) * (size_t)(nfeat > 0 ? nfeat : 1)),
-                 o_pJ = take(sizeof(double) * (size_t)pn * pn), o_pr0 = take(sizeof(double) * pn), o_px0 = take(sizeof(double) * px0_len), o_pcol = take(sizeof(int) * (size_t)(pn > 0 ? pn : 1));
-    const size_t o_st = take(sizeof(BaState)), o_dev = take(sizeof(BaDev));
-    const size_t upload_bytes = off;
+    w.o_X = take(sizeof(double) * (X_FEAT + nfeat)); w.o_vis = take(sizeof(gf_ba_visual_factor) * (nv ? nv : 1)); w.o_imu = take(sizeof(gf_ba_imu_factor));
+    w.o_whl = take(sizeof(gf_ba_wheel_factor)); w.o_plf = take(sizeof(int) * 4); w.o_ps = take(sizeof(int) * (n_work + 1));
+    w.o_pij = take(sizeof(int) * 2 * (size_t)(n_work > 0 ? n_work : 1)); w.o_cf = take(sizeof(int) * (size_t)(nfeat > 0 ? nfeat : 1));
+    w.o_pJ = take(sizeof(double) * (size_t)pn * pn); w.o_pr0 = take(sizeof(double) * pn); w.o_px0 = take(sizeof(double) * px0_len);
+    w.o_pcol = take(sizeof(int) * (size_t)(pn > 0 ? pn : 1)); w.o_st = take(sizeof(BaState));
+    w.upload_bytes = off;
     const size_t NN = (size_t)N * N, mm = (size_t)m * m, nn = (size_t)n * n;
-    const size_t o_sq = take(sizeof(double) * 225), o_Hp = take(sizeof(double) * NN), o_a0 = take(sizeof(double) * acc_size(N, 0)),
-                 o_A = take(sizeof(double) * NN), o_b = take(sizeof(double) * N), o_Amm = take(sizeof(double) * mm), o_Vm = take(sizeof(double) * mm), o_wm = take(sizeof(double) * m),
-                 o_Ainv = take(sizeof(double) * mm), o_T = take(sizeof(double) * (size_t)n * m), o_Ar = take(sizeof(double) * nn), o_Vr = take(sizeof(double) * nn),
-                 o_wr = take(sizeof(double) * n), o_br = take(sizeof(double) * n), o_J0 = take(sizeof(double) * nn), o_r0 = take(sizeof(double) * n), o_sw = take(sizeof(int) * 4),
-                 o_Q = take(sizeof(double) * (size_t)(15 + n) * (15 + n)), o_qb = take(sizeof(double) * (15 + n)), o_ce = take(sizeof(double) * 225);
-    int rc = ensure(s, off);
-    if (rc) return rc;
-    char* hb = (char*)s->hbuf; char* db = (char*)s->dbuf;
-    double* hX = (double*)(hb + o_X);
+    w.o_J0 = take(sizeof(double) * nn); w.o_r0 = take(sizeof(double) * n);
+    w.o_sq = take(sizeof(double) * 225); w.o_Hp = take(sizeof(double) * NN); w.o_a0 = take(sizeof(double) * acc_size(N, 0));
+    w.o_A = take(sizeof(double) * NN); w.o_b = take(sizeof(double) * N); w.o_Amm = take(sizeof(double) * mm); w.o_Vm = take(sizeof(double) * mm);
+    w.o_wm = take(sizeof(double) * m); w.o_Ainv = take(sizeof(double) * mm); w.o_T = take(sizeof(double) * (size_t)n * m);
+    w.o_Ar = take(sizeof(double) * nn); w.o_Vr = take(sizeof(double) * nn); w.o_wr = take(sizeof(double) * n); w.o_br = take(sizeof(double) * n);
+    w.o_Q = take(sizeof(double) * (size_t)(15 + n) * (15 + n)); w.o_qb = take(sizeof(double) * (15 + n)); w.o_ce = take(sizeof(double) * 225);
+    w.bytes = off;
+    return GF_OK;
+}
+
+// dsw: the window's int[4] in the batch table (MargDev::sw)
+static void marg_pack(gf_ba* s, const gf_ba_problem* p, MargWindow& w, int* dsw)
+{
+    const int F = p->n_frames, nfeat = p->n_features, pn = w.pn;
+    const gf_ba_prior* pr = pn ? p->prior : nullptr;
+    char* hb = (char*)s->hbuf + w.base; char* db = (char*)s->dbuf + w.base;
+    double* hX = (double*)(hb + w.o_X);
     memset(hX, 0, sizeof(double) * (X_FEAT + nfeat));
     memcpy(hX + X_POSE, p->para_pose, sizeof(double) * 7 * F);
     if (p->para_speed_bias) memcpy(hX + X_SB, p->para_speed_bias, sizeof(double) * 9 * F);
@@ -2071,71 +2180,57 @@ static int marg_run(gf_ba* s, const gf_ba_problem* p, int mode, gf_ba_prior* out
     if (p->para_ix_wheel && p->para_td_wheel) { memcpy(hX + X_IX, p->para_ix_wheel, sizeof(double) * 3); hX[X_TDW] = p->para_td_wheel[0]; }
     hX[X_PR + 3] = 1.0;
     if (p->para_plane_R && p->para_plane_Z) { memcpy(hX + X_PR, p->para_plane_R, sizeof(double) * 4); hX[X_PZ] = p->para_plane_Z[0]; }
-    ((int*)(hb + o_plf))[0] = 0;                               // the one PlaneFactor of the marginalisation sits on frame 0
+    ((int*)(hb + w.o_plf))[0] = 0;                             // the one PlaneFactor of the marginalisation sits on frame 0
     memcpy(hX + X_FEAT, p->para_feature, sizeof(double) * nfeat);
     {   // state: linearise into buffer 0 (k_ba_eval mode 0 also forms the sqrt-information of IMU(0->1))
-        BaState* h0 = (BaState*)(hb + o_st);
+        BaState* h0 = (BaState*)(hb + w.o_st);
         memset(h0, 0, sizeof(BaState));
         h0->radius = 1e4; h0->mu = 1e-8; h0->need_linearize = 1; h0->cur = 1; h0->first = 1;
     }
     {
-        gf_ba_visual_factor* hv = (gf_ba_visual_factor*)(hb + o_vis);
-        std::vector<int> fill(start.begin(), start.end() - 1);
-        for (const auto& f : vis0) hv[fill[f.imu_j]++] = f;
+        gf_ba_visual_factor* hv = (gf_ba_visual_factor*)(hb + w.o_vis);
+        std::vector<int> fill(w.start.begin(), w.start.end() - 1);
+        for (const auto& f : w.vis0) hv[fill[f.imu_j]++] = f;
     }
-    if (imu01) memcpy(hb + o_imu, imu01, sizeof(gf_ba_imu_factor));
-    if (wheel01) memcpy(hb + o_whl, wheel01, sizeof(gf_ba_wheel_factor));
-    memcpy(hb + o_ps, work_start.data(), sizeof(int) * (n_work + 1));
-    if (n_work) memcpy(hb + o_pij, work_ij.data(), sizeof(int) * 2 * n_work);
-    memcpy(hb + o_cf, lm_col.data(), sizeof(int) * (size_t)(nfeat > 0 ? nfeat : 1));
+    if (w.imu01) memcpy(hb + w.o_imu, w.imu01, sizeof(gf_ba_imu_factor));
+    if (w.wheel01) memcpy(hb + w.o_whl, w.wheel01, sizeof(gf_ba_wheel_factor));
+    memcpy(hb + w.o_ps, w.work_start.data(), sizeof(int) * (w.n_work + 1));
+    if (w.n_work) memcpy(hb + w.o_pij, w.work_ij.data(), sizeof(int) * 2 * w.n_work);
+    memcpy(hb + w.o_cf, w.lm_col.data(), sizeof(int) * (size_t)(nfeat > 0 ? nfeat : 1));
     if (pr) {
-        memcpy(hb + o_pJ, pr->linearized_jacobians, sizeof(double) * (size_t)pn * pn);
-        memcpy(hb + o_pr0, pr->linearized_residuals, sizeof(double) * pn);
-        memcpy(hb + o_px0, pr->x0, sizeof(double) * px0_len);
-        memcpy(hb + o_pcol, pcol.data(), sizeof(int) * pn);
+        memcpy(hb + w.o_pJ, pr->linearized_jacobians, sizeof(double) * (size_t)pn * pn);
+        memcpy(hb + w.o_pr0, pr->linearized_residuals, sizeof(double) * pn);
+        memcpy(hb + w.o_px0, pr->x0, sizeof(double) * w.px0_len);
+        memcpy(hb + w.o_pcol, w.pcol.data(), sizeof(int) * pn);
     }
-    d.X = (double*)(db + o_X); d.Xc = d.X;
-    d.vis = (const gf_ba_visual_factor*)(db + o_vis); d.pair_start = (const int*)(db + o_ps); d.pair_ij = (const int*)(db + o_pij);
-    d.imu = (const gf_ba_imu_factor*)(db + o_imu); d.imu_sqrt = (double*)(db + o_sq); d.wheel = (const gf_ba_wheel_factor*)(db + o_whl);
-    d.plane_frames = (const int*)(db + o_plf);
-    d.col_feat = (const int*)(db + o_cf);
-    d.pJ = (const double*)(db + o_pJ); d.pr0 = (const double*)(db + o_pr0); d.px0 = (const double*)(db + o_px0); d.pcol = (const int*)(db + o_pcol);
-    d.Hp = (double*)(db + o_Hp); d.acc[0] = (double*)(db + o_a0); d.acc[1] = d.acc[0];
-    d.st = (BaState*)(db + o_st);
+    BaDev& d = w.d;
+    d.X = (double*)(db + w.o_X); d.Xc = d.X;
+    d.vis = (const gf_ba_visual_factor*)(db + w.o_vis); d.pair_start = (const int*)(db + w.o_ps); d.pair_ij = (const int*)(db + w.o_pij);
+    d.imu = (const gf_ba_imu_factor*)(db + w.o_imu); d.imu_sqrt = (double*)(db + w.o_sq); d.wheel = (const gf_ba_wheel_factor*)(db + w.o_whl);
+    d.plane_frames = (const int*)(db + w.o_plf);
+    d.col_feat = (const int*)(db + w.o_cf);
+    d.pJ = (const double*)(db + w.o_pJ); d.pr0 = (const double*)(db + w.o_pr0); d.px0 = (const double*)(db + w.o_px0); d.pcol = (const int*)(db + w.o_pcol);
+    d.Hp = (double*)(db + w.o_Hp); d.acc[0] = (double*)(db + w.o_a0); d.acc[1] = d.acc[0];
+    d.st = (BaState*)(db + w.o_st);
     memcpy(d.gravity, p->gravity, sizeof(d.gravity)); d.vis_sqrt_info = p->visual_sqrt_info;
-    const int eval_blocks = n_work + d.n_imu + d.n_wheel + d.n_plane + (pn ? 1 : 0);
-    d.eval_grid = eval_blocks;
-    memcpy(hb + o_dev, &d, sizeof(d));                         // the kernels read the descriptor from the device (a batch of one window)
-    const BaDev* dd = (const BaDev*)(db + o_dev);
-    MargDev q;
-    q.N = N; q.m = m; q.n = n; q.H = d.acc[0]; q.Hp = d.Hp; q.g = d.acc[0] + NN;      // acc layout: [H N*N | g N | ...]
-    q.A = (double*)(db + o_A); q.b = (double*)(db + o_b); q.Amm = (double*)(db + o_Amm); q.Vm = (double*)(db + o_Vm); q.wm = (double*)(db + o_wm);
-    q.Ainv = (double*)(db + o_Ainv); q.T = (double*)(db + o_T); q.Ar = (double*)(db + o_Ar); q.Vr = (double*)(db + o_Vr); q.wr = (double*)(db + o_wr);
-    q.br = (double*)(db + o_br); q.J0 = (double*)(db + o_J0); q.r0 = (double*)(db + o_r0);
-    cudaStream_t st = s->s;
-    GF_CUDA(cudaEventRecord(s->e0, st));
-    GF_CUDA(cudaMemcpyAsync(db, hb, upload_bytes, cudaMemcpyHostToDevice, st));
-    GF_CUDA(cudaMemsetAsync(db + o_Hp, 0, al(sizeof(double) * NN) + al(sizeof(double) * acc_size(N, 0)), st));     // H_prior and the accumulator
-    if (pn) { k_ba_prior_hessian<<<(pn * pn + 255) / 256, 256, 0, st>>>(dd); GF_LAUNCHED(); }
-    if (eval_blocks > 0) { k_ba_eval<<<eval_blocks, PAIR_THREADS, sizeof(double) * 2 * (size_t)pn, st>>>(dd, 0); GF_LAUNCHED(); }
-    k_marg_pack<<<(int)((NN + 255) / 256), 256, 0, st>>>(q); GF_LAUNCHED();
-    const int cdim = (old_ && use_sb) ? 15 : 6;
-    int path = 0;
-    rc = marg_schur_eig(q, cdim, false, (double*)(db + o_Q), (double*)(db + o_qb), (double*)(db + o_ce), (int*)(db + o_sw), (int*)(hb + o_sw), st, &path);
-    if (rc) return rc;
-    GF_CUDA(cudaMemcpyAsync(hb + o_J0, db + o_J0, sizeof(double) * nn, cudaMemcpyDeviceToHost, st));
-    GF_CUDA(cudaMemcpyAsync(hb + o_r0, db + o_r0, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-    GF_CUDA(cudaMemcpyAsync(hb + o_st, db + o_st, sizeof(BaState), cudaMemcpyDeviceToHost, st));
-    GF_CUDA(cudaEventRecord(s->e1, st));
-    GF_CUDA(cudaMemcpyAsync(hb + o_sw, db + o_sw, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));     // sweep counts (not timed)
-    GF_CUDA(cudaStreamSynchronize(st));
-    s->marg_info[0] = path;
-    s->marg_info[1] = (path & GF_MARG_PATH_GENERIC) ? ((int*)(hb + o_sw))[0] : 0;
-    s->marg_info[2] = (path & GF_MARG_PATH_REDUCED_JACOBI) ? ((int*)(hb + o_sw))[1] : 0;
-    if (((BaState*)(hb + o_st))->setup_failed) return set_err(GF_ERR_INVALID_ARG, "IMU covariance is not positive definite");
-    if (device_ms) GF_CUDA(cudaEventElapsedTime(device_ms, s->e0, s->e1));
-    memcpy(out_J, hb + o_J0, sizeof(double) * nn);
-    memcpy(out_r, hb + o_r0, sizeof(double) * n);
+    MargDev& q = w.q;
+    memset(&q, 0, sizeof(q));
+    q.N = w.N; q.m = w.m; q.n = w.n; q.c = w.cdim;
+    q.H = d.acc[0]; q.Hp = d.Hp; q.g = d.acc[0] + (size_t)w.N * w.N;      // acc layout: [H N*N | g N | ...]
+    q.A = (double*)(db + w.o_A); q.b = (double*)(db + w.o_b); q.Amm = (double*)(db + w.o_Amm); q.Vm = (double*)(db + w.o_Vm); q.wm = (double*)(db + w.o_wm);
+    q.Ainv = (double*)(db + w.o_Ainv); q.T = (double*)(db + w.o_T); q.Ar = (double*)(db + w.o_Ar); q.Vr = (double*)(db + w.o_Vr); q.wr = (double*)(db + w.o_wr);
+    q.br = (double*)(db + w.o_br); q.J0 = (double*)(db + w.o_J0); q.r0 = (double*)(db + w.o_r0);
+    q.Q = (double*)(db + w.o_Q); q.qb = (double*)(db + w.o_qb); q.Ceps = (double*)(db + w.o_ce); q.sw = dsw;
+}
+
+static void marg_finish(const gf_ba* s, const gf_ba_problem* p, const MargWindow& w, gf_ba_prior* out, double* out_x0, double* out_J, double* out_r)
+{
+    const char* hb = (const char*)s->hbuf + w.base;
+    const BaDev& d = w.d;
+    const int F = w.F, m = w.m, n = w.n, fdrop = w.fdrop;
+    const bool old_ = w.old_;
+    memcpy(out_J, hb + w.o_J0, sizeof(double) * (size_t)n * n);
+    memcpy(out_r, hb + w.o_r0, sizeof(double) * n);
     // ---- kept blocks after addr_shift (estimator.cpp:3500-3534 / 3583-3621): MARGIN_OLD shifts every frame down by one,
     // MARGIN_SECOND_NEW moves frame F-1 into the slot of the dropped frame F-2 ----
     memset(out, 0, sizeof(*out));
@@ -2152,14 +2247,112 @@ static int marg_run(gf_ba* s, const gf_ba_problem* p, int mode, gf_ba_prior* out
     if (d.col_pr >= 0) { out->block_kind[nb] = GF_BA_BLOCK_PLANE_R; out->block_index[nb] = 0; out->block_idx[nb] = d.col_pr - m; memcpy(xp, p->para_plane_R, 32); xp += 4; nb++; }
     if (d.col_pz >= 0) { out->block_kind[nb] = GF_BA_BLOCK_PLANE_Z; out->block_index[nb] = 0; out->block_idx[nb] = d.col_pz - m; xp[0] = p->para_plane_Z[0]; xp += 1; nb++; }
     out->n_blocks = nb; out->x0 = out_x0; out->linearized_jacobians = out_J; out->linearized_residuals = out_r;
-    return n;
+}
+
+// Windows k = 0..n-1 (problem ps[k] in mode modes[k] on handle hs[k]), every one validated before anything is written or enqueued.
+// The windows with work (all but MARGIN_SECOND_NEW ones whose prior lacks the pose) run on the stream of the first of them, whose
+// buffers also hold the batch table: their BaDev and MargDev descriptors, marg_schur_eig's window lists and the int[4] per window
+// of sweep counts and flag.  kept[k]: what the single call returns for window k.
+static int marg_batch(gf_ba* const* hs, int n, const gf_ba_problem* ps, const int32_t* modes, gf_ba_prior* outs, double* const* x0s,
+                      double* const* Js, double* const* rs, int32_t* kept, float* device_ms, bool multi)
+{
+    std::vector<MargWindow> W(n);
+    for (int k = 0; k < n; k++) {
+        const int rc = (!x0s[k] || !Js[k] || !rs[k]) ? set_err(GF_ERR_INVALID_ARG, "null output buffer") : marg_layout(&ps[k], modes[k], W[k]);
+        if (rc) return multi ? window_err(k, rc) : rc;
+    }
+    std::vector<int> act;
+    for (int k = 0; k < n; k++) { kept[k] = 0; if (!W[k].skip) act.push_back(k); }
+    const int na = (int)act.size();
+    if (na == 0) return GF_OK;
+    gf_ba* lead = hs[act[0]];
+    GF_CUDA(cudaSetDevice(lead->device));
+    const size_t o_mq = al16(sizeof(BaDev) * na), o_lists = o_mq + al16(sizeof(MargDev) * na), o_sw = o_lists + al16(sizeof(int) * MARG_LISTS * na),
+                 table = o_sw + al16(sizeof(int) * 4 * na);
+    for (int a = 0; a < na; a++) {
+        MargWindow& w = W[act[a]];
+        w.base = a == 0 ? table : 0;
+        const int rc = ensure(hs[act[a]], w.base + w.bytes);
+        if (rc) return rc;
+    }
+    char* th = (char*)lead->hbuf; char* td = (char*)lead->dbuf;
+    BaDev* hdesc = (BaDev*)th;
+    MargDev* hq = (MargDev*)(th + o_mq);
+    MargBatch b;
+    b.n = na; b.hq = hq; b.dq = (const MargDev*)(td + o_mq);
+    b.hl = (int*)(th + o_lists); b.dl = (const int*)(td + o_lists);
+    b.hsw = (int*)(th + o_sw); b.dsw = (const int*)(td + o_sw);
+    memset(b.hsw, 0, sizeof(int) * 4 * na);
+    int prior_grid = 0, eval_grid = 0;
+    size_t prior_smem = 0, pack_work = 1;
+    for (int a = 0; a < na; a++) {
+        MargWindow& w = W[act[a]];
+        marg_pack(hs[act[a]], &ps[act[a]], w, (int*)(td + o_sw) + 4 * a);
+        hdesc[a] = w.d; hq[a] = w.q;
+        if (w.pn) prior_grid = std::max(prior_grid, (w.pn * w.pn + 255) / 256);
+        eval_grid = std::max(eval_grid, w.d.eval_grid);
+        prior_smem = std::max(prior_smem, sizeof(double) * 2 * (size_t)w.pn);
+        pack_work = std::max(pack_work, (size_t)w.N * w.N);
+    }
+    std::vector<int> paths(na);
+    marg_plan(b, false, paths.data());
+    const BaDev* wins = (const BaDev*)td;
+    cudaStream_t st = lead->s;
+    GF_CUDA(cudaEventRecord(lead->e0, st));
+    for (int a = 0; a < na; a++) {     // the lead's upload carries the batch table in front of its window
+        const MargWindow& w = W[act[a]];
+        char* db = (char*)hs[act[a]]->dbuf;
+        GF_CUDA(cudaMemcpyAsync(db, hs[act[a]]->hbuf, w.base + w.upload_bytes, cudaMemcpyHostToDevice, st));
+        GF_CUDA(cudaMemsetAsync(db + w.base + w.o_Hp, 0, al16(sizeof(double) * (size_t)w.N * w.N) + al16(sizeof(double) * acc_size(w.N, 0)), st));     // H_prior and the accumulator
+    }
+    if (prior_grid) { k_ba_prior_hessian<<<dim3(prior_grid, na), 256, 0, st>>>(wins); GF_LAUNCHED(); }
+    if (eval_grid > 0) { k_ba_eval<<<dim3(eval_grid, na), PAIR_THREADS, prior_smem, st>>>(wins, 0); GF_LAUNCHED(); }
+    k_marg_pack<<<dim3((unsigned)((pack_work + 255) / 256), na), 256, 0, st>>>(b.dq, b.dl + MARG_ALL * na); GF_LAUNCHED();
+    int rc = marg_schur_eig(b, st, paths.data());
+    if (rc) return rc;
+    for (int a = 0; a < na; a++) {     // solver state | J0 | r0: one range
+        const MargWindow& w = W[act[a]];
+        const size_t o = w.base + w.o_st;
+        GF_CUDA(cudaMemcpyAsync((char*)hs[act[a]]->hbuf + o, (char*)hs[act[a]]->dbuf + o, w.o_r0 + sizeof(double) * w.n - w.o_st, cudaMemcpyDeviceToHost, st));
+    }
+    GF_CUDA(cudaEventRecord(lead->e1, st));
+    GF_CUDA(cudaMemcpyAsync(b.hsw, b.dsw, sizeof(int) * 4 * na, cudaMemcpyDeviceToHost, st));     // sweep counts (not timed)
+    GF_CUDA(cudaStreamSynchronize(st));
+    float ms = 0;
+    GF_CUDA(cudaEventElapsedTime(&ms, lead->e0, lead->e1));
+    for (int a = na - 1; a >= 0; a--) {           // backwards: the error text names the first failing window
+        const int k = act[a];
+        gf_ba* s = hs[k];
+        const MargWindow& w = W[k];
+        s->marg_info[0] = paths[a];
+        s->marg_info[1] = (paths[a] & GF_MARG_PATH_GENERIC) ? b.hsw[4 * a] : 0;
+        s->marg_info[2] = (paths[a] & GF_MARG_PATH_REDUCED_JACOBI) ? b.hsw[4 * a + 1] : 0;
+        if (((const BaState*)((const char*)s->hbuf + w.base + w.o_st))->setup_failed) {
+            rc = set_err(GF_ERR_INVALID_ARG, "IMU covariance is not positive definite");
+            if (multi) window_err(k, rc);
+            kept[k] = GF_ERR_INVALID_ARG;
+            continue;
+        }
+        marg_finish(s, &ps[k], w, &outs[k], x0s[k], Js[k], rs[k]);
+        kept[k] = w.n;
+    }
+    if (device_ms && (multi || rc == GF_OK)) *device_ms = ms;
+    return rc;
+}
+
+static int marg_single(gf_ba* s, const gf_ba_problem* p, int32_t mode, gf_ba_prior* out, double* out_x0, double* out_J, double* out_r, float* device_ms)
+{
+    if (!s || !p || !out || !out_x0 || !out_J || !out_r) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    int32_t kept = 0;
+    const int rc = marg_batch(&s, 1, p, &mode, out, &out_x0, &out_J, &out_r, &kept, device_ms, false);
+    return rc ? rc : kept;
 }
 
 extern "C" {
 
 int gf_ba_marginalize_old(gf_ba* s, const gf_ba_problem* p, gf_ba_prior* out, double* out_x0, double* out_J, double* out_r, float* device_ms)
 {
-    return marg_run(s, p, GF_MARG_OLD, out, out_x0, out_J, out_r, device_ms);
+    return marg_single(s, p, GF_MARG_OLD, out, out_x0, out_J, out_r, device_ms);
 }
 
 /* MARGIN_SECOND_NEW (estimator.cpp:3536-3631): the only factor is the last prior, evaluated at the current state (r = r0 + J0 dx),
@@ -2168,7 +2361,15 @@ int gf_ba_marginalize_old(gf_ba* s, const gf_ba_problem* p, gf_ba_prior* out, do
  * hold that pose (the reference then keeps the prior untouched), or a negative error code. */
 int gf_ba_marginalize_second_new(gf_ba* s, const gf_ba_problem* p, gf_ba_prior* out, double* out_x0, double* out_J, double* out_r, float* device_ms)
 {
-    return marg_run(s, p, GF_MARG_SECOND_NEW, out, out_x0, out_J, out_r, device_ms);
+    return marg_single(s, p, GF_MARG_SECOND_NEW, out, out_x0, out_J, out_r, device_ms);
+}
+
+int gf_ba_marginalize_multi(gf_ba* const* solvers, int n, const gf_ba_problem* problems, const int32_t* modes, gf_ba_prior* outs,
+                            double* const* out_x0, double* const* out_J, double* const* out_r, int32_t* kept, float* device_ms)
+{
+    if (!solvers || !problems || !modes || !outs || !out_x0 || !out_J || !out_r || !kept) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    if (const int rc = check_batch(solvers, n)) return rc;
+    return marg_batch(solvers, n, problems, modes, outs, out_x0, out_J, out_r, kept, device_ms, true);
 }
 
 /* Estimator::double2vector (reference estimator.cpp:2440-2494): after the solve the whole window is rotated about z and
@@ -2330,22 +2531,28 @@ extern "C" int gf_stage_sym_eig(int device, const double* A, int n, int method, 
     std::vector<double> h(nn);
     for (int i = 0; i < n; i++) for (int j = 0; j <= i; j++) h[(size_t)i * n + j] = h[(size_t)j * n + i] = A[(size_t)i * n + j];
     double* dA = nullptr;
-    GF_CUDA(cudaMalloc(&dA, sizeof(double) * (3 * nn + n + 1)));           // A | V | w | sweep count
-    double* dV = dA + nn; double* dw = dV + nn; int* dsw = (int*)(dw + n);
+    GF_CUDA(cudaMalloc(&dA, sizeof(double) * (3 * nn + n) + sizeof(MargDev) + sizeof(int) * 5));     // A | V | w | one-window table: descriptor, list, int[4] sweeps
+    double* dV = dA + nn; double* dw = dV + nn;
+    MargDev* dq = (MargDev*)(dw + n); int* dl = (int*)(dq + 1); int* dsw = dl + 1;
+    MargDev q;
+    memset(&q, 0, sizeof(q));
+    q.n = n; q.Ar = dA; q.Vr = dV; q.wr = dw; q.sw = dsw;
+    const int zeros[5] = {0, 0, 0, 0, 0};                                   // the list {0} and the sweep counts
     cudaError_t e = cudaMemcpy(dA, h.data(), sizeof(double) * nn, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemset(dsw, 0, sizeof(int));
+    if (e == cudaSuccess) e = cudaMemcpy(dq, &q, sizeof(q), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dl, zeros, sizeof(zeros), cudaMemcpyHostToDevice);
     if (e == cudaSuccess && method == 0) {
         e = cudaFuncSetAttribute(k_sym_eig_ql, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        if (e == cudaSuccess) { k_sym_eig_ql<<<1, QL_T, sizeof(double) * (nn + 4 * (size_t)n + 8)>>>(dA, dV, dw, n); GF_LAUNCHED(); }
+        if (e == cudaSuccess) { k_sym_eig_ql<<<1, QL_T, sizeof(double) * (nn + 4 * (size_t)n + 8)>>>(dq, dl); GF_LAUNCHED(); }
     } else if (e == cudaSuccess) {
         const int hp = ((n + 1) & ~1) / 2;
         e = cudaFuncSetAttribute(k_jacobi_eig, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        if (e == cudaSuccess) { k_jacobi_eig<<<1, 1024, (size_t)hp * (2 * sizeof(double) + 2 * sizeof(int)) + 8>>>(dA, dV, dw, n, dsw); GF_LAUNCHED(); }
+        if (e == cudaSuccess) { k_jacobi_eig<<<1, 1024, (size_t)hp * (2 * sizeof(double) + 2 * sizeof(int)) + 8>>>(dq, dl, 1); GF_LAUNCHED(); }
     }
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaMemcpy(V, dV, sizeof(double) * nn, cudaMemcpyDeviceToHost);
     if (e == cudaSuccess) e = cudaMemcpy(w, dw, sizeof(double) * n, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess && sweeps) e = cudaMemcpy(sweeps, dsw, sizeof(int), cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && sweeps) e = cudaMemcpy(sweeps, dsw + 1, sizeof(int), cudaMemcpyDeviceToHost);
     cudaFree(dA);
     if (e != cudaSuccess) { snprintf(g_err, sizeof(g_err), "gf_stage_sym_eig: %s", cudaGetErrorString(e)); return GF_ERR_CUDA; }
     return GF_OK;
@@ -2365,24 +2572,29 @@ extern "C" int gf_stage_marginalize(int device, const double* A, const double* b
     const size_t NN = (size_t)N * N, mm = (size_t)m * m, nn = (size_t)n * n, R = (size_t)c + n;
     const size_t nd = NN + N + 3 * mm + m + (size_t)n * m + 3 * nn + 3 * (size_t)n + R * R + R + 225;
     double* d = nullptr;
-    GF_CUDA(cudaMalloc(&d, sizeof(double) * (nd + 2)));                       // ... | int[4] sweeps and flag
-    int* dsw = (int*)(d + nd);
+    GF_CUDA(cudaMalloc(&d, sizeof(double) * nd + sizeof(MargDev) + sizeof(int) * (MARG_LISTS + 4)));     // ... | one-window table: descriptor, lists, int[4] sweeps and flag
+    MargDev* dq = (MargDev*)(d + nd); int* dl = (int*)(dq + 1); int* dsw = dl + MARG_LISTS;
     MargDev q;
     memset(&q, 0, sizeof(q));
-    q.N = N; q.m = m; q.n = n;
+    q.N = N; q.m = m; q.n = n; q.c = c;
     double* t = d;
     auto take = [&](size_t k) { double* p = t; t += k; return p; };
     q.A = take(NN); q.b = take(N); q.Amm = take(mm); q.Vm = take(mm); q.wm = take(m); q.Ainv = take(mm); q.T = take((size_t)n * m);
     q.Ar = take(nn); q.Vr = take(nn); q.wr = take(n); q.br = take(n); q.J0 = take(nn); q.r0 = take(n);
-    double* dQ = take(R * R); double* dqb = take(R); double* dce = take(225);
-    int h_flag = 0, p = 0, hsw[2] = {0, 0};
+    q.Q = take(R * R); q.qb = take(R); q.Ceps = take(225); q.sw = dsw;
+    int hl[MARG_LISTS], hsw[4] = {0, 0, 0, 0}, p = 0;
+    MargBatch bt;
+    bt.n = 1; bt.hq = &q; bt.dq = dq; bt.hl = hl; bt.dl = dl; bt.hsw = hsw; bt.dsw = dsw;
+    marg_plan(bt, force_generic != 0, &p);
     cudaError_t e = cudaMemcpy(q.A, A, sizeof(double) * NN, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(q.b, b, sizeof(double) * N, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dq, &q, sizeof(q), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(dl, hl, sizeof(hl), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemset(dsw, 0, sizeof(int) * 4);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_sym_eig_ql, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_jacobi_eig, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     if (e == cudaSuccess) {
-        rc = marg_schur_eig(q, c, force_generic != 0, dQ, dqb, dce, dsw, &h_flag, 0, &p);
+        rc = marg_schur_eig(bt, 0, &p);
         if (!rc) e = cudaMemcpy(J0, q.J0, sizeof(double) * nn, cudaMemcpyDeviceToHost);
         if (!rc && e == cudaSuccess) e = cudaMemcpy(r0, q.r0, sizeof(double) * n, cudaMemcpyDeviceToHost);
         if (!rc && e == cudaSuccess) e = cudaMemcpy(hsw, dsw, sizeof(int) * 2, cudaMemcpyDeviceToHost);

@@ -104,6 +104,49 @@ def solve_multi(adjusters, problems):
     return [s.as_dict() for s in sums], [int(v) for v in status]
 
 
+def _prior_buffers(problem):
+    """x0, J0, r0 buffers of the sizes a marginalisation of `problem` may fill (include/gf_b200.h)."""
+    cap = 16 * problem.n_frames + 24
+    return np.zeros(cap), np.zeros(cap * cap), np.zeros(cap)
+
+
+def _prior_from(out, n, x0, J, r):
+    from .ba_problem import Prior
+    nb = out.n_blocks
+    return Prior(list(out.block_kind)[:nb], list(out.block_index)[:nb], list(out.block_idx)[:nb], x0.copy(),
+                 J[:n * n].reshape(n, n).copy(), r[:n].copy())
+
+
+def marginalize_multi(adjusters, problems, modes):
+    """The marginalisations at the end of Estimator::optimization() for several windows in one batched call
+    (gf_ba_marginalize_multi): problems[k] is marginalised on adjusters[k] (distinct BundleAdjusters on one device) as modes[k]
+    says (_lib.MARGIN_OLD / MARGIN_SECOND_NEW).  Returns (priors, statuses): priors[k] is the ba_problem.Prior for the next
+    window, or None when status k is 0 (MARGIN_SECOND_NEW and the prior does not hold the pose) or negative (window k's IMU
+    covariance is singular); argument errors raise GfError.  Every adjuster's last_marg_ms is set to the time of the whole batch."""
+    n = len(adjusters)
+    assert len(problems) == n and len(modes) == n
+    L = _lib.lib()
+    dp = ctypes.POINTER(ctypes.c_double)
+    i32p = ctypes.POINTER(ctypes.c_int32)
+    L.gf_ba_marginalize_multi.argtypes = [ctypes.POINTER(ctypes.c_void_p), ctypes.c_int, ctypes.POINTER(BaProblem), i32p,
+                                          ctypes.POINTER(BaPrior), ctypes.POINTER(dp), ctypes.POINTER(dp), ctypes.POINTER(dp), i32p,
+                                          ctypes.POINTER(ctypes.c_float)]
+    handles = (ctypes.c_void_p * n)(*[a._h.value for a in adjusters])
+    p_array = (BaProblem * n)(*[p.struct() for p in problems])
+    bufs = [_prior_buffers(p) for p in problems]
+    ptrs = [(dp * n)(*[b[j].ctypes.data_as(dp) for b in bufs]) for j in range(3)]
+    mode_arr = np.ascontiguousarray(modes, np.int32)
+    outs, kept, ms = (BaPrior * n)(), np.zeros(n, np.int32), ctypes.c_float(0)
+    rc = L.gf_ba_marginalize_multi(handles, n, p_array, mode_arr.ctypes.data_as(i32p), outs, ptrs[0], ptrs[1], ptrs[2],
+                                   kept.ctypes.data_as(i32p), ctypes.byref(ms))
+    if rc != 0 and not (kept < 0).any():
+        check(rc)
+    for a in adjusters:
+        a.last_marg_ms = float(ms.value)
+    priors = [_prior_from(outs[k], int(kept[k]), *bufs[k]) if kept[k] > 0 else None for k in range(n)]
+    return priors, [int(v) for v in kept]
+
+
 def _capture_buffers(adjuster, problem):
     """A gf_ba_step_capture whose arrays are numpy buffers sized for `problem` (gf_ba_step_dims), and those buffers."""
     L = _lib.lib()
@@ -173,13 +216,11 @@ class BundleAdjuster:
         return s.as_dict()
 
     def _marginalize(self, problem, fn_name):
-        from .ba_problem import Prior
         dp = ctypes.POINTER(ctypes.c_double)
         fn = getattr(self.L, fn_name)
         fn.argtypes = [ctypes.c_void_p, ctypes.POINTER(BaProblem), ctypes.POINTER(BaPrior), dp, dp, dp, ctypes.POINTER(ctypes.c_float)]
         p = problem.struct()
-        cap = 16 * problem.n_frames + 24
-        x0 = np.zeros(cap); J = np.zeros(cap * cap); r = np.zeros(cap)
+        x0, J, r = _prior_buffers(problem)
         out = BaPrior(); ms = ctypes.c_float(0)
         n = fn(self._h, ctypes.byref(p), ctypes.byref(out), x0.ctypes.data_as(dp), J.ctypes.data_as(dp), r.ctypes.data_as(dp), ctypes.byref(ms))
         if n < 0:
@@ -187,9 +228,7 @@ class BundleAdjuster:
         if n == 0:
             return None
         self.last_marg_ms = float(ms.value)
-        nb = out.n_blocks
-        return Prior(list(out.block_kind)[:nb], list(out.block_index)[:nb], list(out.block_idx)[:nb], x0.copy(),
-                     J[:n * n].reshape(n, n).copy(), r[:n].copy())
+        return _prior_from(out, n, x0, J, r)
 
     def marginalize_old(self, problem):
         """MARGIN_OLD on the GPU (estimator.cpp:3334-3535): returns the ba_problem.Prior for the next window (block indices

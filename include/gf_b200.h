@@ -466,6 +466,28 @@ int gf_ba_marginalize_old(gf_ba* s, const gf_ba_problem* p, gf_ba_prior* out, do
  * unchanged: estimator.cpp:3538-3539), or a negative error code. */
 int gf_ba_marginalize_second_new(gf_ba* s, const gf_ba_problem* p, gf_ba_prior* out, double* out_x0, double* out_J, double* out_r,
                                  float* device_ms);
+
+/* The marginalisations of several estimators in one call, as gf_ba_solve_multi batches their solves.  Window k is problems[k]
+ * on solvers[k]'s workspace, marginalised as modes[k] says; the result is exactly what gf_ba_marginalize_old /
+ * gf_ba_marginalize_second_new(solvers[k], &problems[k], &outs[k], out_x0[k], out_J[k], out_r[k], ...) would give (same kernels,
+ * same arithmetic; J0 may differ from a single call in the last bits, as between two single calls, because the Hessian is summed
+ * with atomics), with the buffers of those calls.  Every kernel runs once for all windows that take its path (window =
+ * blockIdx.y, or one CTA per window for the eigensolvers and k_marg_c_elim): the launch count depends on which paths occur
+ * (fast path, literal path, QL or Jacobi on the reduced system), not on n, and the host synchronises at most once mid-batch, to
+ * read every window's fast-path flag together.
+ *   kept[k] (n entries): what the single call returns -- n_k > 0; 0 for MARGIN_SECOND_NEW when the prior does not hold the pose
+ *   (outs[k] and its buffers untouched); GF_ERR_INVALID_ARG when the window's IMU covariance is singular on the device (outs[k]
+ *   untouched; the other windows are written and the call returns GF_ERR_INVALID_ARG).
+ *   1 <= n <= GF_BA_MAX_MULTI (more: GF_ERR_CAPACITY); the handles must be distinct and bound to the same device.  Every window
+ *   is checked as the single call checks it, and modes[k] must be GF_BA_MARGIN_OLD or GF_BA_MARGIN_SECOND_NEW, before anything is
+ *   enqueued; on an argument error nothing is written and gf_last_error() starts with "window k: ".
+ *   gf_ba_last_marg_info(solvers[k]) reports window k.  device_ms (nullable): the CUDA-event time of the whole batch.
+ * All work runs on the stream of the first window with work, driven by the calling thread; no handle of the batch may be used
+ * by another thread during the call. */
+#define GF_BA_MARGIN_OLD 0          /* estimator.cpp:3334-3535 */
+#define GF_BA_MARGIN_SECOND_NEW 1   /* estimator.cpp:3536-3631 */
+int gf_ba_marginalize_multi(gf_ba* const* solvers, int n, const gf_ba_problem* problems, const int32_t* modes, gf_ba_prior* outs,
+                            double* const* out_x0, double* const* out_J, double* const* out_r, int32_t* kept, float* device_ms);
 /* The last marginalisation of this handle: info[0] = GF_MARG_PATH_* bits, info[1] = Jacobi sweeps on Amm (0 on the fast
  * path), info[2] = Jacobi sweeps on the reduced system (0 for QL). */
 int gf_ba_last_marg_info(gf_ba* s, int* info3);
