@@ -4,7 +4,8 @@
 //                       features) is never materialised: tiles test pixels against the kept features in reach
 //   k_eig_max / k_candidates : minMaxLoc(masked) -> threshold -> 3x3 dilate -> local maxima
 //   k_select_finalize : cv::goodFeaturesToTrack's greedy min-distance pass by cell-head rounds (the accepted set is
-//                       exactly the sequential greedy's; the maxCorners cap = top-K of that set by rank), then
+//                       exactly the sequential greedy's; the maxCorners cap = top-K of that set by rank; the rounds stop
+//                       once the top K can no longer change), then
 //                       addPoints, undistortedPts, ptsVelocity, depth and the state of the next frame
 // Arithmetic and ordering follow oracle/fe_cv_restate.c and oracle/fe_oracle.py.
 #pragma once
@@ -303,7 +304,8 @@ __global__ void __launch_bounds__(256) k_candidates(TrackScalars* sc, const floa
 //   A head that outranks the heads of the 8 surrounding cells has no undecided higher-ranked candidate within r
 //   (every candidate of a cell ranks below its head) and no accepted corner within r (else it would be dead), so the
 //   sequential greedy would accept it too.  The globally best head can always decide, so the loop terminates;
-//   measured 5-11 rounds at 640x480.
+//   measured 5-11 rounds at 640x480 to decide every candidate.  Only the first `want` accepted corners by rank are kept,
+//   so the loop stops as soon as `want` corners accepted in earlier rounds outrank every cell head (see the early exit).
 // The single SM is issue-bound on this, so the rounds are kept lean: the head election is two native 32-bit
 // ATOMS.MAX (eig bits, then packed address among the ties; a 64-bit shared atomicMax is a CAS spin loop), a per-cell
 // flag says whether any of the 3x3 cells accepted a corner last round (most candidates skip the distance tests),
@@ -320,7 +322,7 @@ __device__ __forceinline__ int div_cell(int x, float rcp, int cs)
     return q;
 }
 __host__ __device__ inline size_t nms_smem_bytes(int gw, int gh) { return (size_t)(gw + 2) * (gh + 2) * NMS_CELL_BYTES; }
-__device__ __forceinline__ void nms_cells(TrackScalars* sc, const NmsGrid& g, int w, int min_dist, unsigned char* smem_raw, long long* dbg)
+__device__ __forceinline__ void nms_cells(TrackScalars* sc, const NmsGrid& g, int w, int min_dist, int want, unsigned char* smem_raw, long long* dbg)
 {
     const int tid = threadIdx.x, nt = blockDim.x;
     // the grid is padded by one ring of empty cells: the 3x3 neighbourhoods below are nine unconditional loads
@@ -344,13 +346,15 @@ __device__ __forceinline__ void nms_cells(TrackScalars* sc, const NmsGrid& g, in
     const int cell0 = cell_of(key0), cell1 = cell_of(key1);
     for (int c = tid; c < 2 * ncp; c += nt) { head_hi[c] = 0u; head_lo[c] = 0u; acc[c] = -1; flag[c] = 0; }
     for (int i = tid; i < ncell; i += nt) { int cy = i / g.gw, cx = i - cy * g.gw; pidx[i] = (unsigned short)((cy + 1) * gwp + cx + 1); }
-    __shared__ int s_nacc;
-    if (tid == 0) s_nacc = 0;
+    __shared__ int s_nacc, s_above;
+    __shared__ unsigned long long s_u;
+    if (tid == 0) { s_nacc = 0; s_above = 0; s_u = 0ull; }
     int rounds = 0;
     long long tA = 0, tB = 0, tC = 0, tl = gf_clock();
     const long long tstart = tl;
     __syncthreads();
     while (true) {
+        const int nacc_prev = s_nacc;                           // corners accepted by the earlier rounds
         const int p = rounds & 1;
         unsigned int* hh = head_hi + p * ncp;
         unsigned int* hl = head_lo + p * ncp;
@@ -412,6 +416,30 @@ __device__ __forceinline__ void nms_cells(TrackScalars* sc, const NmsGrid& g, in
         for (int c = tid; c < ncp; c += nt) { head_hi[(p ^ 1) * ncp + c] = 0u; head_lo[(p ^ 1) * ncp + c] = 0u; flag[(p ^ 1) * ncp + c] = 0; }
         __syncthreads();
         { long long t_ = gf_clock(); tB += t_ - tl; tl = t_; }
+        // Early exit: every candidate still alive ranks at most U, the best cell head of this round, and so does every corner
+        // a later round could accept.  Once `want` corners accepted earlier rank above U, the first `want` corners of the
+        // accepted set by rank (the output) are fixed, and the rounds stop.
+        if (nacc_prev >= want) {
+            unsigned long long u = 0ull;
+            for (int i = tid; i < ncell; i += nt) {
+                const int c = pidx[i];
+                const unsigned long long hk = ((unsigned long long)hh[c] << 32) | hl[c];
+                u = hk > u ? hk : u;
+            }
+            for (int o = 16; o > 0; o >>= 1) { const unsigned long long t_ = __shfl_xor_sync(0xffffffffu, u, o); u = t_ > u ? t_ : u; }
+            if ((tid & 31) == 0 && u) atomicMax(&s_u, u);
+            __syncthreads();
+            const unsigned long long U = s_u;
+            int above = 0;
+            for (int i = tid; i < min(nacc_prev, g.acc_cap); i += nt) above += g.acc_key[i] > U;
+            above = __reduce_add_sync(0xffffffffu, above);
+            if ((tid & 31) == 0 && above) atomicAdd(&s_above, above);
+            __syncthreads();
+            const bool done = s_above >= want;
+            __syncthreads();                                    // s_u and s_above are read by everyone before they are reset
+            if (tid == 0) { s_u = 0ull; s_above = 0; }
+            if (done) break;
+        }
         // phase C: a head that outranks its 8 neighbours is accepted
         int any = 0;
         int* acc_next = acc + (p ^ 1) * ncp;
@@ -519,13 +547,13 @@ __global__ void __launch_bounds__(1024) k_select_finalize(TrackScalars* sc, Feat
     const int n_box = boxes ? boxes->n : 0;
     if (tid < n_box) s_box[tid] = boxes->b[tid];            // visible after the barriers of nms_cells
     const long long c0 = gf_clock();
-    nms_cells(sc, g, w, min_dist, dyn_smem, fa.dbg);
+    const int n_kept = sc->n_kept;
+    const int want = max(max_cnt - n_kept, 0);
+    nms_cells(sc, g, w, min_dist, want, dyn_smem, fa.dbg);
     const long long c1 = gf_clock();
     const double dt = dt_ptr ? *dt_ptr : 1.0;
     const int depth_cam = depth_cam_cfg && depth_valid_ptr && *depth_valid_ptr;
     const int ncand = sc->n_cand;
-    const int n_kept = sc->n_kept;
-    const int want = max(max_cnt - n_kept, 0);
     const int nacc = sc->n_acc;
     int n_new;
     if (nacc <= (int)blockDim.x) {
