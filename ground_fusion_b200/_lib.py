@@ -67,6 +67,12 @@ def lib():
         L.gf_tracker_track_boxes.argtypes = [vp, d, vp, sz, vp, sz, i, vp, i, vp, ctypes.POINTER(i), vp, vp, ctypes.POINTER(TrackInfo)]
         L.gf_tracker_track_batch_boxes.argtypes = [vp, i, vp, vp, sz, vp, sz, i, vp, vp, vp, vp, vp, vp, vp]
         L.gf_tracker_track_batch_multi_boxes.argtypes = [vp, i, i, vp, vp, sz, vp, sz, i, vp, vp, vp, vp, vp, vp, vp]
+        L.gf_tracker_group_create.argtypes = [ctypes.POINTER(vp), vp, i]
+        L.gf_tracker_group_destroy.argtypes = [vp]
+        L.gf_tracker_group_destroy.restype = None
+        L.gf_tracker_group_submit.argtypes = [vp, vp, vp, sz, vp, sz, i, vp, vp]
+        L.gf_tracker_group_wait.argtypes = [vp, vp, vp, vp, vp, vp]
+        L.gf_tracker_group_track_batch.argtypes = [vp, i, vp, vp, sz, vp, sz, i, vp, vp, vp, vp, vp, vp, vp]
         L.gf_stage_in_boxes.argtypes = [i, vp, i, vp, i, vp]
         L.gf_tracker_set_prediction.argtypes = [vp, vp, vp, i]
         L.gf_tracker_set_equalize.argtypes = [vp, d, i, i]

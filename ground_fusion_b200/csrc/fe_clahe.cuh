@@ -46,7 +46,8 @@ inline int clahe_geometry(ClaheGeom& g, int w, int h, double clip_limit, int til
 }
 
 // grid = tiles_x * tiles_y CTAs; lut: [tiles_y][tiles_x][256]
-__global__ void __launch_bounds__(CLAHE_LUT_THREADS) k_clahe_lut(const uint8_t* src, long long pitch, ClaheGeom g, uint8_t* __restrict__ lut)
+template <int V>
+__device__ __forceinline__ void clahe_lut_tile(const uint8_t* src, long long pitch, const ClaheGeom& g, uint8_t* __restrict__ lut)
 {
     constexpr int NW = CLAHE_LUT_THREADS / 32;
     __shared__ int wh[NW][256];                // per-warp histograms
@@ -119,10 +120,15 @@ __global__ void __launch_bounds__(CLAHE_LUT_THREADS) k_clahe_lut(const uint8_t* 
         lut[(size_t)blockIdx.x * 256 + tid] = (uint8_t)min(max(q, 0), 255);
     }
 }
+__global__ void __launch_bounds__(CLAHE_LUT_THREADS) k_clahe_lut(const uint8_t* src, long long pitch, ClaheGeom g, uint8_t* __restrict__ lut)
+{
+    clahe_lut_tile<0>(src, pitch, g, lut);
+}
 
 // grid = ceil(h / CLAHE_APPLY_ROWS) CTAs, dynamic shared memory tiles_x * tiles_y * 256 bytes.
-__global__ void __launch_bounds__(CLAHE_APPLY_THREADS) k_clahe_apply(const uint8_t* src, long long pitch, ClaheGeom g,
-                                                                     const uint8_t* __restrict__ lut, uint8_t* __restrict__ dst, int dst_pitch)
+template <int V>
+__device__ __forceinline__ void clahe_apply_rows(const uint8_t* src, long long pitch, const ClaheGeom& g, const uint8_t* __restrict__ lut,
+                                                 uint8_t* __restrict__ dst, int dst_pitch)
 {
     extern __shared__ __align__(16) uint8_t s_lut[];
     const int n16 = g.tiles_x * g.tiles_y * 16;
@@ -168,6 +174,11 @@ __global__ void __launch_bounds__(CLAHE_APPLY_THREADS) k_clahe_apply(const uint8
             for (int k = 0; k < 16; k++) if (k < n) dp[k] = out[k];
         }
     }
+}
+__global__ void __launch_bounds__(CLAHE_APPLY_THREADS) k_clahe_apply(const uint8_t* src, long long pitch, ClaheGeom g,
+                                                                     const uint8_t* __restrict__ lut, uint8_t* __restrict__ dst, int dst_pitch)
+{
+    clahe_apply_rows<0>(src, pitch, g, lut, dst, dst_pitch);
 }
 
 inline size_t clahe_lut_bytes(const ClaheGeom& g) { return (size_t)g.tiles_x * g.tiles_y * 256; }

@@ -29,7 +29,9 @@ namespace gf {
 // pyrDown: out(y,x) = (sum_ij k_i k_j P[2y+i-2][2x+j-2] + 128) >> 8, k=[1 4 6 4 1], REFLECT_101
 // ------------------------------------------------------------------------------------------------
 constexpr int PD_TX = 32, PD_TY = 8;
-__global__ void __launch_bounds__(PD_TX* PD_TY) k_pyr_down(Level src, uint8_t* dst, int dw, int dh, int dpitch)
+// one PD_TX x PD_TY tile of the destination (blockIdx.x, blockIdx.y); k_pyr_down and the group form k_pyr_down_g
+template <int V>
+__device__ __forceinline__ void pyr_down_tile(const Level& src, uint8_t* dst, int dw, int dh, int dpitch)
 {
     __shared__ uint8_t tile[2 * PD_TY + 3][2 * PD_TX + 4];
     __shared__ int rowf[2 * PD_TY + 3][PD_TX];
@@ -56,6 +58,10 @@ __global__ void __launch_bounds__(PD_TX* PD_TY) k_pyr_down(Level src, uint8_t* d
         int v = rowf[r][c] + 4 * rowf[r + 1][c] + 6 * rowf[r + 2][c] + 4 * rowf[r + 3][c] + rowf[r + 4][c];
         dst[(size_t)y * dpitch + x] = (uint8_t)((v + 128) >> 8);
     }
+}
+__global__ void __launch_bounds__(PD_TX* PD_TY) k_pyr_down(Level src, uint8_t* dst, int dw, int dh, int dpitch)
+{
+    pyr_down_tile<0>(src, dst, dw, dh, dpitch);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -102,7 +108,8 @@ __device__ __forceinline__ float eig_from_box(double c0, double c1, double c2)
 
 // D in the layout k_box_chain streams: [column block x/32][padded row y+1][channel][x%32]; padded row 0 = D[1],
 // padded row h+1 = D[h-2] (cv::boxFilter's BORDER_REFLECT_101 applied to the cov rows).
-__global__ void __launch_bounds__(EIG_TX) k_cov_rows(Level img, double* __restrict__ Dt)
+template <int V>
+__device__ __forceinline__ void cov_rows_tile(const Level& img, double* __restrict__ Dt)
 {
     constexpr int IH = EIG_BAND + 2, IWW = EIG_TX / 4 + 2, IP = 4 * IWW;   // image tile rows y0-1.., cols x0-4.. as 34 aligned words
     constexpr int CH = EIG_BAND, CW = EIG_TX + 2;         // dx/dy tile rows y0.., cols x0-1..
@@ -182,6 +189,10 @@ __global__ void __launch_bounds__(EIG_TX) k_cov_rows(Level img, double* __restri
         if (y == h - 2) { o = dst + (size_t)(h + 1) * BC_ROW; o[0] = d0; o[32] = d1; o[64] = d2; }
     }
 }
+__global__ void __launch_bounds__(EIG_TX) k_cov_rows(Level img, double* __restrict__ Dt)
+{
+    cov_rows_tile<0>(img, Dt);
+}
 
 // ---- mbarrier / 1-D TMA bulk copy (sm_90+) ----
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -209,7 +220,8 @@ __device__ __forceinline__ bool mbar_try_wait(unsigned long long* bar, unsigned 
 // The running column sums: one CTA of 3 warps per 32-column block, warp q <-> channel q, lane <-> column.
 //   SUM = (0 + D[-1]) + D[0];  per row: s = SUM + D[y+1]; box[y] = (float)s; SUM = s - D[y-1]
 // box: [channel][y][x] floats, row pitch bp = w rounded up to 32 (every lane stores).
-__global__ void __launch_bounds__(96) k_box_chain(const double* __restrict__ Dt, float* __restrict__ box, int bp, int w, int h)
+template <int V>
+__device__ __forceinline__ void box_chain_block(const double* __restrict__ Dt, float* __restrict__ box, int bp, int w, int h)
 {
     extern __shared__ __align__(128) unsigned char bc_smem[];
     __shared__ __align__(8) unsigned long long mbar[BC_NST];
@@ -274,8 +286,13 @@ __global__ void __launch_bounds__(96) k_box_chain(const double* __restrict__ Dt,
         }
     }
 }
+__global__ void __launch_bounds__(96) k_box_chain(const double* __restrict__ Dt, float* __restrict__ box, int bp, int w, int h)
+{
+    box_chain_block<0>(Dt, box, bp, w, h);
+}
 
-__global__ void __launch_bounds__(256) k_eig_from_box(const float* __restrict__ box, int bp, float* __restrict__ eig, int epitch, int w, int h)
+template <int V>
+__device__ __forceinline__ void eig_from_box_tile(const float* __restrict__ box, int bp, float* __restrict__ eig, int epitch, int w, int h)
 {
     const int x = blockIdx.x * 64 + (threadIdx.x & 63);
     const int yb = blockIdx.y * 16 + (threadIdx.x >> 6);
@@ -291,6 +308,10 @@ __global__ void __launch_bounds__(256) k_eig_from_box(const float* __restrict__ 
             eig[(size_t)y * epitch + x] = (a + c) - sqrtf(t * t + b * b);
         }
     }
+}
+__global__ void __launch_bounds__(256) k_eig_from_box(const float* __restrict__ box, int bp, float* __restrict__ eig, int epitch, int w, int h)
+{
+    eig_from_box_tile<0>(box, bp, eig, epitch, w, h);
 }
 
 }  // namespace gf

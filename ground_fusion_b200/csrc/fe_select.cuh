@@ -56,7 +56,8 @@ __device__ __forceinline__ float float_from_order_key(unsigned int k)
 
 // ------------------------------------------------------------------------------------------------
 constexpr int SM_CF_MAX = 6;   // earlier features within min_dist remembered per feature (more: full rescans)
-__global__ void __launch_bounds__(FE_CAP) k_compact_setmask(TrackScalars* sc, FeatArrays fa, int min_dist)
+template <int V>
+__device__ __forceinline__ void compact_setmask(TrackScalars* sc, const FeatArrays& fa, int min_dist)
 {
     __shared__ sort_elem elems[FE_CAP];
     __shared__ float2 c_pt[FE_CAP];
@@ -187,6 +188,10 @@ __global__ void __launch_bounds__(FE_CAP) k_compact_setmask(TrackScalars* sc, Fe
     }
     GF_DBG(0, c1 - c0); GF_DBG(1, c2 - c1); GF_DBG(2, c3 - c2); GF_DBG(3, gf_clock() - c3);
 }
+__global__ void __launch_bounds__(FE_CAP) k_compact_setmask(TrackScalars* sc, FeatArrays fa, int min_dist)
+{
+    compact_setmask<0>(sc, fa, min_dist);
+}
 
 // ------------------------------------------------------------------------------------------------
 // The mask goodFeaturesToTrack sees (setMask, feature_tracker.cpp:56-83) is 255 except inside the integer disks
@@ -232,7 +237,8 @@ __device__ __forceinline__ bool mask_open(const MaskTile& M, const TrackScalars*
 }
 
 // masked maximum of the eig map (cv::minMaxLoc(eig, 0, &maxVal, 0, 0, mask)); one 64x16 tile per CTA of 256 threads
-__global__ void __launch_bounds__(256) k_eig_max(TrackScalars* sc, const float2* kept, const float* eig, int epitch, int w, int h, int r)
+template <int V>
+__device__ __forceinline__ void eig_max_tile(TrackScalars* sc, const float2* kept, const float* eig, int epitch, int w, int h, int r)
 {
     __shared__ MaskTile M;
     __shared__ unsigned int wb[8];
@@ -252,6 +258,10 @@ __global__ void __launch_bounds__(256) k_eig_max(TrackScalars* sc, const float2*
         if (best) atomicMax(&sc->max_key, best);
     }
 }
+__global__ void __launch_bounds__(256) k_eig_max(TrackScalars* sc, const float2* kept, const float* eig, int epitch, int w, int h, int r)
+{
+    eig_max_tile<0>(sc, kept, eig, epitch, w, h, r);
+}
 
 // Candidate list + the cell grid used by the min-distance pass.  cell = max(min_dist, 16) so that a corner's
 // r-neighbourhood is covered by the 3x3 cells around it.
@@ -264,8 +274,9 @@ struct NmsGrid {
 };
 
 // threshold(TOZERO, 0.01*max) -> dilate 3x3 -> val != 0 && val == dilated && mask, on the interior
-__global__ void __launch_bounds__(256) k_candidates(TrackScalars* sc, const float2* kept, const float* eig, int epitch,
-                                                    int w, int h, int r, NmsGrid g)
+template <int V>
+__device__ __forceinline__ void candidates_tile(TrackScalars* sc, const float2* kept, const float* eig, int epitch, int w, int h, int r,
+                                                const NmsGrid& g)
 {
     __shared__ MaskTile M;
     const int x0 = blockIdx.x * MASK_TX, y0 = blockIdx.y * MASK_TY;
@@ -297,6 +308,11 @@ __global__ void __launch_bounds__(256) k_candidates(TrackScalars* sc, const floa
     }
     }
 }
+__global__ void __launch_bounds__(256) k_candidates(TrackScalars* sc, const float2* kept, const float* eig, int epitch,
+                                                    int w, int h, int r, NmsGrid g)
+{
+    candidates_tile<0>(sc, kept, eig, epitch, w, h, r, g);
+}
 
 // cv::goodFeaturesToTrack's greedy min-distance pass, exact, by rounds (single CTA, 1024 threads):
 //   every alive candidate is killed if one of LAST round's accepted corners in its 3x3 cells is closer than r
@@ -322,6 +338,7 @@ __device__ __forceinline__ int div_cell(int x, float rcp, int cs)
     return q;
 }
 __host__ __device__ inline size_t nms_smem_bytes(int gw, int gh) { return (size_t)(gw + 2) * (gh + 2) * NMS_CELL_BYTES; }
+template <int V>
 __device__ __forceinline__ void nms_cells(TrackScalars* sc, const NmsGrid& g, int w, int min_dist, int want, unsigned char* smem_raw, long long* dbg)
 {
     const int tid = threadIdx.x, nt = blockDim.x;
@@ -533,12 +550,13 @@ __device__ __forceinline__ bool in_any_box(const float4* b, int n, float2 p)
 
 // min-distance rounds, then top-K of the accepted corners, addPoints, undistortedPts, ptsVelocity, depth,
 // next-frame state.  Single CTA of 1024 threads; dynamic shared memory for the cell grid (see nms_cells).
-__global__ void __launch_bounds__(1024) k_select_finalize(TrackScalars* sc, FeatArrays fa, NmsGrid g, int w, int max_cnt, int min_dist,
-                                                          CamParams cam, const double* dt_ptr, const uint16_t* depth, int dpitch /*elements*/,
-                                                          int depth_cam_cfg, const int* depth_valid_ptr, int h, OutHeader* out_hdr, gf_obs* out_obs,
-                                                          uint8_t* out_status /* may be null: copy of the LK status of the n_prev input features */,
-                                                          const BoxSet* boxes = nullptr /* the frame's detections, or null */,
-                                                          uint32_t* out_in_box = nullptr /* FE_CAP bits: output i lies inside a box */)
+template <int V>
+__device__ __forceinline__ void select_finalize(TrackScalars* sc, const FeatArrays& fa, const NmsGrid& g, int w, int max_cnt, int min_dist,
+                                                const CamParams& cam, const double* dt_ptr, const uint16_t* depth, int dpitch /*elements*/,
+                                                int depth_cam_cfg, const int* depth_valid_ptr, int h, OutHeader* out_hdr, gf_obs* out_obs,
+                                                uint8_t* out_status /* may be null: copy of the LK status of the n_prev input features */,
+                                                const BoxSet* boxes /* the frame's detections, or null */,
+                                                uint32_t* out_in_box /* FE_CAP bits: output i lies inside a box; may be null */)
 {
     extern __shared__ __align__(16) unsigned char dyn_smem[];
     __shared__ unsigned long long keys[FE_SORT_CAP];
@@ -549,7 +567,7 @@ __global__ void __launch_bounds__(1024) k_select_finalize(TrackScalars* sc, Feat
     const long long c0 = gf_clock();
     const int n_kept = sc->n_kept;
     const int want = max(max_cnt - n_kept, 0);
-    nms_cells(sc, g, w, min_dist, want, dyn_smem, fa.dbg);
+    nms_cells<V>(sc, g, w, min_dist, want, dyn_smem, fa.dbg);
     const long long c1 = gf_clock();
     const double dt = dt_ptr ? *dt_ptr : 1.0;
     const int depth_cam = depth_cam_cfg && depth_valid_ptr && *depth_valid_ptr;
@@ -655,6 +673,14 @@ __global__ void __launch_bounds__(1024) k_select_finalize(TrackScalars* sc, Feat
         sc->n_prev = total; sc->n_id = n_id + n_new; sc->eig_fixups = 0;
     }
     GF_DBG(8, c1 - c0); GF_DBG(9, c2 - c1); GF_DBG(10, gf_clock() - c2); GF_DBG(11, nacc); GF_DBG(12, ncand);
+}
+__global__ void __launch_bounds__(1024) k_select_finalize(TrackScalars* sc, FeatArrays fa, NmsGrid g, int w, int max_cnt, int min_dist,
+                                                          CamParams cam, const double* dt_ptr, const uint16_t* depth, int dpitch /*elements*/,
+                                                          int depth_cam_cfg, const int* depth_valid_ptr, int h, OutHeader* out_hdr, gf_obs* out_obs,
+                                                          uint8_t* out_status, const BoxSet* boxes = nullptr, uint32_t* out_in_box = nullptr)
+{
+    select_finalize<0>(sc, fa, g, w, max_cnt, min_dist, cam, dt_ptr, depth, dpitch, depth_cam_cfg, depth_valid_ptr, h, out_hdr, out_obs, out_status,
+                    boxes, out_in_box);
 }
 
 }  // namespace gf

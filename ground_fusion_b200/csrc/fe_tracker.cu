@@ -84,12 +84,12 @@ __global__ void __launch_bounds__(LK_THREADS) k_lk_stage(Pyramid I, Pyramid J, c
     if (tid == 0) { next_pts[i] = out; status[i] = (uint8_t)st; }
 }
 
-// Prediction pass (feature_tracker.cpp:118-124): maxLevel 1 seeded with predict_pts; counts successes.
-__global__ void __launch_bounds__(LK_THREADS) k_lk_pred(Pyramid prev, Pyramid cur, TrackScalars* sc, FeatArrays fa, const __grid_constant__ LKMapSet M)
+// Prediction pass (feature_tracker.cpp:118-124): maxLevel 1 seeded with predict_pts; counts successes.  Feature blockIdx.x < n_prev.
+template <int V>
+__device__ __forceinline__ void lk_pred_point(const Pyramid& prev, const Pyramid& cur, TrackScalars* sc, const FeatArrays& fa, const LKMapSet& M)
 {
     __shared__ LKSmem sm;
     const int tid = threadIdx.x, i = blockIdx.x;
-    if (i >= sc->n_prev) return;
     lk_tma_init(sm, tid);
     LKTma T{M.prevI, M.curJ, 0u, M.enabled != 0};
     float2 out;
@@ -98,18 +98,23 @@ __global__ void __launch_bounds__(LK_THREADS) k_lk_pred(Pyramid prev, Pyramid cu
     lk_track_point(sm, tid, prev, cur, fa.prev_pts[i], fa.pred_pts[i], true, 1, out, st, iters, fallbacks, pc, T);
     if (tid == 0) { fa.cur_pts[i] = out; fa.status[i] = (uint8_t)st; if (st) atomicAdd(&sc->pred_succ, 1); atomicAdd(&sc->lk_iters, iters); }
 }
+__global__ void __launch_bounds__(LK_THREADS) k_lk_pred(Pyramid prev, Pyramid cur, TrackScalars* sc, FeatArrays fa, const __grid_constant__ LKMapSet M)
+{
+    if ((int)blockIdx.x >= sc->n_prev) return;
+    lk_pred_point<0>(prev, cur, sc, fa, M);
+}
 
 // Forward LK (3 levels) + reverse check (1 level, USE_INITIAL_FLOW) + inBorder + grey<=250
 // (feature_tracker.cpp:118-168).  One CTA of 4 warps per feature.
 #ifndef GF_TRACK_MIN_CTAS
 #define GF_TRACK_MIN_CTAS 3          // 80 registers: three features per SM when several streams share the GPU (2: 110 registers)
 #endif
-__global__ void __launch_bounds__(LK_THREADS, GF_TRACK_MIN_CTAS) k_track(Pyramid prev, Pyramid cur, TrackScalars* sc, FeatArrays fa,
-                                                      const FrameParams* fp, int flow_back, const __grid_constant__ LKMapSet M)
+template <int V>
+__device__ __forceinline__ void track_point(const Pyramid& prev, const Pyramid& cur, TrackScalars* sc, const FeatArrays& fa,
+                                            const FrameParams* fp, int flow_back, const LKMapSet& M)
 {
     __shared__ LKSmem sm;
     const int tid = threadIdx.x, i = blockIdx.x;
-    if (i >= sc->n_prev) return;
     lk_tma_init(sm, tid);
     LKTma T{M.prevI, M.curJ, 0u, M.enabled != 0};
     const float2 p = fa.prev_pts[i];
@@ -145,6 +150,12 @@ __global__ void __launch_bounds__(LK_THREADS, GF_TRACK_MIN_CTAS) k_track(Pyramid
             fa.dbg[64 + 8 * i + 2] = iters - fallbacks; fa.dbg[64 + 8 * i + 3] = fallbacks;
         }
     }
+}
+__global__ void __launch_bounds__(LK_THREADS, GF_TRACK_MIN_CTAS) k_track(Pyramid prev, Pyramid cur, TrackScalars* sc, FeatArrays fa,
+                                                      const FrameParams* fp, int flow_back, const __grid_constant__ LKMapSet M)
+{
+    if ((int)blockIdx.x >= sc->n_prev) return;
+    track_point<0>(prev, cur, sc, fa, fp, flow_back, M);
 }
 
 // setPrediction (feature_tracker.cpp:1006-1027)
@@ -197,6 +208,107 @@ __global__ void __launch_bounds__(FE_CAP) k_remove_ids(TrackScalars* sc, FeatArr
     if (tid == 0) sc->n_prev = s_m;
 }
 
+// ------------------------------------------------------------------------------------------------
+// gf_tracker_group: the kernels of one frame, run once for every member of the group.  Member m's buffers for the step are
+// row m of a table packed on the host and copied to the device with the frame; each kernel takes m from the grid dimension
+// its single-tracker form does not use (z for 2-D grids, y for 1-D ones, y for the single-CTA kernels) and runs the body the
+// single-tracker kernel runs.
+// ------------------------------------------------------------------------------------------------
+struct GroupMember {
+    Pyramid prev, cur;                 // the member's pyramid slots of this step (cur level 0 holds the frame)
+    const LKMapSet* maps;              // its tensor maps for these slots, in global memory (see lk_maps_acquire)
+    TrackScalars* sc;
+    FeatArrays fa;
+    NmsGrid grid;
+    CamParams cam;
+    float* eig; double* cov; float* box;
+    const uint16_t* depth;
+    const uint8_t* raw; uint8_t* lut;  // equalize: the raw frame and the CLAHE LUTs
+    OutHeader* hdr; gf_obs* obs; uint8_t* status; uint32_t* in_box;    // the member's result block of the step
+    FrameParams fp;
+};
+
+// The 16 maps of a member cannot all be __grid_constant__ parameters of a launch that covers up to GF_TRACKER_GROUP_MAX
+// members, so they are read from global memory.  They are written by a host copy when the group is created, long before any
+// launch that reads them; the tensormap-proxy acquire fence orders that write before the TMA unit's reads, as the PTX memory
+// model requires for a tensor map that is not a kernel parameter.  Threads 0 and 32 are the ones that issue the window loads.
+__device__ __forceinline__ void lk_maps_acquire(const LKMapSet* M, int tid)
+{
+    if ((tid == 0 || tid == 32) && M->enabled) {
+        const CUtensorMap* m = M->prevI;       // prevI, curJ, curI, prevJ are contiguous
+        for (int k = 0; k < 4 * LK_MAXLEV; k++)
+            asm volatile("fence.proxy.tensormap::generic.acquire.gpu [%0], 128;" ::"l"(m + k) : "memory");
+    }
+}
+
+__global__ void __launch_bounds__(PD_TX* PD_TY) k_pyr_down_g(const GroupMember* __restrict__ tab, int l)
+{
+    const GroupMember& G = tab[blockIdx.z];
+    const Level& d = G.cur.lv[l];
+    pyr_down_tile<1>(G.cur.lv[l - 1], const_cast<uint8_t*>(d.ptr), d.w, d.h, d.pitch);
+}
+__global__ void __launch_bounds__(EIG_TX) k_cov_rows_g(const GroupMember* __restrict__ tab)
+{
+    const GroupMember& G = tab[blockIdx.z];
+    cov_rows_tile<1>(G.cur.lv[0], G.cov);
+}
+__global__ void __launch_bounds__(96) k_box_chain_g(const GroupMember* __restrict__ tab, int bp, int w, int h)
+{
+    const GroupMember& G = tab[blockIdx.y];
+    box_chain_block<1>(G.cov, G.box, bp, w, h);
+}
+__global__ void __launch_bounds__(256) k_eig_from_box_g(const GroupMember* __restrict__ tab, int bp, int epitch, int w, int h)
+{
+    const GroupMember& G = tab[blockIdx.z];
+    eig_from_box_tile<1>(G.box, bp, G.eig, epitch, w, h);
+}
+__global__ void __launch_bounds__(CLAHE_LUT_THREADS) k_clahe_lut_g(const GroupMember* __restrict__ tab, long long pitch, ClaheGeom g)
+{
+    const GroupMember& G = tab[blockIdx.y];
+    clahe_lut_tile<1>(G.raw, pitch, g, G.lut);
+}
+__global__ void __launch_bounds__(CLAHE_APPLY_THREADS) k_clahe_apply_g(const GroupMember* __restrict__ tab, long long pitch, ClaheGeom g)
+{
+    const GroupMember& G = tab[blockIdx.y];
+    clahe_apply_rows<1>(G.raw, pitch, g, G.lut, const_cast<uint8_t*>(G.cur.lv[0].ptr), G.cur.lv[0].pitch);
+}
+__global__ void __launch_bounds__(LK_THREADS) k_lk_pred_g(const GroupMember* __restrict__ tab)
+{
+    const GroupMember& G = tab[blockIdx.y];
+    if (!G.fp.has_pred || (int)blockIdx.x >= G.sc->n_prev) return;
+    lk_maps_acquire(G.maps, threadIdx.x);
+    lk_pred_point<1>(G.prev, G.cur, G.sc, G.fa, *G.maps);
+}
+__global__ void __launch_bounds__(LK_THREADS, GF_TRACK_MIN_CTAS) k_track_g(const GroupMember* __restrict__ tab, int flow_back)
+{
+    const GroupMember& G = tab[blockIdx.y];
+    if ((int)blockIdx.x >= G.sc->n_prev) return;
+    lk_maps_acquire(G.maps, threadIdx.x);
+    track_point<1>(G.prev, G.cur, G.sc, G.fa, &G.fp, flow_back, *G.maps);
+}
+__global__ void __launch_bounds__(FE_CAP) k_compact_setmask_g(const GroupMember* __restrict__ tab, int min_dist)
+{
+    const GroupMember& G = tab[blockIdx.y];
+    compact_setmask<1>(G.sc, G.fa, min_dist);
+}
+__global__ void __launch_bounds__(256) k_eig_max_g(const GroupMember* __restrict__ tab, int epitch, int w, int h, int r)
+{
+    const GroupMember& G = tab[blockIdx.z];
+    eig_max_tile<1>(G.sc, G.fa.kept_pts, G.eig, epitch, w, h, r);
+}
+__global__ void __launch_bounds__(256) k_candidates_g(const GroupMember* __restrict__ tab, int epitch, int w, int h, int r)
+{
+    const GroupMember& G = tab[blockIdx.z];
+    candidates_tile<1>(G.sc, G.fa.kept_pts, G.eig, epitch, w, h, r, G.grid);
+}
+__global__ void __launch_bounds__(1024) k_select_finalize_g(const GroupMember* __restrict__ tab, int w, int h, int max_cnt, int min_dist,
+                                                            int dpitch, int depth_cam_cfg)
+{
+    const GroupMember& G = tab[blockIdx.y];
+    select_finalize<1>(G.sc, G.fa, G.grid, w, max_cnt, min_dist, G.cam, &G.fp.dt, G.depth, dpitch, depth_cam_cfg, &G.fp.depth_valid, h,
+                    G.hdr, G.obs, G.status, &G.fp.boxes, G.in_box);
+}
+
 }  // namespace gf
 
 using namespace gf;
@@ -244,6 +356,7 @@ struct gf_tracker {
     uint8_t* h_gray; uint16_t* h_depth; OutBlock* h_out[2]; FrameParams* h_fp[2];
     int* h_tmp_ids; double* h_tmp_xyz;
     long long n_submitted, n_waited;     // frame counters; n_submitted - n_waited frames are in flight
+    int group_steps;                     // of those, steps of a gf_tracker_group (collected by gf_tracker_group_wait only)
     double prev_time;
     bool has_pred, depth_valid[2];
     float last_ms;
@@ -604,11 +717,12 @@ static int body_dep2(gf_tracker* t, long long f)
     return GF_OK;
 }
 
-// Runs one piece: replays its CUDA graph (captured on first use) or, in profiling / GF_NO_GRAPH mode, launches it directly.
+// Runs one piece: replays its CUDA graph (captured on first use) or, when `direct` (profiling / GF_NO_GRAPH mode), launches it
+// directly.
 template <class Body>
-static int run_piece(gf_tracker* t, cudaStream_t s, cudaGraphExec_t* exec, int* nk, Body body)
+static int run_piece(bool direct, cudaStream_t s, cudaGraphExec_t* exec, int* nk, Body body)
 {
-    if (!t->use_graph || t->profiling) return body();
+    if (direct) return body();
     if (!*exec) {
         const uint64_t l0 = g_launches.load();
         cudaGraph_t g = nullptr;
@@ -632,6 +746,7 @@ static int run_piece(gf_tracker* t, cudaStream_t s, cudaGraphExec_t* exec, int* 
 static int enqueue_frame(gf_tracker* t, long long f, double time, bool depth_valid, const gf_box* boxes, int n_boxes)
 {
     const int es = (int)(f % 2), key = (int)(f % 6), hp = t->has_pred ? 1 : 0;
+    const bool direct = !t->use_graph || t->profiling;
     t->h_fp[es]->dt = time - t->prev_time;
     t->h_fp[es]->has_pred = hp;
     t->h_fp[es]->depth_valid = depth_valid ? 1 : 0;
@@ -639,7 +754,7 @@ static int enqueue_frame(gf_tracker* t, long long f, double time, bool depth_val
     GF_MARK(0, t->s_up);   // end of upload
     if (t->equalize) {
         const int slot = (int)(f % 3);
-        int rc = run_piece(t, t->s_up, &t->g_clahe[slot], &t->gk_clahe[slot], [&] {
+        int rc = run_piece(direct, t->s_up, &t->g_clahe[slot], &t->gk_clahe[slot], [&] {
             return enqueue_clahe(t->s_up, t->d_raw, t->raw_pitch, t->clahe, t->d_lut, t->d_pyr[slot][0], t->lp[0]);
         });
         if (rc) return rc;
@@ -647,20 +762,20 @@ static int enqueue_frame(gf_tracker* t, long long f, double time, bool depth_val
     GF_CUDA(cudaEventRecord(t->ev_up[es], t->s_up));
     GF_CUDA(cudaStreamWaitEvent(t->s_pyr, t->ev_up[es], 0));
     GF_CUDA(cudaStreamWaitEvent(t->s_eig, t->ev_up[es], 0));
-    int rc = run_piece(t, t->s_pyr, &t->g_pyr[key], &t->gk_pyr[key], [&] { return body_pyr(t, f); });
+    int rc = run_piece(direct, t->s_pyr, &t->g_pyr[key], &t->gk_pyr[key], [&] { return body_pyr(t, f); });
     if (rc) return rc;
     GF_CUDA(cudaEventRecord(t->ev_pyr[es], t->s_pyr));
     GF_MARK(1, t->s_pyr);
     GF_MARK(7, t->s_eig);
-    rc = run_piece(t, t->s_eig, &t->g_eig[key], &t->gk_eig[key], [&] { return body_eig(t, f); });
+    rc = run_piece(direct, t->s_eig, &t->g_eig[key], &t->gk_eig[key], [&] { return body_eig(t, f); });
     if (rc) return rc;
     GF_CUDA(cudaEventRecord(t->ev_eig[es], t->s_eig));
     GF_MARK(8, t->s_eig);
     GF_CUDA(cudaStreamWaitEvent(t->s_main, t->ev_pyr[es], 0));
-    rc = run_piece(t, t->s_main, &t->g_dep1[key][hp], &t->gk_dep1[key][hp], [&] { return body_dep1(t, f, hp != 0); });
+    rc = run_piece(direct, t->s_main, &t->g_dep1[key][hp], &t->gk_dep1[key][hp], [&] { return body_dep1(t, f, hp != 0); });
     if (rc) return rc;
     GF_CUDA(cudaStreamWaitEvent(t->s_main, t->ev_eig[es], 0));
-    rc = run_piece(t, t->s_main, &t->g_dep2[key], &t->gk_dep2[key], [&] { return body_dep2(t, f); });
+    rc = run_piece(direct, t->s_main, &t->g_dep2[key], &t->gk_dep2[key], [&] { return body_dep2(t, f); });
     if (rc) return rc;
     GF_CUDA(cudaEventRecord(t->ev_dep[es], t->s_main));
     GF_CUDA(cudaStreamWaitEvent(t->s_out, t->ev_dep[es], 0));
@@ -679,6 +794,8 @@ extern "C" {
 static int check_submit(gf_tracker* t)
 {
     if (in_flight(t) >= GF_PIPE) return set_err(GF_ERR_INVALID_ARG, "two frames in flight: call gf_tracker_wait first");
+    // a group step works on this tracker's buffers and state from the group's streams: no direct frame may overlap it
+    if (t->group_steps > 0) return set_err(GF_ERR_INVALID_ARG, "a group step is in flight: collect it with gf_tracker_group_wait first");
     if (t->profiling && in_flight(t) > 0) return set_err(GF_ERR_INVALID_ARG, "profiling mode runs one frame at a time");
     return GF_OK;
 }
@@ -734,6 +851,7 @@ int gf_tracker_wait_boxes(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* in_bo
 {
     if (!t) return set_err(GF_ERR_INVALID_ARG, "null tracker");
     if (in_flight(t) == 0) return set_err(GF_ERR_INVALID_ARG, "no frame in flight");
+    if (t->group_steps > 0) return set_err(GF_ERR_INVALID_ARG, "the frame in flight is a group step: collect it with gf_tracker_group_wait");
     GF_CUDA(cudaSetDevice(t->device));
     const int es = (int)(t->n_waited % 2);
     GF_CUDA(cudaEventSynchronize(t->ev_out[es]));
@@ -967,6 +1085,402 @@ int gf_tracker_last_device_ms(gf_tracker* t, float* ms)
 {
     if (!t || !ms) return set_err(GF_ERR_INVALID_ARG, "null argument");
     *ms = t->last_ms;
+    return GF_OK;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------
+// gf_tracker_group: the frame of every member tracked by one set of launches per step.  The orchestration is the tracker's
+// (upload -> pyramid || min-eig map -> dependent chain -> download on five streams, two steps in flight, so step t+1's
+// pyramids and min-eig maps overlap step t's chain); the buffers are the members' own, named per step in a table
+// (GroupMember), so the graphs only alternate with the table and result buffers.
+// ------------------------------------------------------------------------------------------------
+struct gf_tracker_group {
+    int n, device;
+    std::vector<gf_tracker*> m;
+    cudaStream_t s_up, s_pyr, s_eig, s_main, s_out;
+    cudaEvent_t ev_up[2], ev_pyr[2], ev_eig[2], ev_dep[2], ev_t0[2], ev_out[2];
+    // CUDA graphs keyed by step parity and, for the first piece of the chain, by whether any member has a prediction
+    cudaGraphExec_t g_clahe[2], g_pyr[2], g_eig[2], g_dep1[2][2], g_dep2[2];
+    int gk_clahe[2], gk_pyr[2], gk_eig[2], gk_dep1[2][2], gk_dep2[2];
+    bool use_graph, equalize;
+    ClaheGeom clahe;                        // the members' equalize setting when the group was created (see group_submit)
+    LKMapSet* d_maps;                       // [n][3]: the members' lk_maps, read by the LK kernels from global memory
+    GroupMember* d_tab[2]; GroupMember* h_tab[2];
+    // member i's result block of a step is the OutBlock prefix up to obs[max_cnt] at i * out_stride: one D2H copy per step
+    uint8_t* d_out[2]; uint8_t* h_out[2]; size_t out_stride;
+    std::vector<uint8_t> depth_valid[2];    // per step in flight: which members had a depth image
+    long long n_submitted, n_waited;
+};
+
+static inline int group_in_flight(const gf_tracker_group* g) { return (int)(g->n_submitted - g->n_waited); }
+
+static int member_err(int code, int k, const char* what)
+{
+    snprintf(g_err, sizeof(g_err), "member %d: %s", k, what);
+    return code;
+}
+static int member_prefix(int rc, int k)         // an error text raised for one member's arguments, naming the member
+{
+    char keep[sizeof(g_err)];
+    memcpy(keep, g_err, sizeof(keep));
+    snprintf(g_err, sizeof(g_err), "member %d: %s", k, keep);
+    return rc;
+}
+
+// What the members of a group share: every kernel of a step is launched once with this geometry and configuration.
+static const char* group_mismatch(const gf_tracker* a, const gf_tracker* t)
+{
+    if (t->device != a->device) return "bound to another device";
+    if (t->w != a->w || t->h != a->h) return "image size differs from member 0";
+    if (t->cfg.max_cnt != a->cfg.max_cnt) return "max_cnt differs from member 0";
+    if (t->cfg.min_dist != a->cfg.min_dist) return "min_dist differs from member 0";
+    if (t->cfg.flow_back != a->cfg.flow_back) return "flow_back differs from member 0";
+    if (t->cfg.depth_cam != a->cfg.depth_cam) return "depth_cam differs from member 0";
+    if (t->equalize != a->equalize || (t->equalize && memcmp(&t->clahe, &a->clahe, sizeof(ClaheGeom)) != 0))
+        return "equalize setting differs from member 0";
+    return nullptr;
+}
+
+static int group_init(gf_tracker_group* g)
+{
+    const gf_tracker* a = g->m[0];
+    GF_CUDA(cudaStreamCreateWithFlags(&g->s_up, cudaStreamNonBlocking));
+    GF_CUDA(cudaStreamCreateWithFlags(&g->s_pyr, cudaStreamNonBlocking));
+    GF_CUDA(cudaStreamCreateWithFlags(&g->s_eig, cudaStreamNonBlocking));
+    GF_CUDA(cudaStreamCreateWithFlags(&g->s_main, cudaStreamNonBlocking));
+    GF_CUDA(cudaStreamCreateWithFlags(&g->s_out, cudaStreamNonBlocking));
+    g->out_stride = align_up((int)(offsetof(OutBlock, obs) + (size_t)a->cfg.max_cnt * sizeof(gf_obs)), 16);
+    for (int i = 0; i < 2; i++) {
+        GF_CUDA(cudaEventCreateWithFlags(&g->ev_up[i], cudaEventDisableTiming));
+        GF_CUDA(cudaEventCreateWithFlags(&g->ev_pyr[i], cudaEventDisableTiming));
+        GF_CUDA(cudaEventCreateWithFlags(&g->ev_eig[i], cudaEventDisableTiming));
+        GF_CUDA(cudaEventCreateWithFlags(&g->ev_dep[i], cudaEventDisableTiming));
+        GF_CUDA(cudaEventCreate(&g->ev_t0[i]));
+        GF_CUDA(cudaEventCreate(&g->ev_out[i]));
+        GF_CUDA(cudaMalloc(&g->d_tab[i], (size_t)g->n * sizeof(GroupMember)));
+        GF_CUDA(cudaHostAlloc(&g->h_tab[i], (size_t)g->n * sizeof(GroupMember), cudaHostAllocDefault));
+        memset(g->h_tab[i], 0, (size_t)g->n * sizeof(GroupMember));
+        GF_CUDA(cudaMalloc(&g->d_out[i], (size_t)g->n * g->out_stride));
+        GF_CUDA(cudaHostAlloc(&g->h_out[i], (size_t)g->n * g->out_stride, cudaHostAllocDefault));
+        g->depth_valid[i].assign((size_t)g->n, 0);
+    }
+    GF_CUDA(cudaMalloc(&g->d_maps, (size_t)g->n * 3 * sizeof(LKMapSet)));
+    for (int k = 0; k < g->n; k++)
+        GF_CUDA(cudaMemcpy(g->d_maps + 3 * k, g->m[k]->lk_maps, 3 * sizeof(LKMapSet), cudaMemcpyHostToDevice));
+    GF_CUDA(cudaFuncSetAttribute(k_box_chain_g, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BC_SMEM));
+    GF_CUDA(cudaFuncSetAttribute(k_select_finalize_g, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+    GF_CUDA(cudaFuncSetAttribute(k_clahe_apply_g, cudaFuncAttributeMaxDynamicSharedMemorySize, CLAHE_MAX_TILES * CLAHE_MAX_TILES * 256));
+    g->equalize = a->equalize;
+    g->clahe = a->clahe;
+    g->use_graph = getenv("GF_NO_GRAPH") == nullptr;
+    return GF_OK;
+}
+
+// ---- the four capturable pieces of a step (and CLAHE), every kernel once for all members ----
+static int group_body_clahe(gf_tracker_group* g, int gs)
+{
+    const gf_tracker* a = g->m[0];
+    const ClaheGeom& c = g->clahe;
+    k_clahe_lut_g<<<dim3(c.tiles_x * c.tiles_y, g->n), CLAHE_LUT_THREADS, 0, g->s_up>>>(g->d_tab[gs], a->raw_pitch, c); GF_LAUNCHED();
+    k_clahe_apply_g<<<dim3((c.h + CLAHE_APPLY_ROWS - 1) / CLAHE_APPLY_ROWS, g->n), CLAHE_APPLY_THREADS, clahe_lut_bytes(c), g->s_up>>>(
+        g->d_tab[gs], a->raw_pitch, c); GF_LAUNCHED();
+    GF_CUDA(cudaGetLastError());
+    return GF_OK;
+}
+
+static int group_body_pyr(gf_tracker_group* g, int gs)
+{
+    const gf_tracker* a = g->m[0];
+    for (int l = 1; l < 4; l++) {
+        dim3 grid((a->lw[l] + PD_TX - 1) / PD_TX, (a->lh[l] + PD_TY - 1) / PD_TY, g->n), b(PD_TX, PD_TY);
+        k_pyr_down_g<<<grid, b, 0, g->s_pyr>>>(g->d_tab[gs], l); GF_LAUNCHED();
+    }
+    GF_CUDA(cudaGetLastError());
+    return GF_OK;
+}
+
+static int group_body_eig(gf_tracker_group* g, int gs)
+{
+    const gf_tracker* a = g->m[0];
+    const int w = a->w, h = a->h, bp = (w + 31) / 32 * 32;
+    cudaStream_t s = g->s_eig;
+    k_cov_rows_g<<<dim3((w + EIG_TX - 1) / EIG_TX, (h + EIG_BAND - 1) / EIG_BAND, g->n), EIG_TX, 0, s>>>(g->d_tab[gs]); GF_LAUNCHED();
+    k_box_chain_g<<<dim3((w + 31) / 32, g->n), 96, BC_SMEM, s>>>(g->d_tab[gs], bp, w, h); GF_LAUNCHED();
+    k_eig_from_box_g<<<dim3((w + 63) / 64, (h + 15) / 16, g->n), 256, 0, s>>>(g->d_tab[gs], bp, a->epitch, w, h); GF_LAUNCHED();
+    GF_CUDA(cudaGetLastError());
+    return GF_OK;
+}
+
+static int group_body_dep1(gf_tracker_group* g, int gs, bool any_pred)
+{
+    const gf_tracker* a = g->m[0];
+    cudaStream_t s = g->s_main;
+    const dim3 lk(a->cfg.max_cnt, g->n);
+    if (any_pred) { k_lk_pred_g<<<lk, LK_THREADS, 0, s>>>(g->d_tab[gs]); GF_LAUNCHED(); }
+    k_track_g<<<lk, LK_THREADS, 0, s>>>(g->d_tab[gs], a->cfg.flow_back); GF_LAUNCHED();
+    k_compact_setmask_g<<<dim3(1, g->n), FE_CAP, 0, s>>>(g->d_tab[gs], a->cfg.min_dist); GF_LAUNCHED();
+    GF_CUDA(cudaGetLastError());
+    return GF_OK;
+}
+
+static int group_body_dep2(gf_tracker_group* g, int gs)
+{
+    const gf_tracker* a = g->m[0];
+    const int w = a->w, h = a->h, md = a->cfg.min_dist;
+    cudaStream_t s = g->s_main;
+    const dim3 tg((w + MASK_TX - 1) / MASK_TX, (h + MASK_TY - 1) / MASK_TY, g->n);
+    k_eig_max_g<<<tg, 256, 0, s>>>(g->d_tab[gs], a->epitch, w, h, md); GF_LAUNCHED();
+    k_candidates_g<<<tg, 256, 0, s>>>(g->d_tab[gs], a->epitch, w, h, md); GF_LAUNCHED();
+    k_select_finalize_g<<<dim3(1, g->n), 1024, a->grid_cells, s>>>(g->d_tab[gs], w, h, a->cfg.max_cnt, md, a->depth_pitch_el,
+                                                                  a->cfg.depth_cam ? 1 : 0); GF_LAUNCHED();
+    GF_CUDA(cudaGetLastError());
+    return GF_OK;
+}
+
+// One step: member i tracks (times[i], gray[i], depth[i]) with the boxes bx[i][0 .. nb[i]) (box lists already checked).
+static int group_submit(gf_tracker_group* g, const double* times, const void* const* gray, size_t gray_pitch, const void* const* depth,
+                        size_t depth_pitch, bool on_device, const gf_box* const* bx, const int* nb)
+{
+    if (group_in_flight(g) >= GF_PIPE) return set_err(GF_ERR_INVALID_ARG, "two steps in flight: call gf_tracker_group_wait first");
+    const gf_tracker* a = g->m[0];
+    const int w = a->w, h = a->h;
+    if (on_device) {
+        gray_pitch = w; depth_pitch = (size_t)w * 2;
+    } else {
+        if (gray_pitch < (size_t)w) return set_err(GF_ERR_INVALID_ARG, "gray_pitch smaller than width");
+        if (depth && depth_pitch < (size_t)w * 2) return set_err(GF_ERR_INVALID_ARG, "depth_pitch smaller than width*2");
+    }
+    for (int i = 0; i < g->n; i++) {
+        const gf_tracker* t = g->m[i];
+        if (!gray[i]) return member_err(GF_ERR_INVALID_ARG, i, "null frame pointer");
+        if (in_flight(t) != group_in_flight(g)) return member_err(GF_ERR_INVALID_ARG, i, "has a frame in flight outside this group");
+        if (t->profiling) return member_err(GF_ERR_INVALID_ARG, i, "is in profiling mode");
+        // gf_tracker_set_equalize is still accepted on a member that has tracked no frame; the graphs and the frame intake
+        // of the group follow the setting the members had when the group was created
+        if (t->equalize != g->equalize || (g->equalize && memcmp(&t->clahe, &g->clahe, sizeof(ClaheGeom)) != 0))
+            return member_err(GF_ERR_INVALID_ARG, i, "equalize setting changed since the group was created");
+    }
+    GF_CUDA(cudaSetDevice(g->device));
+    const int gs = (int)(g->n_submitted % 2);
+    bool any_pred = false;
+    for (int i = 0; i < g->n; i++) {
+        gf_tracker* t = g->m[i];
+        const long long f = t->n_submitted;
+        const int es = (int)(f % 2), slot = (int)(f % 3);
+        GroupMember& G = g->h_tab[gs][i];
+        G.prev = make_pyr(t, (slot + 2) % 3); G.cur = make_pyr(t, slot);
+        G.maps = g->d_maps + 3 * i + slot;
+        G.sc = t->d_sc; G.fa = t->fa; G.grid = t->grid; G.cam = t->cam;
+        G.eig = t->d_eig[es]; G.cov = t->d_cov; G.box = t->d_box;
+        G.depth = t->d_depth[es]; G.raw = t->d_raw; G.lut = t->d_lut;
+        uint8_t* ob = g->d_out[gs] + (size_t)i * g->out_stride;
+        G.hdr = reinterpret_cast<OutHeader*>(ob + offsetof(OutBlock, hdr)); G.obs = reinterpret_cast<gf_obs*>(ob + offsetof(OutBlock, obs));
+        G.status = ob + offsetof(OutBlock, status); G.in_box = reinterpret_cast<uint32_t*>(ob + offsetof(OutBlock, in_box));
+        G.fp.dt = times[i] - t->prev_time;
+        G.fp.has_pred = t->has_pred ? 1 : 0;
+        G.fp.depth_valid = (depth && depth[i]) ? 1 : 0;
+        put_boxes(G.fp.boxes, bx ? bx[i] : nullptr, nb ? nb[i] : 0);
+        any_pred |= t->has_pred;
+    }
+    const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    cudaStream_t s = g->s_up;
+    GF_CUDA(cudaEventRecord(g->ev_t0[gs], s));
+    GF_CUDA(cudaMemcpyAsync(g->d_tab[gs], g->h_tab[gs], (size_t)g->n * sizeof(GroupMember), cudaMemcpyHostToDevice, s));
+    for (int i = 0; i < g->n; i++) {
+        const gf_tracker* t = g->m[i];
+        const int es = (int)(t->n_submitted % 2);
+        if (g->equalize) GF_CUDA(cudaMemcpy2DAsync(t->d_raw, t->raw_pitch, gray[i], gray_pitch, w, h, kind, s));
+        else GF_CUDA(cudaMemcpy2DAsync(t->d_pyr[t->n_submitted % 3][0], t->lp[0], gray[i], gray_pitch, w, h, kind, s));
+        if (depth && depth[i])
+            GF_CUDA(cudaMemcpy2DAsync(t->d_depth[es], (size_t)t->depth_pitch_el * 2, depth[i], depth_pitch, (size_t)w * 2, h, kind, s));
+    }
+    const bool direct = !g->use_graph;
+    const int hp = any_pred ? 1 : 0;
+    int rc;
+    if (g->equalize && (rc = run_piece(direct, s, &g->g_clahe[gs], &g->gk_clahe[gs], [&] { return group_body_clahe(g, gs); }))) return rc;
+    GF_CUDA(cudaEventRecord(g->ev_up[gs], s));
+    GF_CUDA(cudaStreamWaitEvent(g->s_pyr, g->ev_up[gs], 0));
+    GF_CUDA(cudaStreamWaitEvent(g->s_eig, g->ev_up[gs], 0));
+    if ((rc = run_piece(direct, g->s_pyr, &g->g_pyr[gs], &g->gk_pyr[gs], [&] { return group_body_pyr(g, gs); }))) return rc;
+    GF_CUDA(cudaEventRecord(g->ev_pyr[gs], g->s_pyr));
+    if ((rc = run_piece(direct, g->s_eig, &g->g_eig[gs], &g->gk_eig[gs], [&] { return group_body_eig(g, gs); }))) return rc;
+    GF_CUDA(cudaEventRecord(g->ev_eig[gs], g->s_eig));
+    GF_CUDA(cudaStreamWaitEvent(g->s_main, g->ev_pyr[gs], 0));
+    if ((rc = run_piece(direct, g->s_main, &g->g_dep1[gs][hp], &g->gk_dep1[gs][hp], [&] { return group_body_dep1(g, gs, any_pred); }))) return rc;
+    GF_CUDA(cudaStreamWaitEvent(g->s_main, g->ev_eig[gs], 0));
+    if ((rc = run_piece(direct, g->s_main, &g->g_dep2[gs], &g->gk_dep2[gs], [&] { return group_body_dep2(g, gs); }))) return rc;
+    GF_CUDA(cudaEventRecord(g->ev_dep[gs], g->s_main));
+    GF_CUDA(cudaStreamWaitEvent(g->s_out, g->ev_dep[gs], 0));
+    GF_CUDA(cudaMemcpyAsync(g->h_out[gs], g->d_out[gs], (size_t)g->n * g->out_stride, cudaMemcpyDeviceToHost, g->s_out));
+    GF_CUDA(cudaEventRecord(g->ev_out[gs], g->s_out));
+    for (int i = 0; i < g->n; i++) {          // the members' host-side state advances as enqueue_frame advances it
+        gf_tracker* t = g->m[i];
+        const bool dv = depth && depth[i];
+        t->prev_time = times[i];
+        t->has_pred = false;
+        t->depth_valid[t->n_submitted % 2] = dv;
+        t->n_submitted++;
+        t->group_steps++;
+        g->depth_valid[gs][i] = dv ? 1 : 0;
+    }
+    g->n_submitted++;
+    return GF_OK;
+}
+
+// Collects the oldest step: member i's results at out + i*out_stride, in_box / status_out likewise, n_out[i*n_stride],
+// info[i*n_stride].
+static int group_collect(gf_tracker_group* g, gf_obs* out, size_t out_stride, int* n_out, size_t n_stride, uint8_t* in_box,
+                         uint8_t* status_out, gf_track_info* info)
+{
+    if (group_in_flight(g) == 0) return set_err(GF_ERR_INVALID_ARG, "no step in flight");
+    GF_CUDA(cudaSetDevice(g->device));
+    const int gs = (int)(g->n_waited % 2);
+    GF_CUDA(cudaEventSynchronize(g->ev_out[gs]));
+    float ms = 0.f;
+    GF_CUDA(cudaEventElapsedTime(&ms, g->ev_t0[gs], g->ev_out[gs]));
+    g->n_waited++;
+    for (int i = 0; i < g->n; i++) {
+        gf_tracker* t = g->m[i];
+        t->n_waited++;
+        t->group_steps--;
+        t->last_ms = ms;
+        const uint8_t* ob = g->h_out[gs] + (size_t)i * g->out_stride;
+        const OutHeader& hd = *reinterpret_cast<const OutHeader*>(ob + offsetof(OutBlock, hdr));
+        const uint32_t* bits = reinterpret_cast<const uint32_t*>(ob + offsetof(OutBlock, in_box));
+        int n = hd.n_out;
+        if (t->cfg.depth_cam && !g->depth_valid[gs][i]) n = 0;   // see body_dep2
+        const size_t o = (size_t)i * out_stride, q = (size_t)i * n_stride;
+        if (n_out) n_out[q] = n;
+        if (out && n > 0) memcpy(out + o, ob + offsetof(OutBlock, obs), (size_t)n * sizeof(gf_obs));
+        if (in_box) for (int k = 0; k < n; k++) in_box[o + k] = (uint8_t)((bits[k >> 5] >> (k & 31)) & 1u);
+        if (status_out && hd.n_prev > 0) memcpy(status_out + o, ob + offsetof(OutBlock, status), hd.n_prev);
+        if (info) {
+            gf_track_info& r = info[q];
+            r.n_prev = hd.n_prev; r.n_tracked = hd.n_tracked; r.n_kept = hd.n_kept; r.n_new = hd.n_new;
+            r.n_candidates = hd.n_cand; r.nms_rounds = hd.nms_rounds; r.eig_fixups = hd.eig_fixups; r.lk_iterations = hd.lk_iters;
+        }
+    }
+    return GF_OK;
+}
+
+extern "C" {
+
+void gf_tracker_group_destroy(gf_tracker_group* g)
+{
+    if (!g) return;
+    cudaSetDevice(g->device);
+    cudaDeviceSynchronize();
+    for (; g->n_waited < g->n_submitted; g->n_waited++)       // steps still in flight are complete: the members move on
+        for (gf_tracker* t : g->m) { t->n_waited++; t->group_steps--; }
+    for (int k = 0; k < 2; k++) {
+        for (cudaGraphExec_t e : {g->g_clahe[k], g->g_pyr[k], g->g_eig[k], g->g_dep1[k][0], g->g_dep1[k][1], g->g_dep2[k]})
+            if (e) cudaGraphExecDestroy(e);
+        cudaFree(g->d_tab[k]); cudaFreeHost(g->h_tab[k]); cudaFree(g->d_out[k]); cudaFreeHost(g->h_out[k]);
+        for (cudaEvent_t e : {g->ev_up[k], g->ev_pyr[k], g->ev_eig[k], g->ev_dep[k], g->ev_t0[k], g->ev_out[k]}) if (e) cudaEventDestroy(e);
+    }
+    cudaFree(g->d_maps);
+    for (cudaStream_t s : {g->s_up, g->s_pyr, g->s_eig, g->s_main, g->s_out}) if (s) cudaStreamDestroy(s);
+    cudaGetLastError();
+    delete g;
+}
+
+int gf_tracker_group_create(gf_tracker_group** out, gf_tracker* const* members, int n)
+{
+    if (!out) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    *out = nullptr;
+    if (n > GF_TRACKER_GROUP_MAX) return set_err(GF_ERR_CAPACITY, "more than GF_TRACKER_GROUP_MAX members");
+    if (n < 1 || !members) return set_err(GF_ERR_INVALID_ARG, "a group needs at least one member");
+    for (int k = 0; k < n; k++) {
+        const gf_tracker* t = members[k];
+        if (!t) return member_err(GF_ERR_INVALID_ARG, k, "null tracker");
+        for (int j = 0; j < k; j++) if (members[j] == t) return member_err(GF_ERR_INVALID_ARG, k, "the same tracker listed twice");
+        const char* why = group_mismatch(members[0], t);
+        if (why) return member_err(GF_ERR_INVALID_ARG, k, why);
+        if (in_flight(t) > 0) return member_err(GF_ERR_INVALID_ARG, k, "has a frame in flight");
+        if (t->profiling) return member_err(GF_ERR_INVALID_ARG, k, "is in profiling mode");
+    }
+    GF_CUDA(cudaSetDevice(members[0]->device));
+    gf_tracker_group* g = new (std::nothrow) gf_tracker_group();
+    if (!g) return set_err(GF_ERR_CUDA, "out of host memory");
+    g->n = n; g->device = members[0]->device;
+    g->m.assign(members, members + n);
+    int rc = group_init(g);
+    if (rc) {
+        char keep[sizeof(g_err)];
+        memcpy(keep, g_err, sizeof(keep));
+        gf_tracker_group_destroy(g);
+        memcpy(g_err, keep, sizeof(keep));
+        return rc;
+    }
+    *out = g;
+    return GF_OK;
+}
+
+int gf_tracker_group_submit(gf_tracker_group* g, const double* times, const void* const* gray, size_t gray_pitch,
+                            const void* const* depth, size_t depth_pitch, int on_device, const gf_box* boxes, const int* box_start)
+{
+    if (!g || !times || !gray) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    std::vector<const gf_box*> bx((size_t)g->n, nullptr);
+    std::vector<int> nb((size_t)g->n, 0);
+    if (box_start) {
+        for (int i = 0; i < g->n; i++) {
+            if (box_start[i] < 0) return member_err(GF_ERR_INVALID_ARG, i, "bad box offsets");
+            bx[i] = boxes ? boxes + box_start[i] : nullptr;
+            nb[i] = box_start[i + 1] - box_start[i];
+            int rc = check_boxes(bx[i], nb[i]);
+            if (rc) return member_prefix(rc, i);
+        }
+    }
+    return group_submit(g, times, gray, gray_pitch, depth, depth_pitch, on_device != 0, bx.data(), nb.data());
+}
+
+int gf_tracker_group_wait(gf_tracker_group* g, gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info)
+{
+    if (!g) return set_err(GF_ERR_INVALID_ARG, "null group");
+    return group_collect(g, out, (size_t)g->m[0]->cfg.max_cnt, n_out, 1, in_box, status_out, info);
+}
+
+int gf_tracker_group_track_batch(gf_tracker_group* g, int n_steps, const double* times, const void* const* gray, size_t gray_pitch,
+                                 const void* const* depth, size_t depth_pitch, int on_device, const gf_box* boxes, const int* box_start,
+                                 gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info)
+{
+    if (!g || n_steps < 0 || (n_steps > 0 && (!times || !gray))) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    if (group_in_flight(g) > 0) return set_err(GF_ERR_INVALID_ARG, "a step in flight: call gf_tracker_group_wait first");
+    const int K = g->n, n = n_steps;
+    for (int i = 0; i < K; i++)             // every frame pointer and box list is checked before the first step is submitted
+        for (int k = 0; k < n; k++) {
+            const size_t j = (size_t)i * n + k;
+            if (!gray[j]) return member_err(GF_ERR_INVALID_ARG, i, "null frame pointer");
+            if (box_start) {
+                if (box_start[j] < 0) return member_err(GF_ERR_INVALID_ARG, i, "bad box offsets");
+                int rc = check_boxes(boxes ? boxes + box_start[j] : nullptr, box_start[j + 1] - box_start[j]);
+                if (rc) return member_prefix(rc, i);
+            }
+        }
+    std::vector<double> ts((size_t)K);
+    std::vector<const void*> gp((size_t)K), dp((size_t)K);
+    std::vector<const gf_box*> bx((size_t)K, nullptr);
+    std::vector<int> nb((size_t)K, 0);
+    const size_t cap = (size_t)g->m[0]->cfg.max_cnt;
+    int collected = 0, rc;
+    auto collect = [&]() {
+        const size_t j = (size_t)collected++;
+        return group_collect(g, out ? out + j * cap : nullptr, (size_t)n * cap, n_out ? n_out + j : nullptr, (size_t)n,
+                             in_box ? in_box + j * cap : nullptr, status_out ? status_out + j * cap : nullptr, info ? info + j : nullptr);
+    };
+    for (int k = 0; k < n; k++) {
+        for (int i = 0; i < K; i++) {
+            const size_t j = (size_t)i * n + k;
+            ts[i] = times[j]; gp[i] = gray[j]; dp[i] = depth ? depth[j] : nullptr;
+            if (box_start) { bx[i] = boxes ? boxes + box_start[j] : nullptr; nb[i] = box_start[j + 1] - box_start[j]; }
+        }
+        if ((rc = group_submit(g, ts.data(), gp.data(), gray_pitch, depth ? dp.data() : nullptr, depth_pitch, on_device != 0, bx.data(), nb.data())))
+            return rc;
+        if (group_in_flight(g) == GF_PIPE && (rc = collect())) return rc;
+    }
+    while (group_in_flight(g) > 0) if ((rc = collect())) return rc;
     return GF_OK;
 }
 

@@ -39,6 +39,11 @@ inline int set_err(int code, const char* fmt, const char* a = "", const char* b 
 #define gf_clock() 0LL
 #endif
 
+// Front-end kernel bodies run by a single-tracker kernel and by its group form (gf_tracker_group) are templates on an int V
+// that each kernel instantiates with its own value (0: single tracker, 1: group).  A static __shared__ variable of a device
+// function is one object per instantiation, and with relocatable device code (-dc) the linker places an object that two
+// kernels use at the same offset in both, which would merge their shared-memory layouts.
+
 // BORDER_REFLECT_101; valid for -n < i < 2n-1
 __host__ __device__ __forceinline__ int reflect101(int i, int n)
 {

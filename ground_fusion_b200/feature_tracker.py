@@ -262,6 +262,7 @@ class FeatureTracker:
         st = np.zeros((S, n, a.max_cnt), np.uint8) if want else None
         cnt = np.zeros((S, n), np.int32)
         info = (TrackInfo * (S * n))()
+        ib = None
         if boxes is None:
             check(a.L.gf_tracker_track_batch_multi(h, S, n, t.ctypes.data, g, int(gray_pitch or a.width), d, int(depth_pitch or 2 * a.width),
                                                    int(bool(on_device)), obs.ctypes.data if want else None, cnt.ctypes.data,
@@ -274,15 +275,22 @@ class FeatureTracker:
                                                          int(bool(on_device)), bx.ctypes.data if len(bx) else None, start.ctypes.data,
                                                          obs.ctypes.data if want else None, cnt.ctypes.data, ib.ctypes.data if want else None,
                                                          st.ctypes.data if want else None, info))
+        return FeatureTracker._results(trackers, n, obs, st, cnt, info, ib)
+
+    @staticmethod
+    def _results(trackers, n, obs, st, cnt, info, ib):
+        """Per tracker lists of n (obs, status, info[, in_box]) from the (S, n, max_cnt) result arrays of a multi-stream call;
+        updates every tracker's batch_infos / last_info."""
         for i, tr in enumerate(trackers):
             tr.batch_infos = [info[i * n + k].as_dict() for k in range(n)]
             tr.last_info = tr.batch_infos[-1] if n else {}
-        if not want:
+        if obs is None:
             return None
-        if boxes is not None:
+        if ib is not None:
             return [[(obs[i, k, :cnt[i, k]].copy(), st[i, k, :info[i * n + k].n_prev].copy(), info[i * n + k].as_dict(),
-                      ib[i, k, :cnt[i, k]].view(np.bool_).copy()) for k in range(n)] for i in range(S)]
-        return [[(obs[i, k, :cnt[i, k]].copy(), st[i, k, :info[i * n + k].n_prev].copy(), info[i * n + k].as_dict()) for k in range(n)] for i in range(S)]
+                      ib[i, k, :cnt[i, k]].view(np.bool_).copy()) for k in range(n)] for i in range(len(trackers))]
+        return [[(obs[i, k, :cnt[i, k]].copy(), st[i, k, :info[i * n + k].n_prev].copy(), info[i * n + k].as_dict()) for k in range(n)]
+                for i in range(len(trackers))]
 
     def submitDevice(self, cur_time, d_gray_ptr, d_depth_ptr=None):
         check(self.L.gf_tracker_submit_device(self._h, float(cur_time), d_gray_ptr, d_depth_ptr))
@@ -328,3 +336,88 @@ class FeatureTracker:
         ms = ctypes.c_float(0)
         check(self.L.gf_tracker_last_device_ms(self._h, ctypes.byref(ms)))
         return ms.value
+
+
+class TrackerGroup:
+    """gf_tracker_group: several FeatureTrackers of one geometry and configuration (a multi-camera rig, several robots) that
+    track frame k of their streams in lockstep with one set of kernel launches per step.  Every member's results and state are
+    exactly what its own trackBatch would give; the members stay usable on their own between steps.
+
+    Frames are given as integer addresses, as for trackBatch: host (ideally pinned) or device (on_device, tightly packed)."""
+
+    def __init__(self, trackers):
+        self.members = list(trackers)
+        self.L = _lib.lib()
+        self._h = ctypes.c_void_p()
+        h = (ctypes.c_void_p * len(self.members))(*[tr._h for tr in self.members])
+        check(self.L.gf_tracker_group_create(ctypes.byref(self._h), h, len(self.members)))
+        self.max_cnt = self.members[0].max_cnt
+        S = len(self.members)
+        self._obs = np.zeros((S, self.max_cnt), OBS_DTYPE)
+        self._status = np.zeros((S, self.max_cnt), np.uint8)
+        self._in_box = np.zeros((S, self.max_cnt), np.uint8)
+
+    def close(self):
+        if self._h:
+            self.L.gf_tracker_group_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def submit(self, times, gray_ptrs, depth_ptrs=None, on_device=False, gray_pitch=None, depth_pitch=None, boxes=None):
+        """One step: member i tracks (times[i], gray_ptrs[i], depth_ptrs[i] or None) with the (m, 4) detections boxes[i].
+        Up to two steps may be in flight; collect them in order with wait().  Host frames are read after this call returns:
+        keep them unchanged until wait()."""
+        S = len(self.members)
+        assert len(times) == S and len(gray_ptrs) == S
+        t = np.ascontiguousarray(times, np.float64)
+        g = (ctypes.c_void_p * S)(*[int(p) for p in gray_ptrs])
+        d = (ctypes.c_void_p * S)(*[(int(p) if p else None) for p in depth_ptrs]) if depth_ptrs is not None else None
+        bx, start = _box_csr(boxes) if boxes is not None else (np.zeros((0, 4), np.int64), None)
+        w = self.members[0].width
+        check(self.L.gf_tracker_group_submit(self._h, t.ctypes.data, g, int(gray_pitch or w), d, int(depth_pitch or 2 * w), int(bool(on_device)),
+                                             bx.ctypes.data if len(bx) else None, start.ctypes.data if start is not None else None))
+
+    def wait(self):
+        """The oldest step: per member (obs, status, info, in_box), as trackImageboxRaw plus the status and info of the frame."""
+        S = len(self.members)
+        cnt = np.zeros(S, np.int32)
+        info = (TrackInfo * S)()
+        check(self.L.gf_tracker_group_wait(self._h, self._obs.ctypes.data, cnt.ctypes.data, self._in_box.ctypes.data,
+                                           self._status.ctypes.data, info))
+        out = []
+        for i, tr in enumerate(self.members):
+            tr.last_info = info[i].as_dict()
+            tr.last_status = self._status[i, :info[i].n_prev].copy()
+            out.append((self._obs[i, :cnt[i]].copy(), tr.last_status.copy(), tr.last_info,
+                        self._in_box[i, :cnt[i]].view(np.bool_).copy()))
+        return out
+
+    def trackBatch(self, times, gray_ptrs, depth_ptrs=None, on_device=False, gray_pitch=None, depth_pitch=None, want=True, boxes=None):
+        """n steps in one call (gf_tracker_group_track_batch, two steps in flight).  times / gray_ptrs / depth_ptrs / boxes: per
+        member lists of n entries, and the return value, as FeatureTracker.trackBatchMulti on the members."""
+        S, n = len(self.members), len(times[0])
+        assert len(times) == S and all(len(x) == n for x in times)
+        w = self.members[0].width
+        t = np.ascontiguousarray(times, np.float64).reshape(S * n)
+        g = (ctypes.c_void_p * (S * n))(*[int(p) for row in gray_ptrs for p in row])
+        d = (ctypes.c_void_p * (S * n))(*[(int(p) if p else None) for row in depth_ptrs for p in row]) if depth_ptrs is not None else None
+        obs = np.zeros((S, n, self.max_cnt), OBS_DTYPE) if want else None
+        st = np.zeros((S, n, self.max_cnt), np.uint8) if want else None
+        cnt = np.zeros((S, n), np.int32)
+        info = (TrackInfo * (S * n))()
+        bx, start, ib = np.zeros((0, 4), np.int64), None, None
+        if boxes is not None:
+            assert len(boxes) == S and all(len(x) == n for x in boxes)
+            bx, start = _box_csr([b for row in boxes for b in row])
+            ib = np.zeros((S, n, self.max_cnt), np.uint8) if want else None
+        check(self.L.gf_tracker_group_track_batch(self._h, n, t.ctypes.data, g, int(gray_pitch or w), d, int(depth_pitch or 2 * w),
+                                                  int(bool(on_device)), bx.ctypes.data if len(bx) else None,
+                                                  start.ctypes.data if start is not None else None, obs.ctypes.data if want else None,
+                                                  cnt.ctypes.data, ib.ctypes.data if ib is not None else None,
+                                                  st.ctypes.data if want else None, info))
+        return FeatureTracker._results(self.members, n, obs, st, cnt, info, ib)

@@ -171,6 +171,43 @@ int gf_tracker_track_batch_multi_boxes(gf_tracker* const* trackers, int n_tracke
                                        const gf_box* boxes, const int* box_start, gf_obs* out, int* n_out, uint8_t* in_box,
                                        uint8_t* status_out, gf_track_info* info);
 
+/* A tracker group: n existing trackers (members) that track frame k of their streams in lockstep, one step at a time, with
+ * ONE set of launches per step: every kernel of the frame runs once for the whole group (member = a grid dimension), so the
+ * launch count and the driver calls per step do not grow with n.  Member i's results and its state afterwards are exactly
+ * what gf_tracker_track_batch on that member alone would give (same kernels, same arithmetic).  A step ends with its slowest
+ * member: the group trades per-camera latency for throughput (gf_tracker_track_batch_multi keeps the streams independent).
+ *   _create: 1 <= n <= GF_TRACKER_GROUP_MAX (more: GF_ERR_CAPACITY).  The members must be distinct, bound to the same device,
+ *       with the same width, height, max_cnt, min_dist, flow_back and depth_cam, and the same equalize setting and CLAHE
+ *       geometry (pinhole may differ); none may have a frame in flight or be in profiling mode.  Any other violation is
+ *       GF_ERR_INVALID_ARG, with gf_last_error() starting "member k: " for the member at fault.
+ *   State stays in the members: a step reads and advances each member's features, frame counter, time of the last frame,
+ *       pending prediction and depth flags.  Between steps (no step in flight) a member may be used directly
+ *       (gf_tracker_set_prediction, _remove_ids, _track, batches); the next step continues from there.  A step in flight
+ *       counts as a frame in flight on every member, so direct calls (the _submit calls included) are refused
+ *       until it is collected by gf_tracker_group_wait (gf_tracker_wait on a member refuses to collect it).  A member whose
+ *       equalize setting was changed after the group was created makes _submit fail ("member k: ...").
+ *   _destroy: the members stay usable (a step still in flight is completed and dropped).  Destroying a member that belongs to
+ *       a live group is a caller error.
+ *   _submit: one step, two steps in flight at most (as gf_tracker_submit): member i tracks times[i], gray[i], depth[i] (depth
+ *       nullable, and NULL entries: no depth image); on_device and the pitches as gf_tracker_submit_boxes; boxes / box_start:
+ *       member i's detections are boxes[box_start[i] .. box_start[i + 1]) (n + 1 offsets; box_start NULL: no boxes).  Every
+ *       member's pointers and box list are checked before anything is enqueued: an argument error consumes no frame.
+ *   _wait: collects the oldest step: member i's results at out + i*max_cnt, n_out[i], in_box + i*max_cnt,
+ *       status_out + i*max_cnt, info[i] (each nullable), as gf_tracker_wait_boxes returns them.
+ *   _track_batch: n_steps steps in one call, two in flight, with the arguments and layout of
+ *       gf_tracker_track_batch_multi_boxes (member i = stream i: frame k at [i*n_steps + k]).
+ * gf_tracker_last_device_ms of a member reports the device time of the last collected step. */
+typedef struct gf_tracker_group gf_tracker_group;
+#define GF_TRACKER_GROUP_MAX 64
+int gf_tracker_group_create(gf_tracker_group** out, gf_tracker* const* members, int n);
+void gf_tracker_group_destroy(gf_tracker_group* g);
+int gf_tracker_group_submit(gf_tracker_group* g, const double* times, const void* const* gray, size_t gray_pitch,
+                            const void* const* depth, size_t depth_pitch, int on_device, const gf_box* boxes, const int* box_start);
+int gf_tracker_group_wait(gf_tracker_group* g, gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info);
+int gf_tracker_group_track_batch(gf_tracker_group* g, int n_steps, const double* times, const void* const* gray, size_t gray_pitch,
+                                 const void* const* depth, size_t depth_pitch, int on_device, const gf_box* boxes, const int* box_start,
+                                 gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info);
+
 /* FeatureTracker::setPrediction (feature_tracker.cpp:1006-1027): xyz are camera-frame 3-D points. */
 int gf_tracker_set_prediction(gf_tracker* t, const int32_t* ids, const double* xyz, int n);
 /* FeatureTracker::removeOutliers (feature_tracker.cpp:1029-1045). */
