@@ -14,6 +14,7 @@
 //                          the next frame's camera (the xyz that FeatureTracker::setPrediction takes)
 // One thread per landmark: the work is O(obs^2) <= 121 small FP64 steps per landmark and there are <= a few hundred
 // landmarks; the list bookkeeping (std::list<FeaturePerId>) stays on the host (ground_fusion_b200/feature_manager.py).
+#include <cfloat>
 #include <vector>
 
 #include "gf_common.cuh"
@@ -42,28 +43,45 @@ __device__ __forceinline__ void m3_v(const double* a, const double* b, double* c
 
 struct FmPoses { double P[GF_BA_MAX_FRAMES][3]; double R[GF_BA_MAX_FRAMES][9]; double tic[3]; double ric[9]; };
 
-// smallest-eigenvalue eigenvector of a symmetric 4x4 matrix by cyclic Jacobi (the right singular vector of the DLT matrix A
-// that Eigen::JacobiSVD returns as matrixV().rightCols<1>(), up to sign: only the ratio v2 / v3 is used)
-__device__ inline void smallest_eigvec4(double M[4][4], double v[4])
+// one row of the DLT matrix A folded into the upper-triangular R of A = QR by Givens rotations, so that A is never stored
+__device__ __forceinline__ void qr_add_row4(double R[4][4], double r[4])
+{
+    for (int k = 0; k < 4; k++) {
+        if (r[k] == 0.0) continue;
+        const double h = hypot(R[k][k], r[k]), c = R[k][k] / h, s = r[k] / h;
+        R[k][k] = h;
+        for (int j = k + 1; j < 4; j++) { const double a = R[k][j], b = r[j]; R[k][j] = c * a + s * b; r[j] = c * b - s * a; }
+    }
+}
+// right singular vector of the smallest singular value of R (hence of A) by one-sided (Hestenes) Jacobi on R's columns: the
+// vector Eigen::JacobiSVD returns as matrixV().rightCols<1>(), up to sign (only the ratio v2 / v3 is used).  Working on R, not
+// on A^T A, keeps the error of the null vector at eps kappa(A) instead of eps kappa(A)^2, which matters exactly where the DLT
+// is used: far landmarks and windows that barely move.
+__device__ inline void smallest_right_sv4(double R[4][4], double v[4])
 {
     double V[4][4] = {{1, 0, 0, 0}, {0, 1, 0, 0}, {0, 0, 1, 0}, {0, 0, 0, 1}};
-    for (int sweep = 0; sweep < 30; sweep++) {
-        double off = 0;
-        for (int p = 0; p < 4; p++) for (int q = p + 1; q < 4; q++) off += M[p][q] * M[p][q];
-        if (off < 1e-300) break;
+    for (int sweep = 0; sweep < 20; sweep++) {
+        bool rotated = false;
         for (int p = 0; p < 3; p++)
             for (int q = p + 1; q < 4; q++) {
-                if (M[p][q] == 0.0) continue;
-                const double theta = (M[q][q] - M[p][p]) / (2.0 * M[p][q]);
-                const double t = (theta >= 0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+                double a = 0, b = 0, g = 0;
+                for (int k = 0; k < 4; k++) { a += R[k][p] * R[k][p]; b += R[k][q] * R[k][q]; g += R[k][p] * R[k][q]; }
+                if (fabs(g) <= DBL_EPSILON * sqrt(a) * sqrt(b)) continue;       // columns p, q already orthogonal (or one is zero)
+                const double zeta = (b - a) / (2.0 * g);
+                const double t = (zeta >= 0 ? 1.0 : -1.0) / (fabs(zeta) + hypot(1.0, zeta));
                 const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
-                for (int k = 0; k < 4; k++) { const double a = M[k][p], b = M[k][q]; M[k][p] = c * a - s * b; M[k][q] = s * a + c * b; }
-                for (int k = 0; k < 4; k++) { const double a = M[p][k], b = M[q][k]; M[p][k] = c * a - s * b; M[q][k] = s * a + c * b; }
-                for (int k = 0; k < 4; k++) { const double a = V[k][p], b = V[k][q]; V[k][p] = c * a - s * b; V[k][q] = s * a + c * b; }
+                for (int k = 0; k < 4; k++) { const double x = R[k][p], y = R[k][q]; R[k][p] = c * x - s * y; R[k][q] = s * x + c * y; }
+                for (int k = 0; k < 4; k++) { const double x = V[k][p], y = V[k][q]; V[k][p] = c * x - s * y; V[k][q] = s * x + c * y; }
+                rotated = true;
             }
+        if (!rotated) break;
     }
     int m = 0;
-    for (int k = 1; k < 4; k++) if (M[k][k] < M[m][m]) m = k;
+    double nm = R[0][0] * R[0][0] + R[1][0] * R[1][0] + R[2][0] * R[2][0] + R[3][0] * R[3][0];
+    for (int j = 1; j < 4; j++) {
+        const double n2 = R[0][j] * R[0][j] + R[1][j] * R[1][j] + R[2][j] * R[2][j] + R[3][j] * R[3][j];
+        if (n2 < nm) { nm = n2; m = j; }
+    }
     for (int k = 0; k < 4; k++) v[k] = V[k][m];
 }
 
@@ -118,7 +136,7 @@ __global__ void k_fm_triangulate(int n, const int* __restrict__ start, const int
     // ---- triangulate: DLT over all observations, reference frame = start frame ----
     double t0[3], R0[9], R0T[9];
     cam(s0, t0, R0); m3_T(R0, R0T);
-    double M[4][4] = {{0}};
+    double QR[4][4] = {{0}};
     for (int a = 0; a < m; a++) {
         double t1[3], R1[9];
         cam(s0 + a, t1, R1);
@@ -130,12 +148,14 @@ __global__ void k_fm_triangulate(int n, const int* __restrict__ start, const int
         const double f[3] = {p[3 * a] / nrm, p[3 * a + 1] / nrm, p[3 * a + 2] / nrm};
         double r0[4], r1[4];
         for (int c = 0; c < 4; c++) { r0[c] = f[0] * P[2][c] - f[2] * P[0][c]; r1[c] = f[1] * P[2][c] - f[2] * P[1][c]; }
-        for (int u = 0; u < 4; u++) for (int v = 0; v < 4; v++) M[u][v] += r0[u] * r0[v] + r1[u] * r1[v];
+        qr_add_row4(QR, r0); qr_add_row4(QR, r1);
     }
     double v[4];
-    smallest_eigvec4(M, v);
+    smallest_right_sv4(QR, v);
     double d = v[2] / v[3]; int fl = 2;
-    if (!(d >= 0.1)) { d = init_depth; fl = 0; }
+    // NaN and +inf (v3 == 0: a window without translation leaves the depth undetermined) never reach estimated_depth, whose
+    // inverse the solve takes
+    if (!(d >= 0.1) || isinf(d)) { d = init_depth; fl = 0; }
     est[i] = d; flag[i] = fl;
 }
 

@@ -546,7 +546,8 @@ int gf_ba_double2vector(const gf_ba_problem* p, const double* R0_before, const d
 /* FeatureManager::triangulateWithDepth (:726-799) followed by FeatureManager::triangulate (:668-723), as processImage calls
  * them (estimator.cpp:1090-1102): landmarks with >= 4 observations and estimated_depth <= 0 get a depth -- the mean of the
  * RGB-D depths (0.1 .. depth_threshold) that re-project within 10/460 into another frame (estimate_flag 1), else the DLT
- * depth over all observations (flag 2); results < 0.1 become init_depth (flag 0).  Ps [n_frames][3], Rs [n_frames][9] row-major. */
+ * depth over all observations (flag 2); results < 0.1, NaN or inf (a window without translation) become init_depth (flag 0).
+ * Ps [n_frames][3], Rs [n_frames][9] row-major. */
 int gf_fm_triangulate(int device, int n_features, const int32_t* start_frame, const int32_t* n_obs, const int32_t* obs_offset, int n_obs_total,
                       const double* points, const double* depths, double* estimated_depth, int32_t* estimate_flag,
                       int n_frames, const double* Ps, const double* Rs, const double* tic, const double* ric, double depth_threshold, double init_depth);

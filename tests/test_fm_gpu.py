@@ -3,6 +3,7 @@ replay pipeline on the GPU (FeatureTracker + FeatureManager + BundleAdjuster) ag
 import numpy as np
 import pytest
 
+from fm_ref import K, Scene, dlt_ref, ratio
 from test_fm_oracle import fill, scene
 
 pytestmark = pytest.mark.gpu
@@ -26,9 +27,13 @@ def test_triangulation_matches_oracle(seed, thr, dn):
     for x, y in zip(a.feature, b.feature):
         assert x.estimate_flag == y.estimate_flag, x.feature_id
         flags.add(x.estimate_flag)
-        if x.estimated_depth > 0:
-            # flag 2: smallest singular vector of an ill-conditioned 2m x 4 system (SVD on the CPU, eigenvector of A^T A on the GPU)
-            assert abs(x.estimated_depth - y.estimated_depth) <= (1e-6 if x.estimate_flag == 2 else 1e-10) * x.estimated_depth, (x.feature_id, x.estimated_depth, y.estimated_depth)
+        if x.estimate_flag == 2:
+            # the DLT depth against its high-precision reference and error bar (tests/fm_ref.py)
+            lm = dict(start=x.start_frame, pts=np.array([f.point for f in x.feature_per_frame]), dep=np.array([f.depth for f in x.feature_per_frame]))
+            want, sc_ = dlt_ref(Scene("", Ps, Rs, np.zeros(3), np.eye(3), thr, [lm]), lm)[:2]
+            assert ratio(y.estimated_depth, want, sc_) <= K["dlt"], (x.feature_id, want, y.estimated_depth)
+        elif x.estimated_depth > 0:
+            assert abs(x.estimated_depth - y.estimated_depth) <= 1e-10 * x.estimated_depth, (x.feature_id, x.estimated_depth, y.estimated_depth)
         else:
             assert y.estimated_depth < 0
     assert len(flags) >= 2
