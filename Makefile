@@ -19,19 +19,26 @@ $(BUILD)/ba_solver.o: $(CSRC)/ba_solver.cu $(HDRS)
 	@mkdir -p $(BUILD); $(NVCC) $(filter-out -fmad=false,$(NVFLAGS)) -dc -o $@ $< -Xptxas -v 2> build_ptxas_ba.log || (cat build_ptxas_ba.log; false)
 $(BUILD)/fm_kernels.o: $(CSRC)/fm_kernels.cu $(HDRS)
 	@mkdir -p $(BUILD); $(NVCC) $(filter-out -fmad=false,$(NVFLAGS)) -dc -o $@ $<
-$(OUT): $(BUILD)/fe_tracker.o $(BUILD)/ba_solver.o $(BUILD)/fm_kernels.o
+# dense map: -fmad=false (bit-exact with oracle/dm_oracle.c, built with -ffp-contract=off)
+$(BUILD)/dm_map.o: $(CSRC)/dm_map.cu $(HDRS)
+	@mkdir -p $(BUILD); $(NVCC) $(NVFLAGS) -dc -o $@ $< -Xptxas -v 2> build_ptxas_dm.log || (cat build_ptxas_dm.log; false)
+$(OUT): $(BUILD)/fe_tracker.o $(BUILD)/ba_solver.o $(BUILD)/fm_kernels.o $(BUILD)/dm_map.o
 	$(NVCC) $(ARCH) -shared -o $@ $^
-	@cat build_ptxas_fe.log build_ptxas_ba.log > build_ptxas.log
+	@cat build_ptxas_fe.log build_ptxas_ba.log build_ptxas_dm.log > build_ptxas.log
 
-oracle:
+oracle: oracle/_build/libgf_oracle_dm.so
 	$(MAKE) -C oracle
+# the dense map's sequential restatement (tests and tools/bench_dense_map.py only): -O3 -ffp-contract=off as oracle/Makefile's
+# libgf_oracle_ba.so, plus -msse2 -mfpmath=sse as its libgf_oracle_fe.so
+oracle/_build/libgf_oracle_dm.so: oracle/dm_oracle.c
+	@mkdir -p oracle/_build; gcc -O3 -ffp-contract=off -msse2 -mfpmath=sse -shared -fPIC -o $@ $< -lm
 
 # development aid: the same library with the clock64() phase counters compiled in (GF_B200_LIB=... selects it)
-profile: $(SRCS) $(HDRS) $(BUILD)/fm_kernels.o
+profile: $(SRCS) $(HDRS) $(BUILD)/fm_kernels.o $(BUILD)/dm_map.o
 	@mkdir -p $(BUILD)
 	$(NVCC) $(NVFLAGS) -DGF_PROFILE -dc -o $(BUILD)/fe_tracker_prof.o $(CSRC)/fe_tracker.cu
 	$(NVCC) $(filter-out -fmad=false,$(NVFLAGS)) -DGF_PROFILE -dc -o $(BUILD)/ba_solver_prof.o $(CSRC)/ba_solver.cu
-	$(NVCC) $(ARCH) -shared -o ground_fusion_b200/libgf_b200_prof.so $(BUILD)/fe_tracker_prof.o $(BUILD)/ba_solver_prof.o $(BUILD)/fm_kernels.o
+	$(NVCC) $(ARCH) -shared -o ground_fusion_b200/libgf_b200_prof.so $(BUILD)/fe_tracker_prof.o $(BUILD)/ba_solver_prof.o $(BUILD)/fm_kernels.o $(BUILD)/dm_map.o
 
 clean:
 	rm -f $(OUT) build_ptxas.log; $(MAKE) -C oracle clean

@@ -6,12 +6,15 @@
 //   harness ba <in> <out>   one window through Estimator::optimization()
 //   harness ba-multi <in> <out>  several estimators' windows, each round through one Estimator::optimizationMulti call
 //   harness ba-seq <in> <out>    the same input through each estimator's optimization() in turn
+//   harness dm <in> <out>   keyframes and pose corrections through DenseMap (PoseGraph's octree blocks); after each call the
+//                           returned point_rgbd (add only), the cloud and the filtered cloud's indices
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <memory>
 #include <vector>
 
+#include "dense_map.h"
 #include "estimator_ba.h"
 #include "feature_tracker.h"
 
@@ -158,10 +161,61 @@ static int run_ba_multi(const char *in, const char *out, bool batched)
     return 0;
 }
 
+// Input: w, h, pinhole[8], depth_dist, depth_boundary, qic[9] (row-major), tic[3], max_points, max_keyframes, n_ops; each op is
+// int 0 + R[9] (row-major) + P[3] + rgb (h x w x 3) + depth (h x w u16), or int 1 + n + n x (R[9], P[3]).
+static int run_dm(const char *in, const char *out)
+{
+    FILE *f = fopen(in, "rb"), *o = fopen(out, "wb");
+    if (!f || !o) return 2;
+    const int w = rd1<int>(f), h = rd1<int>(f);
+    double p[8], q[9];
+    rd(f, p, sizeof(p));
+    const int dd = rd1<int>(f), db = rd1<int>(f);
+    rd(f, q, sizeof(q));
+    Eigen::Matrix3d qic; Eigen::Vector3d tic;
+    for (int i = 0; i < 9; i++) qic(i / 3, i % 3) = q[i];
+    rd(f, tic.data(), 24);
+    const int max_points = rd1<int>(f), max_keyframes = rd1<int>(f), n_ops = rd1<int>(f);
+    DenseMap map(w, h, p, dd, db, qic, tic, max_points, max_keyframes);
+    auto pose = [&](Eigen::Matrix3d &R, Eigen::Vector3d &P) {
+        double r[9]; rd(f, r, sizeof(r));
+        for (int i = 0; i < 9; i++) R(i / 3, i % 3) = r[i];
+        rd(f, P.data(), 24);
+    };
+    std::vector<unsigned char> rgb((size_t)w * h * 3);
+    std::vector<unsigned short> depth((size_t)w * h);
+    for (int op = 0; op < n_ops; op++) {
+        if (rd1<int>(f) == 0) {
+            Eigen::Matrix3d R; Eigen::Vector3d P;
+            pose(R, P);
+            rd(f, rgb.data(), rgb.size()); rd(f, depth.data(), depth.size() * 2);
+            const auto pts = map.addKeyFrame(R, P, cv::Mat(h, w, CV_8UC3, rgb.data()), cv::Mat(h, w, CV_16UC1, depth.data()));
+            const int m = (int)pts.size();
+            fwrite(&m, 4, 1, o);
+            for (auto &v : pts) fwrite(v.data(), 4, 6, o);
+        } else {
+            const int n = rd1<int>(f);
+            std::vector<Eigen::Matrix3d> Rs(n); std::vector<Eigen::Vector3d> Ps(n);
+            for (int k = 0; k < n; k++) pose(Rs[k], Ps[k]);
+            map.updatePath(Rs, Ps);
+        }
+        std::vector<float> xyz; std::vector<unsigned char> col; std::vector<int32_t> idx;
+        map.cloud(xyz, col);
+        const int n = (int)(xyz.size() / 3);
+        fwrite(&n, 4, 1, o); fwrite(xyz.data(), 4, xyz.size(), o); fwrite(col.data(), 1, col.size(), o);
+        map.filtered(xyz, col, idx);
+        const int nf = (int)idx.size();
+        fwrite(&nf, 4, 1, o); fwrite(idx.data(), 4, idx.size(), o);
+    }
+    fclose(f); fclose(o);
+    return 0;
+}
+
 int main(int argc, char **argv)
 {
-    if (argc != 4) { std::fprintf(stderr, "usage: harness fe|fe-eq|fe-box|ba|ba-multi|ba-seq <in> <out>\n"); return 2; }
+    if (argc != 4) { std::fprintf(stderr, "usage: harness fe|fe-eq|fe-box|ba|ba-multi|ba-seq|dm <in> <out>\n"); return 2; }
     if (!std::strcmp(argv[1], "fe-eq")) EQUALIZE = 1;
+    if (!std::strcmp(argv[1], "dm")) return run_dm(argv[2], argv[3]);
     if (!std::strcmp(argv[1], "ba-multi") || !std::strcmp(argv[1], "ba-seq")) return run_ba_multi(argv[2], argv[3], argv[1][3] == 'm');
     return argv[1][0] == 'f' ? run_fe(argv[2], argv[3], !std::strcmp(argv[1], "fe-box")) : run_ba(argv[2], argv[3]);
 }

@@ -8,6 +8,7 @@
 #include <memory>
 #define CV_8UC1 0
 #define CV_16UC1 2
+#define CV_8UC3 16
 namespace cv {
 struct Point2f { float x = 0, y = 0; Point2f() {} Point2f(float a, float b) : x(a), y(b) {} };
 class Mat {
@@ -23,7 +24,7 @@ public:
     template <class T> T *ptr(int r = 0) { return (T *)(data + step * r); }
     template <class T> const T *ptr(int r = 0) const { return (const T *)(data + step * r); }
 private:
-    size_t esz() const { return type_ == CV_16UC1 ? 2 : 1; }
+    size_t esz() const { return type_ == CV_16UC1 ? 2 : type_ == CV_8UC3 ? 3 : 1; }
     int type_ = CV_8UC1;
     std::shared_ptr<unsigned char[]> own_;
 };

@@ -22,6 +22,15 @@ class TrackerCfg(ctypes.Structure):
                 ("depth_cam", ctypes.c_int), ("pinhole", ctypes.c_double * 8)]
 
 
+class DenseMapCfg(ctypes.Structure):
+    _fields_ = [("width", ctypes.c_int), ("height", ctypes.c_int), ("pinhole", ctypes.c_double * 8), ("depth_dist", ctypes.c_int),
+                ("depth_boundary", ctypes.c_int), ("ric", ctypes.c_double * 9), ("tic", ctypes.c_double * 3), ("max_points", ctypes.c_int),
+                ("max_keyframes", ctypes.c_int)]
+
+
+DENSE_MAP_CLOUD, DENSE_MAP_FILTERED = 0, 1      # gf_dense_map_read's `which`
+
+
 class Obs(ctypes.Structure):
     _fields_ = [("id", ctypes.c_int32), ("track_cnt", ctypes.c_int32), ("v", ctypes.c_double * 8)]
 
@@ -87,6 +96,15 @@ def lib():
         L.gf_stage_lk.argtypes = [i, vp, vp, i, i, vp, vp, i, i, i, vp]
         L.gf_stage_gftt.argtypes = [i, vp, i, i, vp, i, i, i, vp, ctypes.POINTER(i), ctypes.POINTER(TrackInfo)]
         L.gf_stage_setmask_order.argtypes = [i, vp, i, vp]
+        L.gf_dense_map_create.argtypes = [ctypes.POINTER(vp), i, ctypes.POINTER(DenseMapCfg)]
+        L.gf_dense_map_destroy.argtypes = [vp]
+        L.gf_dense_map_destroy.restype = None
+        L.gf_dense_map_add_keyframe.argtypes = [vp, vp, vp, vp, sz, vp, sz, i, ctypes.POINTER(i)]
+        L.gf_dense_map_update_poses.argtypes = [vp, i, vp, vp]
+        L.gf_dense_map_size.argtypes = [vp, ctypes.POINTER(i), ctypes.POINTER(i), ctypes.POINTER(i)]
+        L.gf_dense_map_read.argtypes = [vp, i, vp, vp, vp]
+        L.gf_dense_map_keyframe_points.argtypes = [vp, i, vp, ctypes.POINTER(i)]
+        L.gf_stage_radius_filter.argtypes = [i, vp, i, d, i, vp]
         _LIB = L
     return _LIB
 

@@ -10,6 +10,7 @@
 // Arithmetic and ordering follow oracle/fe_cv_restate.c and oracle/fe_oracle.py.
 #pragma once
 #include "fe_sort.cuh"
+#include "gf_camera.cuh"
 #include "gf_common.cuh"
 
 namespace gf {
@@ -498,39 +499,6 @@ __device__ __forceinline__ void nms_cells(TrackScalars* sc, const NmsGrid& g, in
 }
 
 // ------------------------------------------------------------------------------------------------
-struct CamParams { double fx, fy, cx, cy, k1, k2, p1, p2; int no_distortion; };
-
-__device__ __forceinline__ void cam_distortion(const CamParams& c, double x, double y, double& dx, double& dy)
-{   // PinholeCamera::distortion, camera_models/src/camera_models/PinholeCamera.cc:646-662
-    double mx2 = x * x, my2 = y * y, mxy = x * y;
-    double rho2 = mx2 + my2;
-    double rad = c.k1 * rho2 + c.k2 * rho2 * rho2;
-    dx = x * rad + 2.0 * c.p1 * mxy + c.p2 * (rho2 + 2.0 * mx2);
-    dy = y * rad + 2.0 * c.p2 * mxy + c.p1 * (rho2 + 2.0 * my2);
-}
-__device__ __forceinline__ void cam_lift(const CamParams& c, double u, double v, double& ox, double& oy)
-{   // PinholeCamera::liftProjective, PinholeCamera.cc:450-510 (recursive distortion model, n = 8)
-    double ik11 = 1.0 / c.fx, ik13 = -c.cx / c.fx, ik22 = 1.0 / c.fy, ik23 = -c.cy / c.fy;
-    double mx_d = ik11 * u + ik13, my_d = ik22 * v + ik23;
-    if (c.no_distortion) { ox = mx_d; oy = my_d; return; }
-    double dx, dy;
-    cam_distortion(c, mx_d, my_d, dx, dy);
-    double mx_u = mx_d - dx, my_u = my_d - dy;
-    for (int i = 1; i < 8; i++) {
-        cam_distortion(c, mx_u, my_u, dx, dy);
-        mx_u = mx_d - dx;
-        my_u = my_d - dy;
-    }
-    ox = mx_u; oy = my_u;
-}
-__device__ __forceinline__ void cam_project(const CamParams& c, double X, double Y, double Z, double& u, double& v)
-{   // PinholeCamera::spaceToPlane, PinholeCamera.cc:520-541
-    double x = X / Z, y = Y / Z;
-    if (!c.no_distortion) { double dx, dy; cam_distortion(c, x, y, dx, dy); x = x + dx; y = y + dy; }
-    u = c.fx * x + c.cx;
-    v = c.fy * y + c.cy;
-}
-
 struct OutHeader { int n_out, n_prev, n_tracked, n_kept, n_new, n_cand, nms_rounds, eig_fixups, lk_iters, pad; };
 
 // The detections of one frame (trackImagebox, feature_tracker.cpp:374-678), converted on the host: box k is

@@ -413,14 +413,6 @@ static int make_lk_maps(LKMapSet* M, const Pyramid& prev, const Pyramid& cur, in
     return GF_OK;
 }
 
-static CamParams make_cam(const double* p)
-{
-    CamParams c;
-    c.fx = p[0]; c.fy = p[1]; c.cx = p[2]; c.cy = p[3]; c.k1 = p[4]; c.k2 = p[5]; c.p1 = p[6]; c.p2 = p[7];
-    c.no_distortion = (p[4] == 0.0 && p[5] == 0.0 && p[6] == 0.0 && p[7] == 0.0);
-    return c;
-}
-
 static int select_device(int device)
 {
     int n = 0;

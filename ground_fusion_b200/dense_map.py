@@ -1,0 +1,110 @@
+"""Dense colour map on the GPU: the keyframe point map of the reference's dense_map node (PoseGraph's octree blocks,
+dense_map/src/pose_graph.cpp:191-239 and 997-1058, fed by the node's sampling loop, pose_graph_node.cpp:598-623).
+
+DenseMap wraps gf_dense_map_* (include/gf_b200.h); method names follow the reference.  There is no CPU fallback."""
+import ctypes
+
+import numpy as np
+
+from . import _lib
+
+
+def _p(a):
+    return a.ctypes.data_as(ctypes.c_void_p)
+
+
+class DenseMap:
+    """width, height, pinhole (fx fy cx cy k1 k2 p1 p2): cam0_calib; depth_dist / depth_boundary: DEPTH_DIST / DEPTH_BOUNDARY;
+    ric (3x3), tic (3): camera to body.  max_points bounds the points all keyframes keep together, max_keyframes the keyframes."""
+
+    def __init__(self, width, height, pinhole, depth_dist=10, depth_boundary=10, ric=np.eye(3), tic=np.zeros(3),
+                 max_points=1 << 20, max_keyframes=4096, device=0):
+        cfg = _lib.DenseMapCfg()
+        cfg.width, cfg.height, cfg.depth_dist, cfg.depth_boundary = width, height, depth_dist, depth_boundary
+        cfg.pinhole[:] = [float(v) for v in pinhole]
+        cfg.ric[:] = [float(v) for v in np.asarray(ric, float).reshape(9)]
+        cfg.tic[:] = [float(v) for v in np.asarray(tic, float).reshape(3)]
+        cfg.max_points, cfg.max_keyframes = max_points, max_keyframes
+        self.width, self.height = width, height
+        self._m = ctypes.c_void_p()
+        _lib.check(_lib.lib().gf_dense_map_create(ctypes.byref(self._m), device, ctypes.byref(cfg)))
+
+    def close(self):
+        if self._m:
+            _lib.lib().gf_dense_map_destroy(self._m)
+            self._m = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def addKeyFrame(self, R, P, rgb, depth):
+        """One keyframe with body pose (R, P): rgb (H, W, 3) uint8 and depth (H, W) uint16 millimetres, numpy arrays (rows may be
+        padded) or CUDA tensors.  Returns the number of points inserted."""
+        R = np.ascontiguousarray(R, np.float64).reshape(9)
+        P = np.ascontiguousarray(P, np.float64).reshape(3)
+        n = ctypes.c_int()
+        h, w = self.height, self.width
+        if tuple(rgb.shape) != (h, w, 3) or tuple(depth.shape) != (h, w):
+            raise ValueError("rgb must be (%d, %d, 3) and depth (%d, %d)" % (h, w, h, w))
+        if hasattr(rgb, "is_cuda") and rgb.is_cuda:
+            import torch
+            if rgb.dtype != torch.uint8 or depth.dtype not in (torch.int16, torch.uint16) or not depth.is_cuda:
+                raise ValueError("CUDA frames: rgb uint8, depth int16 / uint16 (the millimetres' bits), both on the device")
+            if rgb.stride(2) != 1 or rgb.stride(1) != 3 or depth.stride(1) != 1:
+                raise ValueError("rows must be packed pixels")
+            args = (ctypes.c_void_p(rgb.data_ptr()), rgb.stride(0), ctypes.c_void_p(depth.data_ptr()), depth.stride(0) * 2, 1)
+        else:
+            if rgb.dtype != np.uint8 or depth.dtype != np.uint16:
+                raise ValueError("rgb must be uint8 and depth uint16")
+            if rgb.strides[1:] != (3, 1) or depth.strides[1] != 2:
+                raise ValueError("rows must be packed pixels")
+            args = (_p(rgb), rgb.strides[0], _p(depth), depth.strides[0], 0)
+        _lib.check(_lib.lib().gf_dense_map_add_keyframe(self._m, _p(R), _p(P), *args, ctypes.byref(n)))
+        return n.value
+
+    def updatePath(self, Rs, Ps):
+        """The rebuild after a pose-graph correction: Rs (n, 3, 3), Ps (n, 3), one pose per keyframe added."""
+        Rs = np.ascontiguousarray(Rs, np.float64).reshape(-1, 9)
+        Ps = np.ascontiguousarray(Ps, np.float64).reshape(-1, 3)
+        if len(Rs) != len(Ps):
+            raise ValueError("Rs and Ps differ in length")
+        _lib.check(_lib.lib().gf_dense_map_update_poses(self._m, len(Rs), _p(Rs), _p(Ps)))
+
+    def size(self):
+        """(points in the cloud, points the filter keeps, keyframes)."""
+        a, b, c = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+        _lib.check(_lib.lib().gf_dense_map_size(self._m, ctypes.byref(a), ctypes.byref(b), ctypes.byref(c)))
+        return a.value, b.value, c.value
+
+    def _read(self, which, n):
+        xyz, rgb, idx = np.zeros((n, 3), np.float32), np.zeros((n, 3), np.uint8), np.zeros(n, np.int32)
+        _lib.check(_lib.lib().gf_dense_map_read(self._m, which, _p(xyz), _p(rgb), _p(idx)))
+        return xyz, rgb, idx
+
+    def cloud(self):
+        """(xyz float32 (n, 3), rgb uint8 (n, 3)) of the accumulated cloud, in insertion order."""
+        xyz, rgb, _ = self._read(_lib.DENSE_MAP_CLOUD, self.size()[0])
+        return xyz, rgb
+
+    def filtered(self):
+        """(xyz, rgb, idx) of the points RadiusOutlierRemoval keeps, in cloud order; idx = their indices in cloud()."""
+        return self._read(_lib.DENSE_MAP_FILTERED, self.size()[1])
+
+    def keyframePoints(self, k):
+        """Keyframe k's kept points (KeyFrame::point_rgbd): float32 (n, 6), camera-frame x y z and r g b."""
+        n = ctypes.c_int()
+        _lib.check(_lib.lib().gf_dense_map_keyframe_points(self._m, k, None, ctypes.byref(n)))
+        out = np.zeros((n.value, 6), np.float32)
+        _lib.check(_lib.lib().gf_dense_map_keyframe_points(self._m, k, _p(out), ctypes.byref(n)))
+        return out
+
+
+def radius_filter(xyz, radius=0.8, min_pts=10, device=0):
+    """The map's radius filter over any float32 point set (gf_stage_radius_filter): bool keep mask."""
+    xyz = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)
+    keep = np.zeros(len(xyz), np.uint8)
+    _lib.check(_lib.lib().gf_stage_radius_filter(device, _p(xyz), len(xyz), float(radius), int(min_pts), _p(keep)))
+    return keep.astype(bool)

@@ -181,17 +181,23 @@ class WindowEstimator:
             self.fm.removeFront(self.frame_count)                 # slideWindowNew (estimator.cpp:3839-3851)
 
 
-def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=True, max_iter=8, feedback=False, use_mcc=False, boxes=None):
+def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=True, max_iter=8, feedback=False, use_mcc=False, boxes=None,
+           dense_map=None):
     """Runs n_frames of `stream` through tracker -> fm -> ba.  Returns dict(t, P_est, P_gt, R_est, R_gt, keyframes, ...).
     tracker.trackImage(t, gray, depth) -> {id: v[8]};  fm / ba: see WindowEstimator.  feedback: the estimator calls the tracker's
     removeOutliers / setPrediction after every optimisation (the reference with MULTIPLE_THREAD 0).
     boxes: USE_YOLO -- the detections of frame k in boxes[k] ((m, 4) xmin, ymin, xmax, ymax).  A frame with detections goes
     through tracker.trackImagebox(t, boxes[k], gray, depth), one without through trackImage, as sync_process does
-    (rosNodeTest.cpp:433-439, 519-540)."""
+    (rosNodeTest.cpp:433-439, 519-540).
+    dense_map: a map with addKeyFrame(R, P, rgb, depth) (DenseMap, or the oracle's), fed as pubKeyframe feeds the mapping node
+    (visualization.cpp): after every MARGIN_OLD, the pose of window frame WINDOW_SIZE - 2 with that frame's colour and depth
+    images (stream.color / stream.frame), unless its position equals the previous keyframe's exactly, as the node skips it.  It is returned under "dense_map"."""
     imu = ImuFromStream(stream)
     est = WindowEstimator(fm, ba, imu_propagate=imu_propagate, max_iter=max_iter, tracker=tracker if feedback else None, use_mcc=use_mcc)
     out_t, out_P, out_R, gt_P, gt_R, iters = [], [], [], [], [], []
     t_prev = None
+    slot = [0] * (WINDOW_SIZE + 1)                      # stream frame held by each window slot (Headers[])
+    last_P = None                                       # position of the last keyframe fed to dense_map
     for k in range(n_frames):
         t, gray, depth = stream.frame(k)
         if t_prev is not None:                          # IMU samples of (t_prev, t]
@@ -208,14 +214,28 @@ def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=Tru
         if not est.nonlinear:                           # initialisation is out of scope: ground-truth states while the window fills
             R_wb, P = imu.pose_t(t)
             est.set_state(est.frame_count, R_wb, P, imu.velocity(t))
+        slot[est.frame_count] = k
         res = est.processImage(image)
         t_prev = t
+        if res is not None:                             # the window slid: slideWindow's shift of Headers[]
+            if est.margin_old:
+                slot[:WINDOW_SIZE] = slot[1:]
+            else:
+                slot[WINDOW_SIZE - 1] = slot[WINDOW_SIZE]
+            # the node skips a keyframe whose position equals the previous one exactly (pose_graph_node.cpp:660, SKIP_DIS 0)
+            if dense_map is not None and est.margin_old and not np.array_equal(est.Ps[WINDOW_SIZE - 2], last_P):
+                j = slot[WINDOW_SIZE - 2]
+                last_P = est.Ps[WINDOW_SIZE - 2].copy()
+                dense_map.addKeyFrame(est.Rs[WINDOW_SIZE - 2], last_P, stream.color(j), stream.frame(j)[2])
         if res is not None:
             R_wb, P = imu.pose_t(t)
             out_t.append(t); out_P.append(res[0]); out_R.append(res[1]); gt_P.append(P); gt_R.append(R_wb)
             iters.append(est.last_summary["iterations"] if isinstance(est.last_summary, dict) else est.last_summary.get("iterations"))
     P_est, P_gt = np.array(out_P), np.array(gt_P)
     ate = float(np.sqrt(np.mean(np.sum((P_est - P_gt) ** 2, axis=1)))) if len(P_est) else float("nan")
-    return {"t": np.array(out_t), "P_est": P_est, "P_gt": P_gt, "R_est": np.array(out_R), "R_gt": np.array(gt_R), "ate_m": ate,
-            "n_margin_old": est.n_old, "n_margin_second_new": est.n_second_new, "iterations": iters,
-            "n_removed": est.n_removed, "n_predicted": est.n_predicted}
+    out = {"t": np.array(out_t), "P_est": P_est, "P_gt": P_gt, "R_est": np.array(out_R), "R_gt": np.array(gt_R), "ate_m": ate,
+           "n_margin_old": est.n_old, "n_margin_second_new": est.n_second_new, "iterations": iters,
+           "n_removed": est.n_removed, "n_predicted": est.n_predicted}
+    if dense_map is not None:
+        out["dense_map"] = dense_map
+    return out

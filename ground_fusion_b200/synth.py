@@ -166,3 +166,11 @@ class SyntheticStream:
         gray = np.clip(np.rint(img), 0, 255).astype(np.uint8)
         depth = np.where((depth_m > 0) & (depth_m < 10.0), np.rint(depth_m * 1000.0), 0).astype(np.uint16)
         return k / self.fps, gray, depth
+
+    def color(self, k):
+        """An RGB8 image of frame k for the dense map, derived from frame(k)'s gray image: the saturated boxes of the texture
+        (gray >= 246) are white in all three channels, so the mapping node's white test (> 240) has pixels on both sides."""
+        gray = self.frame(k)[1].astype(np.int32)
+        rgb = np.stack([gray, gray * 7 // 8 + 32, 255 - gray], axis=-1)
+        rgb[gray >= 246] = gray[gray >= 246][:, None]
+        return rgb.astype(np.uint8)

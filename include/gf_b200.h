@@ -576,6 +576,50 @@ int gf_fm_reprojection_errors(int device, int n_features, const int32_t* start_f
 int gf_fm_predict_next(int device, int n, const int32_t* first_frame, const double* uv_first, const double* estimated_depth, int n_frames, int frame_count,
                        const double* Ps, const double* Rs, const double* tic, const double* ric, double* pts_cam);
 
+/* ------------------------------------------------------------------------------------------------
+ * Dense colour map (dense_map/src/pose_graph.cpp, pose_graph_node.cpp): the keyframe point sampling of the mapping node,
+ * PoseGraph's voxel-density insertion (OctreePointCloudDensity, 0.01 m voxels), its RadiusOutlierRemoval (0.8 m, 10
+ * neighbours) and updatePath's rebuild after a pose-graph correction.  Loop detection and the pose-graph optimisation stay
+ * with the caller, which passes the corrected keyframe poses.  DESIGN.md "Dense colour map" has the semantics.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct gf_dense_map gf_dense_map; /* opaque: one map, bound to one GPU and one stream */
+
+typedef struct gf_dense_map_cfg {
+    int width, height;       /* image size (COL, ROW) */
+    double pinhole[8];       /* fx fy cx cy k1 k2 p1 p2, as gf_tracker_cfg (cam0_calib) */
+    int depth_dist;          /* DEPTH_DIST: sample every depth_dist-th pixel, >= 1 */
+    int depth_boundary;      /* DEPTH_BOUNDARY: samples in [b, COL - b) x [b, ROW - b); 2 b < width and height */
+    double ric[9];           /* qic (row-major) and tic: camera to body */
+    double tic[3];
+    int max_points;          /* capacity: points kept by all keyframes together (the cloud never holds more) */
+    int max_keyframes;       /* capacity: keyframes */
+} gf_dense_map_cfg;
+
+enum { GF_DENSE_MAP_CLOUD = 0, GF_DENSE_MAP_FILTERED = 1 };
+
+int gf_dense_map_create(gf_dense_map** map, int device, const gf_dense_map_cfg* cfg);
+void gf_dense_map_destroy(gf_dense_map* map);
+/* One keyframe: sample (pose_graph_node.cpp:598-623), insert with pose (R row-major, P) under the z band and the density gate
+ * < 3 (pose_graph.cpp:191-221), then filter (:228-239).  rgb: RGB8 rows of rgb_pitch bytes; depth: uint16 millimetres, rows of
+ * depth_pitch bytes; both HOST pointers, or device pointers when on_device != 0.  n_inserted (nullable): points added.
+ * GF_ERR_CAPACITY (max_keyframes, max_points) and GF_ERR_INVALID_ARG (a point outside the octree's box) leave the map unchanged. */
+int gf_dense_map_add_keyframe(gf_dense_map* map, const double* R, const double* P, const uint8_t* rgb, size_t rgb_pitch,
+                              const uint16_t* depth, size_t depth_pitch, int on_device, int* n_inserted);
+/* PoseGraph::updatePath's rebuild (:997-1058): a fresh octree over the wider box, every keyframe's kept points re-inserted in
+ * keyframe order with its new pose (R [n][9], P [n][3]) under the gate < 5 and no z band, then a full filter.  n_keyframes must
+ * equal the number of keyframes added (GF_ERR_INVALID_ARG otherwise, map unchanged). */
+int gf_dense_map_update_poses(gf_dense_map* map, int n_keyframes, const double* R, const double* P);
+int gf_dense_map_size(gf_dense_map* map, int* n_cloud, int* n_filtered, int* n_keyframes);
+/* Host copies in cloud order of the whole cloud (which = GF_DENSE_MAP_CLOUD) or of the points the filter keeps
+ * (GF_DENSE_MAP_FILTERED): xyz [n][3], rgb [n][3], idx [n] = each point's index in the cloud.  Each output is nullable. */
+int gf_dense_map_read(gf_dense_map* map, int which, float* xyz, uint8_t* rgb, int32_t* idx);
+/* Keyframe k's kept points (KeyFrame::point_rgbd after insertion): out6 [n][6] = camera-frame x y z and r g b; *n = their number
+ * (out6 NULL: only the number). */
+int gf_dense_map_keyframe_points(gf_dense_map* map, int k, float* out6, int* n);
+/* The map's radius filter over n host points: keep[i] = 1 iff more than min_pts points (itself included) lie at float squared
+ * distance < float(radius^2). */
+int gf_stage_radius_filter(int device, const float* xyz, int n, double radius, int min_pts, uint8_t* keep);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif
