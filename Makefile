@@ -6,7 +6,7 @@ OUT  := ground_fusion_b200/libgf_b200.so
 # -fmad=false: the front end is bit-exact with OpenCV's separately-rounded float ops (FMA only where written)
 NVFLAGS := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden -fmad=false
 SRCS := $(wildcard $(CSRC)/*.cu)
-HDRS := $(wildcard $(CSRC)/*.cuh) include/gf_b200.h
+HDRS := $(wildcard $(CSRC)/*.cuh) $(CSRC)/gm_math.h include/gf_b200.h
 
 all: $(OUT) oracle
 
@@ -22,23 +22,29 @@ $(BUILD)/fm_kernels.o: $(CSRC)/fm_kernels.cu $(HDRS)
 # dense map: -fmad=false (bit-exact with oracle/dm_oracle.c, built with -ffp-contract=off)
 $(BUILD)/dm_map.o: $(CSRC)/dm_map.cu $(HDRS)
 	@mkdir -p $(BUILD); $(NVCC) $(NVFLAGS) -dc -o $@ $< -Xptxas -v 2> build_ptxas_dm.log || (cat build_ptxas_dm.log; false)
-$(OUT): $(BUILD)/fe_tracker.o $(BUILD)/ba_solver.o $(BUILD)/fm_kernels.o $(BUILD)/dm_map.o
+# occupancy grid: -fmad=false (bit-exact with oracle/gm_oracle.c's shared mode, built with -ffp-contract=off)
+$(BUILD)/gm_grid.o: $(CSRC)/gm_grid.cu $(HDRS)
+	@mkdir -p $(BUILD); $(NVCC) $(NVFLAGS) -dc -o $@ $< -Xptxas -v 2> build_ptxas_gm.log || (cat build_ptxas_gm.log; false)
+$(OUT): $(BUILD)/fe_tracker.o $(BUILD)/ba_solver.o $(BUILD)/fm_kernels.o $(BUILD)/dm_map.o $(BUILD)/gm_grid.o
 	$(NVCC) $(ARCH) -shared -o $@ $^
-	@cat build_ptxas_fe.log build_ptxas_ba.log build_ptxas_dm.log > build_ptxas.log
+	@cat build_ptxas_fe.log build_ptxas_ba.log build_ptxas_dm.log build_ptxas_gm.log > build_ptxas.log
 
-oracle: oracle/_build/libgf_oracle_dm.so
+oracle: oracle/_build/libgf_oracle_dm.so oracle/_build/libgf_oracle_gm.so
 	$(MAKE) -C oracle
 # the dense map's sequential restatement (tests and tools/bench_dense_map.py only): -O3 -ffp-contract=off as oracle/Makefile's
 # libgf_oracle_ba.so, plus -msse2 -mfpmath=sse as its libgf_oracle_fe.so
 oracle/_build/libgf_oracle_dm.so: oracle/dm_oracle.c
 	@mkdir -p oracle/_build; gcc -O3 -ffp-contract=off -msse2 -mfpmath=sse -shared -fPIC -o $@ $< -lm
+# the occupancy grid's sequential restatement, built like libgf_oracle_dm.so; it includes the kernel's shared log / exp
+oracle/_build/libgf_oracle_gm.so: oracle/gm_oracle.c $(CSRC)/gm_math.h
+	@mkdir -p oracle/_build; gcc -O3 -ffp-contract=off -msse2 -mfpmath=sse -shared -fPIC -o $@ $< -lm
 
 # development aid: the same library with the clock64() phase counters compiled in (GF_B200_LIB=... selects it)
-profile: $(SRCS) $(HDRS) $(BUILD)/fm_kernels.o $(BUILD)/dm_map.o
+profile: $(SRCS) $(HDRS) $(BUILD)/fm_kernels.o $(BUILD)/dm_map.o $(BUILD)/gm_grid.o
 	@mkdir -p $(BUILD)
 	$(NVCC) $(NVFLAGS) -DGF_PROFILE -dc -o $(BUILD)/fe_tracker_prof.o $(CSRC)/fe_tracker.cu
 	$(NVCC) $(filter-out -fmad=false,$(NVFLAGS)) -DGF_PROFILE -dc -o $(BUILD)/ba_solver_prof.o $(CSRC)/ba_solver.cu
-	$(NVCC) $(ARCH) -shared -o ground_fusion_b200/libgf_b200_prof.so $(BUILD)/fe_tracker_prof.o $(BUILD)/ba_solver_prof.o $(BUILD)/fm_kernels.o $(BUILD)/dm_map.o
+	$(NVCC) $(ARCH) -shared -o ground_fusion_b200/libgf_b200_prof.so $(BUILD)/fe_tracker_prof.o $(BUILD)/ba_solver_prof.o $(BUILD)/fm_kernels.o $(BUILD)/dm_map.o $(BUILD)/gm_grid.o
 
 clean:
 	rm -f $(OUT) build_ptxas.log; $(MAKE) -C oracle clean

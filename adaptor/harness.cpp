@@ -8,6 +8,8 @@
 //   harness ba-seq <in> <out>    the same input through each estimator's optimization() in turn
 //   harness dm <in> <out>   keyframes and pose corrections through DenseMap (PoseGraph's octree blocks); after each call the
 //                           returned point_rgbd (add only), the cloud and the filtered cloud's indices
+//   harness gm <in> <out>   keyframes' point_rgbd and pose corrections through GridMapper (the grid_mapping tool); after each
+//                           call bel, the map.png pixels and the OccupancyGrid data
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -17,6 +19,7 @@
 #include "dense_map.h"
 #include "estimator_ba.h"
 #include "feature_tracker.h"
+#include "grid_map.h"
 
 int MAX_CNT = 150, MIN_DIST = 30, FLOW_BACK = 1, EQUALIZE = 0;
 int USE_IMU = 1, NUM_ITERATIONS = 8, ESTIMATE_TD = 0;
@@ -211,11 +214,55 @@ static int run_dm(const char *in, const char *out)
     return 0;
 }
 
+// Input: size_x, size_y, init_x, init_y, cell_size, p_occ, p_free, p_prior, qic[9] (row-major), tic[3], max_points,
+// max_keyframes, max_records, n_ops; each op is int 0 + R[9] + P[3] + n + n x 6 floats (point_rgbd), or int 1 + n + n x (R[9], P[3]).
+static int run_gm(const char *in, const char *out)
+{
+    FILE *f = fopen(in, "rb"), *o = fopen(out, "wb");
+    if (!f || !o) return 2;
+    int sz[4];
+    rd(f, sz, sizeof(sz));
+    double c[4], q[9];
+    rd(f, c, sizeof(c));
+    rd(f, q, sizeof(q));
+    Eigen::Matrix3d qic; Eigen::Vector3d tic;
+    for (int i = 0; i < 9; i++) qic(i / 3, i % 3) = q[i];
+    rd(f, tic.data(), 24);
+    const int max_points = rd1<int>(f), max_keyframes = rd1<int>(f), max_records = rd1<int>(f), n_ops = rd1<int>(f);
+    GridMapper map(qic, tic, sz[0], sz[1], sz[2], sz[3], c[0], c[1], c[2], c[3], max_points, max_keyframes, max_records);
+    auto pose = [&](Eigen::Matrix3d &R, Eigen::Vector3d &P) {
+        double r[9]; rd(f, r, sizeof(r));
+        for (int i = 0; i < 9; i++) R(i / 3, i % 3) = r[i];
+        rd(f, P.data(), 24);
+    };
+    for (int op = 0; op < n_ops; op++) {
+        if (rd1<int>(f) == 0) {
+            Eigen::Matrix3d R; Eigen::Vector3d P;
+            pose(R, P);
+            std::vector<Eigen::Matrix<float, 6, 1>> pts(rd1<int>(f));
+            for (auto &v : pts) rd(f, v.data(), 24);
+            map.addKeyFrame(R, P, pts);
+        } else {
+            const int n = rd1<int>(f);
+            std::vector<Eigen::Matrix3d> Rs(n); std::vector<Eigen::Vector3d> Ps(n);
+            for (int k = 0; k < n; k++) pose(Rs[k], Ps[k]);
+            map.updatePath(Rs, Ps);
+        }
+        const auto bel = map.bel();
+        const auto img = map.image();
+        const auto occ = map.occupancy();
+        fwrite(bel.data(), 8, bel.size(), o); fwrite(img.data(), 1, img.size(), o); fwrite(occ.data(), 1, occ.size(), o);
+    }
+    fclose(f); fclose(o);
+    return 0;
+}
+
 int main(int argc, char **argv)
 {
-    if (argc != 4) { std::fprintf(stderr, "usage: harness fe|fe-eq|fe-box|ba|ba-multi|ba-seq|dm <in> <out>\n"); return 2; }
+    if (argc != 4) { std::fprintf(stderr, "usage: harness fe|fe-eq|fe-box|ba|ba-multi|ba-seq|dm|gm <in> <out>\n"); return 2; }
     if (!std::strcmp(argv[1], "fe-eq")) EQUALIZE = 1;
     if (!std::strcmp(argv[1], "dm")) return run_dm(argv[2], argv[3]);
+    if (!std::strcmp(argv[1], "gm")) return run_gm(argv[2], argv[3]);
     if (!std::strcmp(argv[1], "ba-multi") || !std::strcmp(argv[1], "ba-seq")) return run_ba_multi(argv[2], argv[3], argv[1][3] == 'm');
     return argv[1][0] == 'f' ? run_fe(argv[2], argv[3], !std::strcmp(argv[1], "fe-box")) : run_ba(argv[2], argv[3]);
 }

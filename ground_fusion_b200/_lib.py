@@ -31,6 +31,16 @@ class DenseMapCfg(ctypes.Structure):
 DENSE_MAP_CLOUD, DENSE_MAP_FILTERED = 0, 1      # gf_dense_map_read's `which`
 
 
+class GridMapCfg(ctypes.Structure):
+    _fields_ = [("size_x", ctypes.c_int), ("size_y", ctypes.c_int), ("init_x", ctypes.c_int), ("init_y", ctypes.c_int),
+                ("cell_size", ctypes.c_double), ("p_occ", ctypes.c_double), ("p_free", ctypes.c_double), ("p_prior", ctypes.c_double),
+                ("ric", ctypes.c_double * 9), ("tic", ctypes.c_double * 3), ("max_points", ctypes.c_int), ("max_keyframes", ctypes.c_int),
+                ("max_records", ctypes.c_int)]
+
+
+GRID_MAP_BEL, GRID_MAP_IMAGE, GRID_MAP_OCCUPANCY = 0, 1, 2      # gf_grid_map_read's `which`
+
+
 class Obs(ctypes.Structure):
     _fields_ = [("id", ctypes.c_int32), ("track_cnt", ctypes.c_int32), ("v", ctypes.c_double * 8)]
 
@@ -105,6 +115,14 @@ def lib():
         L.gf_dense_map_read.argtypes = [vp, i, vp, vp, vp]
         L.gf_dense_map_keyframe_points.argtypes = [vp, i, vp, ctypes.POINTER(i)]
         L.gf_stage_radius_filter.argtypes = [i, vp, i, d, i, vp]
+        L.gf_grid_map_create.argtypes = [ctypes.POINTER(vp), i, ctypes.POINTER(GridMapCfg)]
+        L.gf_grid_map_destroy.argtypes = [vp]
+        L.gf_grid_map_destroy.restype = None
+        L.gf_grid_map_add_keyframe.argtypes = [vp, vp, vp, vp, i, i, i]
+        L.gf_grid_map_update_poses.argtypes = [vp, i, vp, vp]
+        L.gf_grid_map_read.argtypes = [vp, i, vp]
+        L.gf_grid_map_size.argtypes = [vp] + [ctypes.POINTER(i)] * 4
+        L.gf_grid_map_stats.argtypes = [vp, vp]
         _LIB = L
     return _LIB
 

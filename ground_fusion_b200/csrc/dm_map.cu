@@ -16,6 +16,7 @@
 #include <vector>
 
 #include "gf_camera.cuh"
+#include "gf_pose.cuh"
 
 using namespace gf;
 
@@ -51,26 +52,7 @@ static void dm_octree_anchor(const double lo[3], const double hi[3], double mn[3
 static const double BOX_INIT_LO[3] = {-10000, -1000, -10000}, BOX_REBUILD_LO[3] = {-10000, -10000, -10000}, BOX_HI[3] = {10000, 10000, 10000};
 
 struct Anchor { double mn[3], mx[3]; };
-struct Pose { double R[9], P[3]; };                // row-major R; world = R x + P
-struct Ext { double ric[9], tic[3]; };
 
-__device__ __forceinline__ void mv3(const double* M, const double* x, double* y)
-{   // Eigen's Matrix3d * Vector3d without FMA: ((m0 x0 + m1 x1) + m2 x2) per row
-    const double y0 = M[0] * x[0] + M[1] * x[1] + M[2] * x[2];
-    const double y1 = M[3] * x[0] + M[4] * x[1] + M[5] * x[2];
-    const double y2 = M[6] * x[0] + M[7] * x[1] + M[8] * x[2];
-    y[0] = y0; y[1] = y1; y[2] = y2;
-}
-// pointWorld = R * (qic * point + tic) + P (:197), rounded to PointXYZRGB's floats
-__device__ __forceinline__ void to_world(const Ext& e, const Pose& T, const float* l, double* w)
-{
-    const double p[3] = {(double)l[0], (double)l[1], (double)l[2]};
-    double a[3], b[3];
-    mv3(e.ric, p, a);
-    for (int k = 0; k < 3; k++) a[k] = a[k] + e.tic[k];
-    mv3(T.R, a, b);
-    for (int k = 0; k < 3; k++) w[k] = b[k] + T.P[k];
-}
 // the voxel key of a float point inside the anchored box, packed 3 x 21 bits; INVALID (and *bad set) outside the box
 __device__ __forceinline__ uint64_t dm_voxel_key(const Anchor& A, const float* f, int* bad)
 {

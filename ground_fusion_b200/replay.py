@@ -182,7 +182,7 @@ class WindowEstimator:
 
 
 def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=True, max_iter=8, feedback=False, use_mcc=False, boxes=None,
-           dense_map=None):
+           dense_map=None, grid_map=None):
     """Runs n_frames of `stream` through tracker -> fm -> ba.  Returns dict(t, P_est, P_gt, R_est, R_gt, keyframes, ...).
     tracker.trackImage(t, gray, depth) -> {id: v[8]};  fm / ba: see WindowEstimator.  feedback: the estimator calls the tracker's
     removeOutliers / setPrediction after every optimisation (the reference with MULTIPLE_THREAD 0).
@@ -191,13 +191,19 @@ def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=Tru
     (rosNodeTest.cpp:433-439, 519-540).
     dense_map: a map with addKeyFrame(R, P, rgb, depth) (DenseMap, or the oracle's), fed as pubKeyframe feeds the mapping node
     (visualization.cpp): after every MARGIN_OLD, the pose of window frame WINDOW_SIZE - 2 with that frame's colour and depth
-    images (stream.color / stream.frame), unless its position equals the previous keyframe's exactly, as the node skips it.  It is returned under "dense_map"."""
+    images (stream.color / stream.frame), unless its position equals the previous keyframe's exactly, as the node skips it.  It is returned under "dense_map".
+    grid_map: an occupancy grid with addKeyFrame(R, P, points) (GridMap, or the oracle's); requires dense_map.  After dense-map
+    keyframe k it gets the same pose and dense_map.keyframePoints(k), the point_rgbd the grid_mapping tool reads.  It is returned
+    under "grid_map"."""
+    if grid_map is not None and dense_map is None:
+        raise ValueError("grid_map requires dense_map")
     imu = ImuFromStream(stream)
     est = WindowEstimator(fm, ba, imu_propagate=imu_propagate, max_iter=max_iter, tracker=tracker if feedback else None, use_mcc=use_mcc)
     out_t, out_P, out_R, gt_P, gt_R, iters = [], [], [], [], [], []
     t_prev = None
     slot = [0] * (WINDOW_SIZE + 1)                      # stream frame held by each window slot (Headers[])
     last_P = None                                       # position of the last keyframe fed to dense_map
+    n_dm = 0                                            # keyframes fed to dense_map
     for k in range(n_frames):
         t, gray, depth = stream.frame(k)
         if t_prev is not None:                          # IMU samples of (t_prev, t]
@@ -227,6 +233,9 @@ def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=Tru
                 j = slot[WINDOW_SIZE - 2]
                 last_P = est.Ps[WINDOW_SIZE - 2].copy()
                 dense_map.addKeyFrame(est.Rs[WINDOW_SIZE - 2], last_P, stream.color(j), stream.frame(j)[2])
+                if grid_map is not None:
+                    grid_map.addKeyFrame(est.Rs[WINDOW_SIZE - 2], last_P, dense_map.keyframePoints(n_dm))
+                n_dm += 1
         if res is not None:
             R_wb, P = imu.pose_t(t)
             out_t.append(t); out_P.append(res[0]); out_R.append(res[1]); gt_P.append(P); gt_R.append(R_wb)
@@ -238,4 +247,6 @@ def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=Tru
            "n_removed": est.n_removed, "n_predicted": est.n_predicted}
     if dense_map is not None:
         out["dense_map"] = dense_map
+    if grid_map is not None:
+        out["grid_map"] = grid_map
     return out

@@ -620,6 +620,49 @@ int gf_dense_map_keyframe_points(gf_dense_map* map, int k, float* out6, int* n);
  * distance < float(radius^2). */
 int gf_stage_radius_filter(int device, const float* xyz, int n, double radius, int min_pts, uint8_t* keep);
 
+/* ------------------------------------------------------------------------------------------------
+ * Occupancy grid (support_files/grid_mapping: main.cpp, grid_mapper.cpp, grid_map.cpp): the 2-D log-odds grid the reference
+ * builds offline from every keyframe's point_rgbd and corrected pose, here built online.  Keyframe points whose world height
+ * lies in [0.1, 0.5] m cast a ray from the body position in steps of one cell; every cell on the way gets the inverse sensor
+ * model's free / occupied / prior update.  After any sequence of calls bel equals the tool's over the same keyframes in the
+ * same order with the poses last passed, with the tool's log / exp replaced by the shared double-double ones of
+ * csrc/gm_math.h.  DESIGN.md "Occupancy grid" has the semantics.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct gf_grid_map gf_grid_map; /* opaque: one grid, bound to one GPU and one stream */
+
+typedef struct gf_grid_map_cfg {
+    int size_x, size_y;      /* cells (1500 x 500 in the tool); size_x * size_y < 2^30 */
+    int init_x, init_y;      /* the cell of world (0, 0) (750, 250) */
+    double cell_size;        /* metres (0.05), > 0 */
+    double p_occ, p_free, p_prior; /* inverse sensor model (0.6, 0.4, 0.5), each in (0, 1) */
+    double ric[9];           /* qic (row-major) and tic: camera to body */
+    double tic[3];
+    int max_points;          /* capacity: points of all keyframes together */
+    int max_keyframes;       /* capacity: keyframes */
+    int max_records;         /* ray steps sorted at once; a call with more is processed in chunks of this many */
+} gf_grid_map_cfg;
+
+enum { GF_GRID_MAP_BEL = 0, GF_GRID_MAP_IMAGE = 1, GF_GRID_MAP_OCCUPANCY = 2 };
+
+int gf_grid_map_create(gf_grid_map** map, int device, const gf_grid_map_cfg* cfg);
+void gf_grid_map_destroy(gf_grid_map* map);
+/* One keyframe with body pose (R row-major, P) applied on top of the grid: n camera-frame points, rows of stride_floats floats
+ * (x y z first; 6 takes gf_dense_map_keyframe_points' rows as they are), a HOST pointer or a device pointer when on_device != 0.
+ * GF_ERR_INVALID_ARG (a non-finite pose or point) and GF_ERR_CAPACITY (max_keyframes, max_points, a ray of more than 2^24 steps)
+ * leave the grid unchanged. */
+int gf_grid_map_add_keyframe(gf_grid_map* map, const double* R, const double* P, const float* pts, int n, int stride_floats, int on_device);
+/* The rebuild after a pose correction: the grid back to 0.5, then every keyframe applied again in order with its new pose
+ * (R [n][9], P [n][3]).  n_keyframes must equal the number of keyframes added (GF_ERR_INVALID_ARG otherwise, grid unchanged). */
+int gf_grid_map_update_poses(gf_grid_map* map, int n_keyframes, const double* R, const double* P);
+/* Host copy of GF_GRID_MAP_BEL: double [size_x * size_y], bel(x, y) at x + size_x * y (Eigen's column-major order);
+ * GF_GRID_MAP_IMAGE: uint8 [size_x][size_y], the pixels GridMap::saveMap writes to map.png; GF_GRID_MAP_OCCUPANCY: int8
+ * [size_x * size_y], the nav_msgs/OccupancyGrid data the mapping node publishes from that image (-1 unknown, else 0..100). */
+int gf_grid_map_read(gf_grid_map* map, int which, void* out);
+int gf_grid_map_size(gf_grid_map* map, int* size_x, int* size_y, int* n_keyframes, int* n_points);
+/* Of the last add_keyframe / update_poses: out4 = ray steps (records), updates applied, updates the exact shortcuts skipped
+ * (a repeated no-op update, a cell at 0 or 1) and the longest per-cell run within one chunk. */
+int gf_grid_map_stats(gf_grid_map* map, int64_t* out4);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif
