@@ -19,15 +19,18 @@ $(BUILD)/ba_solver.o: $(CSRC)/ba_solver.cu $(HDRS)
 	@mkdir -p $(BUILD); $(NVCC) $(filter-out -fmad=false,$(NVFLAGS)) -dc -o $@ $< -Xptxas -v 2> build_ptxas_ba.log || (cat build_ptxas_ba.log; false)
 $(BUILD)/fm_kernels.o: $(CSRC)/fm_kernels.cu $(HDRS)
 	@mkdir -p $(BUILD); $(NVCC) $(filter-out -fmad=false,$(NVFLAGS)) -dc -o $@ $<
+# landmark table: the flags of fm_kernels.o, whose arithmetic (fm_device.cuh) it shares bit for bit
+$(BUILD)/fm_window.o: $(CSRC)/fm_window.cu $(HDRS)
+	@mkdir -p $(BUILD); $(NVCC) $(filter-out -fmad=false,$(NVFLAGS)) -dc -o $@ $< -Xptxas -v 2> build_ptxas_fmw.log || (cat build_ptxas_fmw.log; false)
 # dense map: -fmad=false (bit-exact with oracle/dm_oracle.c, built with -ffp-contract=off)
 $(BUILD)/dm_map.o: $(CSRC)/dm_map.cu $(HDRS)
 	@mkdir -p $(BUILD); $(NVCC) $(NVFLAGS) -dc -o $@ $< -Xptxas -v 2> build_ptxas_dm.log || (cat build_ptxas_dm.log; false)
 # occupancy grid: -fmad=false (bit-exact with oracle/gm_oracle.c's shared mode, built with -ffp-contract=off)
 $(BUILD)/gm_grid.o: $(CSRC)/gm_grid.cu $(HDRS)
 	@mkdir -p $(BUILD); $(NVCC) $(NVFLAGS) -dc -o $@ $< -Xptxas -v 2> build_ptxas_gm.log || (cat build_ptxas_gm.log; false)
-$(OUT): $(BUILD)/fe_tracker.o $(BUILD)/ba_solver.o $(BUILD)/fm_kernels.o $(BUILD)/dm_map.o $(BUILD)/gm_grid.o
+$(OUT): $(BUILD)/fe_tracker.o $(BUILD)/ba_solver.o $(BUILD)/fm_kernels.o $(BUILD)/fm_window.o $(BUILD)/dm_map.o $(BUILD)/gm_grid.o
 	$(NVCC) $(ARCH) -shared -o $@ $^
-	@cat build_ptxas_fe.log build_ptxas_ba.log build_ptxas_dm.log build_ptxas_gm.log > build_ptxas.log
+	@cat build_ptxas_fe.log build_ptxas_ba.log build_ptxas_dm.log build_ptxas_gm.log build_ptxas_fmw.log > build_ptxas.log
 
 oracle: oracle/_build/libgf_oracle_dm.so oracle/_build/libgf_oracle_gm.so
 	$(MAKE) -C oracle
@@ -40,11 +43,11 @@ oracle/_build/libgf_oracle_gm.so: oracle/gm_oracle.c $(CSRC)/gm_math.h
 	@mkdir -p oracle/_build; gcc -O3 -ffp-contract=off -msse2 -mfpmath=sse -shared -fPIC -o $@ $< -lm
 
 # development aid: the same library with the clock64() phase counters compiled in (GF_B200_LIB=... selects it)
-profile: $(SRCS) $(HDRS) $(BUILD)/fm_kernels.o $(BUILD)/dm_map.o $(BUILD)/gm_grid.o
+profile: $(SRCS) $(HDRS) $(BUILD)/fm_kernels.o $(BUILD)/fm_window.o $(BUILD)/dm_map.o $(BUILD)/gm_grid.o
 	@mkdir -p $(BUILD)
 	$(NVCC) $(NVFLAGS) -DGF_PROFILE -dc -o $(BUILD)/fe_tracker_prof.o $(CSRC)/fe_tracker.cu
 	$(NVCC) $(filter-out -fmad=false,$(NVFLAGS)) -DGF_PROFILE -dc -o $(BUILD)/ba_solver_prof.o $(CSRC)/ba_solver.cu
-	$(NVCC) $(ARCH) -shared -o ground_fusion_b200/libgf_b200_prof.so $(BUILD)/fe_tracker_prof.o $(BUILD)/ba_solver_prof.o $(BUILD)/fm_kernels.o $(BUILD)/dm_map.o $(BUILD)/gm_grid.o
+	$(NVCC) $(ARCH) -shared -o ground_fusion_b200/libgf_b200_prof.so $(BUILD)/fe_tracker_prof.o $(BUILD)/ba_solver_prof.o $(BUILD)/fm_kernels.o $(BUILD)/fm_window.o $(BUILD)/dm_map.o $(BUILD)/gm_grid.o
 
 clean:
 	rm -f $(OUT) build_ptxas.log; $(MAKE) -C oracle clean

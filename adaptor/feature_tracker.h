@@ -40,6 +40,8 @@ class FeatureTracker
     void setPinhole(double fx, double fy, double cx, double cy, double k1, double k2, double p1, double p2, int depth);
     void setPrediction(std::map<int, Eigen::Vector3d> &predictPts);
     void removeOutliers(std::set<int> &removePtsIds);
+    // the library's tracker (null before the first frame), for FeatureManager::addFeatureCheckParallax(frame_count, tracker, td)
+    const gf_tracker *handle() const { return gf_; }
 
     int row = 0, col = 0;
     std::vector<cv::Point2f> cur_pts;

@@ -10,14 +10,27 @@
 //                           returned point_rgbd (add only), the cloud and the filtered cloud's indices
 //   harness gm <in> <out>   keyframes' point_rgbd and pose corrections through GridMapper (the grid_mapping tool); after each
 //                           call bel, the map.png pixels and the OccupancyGrid data
+//   harness fm <in> <out>   a call script through FeatureManager (the landmark table on the GPU); after each call its return
+//                           values and the whole table (FeatureManager::features)
+//   harness fm-bench <in> <out>  host time per frame of the FeatureManager stage from C++ alone: the calls one processImage makes
+//                           around the solve, once over a std::list on the host with the stateless gf_fm_* calls and once over
+//                           gf_fm_window, alternating; <out> is one JSON object (tools/bench_fm_window.py reads it)
+#include <algorithm>
+#include <array>
+#include <chrono>
+#include <list>
+#include <unordered_map>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <memory>
+#include <set>
 #include <vector>
 
 #include "dense_map.h"
 #include "estimator_ba.h"
+#include "feature_manager.h"
 #include "feature_tracker.h"
 #include "grid_map.h"
 
@@ -257,12 +270,297 @@ static int run_gm(const char *in, const char *out)
     return 0;
 }
 
+// ops: 0 add (fc, td, n, n x (id, v[8])) -> margin_old, 3 counters, parallax; 1 triangulate (fc, poses); 2 fillProblem -> rows, para, const;
+// 3 setDepth (n, x); 4 removeFailures; 5 removeOutlier (n, ids); 6 removeBackShiftDepth (R, P, R, P); 7 removeBack; 8 removeFront (fc);
+// 9 outliersRejection (poses) -> ids; 10 movingConsistencyCheckW (poses) -> ids; 11 predictPtsInNextFrame (fc, poses) -> (id, xyz);
+// poses: Ps [11][3], Rs [11][9] row-major, tic, ric
+static int run_fm(const char *in, const char *out)
+{
+    FILE *f = fopen(in, "rb"), *o = fopen(out, "wb");
+    if (!f || !o) return 2;
+    const double min_parallax = rd1<double>(f), depth_threshold = rd1<double>(f), init_depth = rd1<double>(f);
+    const int cap = rd1<int>(f), n_ops = rd1<int>(f);
+    gf_device::FeatureManager fm(min_parallax, depth_threshold, init_depth, cap);
+    Eigen::Vector3d Ps[11], tic; Eigen::Matrix3d Rs[11], ric;
+    auto mat = [&](Eigen::Matrix3d &M) { double r[9]; rd(f, r, sizeof(r)); for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) M(i, j) = r[3 * i + j]; };
+    auto poses = [&]() {
+        for (auto &P : Ps) rd(f, P.data(), 24);
+        for (auto &R : Rs) mat(R);
+        rd(f, tic.data(), 24); mat(ric);
+    };
+    auto put_ids = [&](const std::set<int> &s) { const int n = (int)s.size(); fwrite(&n, 4, 1, o); for (int id : s) fwrite(&id, 4, 1, o); };
+    for (int k = 0; k < n_ops; k++) {
+        const int op = rd1<int>(f);
+        if (op == 0) {
+            const int fc = rd1<int>(f); const double td = rd1<double>(f); const int n = rd1<int>(f);
+            std::map<int, std::vector<std::pair<int, Eigen::Matrix<double, 8, 1>>>> image;
+            for (int i = 0; i < n; i++) { const int id = rd1<int>(f); Eigen::Matrix<double, 8, 1> v; rd(f, v.data(), 64); image[id].emplace_back(0, v); }
+            const int margin = fm.addFeatureCheckParallax(fc, image, td);
+            const int c[4] = {margin, fm.last_track_num, fm.new_feature_num, fm.long_track_num};
+            fwrite(c, 4, 4, o); fwrite(&fm.last_average_parallax, 8, 1, o);
+        } else if (op == 1) { const int fc = rd1<int>(f); poses(); fm.triangulate(fc, Ps, Rs, tic, ric); }
+        else if (op == 2) {
+            std::vector<gf_ba_visual_factor> rows; std::vector<double> para; std::vector<uint8_t> cst;
+            fm.fillProblem(rows, para, cst);
+            const int n[2] = {(int)rows.size(), (int)para.size()};
+            fwrite(n, 4, 2, o); fwrite(rows.data(), sizeof(gf_ba_visual_factor), rows.size(), o); fwrite(para.data(), 8, para.size(), o); fwrite(cst.data(), 1, cst.size(), o);
+        } else if (op == 3) { std::vector<double> x(rd1<int>(f)); rd(f, x.data(), 8 * x.size()); fm.setDepth(x); }
+        else if (op == 4) fm.removeFailures();
+        else if (op == 5) { std::set<int> s; for (int n = rd1<int>(f); n > 0; n--) s.insert(rd1<int>(f)); fm.removeOutlier(s); }
+        else if (op == 6) { Eigen::Matrix3d R0, R1; Eigen::Vector3d P0, P1; mat(R0); rd(f, P0.data(), 24); mat(R1); rd(f, P1.data(), 24); fm.removeBackShiftDepth(R0, P0, R1, P1); }
+        else if (op == 7) fm.removeBack();
+        else if (op == 8) fm.removeFront(rd1<int>(f));
+        else if (op == 9 || op == 10) {
+            poses();
+            std::set<int> s;
+            if (op == 9) fm.outliersRejection(s, Ps, Rs, tic, ric); else fm.movingConsistencyCheckW(s, Ps, Rs, tic, ric);
+            put_ids(s);
+        } else if (op == 11) {
+            const int fc = rd1<int>(f); poses();
+            auto pred = fm.predictPtsInNextFrame(fc, Ps, Rs, tic, ric);
+            const int n = (int)pred.size(); fwrite(&n, 4, 1, o);
+            for (auto &kv : pred) { fwrite(&kv.first, 4, 1, o); fwrite(kv.second.data(), 8, 3, o); }
+        } else return 2;
+        const auto tab = fm.features();
+        const int n = (int)tab.size(); fwrite(&n, 4, 1, o);
+        for (auto &it : tab) {
+            const int h[5] = {it.feature_id, it.start_frame, (int)it.feature_per_frame.size(), it.estimate_flag, it.solve_flag};
+            fwrite(h, 4, 5, o); fwrite(&it.estimated_depth, 8, 1, o);
+            for (auto &r : it.feature_per_frame) fwrite(r.data(), 8, 9, o);
+        }
+    }
+    fclose(f); fclose(o);
+    return 0;
+}
+
+// ---- fm-bench: the FeatureManager stage in C++, host lists + stateless calls against the resident table ----
+namespace fmb {
+static void ok(int rc, const char *what) { if (rc != GF_OK) { std::fprintf(stderr, "%s: %s\n", what, gf_last_error()); std::exit(3); } }
+struct Obs { int id; double v[8]; };
+struct Poses { double P[33], R[99], tic[3], ric[9]; };
+struct Lm { int id, start; double est = -1; int eflag = 0, sflag = 0; std::vector<std::array<double, 9>> obs; int end() const { return start + (int)obs.size() - 1; } };
+constexpr int W = 10;
+constexpr double FOCAL = 600.0, INIT_DEPTH = 5.0;
+
+// FeatureManager as the reference keeps it: a std::list on the host; the per-landmark loops are the stateless library calls
+struct HostFM {
+    std::list<Lm> feature;
+    double min_parallax, depth_threshold;
+    std::vector<int32_t> start, nobs, off, flag, cnt; std::vector<double> pts, dep, est, e2, e3;
+    void flatten(const std::vector<Lm *> &f, bool with_depth)
+    {
+        const size_t n = f.size();
+        start.resize(n); nobs.resize(n); off.resize(n); est.resize(n); flag.resize(n); pts.clear(); dep.clear();
+        int o = 0;
+        for (size_t i = 0; i < n; i++) {
+            start[i] = f[i]->start; nobs[i] = (int)f[i]->obs.size(); off[i] = o; est[i] = f[i]->est; flag[i] = f[i]->eflag; o += nobs[i];
+            for (auto &r : f[i]->obs) { pts.insert(pts.end(), r.begin(), r.begin() + 3); if (with_depth) dep.push_back(r[7]); }
+        }
+    }
+    bool add(int fc, const std::vector<Obs> &image, double td)
+    {
+        std::unordered_map<int, Lm *> index;
+        index.reserve(feature.size() * 2);
+        for (auto &it : feature) index[it.id] = &it;
+        int last = 0, fresh = 0, lng = 0;
+        for (auto &o : image) {
+            std::array<double, 9> row;
+            std::copy(o.v, o.v + 8, row.begin()); row[8] = td;
+            auto f = index.find(o.id);
+            if (f == index.end()) { feature.emplace_back(); Lm &l = feature.back(); l.id = o.id; l.start = fc; l.obs.push_back(row); fresh++; }
+            else { f->second->obs.push_back(row); last++; lng += f->second->obs.size() >= 4; }
+        }
+        if (fc < 2 || last < 20 || lng < 40 || fresh > 0.5 * last) return true;
+        std::vector<double> pi, pj;
+        for (auto &it : feature)
+            if (it.start <= fc - 2 && it.end() >= fc - 1) {
+                auto &a = it.obs[fc - 2 - it.start]; auto &b = it.obs[fc - 1 - it.start];
+                pi.insert(pi.end(), a.begin(), a.begin() + 3); pj.insert(pj.end(), b.begin(), b.begin() + 3);
+            }
+        if (pi.empty()) return true;
+        double sum = 0;
+        ok(gf_fm_parallax(0, (int)pi.size() / 3, pi.data(), pj.data(), &sum), "gf_fm_parallax");
+        return sum / (pi.size() / 3) >= min_parallax;
+    }
+    void triangulate(const Poses &p)
+    {
+        std::vector<Lm *> f;
+        for (auto &it : feature) f.push_back(&it);
+        if (f.empty()) return;
+        flatten(f, true);
+        ok(gf_fm_triangulate(0, (int)f.size(), start.data(), nobs.data(), off.data(), (int)dep.size(), pts.data(), dep.data(), est.data(), flag.data(), 11, p.P, p.R,
+                             p.tic, p.ric, depth_threshold, INIT_DEPTH), "gf_fm_triangulate");
+        for (size_t i = 0; i < f.size(); i++) { f[i]->est = est[i]; f[i]->eflag = flag[i]; }
+    }
+    void fill(std::vector<gf_ba_visual_factor> &rows, std::vector<double> &para, std::vector<uint8_t> &cst)
+    {
+        rows.clear(); para.clear(); cst.clear();
+        for (auto &it : feature) {
+            if (it.obs.size() < 4) continue;
+            const int k = (int)para.size();
+            para.push_back(1.0 / it.est); cst.push_back(it.eflag == 1);
+            for (size_t a = 1; a < it.obs.size(); a++) {
+                gf_ba_visual_factor v{};
+                v.imu_i = it.start; v.imu_j = it.start + (int)a; v.feature = k;
+                for (int c = 0; c < 3; c++) { v.pts_i[c] = it.obs[0][c]; v.pts_j[c] = it.obs[a][c]; }
+                for (int c = 0; c < 2; c++) { v.vel_i[c] = it.obs[0][5 + c]; v.vel_j[c] = it.obs[a][5 + c]; }
+                v.td_i = it.obs[0][8]; v.td_j = it.obs[a][8];
+                rows.push_back(v);
+            }
+        }
+    }
+    void setDepth(const std::vector<double> &x)
+    {
+        size_t k = 0;
+        for (auto &it : feature) if (it.obs.size() >= 4) { it.est = 1.0 / x[k++]; it.sflag = it.est < 0 ? 2 : 1; }
+    }
+    std::vector<int> moving(const Poses &p)
+    {
+        std::vector<Lm *> f;
+        for (auto &it : feature) if (it.obs.size() >= 2 && it.start < W - 2 && !(it.est < 0)) f.push_back(&it);
+        std::vector<int> out;
+        if (f.empty()) return out;
+        flatten(f, false);
+        e2.resize(f.size()); e3.resize(f.size()); cnt.resize(f.size());
+        ok(gf_fm_reprojection_errors(0, (int)f.size(), start.data(), nobs.data(), off.data(), (int)pts.size() / 3, pts.data(), est.data(), 11, p.P, p.R, p.tic, p.ric,
+                                     e2.data(), e3.data(), cnt.data()), "gf_fm_reprojection_errors");
+        for (size_t i = 0; i < f.size(); i++) if (cnt[i] > 0 && (FOCAL * e2[i] / cnt[i] > 10 || e3[i] / cnt[i] > 2.0)) out.push_back(f[i]->id);
+        return out;
+    }
+    void removeIds(const std::vector<int> &ids) { feature.remove_if([&](const Lm &l) { return std::find(ids.begin(), ids.end(), l.id) != ids.end(); }); }
+    int predict(int fc, const Poses &p, std::vector<double> &xyz)
+    {
+        std::vector<int32_t> first; std::vector<double> uv, d;
+        for (auto &it : feature) if (it.est > 0 && it.obs.size() >= 2 && it.end() == fc) { first.push_back(it.start); uv.insert(uv.end(), it.obs[0].begin(), it.obs[0].begin() + 3); d.push_back(it.est); }
+        xyz.resize(3 * first.size());
+        if (!first.empty()) ok(gf_fm_predict_next(0, (int)first.size(), first.data(), uv.data(), d.data(), 11, fc, p.P, p.R, p.tic, p.ric, xyz.data()), "gf_fm_predict_next");
+        return (int)first.size();
+    }
+    void removeBackShiftDepth(const Poses &p)
+    {
+        std::vector<Lm *> moved; std::vector<double> uv, d;
+        for (auto it = feature.begin(); it != feature.end();) {
+            if (it->start != 0) { it->start--; ++it; continue; }
+            const auto first = it->obs.front();
+            it->obs.erase(it->obs.begin());
+            if (it->obs.size() < 2) { it = feature.erase(it); continue; }
+            moved.push_back(&*it); uv.insert(uv.end(), first.begin(), first.begin() + 3); d.push_back(it->est); ++it;
+        }
+        if (moved.empty()) return;
+        ok(gf_fm_back_shift_depth(0, (int)moved.size(), uv.data(), d.data(), p.R, p.P, p.R + 9, p.P + 3, INIT_DEPTH), "gf_fm_back_shift_depth");
+        for (size_t i = 0; i < moved.size(); i++) moved[i]->est = d[i];
+    }
+    void removeFront(int fc)
+    {
+        for (auto it = feature.begin(); it != feature.end();) {
+            if (it->start == fc) { it->start--; ++it; continue; }
+            if (it->end() < fc - 1) { ++it; continue; }
+            it->obs.erase(it->obs.begin() + (W - 1 - it->start));
+            if (it->obs.empty()) it = feature.erase(it); else ++it;
+        }
+    }
+    void removeFailures() { feature.remove_if([](const Lm &l) { return l.sflag == 2; }); }
+};
+
+struct Pass { double stage_us, fill_us; long factors; };
+static double median(std::vector<double> v) { std::sort(v.begin(), v.end()); return v.empty() ? 0 : v[v.size() / 2]; }
+using clk = std::chrono::steady_clock;
+static double us(clk::time_point a, clk::time_point b) { return std::chrono::duration<double, std::micro>(b - a).count(); }
+
+// one pass of the stream; `win` null: the host list.  The same calls in the same order on both arms; the solve is left out
+// (setDepth gets the depth vector back), and at most three of the ids the consistency check flags are removed per frame.
+static Pass pass(const std::vector<std::vector<Obs>> &frames, const Poses &p, double min_parallax, double depth_threshold, gf_fm_window *win)
+{
+    HostFM h; h.min_parallax = min_parallax; h.depth_threshold = depth_threshold;
+    if (win) ok(gf_fm_window_clear(win), "clear");
+    std::vector<double> t_stage, t_fill, para(8192), xyz(3 * 8192);
+    std::vector<gf_ba_visual_factor> rows; std::vector<uint8_t> cst(8192); std::vector<gf_obs> obs; std::vector<int32_t> ids(8192);
+    if (win) rows.resize(8192 * 10);
+    long factors = 0;
+    for (size_t k = 0; k < frames.size(); k++) {
+        const int fc = (int)std::min<size_t>(k, W);
+        const auto t0 = clk::now();
+        int margin = 0;
+        if (win) {
+            obs.resize(frames[k].size());
+            for (size_t i = 0; i < obs.size(); i++) { obs[i].id = frames[k][i].id; obs[i].track_cnt = 0; std::copy(frames[k][i].v, frames[k][i].v + 8, obs[i].v); }
+            int32_t c4[4]; double par;
+            ok(gf_fm_window_add_frame(win, fc, obs.data(), (int)obs.size(), nullptr, 0.0, &margin, c4, &par), "add_frame");
+        } else margin = h.add(fc, frames[k], 0.0);
+        if (fc < W) continue;
+        int nf = 0, nv = 0, n = 0;
+        if (win) ok(gf_fm_window_triangulate(win, fc, p.P, p.R, p.tic, p.ric), "triangulate"); else h.triangulate(p);
+        const auto t1 = clk::now();
+        if (win) ok(gf_fm_window_fill_problem(win, rows.data(), (int)rows.size(), &nv, para.data(), cst.data(), &nf), "fill_problem");
+        else { std::vector<double> pf; std::vector<uint8_t> c; h.fill(rows, pf, c); nv = (int)rows.size(); nf = (int)pf.size(); std::copy(pf.begin(), pf.end(), para.begin()); }
+        t_fill.push_back(us(t1, clk::now())); factors = nv;
+        std::vector<int> bad;
+        if (win) {
+            ok(gf_fm_window_set_depth(win, para.data(), nf), "set_depth");
+            ok(gf_fm_window_outliers(win, p.P, p.R, p.tic, p.ric, GF_FM_OUTLIERS_MOVING, ids.data(), &n), "outliers");
+            bad.assign(ids.begin(), ids.begin() + n);
+        } else { h.setDepth(std::vector<double>(para.begin(), para.begin() + nf)); bad = h.moving(p); }
+        std::sort(bad.begin(), bad.end());
+        if (bad.size() > 3) bad.resize(3);
+        if (win) {
+            std::vector<int32_t> b(bad.begin(), bad.end());
+            ok(gf_fm_window_remove_ids(win, b.data(), (int)b.size()), "remove_ids");
+            ok(gf_fm_window_predict_next(win, fc, p.P, p.R, p.tic, p.ric, ids.data(), xyz.data(), &n), "predict_next");
+            if (margin || k % 3 == 0) ok(gf_fm_window_remove_back_shift_depth(win, p.R, p.P, p.R + 9, p.P + 3), "remove_back_shift_depth");
+            else ok(gf_fm_window_remove_front(win, fc), "remove_front");
+            ok(gf_fm_window_remove_failures(win), "remove_failures");
+            ok(gf_fm_window_size(win, &n), "size");                 // the frame's work has finished on the device before the clock stops
+        } else {
+            h.removeIds(bad); h.predict(fc, p, xyz);
+            if (margin || k % 3 == 0) h.removeBackShiftDepth(p); else h.removeFront(fc);
+            h.removeFailures();
+        }
+        t_stage.push_back(us(t0, clk::now()));
+    }
+    return {median(t_stage), median(t_fill), factors};
+}
+}  // namespace fmb
+
+static int run_fm_bench(const char *in, const char *out)
+{
+    using namespace fmb;
+    FILE *f = fopen(in, "rb"), *o = fopen(out, "w");
+    if (!f || !o) return 2;
+    const int rounds = rd1<int>(f), n_frames = rd1<int>(f);
+    const double min_parallax = rd1<double>(f), depth_threshold = rd1<double>(f);
+    Poses p; rd(f, &p, sizeof(p));
+    std::vector<std::vector<Obs>> frames(n_frames);
+    for (auto &fr : frames) { fr.resize(rd1<int>(f)); for (auto &ob : fr) { ob.id = rd1<int>(f); rd(f, ob.v, 64); } }
+    gf_fm_window_cfg c{};
+    c.max_features = 8192; c.window_size = 10; c.min_parallax = min_parallax; c.depth_threshold = depth_threshold; c.init_depth = INIT_DEPTH;
+    gf_fm_window *win = nullptr;
+    ok(gf_fm_window_create(&win, 0, &c), "gf_fm_window_create");
+    const Pass wa = pass(frames, p, min_parallax, depth_threshold, nullptr), wb = pass(frames, p, min_parallax, depth_threshold, win);    // warm-up
+    std::vector<Pass> a, b;
+    for (int r = 0; r < rounds; r++) { a.push_back(pass(frames, p, min_parallax, depth_threshold, nullptr)); b.push_back(pass(frames, p, min_parallax, depth_threshold, win)); }
+    gf_fm_window_destroy(win);
+    auto put = [&](const char *name, const std::vector<Pass> &v, bool last) {
+        std::vector<double> s, fl;
+        for (auto &x : v) { s.push_back(x.stage_us); fl.push_back(x.fill_us); }
+        std::fprintf(o, "\"%s\": {\"stage_us\": {\"median\": %.3f, \"min\": %.3f, \"max\": %.3f}, \"factor_loop_us\": {\"median\": %.3f, \"min\": %.3f, \"max\": %.3f}}%s",
+                     name, median(s), *std::min_element(s.begin(), s.end()), *std::max_element(s.begin(), s.end()), median(fl),
+                     *std::min_element(fl.begin(), fl.end()), *std::max_element(fl.begin(), fl.end()), last ? "" : ", ");
+    };
+    std::fprintf(o, "{\"factors_per_window\": [%ld, %ld], ", wa.factors, wb.factors);
+    put("stateless_calls_host_list", a, false); put("gf_fm_window", b, true);
+    std::fprintf(o, "}\n");
+    fclose(f); fclose(o);
+    return 0;
+}
+
 int main(int argc, char **argv)
 {
-    if (argc != 4) { std::fprintf(stderr, "usage: harness fe|fe-eq|fe-box|ba|ba-multi|ba-seq|dm|gm <in> <out>\n"); return 2; }
+    if (argc != 4) { std::fprintf(stderr, "usage: harness fe|fe-eq|fe-box|ba|ba-multi|ba-seq|dm|gm|fm|fm-bench <in> <out>\n"); return 2; }
     if (!std::strcmp(argv[1], "fe-eq")) EQUALIZE = 1;
     if (!std::strcmp(argv[1], "dm")) return run_dm(argv[2], argv[3]);
     if (!std::strcmp(argv[1], "gm")) return run_gm(argv[2], argv[3]);
+    if (!std::strcmp(argv[1], "fm")) return run_fm(argv[2], argv[3]);
+    if (!std::strcmp(argv[1], "fm-bench")) return run_fm_bench(argv[2], argv[3]);
     if (!std::strcmp(argv[1], "ba-multi") || !std::strcmp(argv[1], "ba-seq")) return run_ba_multi(argv[2], argv[3], argv[1][3] == 'm');
     return argv[1][0] == 'f' ? run_fe(argv[2], argv[3], !std::strcmp(argv[1], "fe-box")) : run_ba(argv[2], argv[3]);
 }

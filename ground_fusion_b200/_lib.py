@@ -41,6 +41,15 @@ class GridMapCfg(ctypes.Structure):
 GRID_MAP_BEL, GRID_MAP_IMAGE, GRID_MAP_OCCUPANCY = 0, 1, 2      # gf_grid_map_read's `which`
 
 
+class FmWindowCfg(ctypes.Structure):
+    _fields_ = [("max_features", ctypes.c_int), ("window_size", ctypes.c_int), ("min_parallax", ctypes.c_double),
+                ("depth_threshold", ctypes.c_double), ("init_depth", ctypes.c_double)]
+
+
+FM_WINDOW_ROWS, FM_WINDOW_ROW_DOUBLES = 11, 9
+FM_OUTLIERS_REPROJECTION, FM_OUTLIERS_MOVING = 0, 1            # gf_fm_window_outliers' `mode`
+
+
 class Obs(ctypes.Structure):
     _fields_ = [("id", ctypes.c_int32), ("track_cnt", ctypes.c_int32), ("v", ctypes.c_double * 8)]
 
@@ -123,6 +132,27 @@ def lib():
         L.gf_grid_map_read.argtypes = [vp, i, vp]
         L.gf_grid_map_size.argtypes = [vp] + [ctypes.POINTER(i)] * 4
         L.gf_grid_map_stats.argtypes = [vp, vp]
+        ip, dp = ctypes.POINTER(i), ctypes.POINTER(d)
+        L.gf_fm_window_create.argtypes = [ctypes.POINTER(vp), i, ctypes.POINTER(FmWindowCfg)]
+        L.gf_fm_window_destroy.argtypes = [vp]
+        L.gf_fm_window_destroy.restype = None
+        L.gf_fm_window_clear.argtypes = [vp]
+        L.gf_fm_window_add_frame.argtypes = [vp, i, vp, i, vp, d, ip, vp, dp]
+        L.gf_fm_window_add_frame_from_tracker.argtypes = [vp, vp, i, d, ip, vp, dp]
+        L.gf_fm_window_triangulate.argtypes = [vp, i, vp, vp, vp, vp]
+        L.gf_fm_window_fill_problem.argtypes = [vp, vp, i, ip, vp, vp, ip]
+        L.gf_fm_window_set_depth.argtypes = [vp, vp, i]
+        L.gf_fm_window_remove_failures.argtypes = [vp]
+        L.gf_fm_window_clear_depth.argtypes = [vp]
+        L.gf_fm_window_remove_ids.argtypes = [vp, vp, i]
+        L.gf_fm_window_remove_back_shift_depth.argtypes = [vp, vp, vp, vp, vp]
+        L.gf_fm_window_remove_back.argtypes = [vp]
+        L.gf_fm_window_remove_front.argtypes = [vp, i]
+        L.gf_fm_window_outliers.argtypes = [vp, vp, vp, vp, vp, i, vp, ip]
+        L.gf_fm_window_predict_next.argtypes = [vp, i, vp, vp, vp, vp, vp, vp, ip]
+        L.gf_fm_window_read.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, i, ip]
+        L.gf_fm_window_size.argtypes = [vp, ip]
+        L.gf_fm_window_last_device_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
         _LIB = L
     return _LIB
 

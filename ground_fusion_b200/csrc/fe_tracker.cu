@@ -360,6 +360,8 @@ struct gf_tracker {
     double prev_time;
     bool has_pred, depth_valid[2];
     float last_ms;
+    long long out_frame1;                // 1 + the index of the frame gf_tracker_wait* last returned (its results are in slot index % 2 until
+                                         // frame index + GF_PIPE is submitted); 0: none, or a group step
 };
 
 static inline int in_flight(const gf_tracker* t) { return (int)(t->n_submitted - t->n_waited); }
@@ -848,6 +850,7 @@ int gf_tracker_wait_boxes(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* in_bo
     const int es = (int)(t->n_waited % 2);
     GF_CUDA(cudaEventSynchronize(t->ev_out[es]));
     t->n_waited++;
+    t->out_frame1 = t->n_waited;         // n_waited was just advanced: 1 + this frame's index
     GF_CUDA(cudaEventElapsedTime(&t->last_ms, t->ev_t0[es], t->ev_out[es]));
     if (t->profiling) {
         cudaEvent_t b[8] = {t->ev_t0[es], t->ev_st[0], t->ev_st[1], t->ev_st[2], t->ev_st[3], t->ev_st[4], t->ev_st[5], t->ev_out[es]};
@@ -1321,6 +1324,22 @@ static int group_submit(gf_tracker_group* g, const double* times, const void* co
     return GF_OK;
 }
 
+int gf::tracker_last_out(const gf_tracker* t, TrackerOut* o)
+{
+    if (!t) return set_err(GF_ERR_INVALID_ARG, "null tracker");
+    if (t->out_frame1 == 0) return set_err(GF_ERR_INVALID_ARG, "the tracker has returned no frame of its own yet");
+    const long long f = t->out_frame1 - 1;
+    // frame f + GF_PIPE runs in frame f's result slot: once it is submitted the slot, its header and its event belong to that frame
+    if (t->n_submitted - f > GF_PIPE)
+        return set_err(GF_ERR_INVALID_ARG, "the frame the tracker last returned is no longer on the device: a later frame was submitted into its result slot");
+    const int es = (int)(f % GF_PIPE);
+    o->device = t->device;
+    o->n = (t->cfg.depth_cam && !t->depth_valid[es]) ? 0 : t->h_out[es]->hdr.n_out;   // as gf_tracker_wait_boxes
+    o->obs = t->d_out[es]->obs; o->in_box = t->d_out[es]->in_box;
+    o->downloaded = t->ev_out[es];
+    return GF_OK;
+}
+
 // Collects the oldest step: member i's results at out + i*out_stride, in_box / status_out likewise, n_out[i*n_stride],
 // info[i*n_stride].
 static int group_collect(gf_tracker_group* g, gf_obs* out, size_t out_stride, int* n_out, size_t n_stride, uint8_t* in_box,
@@ -1337,6 +1356,7 @@ static int group_collect(gf_tracker_group* g, gf_obs* out, size_t out_stride, in
         gf_tracker* t = g->m[i];
         t->n_waited++;
         t->group_steps--;
+        t->out_frame1 = 0;
         t->last_ms = ms;
         const uint8_t* ob = g->h_out[gs] + (size_t)i * g->out_stride;
         const OutHeader& hd = *reinterpret_cast<const OutHeader*>(ob + offsetof(OutBlock, hdr));

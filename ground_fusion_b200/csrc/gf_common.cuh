@@ -64,6 +64,11 @@ struct Pyramid {
 };
 
 
+// Where the frame a tracker last returned through gf_tracker_wait* lies on the device, for gf_fm_window_add_frame_from_tracker
+// (fe_tracker.cu): n observations, the in_box bits, and the event recorded after that frame's download.
+struct TrackerOut { int device, n; const gf_obs* obs; const uint32_t* in_box; cudaEvent_t downloaded; };
+int tracker_last_out(const gf_tracker* t, TrackerOut* o);
+
 // Programmatic dependent launch (PDL): a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may become
 // resident as soon as every CTA of its predecessor has executed gf_pdl_trigger (or exited); it must not touch anything the
 // predecessor chain writes before gf_pdl_wait, which returns once the predecessor grid has completed and its writes are visible.

@@ -119,7 +119,8 @@ class WindowEstimator:
     # estimator.cpp:2890-3636
     def optimization(self):
         W = WINDOW_SIZE
-        feats = list(self.fm.iter_ba_features())
+        on_device = hasattr(self.fm, "fillProblem")      # FeatureWindow: the visual factors come from the resident table
+        feats = [] if on_device else list(self.fm.iter_ba_features())
         pb = Problem(W + 1, len(feats))
         for i in range(W + 1):                           # vector2double (estimator.cpp:2276-2353)
             pb.para_pose[i, :3] = self.Ps[i]; pb.para_pose[i, 3:] = R_to_q(self.Rs[i])
@@ -136,7 +137,10 @@ class WindowEstimator:
             for a in range(1, len(obs)):
                 pj, vj, tj = obs[a]
                 rows.append((start, start + a, k, p0, pj, v0, vj, t0, tj))
-        pb.set_visual(rows)
+        if on_device:
+            n_feat = self.fm.fillProblem(pb)
+        else:
+            pb.set_visual(rows); n_feat = len(feats)
         pb.set_imu([self.pre[j].as_dict(j - 1, j) for j in range(1, W + 1) if self.pre[j] is not None and self.pre[j].sum_dt <= 10.0])
         pb.prior = self.prior
         R0_before, P0_before = self.Rs[0].copy(), self.Ps[0].copy()
@@ -146,7 +150,7 @@ class WindowEstimator:
         Rs, Ps, Vs = double2vector(pb, R0_before, P0_before, True)
         self.Rs, self.Ps, self.Vs = Rs, Ps, Vs
         self.Bas = pb.para_speed_bias[:, 3:6].copy(); self.Bgs = pb.para_speed_bias[:, 6:9].copy()
-        self.fm.setDepth(pb.para_feature[:len(feats)])
+        self.fm.setDepth(pb.para_feature[:n_feat])
         # the prior of the next window is linearised at the solved blocks as they stand (vector2double at estimator.cpp:3337 re-reads
         # the rotated state; the rotation is the identity up to the yaw fix of a window that has a prior)
         for i in range(W + 1):

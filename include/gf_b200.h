@@ -577,6 +577,97 @@ int gf_fm_predict_next(int device, int n, const int32_t* first_frame, const doub
                        const double* Ps, const double* Rs, const double* tic, const double* ric, double* pts_cam);
 
 /* ------------------------------------------------------------------------------------------------
+ * gf_fm_window: one FeatureManager (feature_manager.h:90-150) whose landmark table -- the reference's std::list<FeaturePerId> --
+ * stays on the GPU between frames, on the handle's own stream, with no allocation after creation.  It runs the arithmetic of
+ * the stateless gf_fm_* calls above on the resident table (the results are bit-equal), takes the tracker's observations where
+ * gf_tracker left them on the device, and emits the visual factors of gf_ba_problem.
+ *
+ * Per landmark, in LIST ORDER: feature_id, start_frame, n_obs, estimated_depth, estimate_flag, solve_flag and up to
+ * GF_FM_WINDOW_ROWS observation rows [x y z u v vx vy depth td].  The list order is the reference's: the new landmarks of a
+ * frame are appended in increasing id, every removal keeps the order of the rest.  It is not sorted by id.
+ *
+ * Every call checks its arguments before it changes anything; after an error the table is as it was.  Poses are Ps [11][3],
+ * Rs [11][9] row-major, tic [3], ric [9]; a non-finite pose or a frame_count outside 0..WINDOW_SIZE is GF_ERR_INVALID_ARG.
+ * Calls that return nothing (triangulate, set_depth, clear_depth, the removals, clear) only enqueue work; the others
+ * synchronise the handle's stream once.  All pointers are HOST pointers.  A handle is used from one thread at a time.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct gf_fm_window gf_fm_window; /* opaque: one FeatureManager, bound to one GPU and one stream */
+#define GF_FM_WINDOW_ROWS 11           /* WINDOW_SIZE + 1 observations per landmark */
+#define GF_FM_WINDOW_ROW_DOUBLES 9
+#define GF_FM_WINDOW_MAX_FRAME_OBS 2048 /* observations one add_frame takes */
+
+typedef struct gf_fm_window_cfg {
+    int max_features;        /* capacity of the table in landmarks, <= 8192; 0: 2048 */
+    int window_size;         /* WINDOW_SIZE: 10 (or 0 for it); anything else is GF_ERR_UNSUPPORTED */
+    double min_parallax;     /* MIN_PARALLAX, already divided by FOCAL_LENGTH (parameters.cpp:345-346) */
+    double depth_threshold;  /* parameters.cpp:172 */
+    double init_depth;       /* INIT_DEPTH (parameters.cpp:478) */
+} gf_fm_window_cfg;
+
+int gf_fm_window_create(gf_fm_window** out, int device, const gf_fm_window_cfg* cfg);
+void gf_fm_window_destroy(gf_fm_window* w);
+/* FeatureManager::clearState: the empty table */
+int gf_fm_window_clear(gf_fm_window* w);
+/* FeatureManager::addFeatureCheckParallax (:57-116) with the n observations of one frame (ids distinct and >= 0), without those
+ * whose in_box[i] is set (nullable: none).  An observation of a known landmark is appended to its list, whether or not the
+ * landmark was seen in the previous frame, as the reference does; the others start new landmarks.  *margin_old = the keyframe
+ * decision (1: MARGIN_OLD); counters4 = last_track_num, new_feature_num, long_track_num, landmarks in the table afterwards;
+ * *last_average_parallax in pixels at FOCAL_LENGTH (0 when the parallax test was not reached).  The parallax is summed in a
+ * fixed order: two runs give the same bits.  More new landmarks than fit: GF_ERR_CAPACITY.  A landmark holds WINDOW_SIZE + 1
+ * observation rows, one per window frame, so an observation of a landmark with start_frame + n_obs > WINDOW_SIZE (the frame at
+ * WINDOW_SIZE added a second time without a slide in between) is GF_ERR_INVALID_ARG; the reference's list would grow. */
+int gf_fm_window_add_frame(gf_fm_window* w, int frame_count, const gf_obs* obs, int n, const uint8_t* in_box, double td, int* margin_old,
+                           int32_t* counters4, double* last_average_parallax);
+/* The same with the frame `tracker` last returned through gf_tracker_wait* / gf_tracker_track*, read where the tracker left it
+ * on the device (its observations and its in_box flags), ordered after the tracker's download of that frame.  The tracker is
+ * only read.  With the pipelined calls the tracker has two result slots: the returned frame k stays on the device while frame
+ * k + 1 is in flight (submit k + 1, wait k, add_frame_from_tracker is fine), and is gone once frame k + 2 has been submitted.
+ * GF_ERR_INVALID_ARG if the tracker has returned no frame, returned its last one as a step of a gf_tracker_group, has had a
+ * later frame submitted into that frame's result slot, or is bound to another device; the table is unchanged. */
+int gf_fm_window_add_frame_from_tracker(gf_fm_window* w, const gf_tracker* tracker, int frame_count, double td, int* margin_old, int32_t* counters4,
+                                        double* last_average_parallax);
+/* triangulateWithDepth followed by triangulate (gf_fm_triangulate) over the table */
+int gf_fm_window_triangulate(gf_fm_window* w, int frame_count, const double* Ps, const double* Rs, const double* tic, const double* ric);
+/* The visual part of a gf_ba_problem (estimator.cpp:3268-3297, getDepthVector): the landmarks with n_obs >= 4 in list order are
+ * features 0 .. *n_features - 1 with para_feature[k] = 1 / estimated_depth and feature_const[k] = (estimate_flag == 1); each
+ * contributes one factor per observation after its first, (start_frame, start_frame + a, k), in that order.  visual_out
+ * (nullable: only the feature arrays) holds cap rows, fewer than needed is GF_ERR_CAPACITY; para_feature and feature_const
+ * (nullable) hold max_features entries. */
+int gf_fm_window_fill_problem(gf_fm_window* w, gf_ba_visual_factor* visual_out, int cap, int* n_visual, double* para_feature, uint8_t* feature_const,
+                              int* n_features);
+/* FeatureManager::setDepth (:249-267) with the solved para_feature: n must be the n_features the last fill_problem returned,
+ * with no frame added and no landmark removed since (GF_ERR_INVALID_ARG otherwise). */
+int gf_fm_window_set_depth(gf_fm_window* w, const double* para_feature, int n);
+/* removeFailures (solve_flag == 2), clearDepth (every estimated_depth = -1), removeOutlier (ids not in the table are ignored) */
+int gf_fm_window_remove_failures(gf_fm_window* w);
+int gf_fm_window_clear_depth(gf_fm_window* w);
+int gf_fm_window_remove_ids(gf_fm_window* w, const int32_t* ids, int n);
+/* removeBackShiftDepth (:818-856; marg / new: the camera poses R [9], P [3] of the marginalised and the new first frame; a
+ * landmark left with fewer than two observations goes), removeBack and removeFront (frame_count must be WINDOW_SIZE; a landmark
+ * left without observations goes) */
+int gf_fm_window_remove_back_shift_depth(gf_fm_window* w, const double* marg_R, const double* marg_P, const double* new_R, const double* new_P);
+int gf_fm_window_remove_back(gf_fm_window* w);
+int gf_fm_window_remove_front(gf_fm_window* w, int frame_count);
+/* Estimator::outliersRejection (mode GF_FM_OUTLIERS_REPROJECTION: n_obs >= 4, mean reprojection error over 3 px at FOCAL_LENGTH)
+ * and movingConsistencyCheckW (GF_FM_OUTLIERS_MOVING: n_obs >= 2, start_frame < WINDOW_SIZE - 2, depth >= 0, mean error over
+ * 10 px or mean 3-D error over 2): the ids in list order; ids_out holds max_features entries. */
+#define GF_FM_OUTLIERS_REPROJECTION 0
+#define GF_FM_OUTLIERS_MOVING 1
+int gf_fm_window_outliers(gf_fm_window* w, const double* Ps, const double* Rs, const double* tic, const double* ric, int mode, int32_t* ids_out, int* n);
+/* Estimator::predictPtsInNextFrame: ids_out / xyz_out [n][3] (max_features entries each, list order) are the arguments of
+ * gf_tracker_set_prediction; *n = 0 when frame_count < 2. */
+int gf_fm_window_predict_next(gf_fm_window* w, int frame_count, const double* Ps, const double* Rs, const double* tic, const double* ric, int32_t* ids_out,
+                              double* xyz_out, int* n);
+/* The table in list order: every array (nullable) holds cap entries, obs cap * GF_FM_WINDOW_ROWS * GF_FM_WINDOW_ROW_DOUBLES
+ * doubles (landmark i's row a at (i * GF_FM_WINDOW_ROWS + a) * GF_FM_WINDOW_ROW_DOUBLES, rows from n_obs[i] on unspecified).
+ * *n = the number of landmarks; more than cap is GF_ERR_CAPACITY with *n set. */
+int gf_fm_window_read(gf_fm_window* w, int32_t* feature_id, int32_t* start_frame, int32_t* n_obs, double* estimated_depth, int32_t* estimate_flag,
+                      int32_t* solve_flag, double* obs, int cap, int* n);
+int gf_fm_window_size(gf_fm_window* w, int* n);
+/* Device time of the last call's work on the handle's stream, from CUDA events (waits for that work) */
+int gf_fm_window_last_device_ms(gf_fm_window* w, float* ms);
+
+/* ------------------------------------------------------------------------------------------------
  * Dense colour map (dense_map/src/pose_graph.cpp, pose_graph_node.cpp): the keyframe point sampling of the mapping node,
  * PoseGraph's voxel-density insertion (OctreePointCloudDensity, 0.01 m voxels), its RadiusOutlierRemoval (0.8 m, 10
  * neighbours) and updatePath's rebuild after a pose-graph correction.  Loop detection and the pose-graph optimisation stay
