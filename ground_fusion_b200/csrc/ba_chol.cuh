@@ -10,6 +10,7 @@
 // Tile storage ("fragment order"): tile element [r][c] at  (c/4)*32 + r*4 + c%4 , so that the k-half h of a tile is the
 // contiguous run [h*32, h*32+32): lane l of an m8n8k4 operand fragment reads element h*32 + l.
 #pragma once
+#include <cfloat>
 #include "gf_common.cuh"
 
 #ifndef GF_CHOL_STAMP
@@ -36,7 +37,7 @@ __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double
 __host__ __device__ __forceinline__ int tix(int I, int J) { return I * (I + 1) / 2 + J; }
 
 // Factor tiles live in shared memory up to `cap` tiles, beyond that in a global (L2-resident) spill buffer.  SPILL = false is
-// the common case (everything fits: <= 27 block rows, nc <= 215): the accessors are plain LDS / STS with no second path.
+// the common case (everything fits: <= 26 block rows = 351 tiles, nc <= 207): the accessors are plain LDS / STS with no second path.
 // The tile slots start at offset 0 of the dynamic shared memory of the calling kernel.  Their 32-bit shared address is taken
 // ONCE (ch_tiles_u32, made opaque to the compiler) and every access in the hot loops is an explicit ld.shared / st.shared with
 // an immediate offset: left to itself nvcc rematerialises the address of the extern array (S2R SR_CgaCtaId + shifts, a
@@ -86,8 +87,9 @@ struct TileStoreT {
 // sqrt and 1/sqrt of a positive, normal double without the special-case branch of the CUDA math library (a branch would
 // cut the factorisation below into basic blocks the scheduler cannot overlap).  The argument is brought into [1, 4) by its
 // even exponent, the seed is the single-precision MUFU.RSQ (2^-22), two coupled Newton / Goldschmidt steps (g -> sqrt(x),
-// h -> 1 / (2 sqrt(x))) square the error twice and a last correction fixes the square root itself.  Zero, negative and
-// non-finite x are the caller's failure case (the result is then garbage and never used).
+// h -> 1 / (2 sqrt(x))) square the error twice and a last correction fixes the square root itself.  Zero, negative,
+// subnormal and non-finite x are the caller's failure case (the result is then garbage and never used: the exponent trick
+// gives 1e-310 a root of 1.06e-154 and +inf a finite one, so chol8_inv accepts a pivot only in [DBL_MIN, DBL_MAX]).
 __device__ __forceinline__ void sqrt_rsqrt(double x, double& sq, double& rs)
 {
     const int hi = __double2hiint(x), lo = __double2loint(x);
@@ -124,7 +126,7 @@ __device__ __forceinline__ bool chol8_inv(const double* __restrict__ S8, int nco
     for (int k = 0; k < 8; k++) {
         const bool live = k < ncol;
         const double dk = live ? a[k][k] : 1.0;
-        ok = ok && (dk > 0.0);
+        ok = ok & (dk >= DBL_MIN) & (dk <= DBL_MAX);      // positive and normal (NaN fails both); a select, not a branch
         double sq, r;
         sqrt_rsqrt(dk, sq, r);
         inv[k] = r;
@@ -237,7 +239,7 @@ __device__ __forceinline__ void c_to_frags(double c0, double c1, int lane, doubl
 // issue latency of a few warps on ONE SM, so every instruction next to an MMA counts.
 // A: tiles [0, cap) already sit in their slots, row-major (chol_issue_load); others are read from Ag.  L: fragment order, same
 // slots.  Linv: n8 tiles (fragment order), kept for the back substitution.  S8: 2 scratch tiles.  Ld: the factor of the last
-// diagonal tile, row-major (it holds the tail of z).  Returns false if a pivot was not positive.
+// diagonal tile, row-major (it holds the tail of z).  Returns false if a pivot was not a positive normal number.
 constexpr int CH_BULK = ST_WARPS - 1;
 template <int R, bool SPILL>
 __device__ __forceinline__ bool chol_factor(const double* __restrict__ Ag, const TileStoreT<SPILL>& T, double* Linv, double* S8, double* Ld,

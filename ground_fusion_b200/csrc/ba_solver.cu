@@ -17,6 +17,7 @@
 //                   last CTA of k_ba_eval(1) to finish.
 // All four are enqueued for every iteration up front; kernels return immediately once the state says "done",
 // so the host synchronises exactly once per solve.
+#include <cmath>
 #include <stdlib.h>
 #include <new>
 #include <type_traits>
@@ -2466,6 +2467,12 @@ __global__ void __launch_bounds__(ST_THREADS) k_stage_chol(const double* Ag, dou
 extern "C" int gf_stage_spd_solve(int device, const double* A, const double* b, int n, double* x, int tile_cap)
 {
     if (!A || !b || !x || n < 1 || n > MAX_NC) return set_err(GF_ERR_INVALID_ARG, "bad argument (1 <= n <= 383)");
+    // a non-finite entry would reach x through the factor's MMAs (0 * inf = NaN) without failing a pivot test
+    for (int i = 0; i < n; i++) {
+        if (!std::isfinite(b[i])) return set_err(GF_ERR_INVALID_ARG, "b is not finite");
+        for (int j = 0; j <= i; j++)
+            if (!std::isfinite(A[(size_t)i * n + j])) return set_err(GF_ERR_INVALID_ARG, "A is not finite (lower triangle)");
+    }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return set_err(GF_ERR_NO_DEVICE, "no CUDA device visible; libgf_b200 has no CPU fallback");
     if (device < 0 || device >= ndev) return set_err(GF_ERR_INVALID_ARG, "device index out of range");
@@ -2503,7 +2510,7 @@ extern "C" int gf_stage_spd_solve(int device, const double* A, const double* b, 
     if (e == cudaSuccess && !fail) e = cudaMemcpy(x, dy, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost);
     cudaFree(dA); cudaFree(dL); cudaFree(dy); cudaFree(df);
     if (e != cudaSuccess) { snprintf(g_err, sizeof(g_err), "gf_stage_spd_solve: %s", cudaGetErrorString(e)); return GF_ERR_CUDA; }
-    if (fail) return set_err(GF_ERR_INVALID_ARG, "matrix is not positive definite");
+    if (fail) return set_err(GF_ERR_INVALID_ARG, "matrix is not positive definite (a pivot is not a positive normal number)");
     return GF_OK;
 }
 

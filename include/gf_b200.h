@@ -264,7 +264,8 @@ int gf_stage_setmask_order(int device, const int32_t* track_cnt, int n, int32_t*
  * tensor-core MMAs + back substitution; replaces Ceres' dense Cholesky of the reduced camera system, call site
  * estimator.cpp:3303-3318): x = A^-1 b for a symmetric positive definite A (n x n row-major, lower triangle read),
  * 1 <= n <= 383.  tile_cap < 0: default number of factor tiles kept in shared memory; smaller values force the L2 spill
- * path (tests). */
+ * path (tests).  A non-finite entry of b or of A's lower triangle is GF_ERR_INVALID_ARG, and so is a pivot of the
+ * factorisation that is not a positive normal number ("not positive definite"; x is then left unchanged). */
 int gf_stage_spd_solve(int device, const double* A, const double* b, int n, double* x, int tile_cap);
 
 /* The marginalisation's symmetric eigensolvers on their own (A n x n row-major, lower triangle read; w[n], V n x n row-major
