@@ -22,6 +22,15 @@
 // barrier every warp sums the per-warp partials itself (lk_bsum_int).  When all ten chains are within the bound (99.5 %
 // of the iterations of the C2 synthetic stream) that sum replaces the sequential chains.  Otherwise the threads store
 // their terms in chain order and warp 0 runs lk_chain on them.
+//
+// The CTA has two warp roles (lk_track_point).  Consumer warps 0..3 run the iterations of level l; producer warps 4..7
+// meanwhile build level l-1 -- Scharr, the template, the gradient-matrix terms and chains, minEig and D -- into the other
+// of two level buffers.  A level's setup depends only on the point p and the staged template window, so only the
+// coarsest level of a pass waits for its setup.  Each role synchronises on its own named barrier; the roles meet once
+// per level at a 256-thread named barrier, whatever path the level took.  The producers also fetch each level's first
+// search window, placed from the pass's initial guess, so a level restages only when its iterate leaves that window.
+// fe_lk_single.cuh keeps the single-role form (all 8 warps set up a level, then iterate it), which fe_tracker.cu launches
+// while several trackers share the GPU.
 #pragma once
 #include <cuda.h>          // CUtensorMap (types only: the encoder is fetched with cudaGetDriverEntryPoint, fe_tracker.cu)
 #include "gf_common.cuh"
@@ -43,28 +52,45 @@ constexpr int LK_BCHAIN = 42;                       // pair terms per chain of t
 constexpr int LK_AT = 4 * LK_CHAIN + LK_TAIL;       // 441 terms per A quantity
 constexpr int LK_BT = 4 * LK_BCHAIN + LK_TAIL;      // 273 terms per b component (168 pair units + 105 tail pixels)
 constexpr int LK_Q = 5 * LK_TAIL;                   // slots per quantity: [step 0..104][chain 0..4], short chains padded with +0.0f
-// Units of the b terms per thread (lk_unit): thread u < 4 * LK_BCHAIN holds pair unit u, of chain u & 3; the others hold
-// tail units (chain 4).  So warps 0..LK_PAIR_WARPS-1 carry pair units and warps LK_TAIL_WARP0.. carry tail units.
-constexpr int LK_PAIR_WARPS = (4 * LK_BCHAIN + 31) / 32;            // 6
-constexpr int LK_TAIL_WARP0 = 4 * LK_BCHAIN / 32;                   // 5
-constexpr int LK_TAIL_WARPS = LK_THREADS / 32 - LK_TAIL_WARP0;       // 3
-constexpr int LK_BSLOTS = 5 * LK_PAIR_WARPS;         // per-warp partials; the tail chain's slots beyond LK_TAIL_WARPS stay 0
-static_assert(LK_PAIR_WARPS >= LK_TAIL_WARPS, "lk_bsum_int sums LK_PAIR_WARPS partials per chain");
+// Warp roles: consumer warps 0..LK_CWARPS-1 iterate, the others (producers) build the next level.
+constexpr int LK_CWARPS = 4;
+constexpr int LK_CTHREADS = 32 * LK_CWARPS;                 // 128
+constexpr int LK_PTHREADS = LK_THREADS - LK_CTHREADS;       // 128
+// Units of the b terms per consumer thread t (lk_iterate): pair unit t, and pair unit t + 128 (t < 40) or tail unit t - 40
+// (t >= 40), plus tail unit t + 48 for 40 <= t < 57 -- at most four pixels per thread.  Pair units u and u + 128 belong to
+// the same chain (u & 3), so every thread holds one pair chain and the tail chain.
+constexpr int LK_PAIR2 = 4 * LK_BCHAIN - LK_CTHREADS;       // 40 threads hold a second pair unit
+constexpr int LK_TAIL2 = LK_TAIL - (LK_CTHREADS - LK_PAIR2); // 17 threads hold a second tail unit
+static_assert(LK_CTHREADS == 128 && LK_PAIR2 > 0 && LK_TAIL2 > 0 && LK_PAIR2 + LK_TAIL2 <= LK_CTHREADS, "unit map of lk_iterate");
+constexpr int LK_BSLOTS = 5 * LK_CWARPS;    // per-warp partials: slot w*4 + k pair chain k of warp w, slot 4*LK_CWARPS + w its tail
+// named barriers (0 is __syncthreads)
+constexpr int LK_BAR_HANDOFF = 1, LK_BAR_CONS = 2, LK_BAR_PROD = 3;
+
+// One built level: the gradient matrix, scaled, and whether the level is tracked at all (inside the image, minEig and
+// the determinant above OpenCV's thresholds).
+struct LKLevelA { float A11, A12, A22, D; int ok, pad_[3]; };
 
 struct __align__(128) LKSmem {
     uint8_t ireg[LK_MAXLEV][LK_IREG * LK_IPITCH];   // per level: raw bytes, row r at r*32, first needed column at byte xoff
-    uint8_t jreg[LK_JR * LK_JPITCH];                // 128-byte aligned like ireg[l]: both are TMA box destinations
-    int16_t sch[LK_SCH * LK_SCH * 2];
-    short4 tpl[LK_NPIX + 1];               // template patch per pixel: (I*32, Ix, Iy, 0), one 8-byte load per pixel
-    float terms[3 * LK_Q];                 // [quantity][step][chain]; slots beyond a chain's length hold +0.0f (x + 0 is exact)
-    float sums[4];                         // chain results broadcast from warp 0
+    uint8_t jreg[2][LK_JR * LK_JPITCH];             // search window of level l in [l & 1]; 128-byte aligned like ireg[l]: TMA box destinations
+    int16_t sch[LK_SCH * LK_SCH * 2];               // producers only
+    short4 tpl[2][LK_NPIX + 1];            // per level buffer: template patch per pixel (I*32, Ix, Iy, 0), one 8-byte load
+    float aterms[3 * LK_Q];                // A terms [quantity][step][chain] (producers); slots beyond a chain's length hold +0.0f
+    float bterms[2 * LK_Q];                // b terms of the sequential fallback (consumers), same layout
+    LKLevelA lv[2];                        // per level buffer: the built gradient matrix
+    float bsums[2];                        // fallback b chain results broadcast from warp 0
+    float2 res;                            // result of the pass, broadcast from consumer thread 0
+    int res_status;
     // [iteration parity][slot][x+, x-, y+, y-]: per-warp sums of the positive b terms and of the magnitudes of the negative
-    // ones of one chain; slot w*4 + k: pair chain k of warp w, slot 4*LK_PAIR_WARPS + w - LK_TAIL_WARP0: tail chain of warp w
-    // (the tail chain's remaining slots are zeroed once per point, so every chain sums LK_PAIR_WARPS slots)
+    // ones of one chain (slots as LK_BSLOTS)
     alignas(16) unsigned bpart[2][LK_BSLOTS][4];
-    unsigned long long mbar;               // completion barrier of the window loads
+    unsigned long long mbar_i;             // completion barrier of the template window loads (all threads wait)
+    unsigned long long mbar_p[2];          // completion barriers of the producers' first search window of level l, [l & 1]
+                                           // (consumers wait; level l+2 reuses a barrier only after level l's wait)
+    unsigned long long mbar_j;             // completion barrier of the search windows restaged within a level (consumers wait)
 };
-static_assert((LK_IREG * LK_IPITCH) % 128 == 0 && (LK_MAXLEV * LK_IREG * LK_IPITCH) % 128 == 0, "TMA destinations must be 128-byte aligned");
+static_assert((LK_IREG * LK_IPITCH) % 128 == 0 && (LK_MAXLEV * LK_IREG * LK_IPITCH) % 128 == 0 && (LK_JR * LK_JPITCH) % 128 == 0,
+              "TMA destinations must be 128-byte aligned");
 
 // ---- 2-D TMA staging of the LK windows --------------------------------------------------------------------------------
 // A window that lies inside its pyramid level is one cp.async.bulk.tensor.2d box: LK_IPITCH x LK_IREG bytes for a template
@@ -78,27 +104,33 @@ struct LKMapSet {
     CUtensorMap curI[LK_MAXLEV], prevJ[LK_MAXLEV];   // reverse pass
     int enabled, pad_[15];
 };
-struct LKTma { const CUtensorMap* mi; const CUtensorMap* mj; unsigned phase; bool on; };
+// phase_i: the template windows' barrier (every thread waits on it); phase_p (bit b: S.mbar_p[b]), phase_j: the search
+// windows' barriers (only consumers wait, so only their copies advance)
+struct LKTma { const CUtensorMap* mi; const CUtensorMap* mj; unsigned phase_i, phase_p, phase_j; bool on; };
 
 __device__ __forceinline__ void lk_tma_box(void* dst, const CUtensorMap* map, int x, int y, unsigned long long* bar)
 {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                  ::"r"(smem_u32(dst)), "l"(map), "r"(x), "r"(y), "r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void lk_tma_wait(LKSmem& S, LKTma& T)
+__device__ __forceinline__ void lk_tma_wait(unsigned long long* bar, unsigned& phase)
 {
-    while (!mbar_try_wait(&S.mbar, T.phase)) { }
-    T.phase ^= 1u;
+    while (!mbar_try_wait(bar, phase)) { }
+    phase ^= 1u;
 }
 // once per kernel, before the first lk_track_point
 __device__ __forceinline__ void lk_tma_init(LKSmem& S, int tid)
 {
     if (tid == 0) {
-        mbar_init(&S.mbar, 1);
+        mbar_init(&S.mbar_i, 1);
+        mbar_init(&S.mbar_p[0], 1);
+        mbar_init(&S.mbar_p[1], 1);
+        mbar_init(&S.mbar_j, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
 }
+__device__ __forceinline__ void lk_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 template <int RW, int RH>
 __device__ __forceinline__ bool lk_inside(const Level& L, int x0, int y0)
 {
@@ -204,34 +236,29 @@ __device__ __forceinline__ void lk_split(int v, unsigned& pos, unsigned& neg)
     neg += v < 0 ? (unsigned)-v : 0u;
 }
 
-// Per-warp integer partials of the b chains from this thread's share v = (x+, x-, y+, y-) of its chain's terms.
-// No sum can wrap: a term is below 2^26 in magnitude (|d| <= 8160, |g| <= 4080, two products per pair), and a whole
-// chain (42 pair terms or 105 tail products) stays below 2^32.
-__device__ __forceinline__ void lk_bpart_write(unsigned (*P)[4], int tid, const unsigned (&v)[4])
+// Per-warp integer partials of the b chains from a consumer thread's shares (x+, x-, y+, y-) of its pair chain (v, chain
+// lane & 3) and of the tail chain (tv).  No sum can wrap: a term is below 2^26 in magnitude (|d| <= 8160, |g| <= 4080,
+// two products per pair), and a whole chain (42 pair terms or 105 tail products) stays below 2^32.
+__device__ __forceinline__ void lk_bpart_write(unsigned (*P)[4], int tid, const unsigned (&v)[4], const unsigned (&tv)[4])
 {
     const int w = tid >> 5, lane = tid & 31;
-    const bool pair = tid < 4 * LK_BCHAIN;
-    if (w < LK_PAIR_WARPS) {
-        // Reduce-scatter over the 8 lanes of each pair chain (equal lane & 3), four shuffles, three deep: across lane bit 4
-        // a lane keeps values {0,1} or {2,3}, across bit 3 one of them, across bit 2 it completes value (lane >> 3) & 3.
-        const bool h4 = lane & 16, h3 = lane & 8;
-        unsigned a0 = pair ? (h4 ? v[2] : v[0]) : 0u, a1 = pair ? (h4 ? v[3] : v[1]) : 0u;
-        const unsigned s0 = pair ? (h4 ? v[0] : v[2]) : 0u, s1 = pair ? (h4 ? v[1] : v[3]) : 0u;
-        a0 += __shfl_xor_sync(0xffffffffu, s0, 16);
-        a1 += __shfl_xor_sync(0xffffffffu, s1, 16);
-        unsigned c = (h3 ? a1 : a0) + __shfl_xor_sync(0xffffffffu, h3 ? a0 : a1, 8);
-        c += __shfl_xor_sync(0xffffffffu, c, 4);
-        if (!(lane & 4)) P[w * 4 + (lane & 3)][(lane >> 3) & 3] = c;
-    }
-    if (w >= LK_TAIL_WARP0) {           // every tail unit belongs to chain 4
-        unsigned s[4];
+    // Reduce-scatter over the 8 lanes of each pair chain (equal lane & 3), four shuffles, three deep: across lane bit 4
+    // a lane keeps values {0,1} or {2,3}, across bit 3 one of them, across bit 2 it completes value (lane >> 3) & 3.
+    const bool h4 = lane & 16, h3 = lane & 8;
+    unsigned a0 = h4 ? v[2] : v[0], a1 = h4 ? v[3] : v[1];
+    const unsigned s0 = h4 ? v[0] : v[2], s1 = h4 ? v[1] : v[3];
+    a0 += __shfl_xor_sync(0xffffffffu, s0, 16);
+    a1 += __shfl_xor_sync(0xffffffffu, s1, 16);
+    unsigned c = (h3 ? a1 : a0) + __shfl_xor_sync(0xffffffffu, h3 ? a0 : a1, 8);
+    c += __shfl_xor_sync(0xffffffffu, c, 4);
+    if (!(lane & 4)) P[w * 4 + (lane & 3)][(lane >> 3) & 3] = c;
+    unsigned s[4];
 #pragma unroll
-        for (int k = 0; k < 4; k++) s[k] = __reduce_add_sync(0xffffffffu, pair ? 0u : v[k]);
-        if (lane == 0) *reinterpret_cast<uint4*>(P[4 * LK_PAIR_WARPS + w - LK_TAIL_WARP0]) = make_uint4(s[0], s[1], s[2], s[3]);
-    }
+    for (int k = 0; k < 4; k++) s[k] = __reduce_add_sync(0xffffffffu, tv[k]);
+    if (lane == 0) *reinterpret_cast<uint4*>(P[4 * LK_CWARPS + w]) = make_uint4(s[0], s[1], s[2], s[3]);
 }
 
-// b1 and b2 from the per-warp integer partials, computed by every warp, when all ten chains are within the exactness
+// b1 and b2 from the per-warp integer partials, computed by every consumer warp, when all ten chains are within the exactness
 // bound; returns whether they are (the same answer in every warp).  Lane comp*8 + c (c < 5) sums chain c of component comp.
 // OpenCV's combination t + ((c0 + c2) + (c1 + c3)) then pairs c0/c2 and c1/c3 across lane bit 1 and the two pair sums
 // across lane bit 0; float addition is commutative, so the bits do not depend on which lane of a pair adds.
@@ -243,8 +270,8 @@ __device__ __forceinline__ bool lk_bsum_int(const unsigned (*P)[4], int lane, fl
     if (comp < 2 && c < 5) {
         unsigned pos = 0, neg = 0;
 #pragma unroll
-        for (int w = 0; w < LK_PAIR_WARPS; w++) {
-            const uint2 v = reinterpret_cast<const uint2*>(P[c < 4 ? w * 4 + c : 4 * LK_PAIR_WARPS + w])[comp];
+        for (int w = 0; w < LK_CWARPS; w++) {
+            const uint2 v = reinterpret_cast<const uint2*>(P[c < 4 ? w * 4 + c : 4 * LK_CWARPS + w])[comp];
             pos += v.x;
             neg += v.y;
         }
@@ -278,51 +305,61 @@ __device__ __forceinline__ void lk_origin(float2 p, int l, float& ppx, float& pp
     ipy = __float2int_rd(ppy);
 }
 
-// A thread's fixed share of the mismatch terms: one unit of the chain layout (a pmaddwd pair or a tail pixel) plus,
-// for 17 threads, a second tail pixel -- at most two pixels per thread, the same for every level and iteration.
-struct LKUnit { int i0, i1, slot, off0, off1; };
-__device__ __forceinline__ LKUnit lk_unit(int u)
+// Search window a level starts with when the pass's initial guess g needs no correction from the coarser levels: origin
+// floor(g / 2^l - 10) - 9, as lk_iterate places it; false when that guess is out of range (the level's first iteration
+// then ends the level).  The producers stage these windows (lk_build).  A window only caches the image, so a
+// level whose iterate leaves it restages, and a better or worse guess changes no result.
+__device__ __forceinline__ bool lk_jwin0(float2 g, int l, const Level& J, int& jx0, int& jy0)
 {
-    LKUnit U;
-    if (u < 4 * LK_BCHAIN) {
-        int y = u >> 3, r = u & 7, k = r & 3, hh = r >> 2;
-        U.i0 = y * LK_WIN + 8 * hh + k;
-        U.i1 = U.i0 + 4;
-        U.slot = (y * 2 + hh) * 5 + k;
-    } else {
-        int t = u - 4 * LK_BCHAIN, y = t / 5, x = 16 + (t - y * 5);
-        U.i0 = U.i1 = y * LK_WIN + x;
-        U.slot = t * 5 + 4;
-    }
-    U.off0 = (U.i0 / LK_WIN) * LK_JPITCH + (U.i0 % LK_WIN);
-    U.off1 = (U.i1 / LK_WIN) * LK_JPITCH + (U.i1 % LK_WIN);
-    return U;
+    const float sc = (float)(1. / (double)(1 << l));
+    const int iqx = __float2int_rd(g.x * sc - 10.f), iqy = __float2int_rd(g.y * sc - 10.f);
+    jx0 = iqx - 9;
+    jy0 = iqy - 9;
+    return !(iqx < -LK_WIN || iqx >= J.w || iqy < -LK_WIN || iqy >= J.h);
 }
 
-// One pyramid level for one point.  All LK_THREADS threads of the CTA call this with identical scalar arguments
-// and keep identical copies of the scalar state; warp 0 owns the sequential chains.  The level's 24x24 window of I
-// is already staged in S.ireg[level] (lk_track_point).
-__device__ __forceinline__ void lk_level(LKSmem& S, int tid, const Level& I, const Level& J, float2 p,
-                                         float& nx, float& ny, int level, int& status, int& iters, int& fallbacks,
-                                         long long* pc, LKTma& T)
+// Producer role: builds one pyramid level of point p into level buffer buf -- the template patch S.tpl[buf] and the
+// gradient matrix S.lv[buf] -- from the staged window S.ireg[level], and fetches the level's first search window
+// (from the pass's initial guess g) into S.jreg[level & 1].  Run by the LK_PTHREADS producer threads (pt is the
+// index among them) with identical arguments; warp 0 of the role runs the A chains.  The role's barriers are all
+// skipped together when the level lies outside the image.
+__device__ __forceinline__ void lk_build(LKSmem& S, int pt, const Level& I, const Level& J, float2 p, float2 g, int level,
+                                         int buf, const LKTma& T)
 {
-    [[maybe_unused]] long long tl = gf_clock();
-    const float FLT_SCALE = 1.f / (1 << 20);
+    const bool tma_on = T.on;
+    // ---- the level's first search window (lk_jwin0) into S.jreg[level & 1], whose last readers (the consumers of level
+    //      level+2) passed the hand-over before this build.  A box completes on S.mbar_p[level & 1], which the consumers
+    //      wait on; gathered bytes are published by the next hand-over ----
+    {
+        int jx0, jy0;
+        if (lk_jwin0(g, level, J, jx0, jy0)) {
+            if (tma_on && lk_inside<LK_JR, LK_JR>(J, jx0, jy0)) {
+                if (pt == 0) {
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                    mbar_expect_tx(&S.mbar_p[level & 1], LK_JR * LK_JPITCH);
+                    lk_tma_box(S.jreg[level & 1], T.mj + level, jx0 & ~15, jy0, &S.mbar_p[level & 1]);
+                }
+            } else {
+                lk_stage_part<LK_JR, LK_JR, LK_JPITCH>(S.jreg[level & 1], J, jx0, jy0, pt, LK_PTHREADS);
+            }
+        }
+    }
     float ppx, ppy;
     int ipx, ipy;
     lk_origin(p, level, ppx, ppy, ipx, ipy);
+    LKLevelA& R = S.lv[buf];
     if (ipx < -LK_WIN || ipx >= I.w || ipy < -LK_WIN || ipy >= I.h) {
-        if (level == 0) status = 0;
+        if (pt == 0) R.ok = 0;
         return;
     }
-    float a = ppx - (float)ipx, b = ppy - (float)ipy;
+    const float a = ppx - (float)ipx, b = ppy - (float)ipy;
     int iw00, iw01, iw10, iw11;
     lk_weights(a, b, iw00, iw01, iw10, iw11);
     const uint8_t* ireg = S.ireg[level];
-    const int ioff = lk_stage_offset<LK_IREG, LK_IREG>(I, ipx - 1, ipy - 1, T.on);
-    __syncthreads();     // previous level's readers of sch / tpl / terms are done
-    // ---- Scharr derivative at the 22x22 integer positions (0 outside the image) ----
-    for (int i = tid; i < LK_SCH * LK_SCH; i += LK_THREADS) {
+    const int ioff = lk_stage_offset<LK_IREG, LK_IREG>(I, ipx - 1, ipy - 1, tma_on);
+    // ---- Scharr derivative at the 22x22 integer positions (0 outside the image).  The previous build's readers of
+    //      S.sch passed its second role barrier before this build began ----
+    for (int i = pt; i < LK_SCH * LK_SCH; i += LK_PTHREADS) {
         int r = i / LK_SCH, c = i - r * LK_SCH;
         int X = ipx + c, Y = ipy + r;
         int ix = 0, iy = 0;
@@ -337,10 +374,11 @@ __device__ __forceinline__ void lk_level(LKSmem& S, int tid, const Level& I, con
         }
         reinterpret_cast<int*>(S.sch)[i] = (ix & 0xffff) | (iy << 16);
     }
-    __syncthreads();
-    LKP(1);
-    // ---- bilinear 21x21 patches I*32, (Ix, Iy), and the gradient-matrix terms in chain order ----
-    for (int i = tid; i < LK_NPIX; i += LK_THREADS) {
+    lk_bar(LK_BAR_PROD, LK_PTHREADS);
+    // ---- bilinear 21x21 patches I*32, (Ix, Iy), and the gradient-matrix terms in chain order.  The previous build's
+    //      A chains finished before warp 0 of the role reached the barrier above ----
+    short4* tpl = S.tpl[buf];
+    for (int i = pt; i < LK_NPIX; i += LK_PTHREADS) {
         int y = i / LK_WIN, x = i - y * LK_WIN;
         const uint8_t* q = ireg + (y + 1) * LK_IPITCH + ioff + (x + 1);
         int iv = q[0] * iw00 + q[1] * iw01 + q[LK_IPITCH] * iw10 + q[LK_IPITCH + 1] * iw11;
@@ -349,73 +387,76 @@ __device__ __forceinline__ void lk_level(LKSmem& S, int tid, const Level& I, con
         int dxv = s[0] * iw00 + s[2] * iw01 + s[2 * LK_SCH] * iw10 + s[2 * LK_SCH + 2] * iw11;
         int dyv = s[1] * iw00 + s[3] * iw01 + s[2 * LK_SCH + 1] * iw10 + s[2 * LK_SCH + 3] * iw11;
         int gx = (int16_t)lk_descale(dxv, 14), gy = (int16_t)lk_descale(dyv, 14);
-        S.tpl[i] = make_short4((short)pv, (short)gx, (short)gy, 0);
+        tpl[i] = make_short4((short)pv, (short)gx, (short)gy, 0);
         // products are exact integers below 2^24, so (float)(int product) == fx*fy of OpenCV's float path
         int slot = (x < 16) ? (y * 4 + (x >> 2)) * 5 + (x & 3) : (y * 5 + (x - 16)) * 5 + 4;     // [step][chain]
-        S.terms[slot] = (float)(gx * gx);
-        S.terms[LK_Q + slot] = (float)(gx * gy);
-        S.terms[2 * LK_Q + slot] = (float)(gy * gy);
+        S.aterms[slot] = (float)(gx * gx);
+        S.aterms[LK_Q + slot] = (float)(gx * gy);
+        S.aterms[2 * LK_Q + slot] = (float)(gy * gy);
     }
-    __syncthreads();
-    LKP(2);
-    // ---- gradient matrix, OpenCV lane order: warp 0 runs the 15 chains while the other warps already stage the
-    //      search window of the first iteration (its position does not depend on A) ----
-    float qx = nx - 10.f, qy = ny - 10.f;
-    int jx0 = 0, jy0 = 0, joff = 0;
-    bool jvalid = false;
-    {
-        int iqx = __float2int_rd(qx), iqy = __float2int_rd(qy);
-        const bool inwin = !(iqx < -LK_WIN || iqx >= J.w || iqy < -LK_WIN || iqy >= J.h);
-        if (inwin) { jx0 = iqx - 9; jy0 = iqy - 9; jvalid = true; }
-        if (tid < 32) {
-            const float acc = lk_chain(S.terms, tid, 3);
+    lk_bar(LK_BAR_PROD, LK_PTHREADS);
+    // ---- gradient matrix, OpenCV lane order, minEig and the determinant ----
+    if (pt < 32) {
+        const float acc = lk_chain(S.aterms, pt, 3);
+        float sum[3];
 #pragma unroll
-            for (int q = 0; q < 3; q++) {
-                float l0 = __shfl_sync(0xffffffffu, acc, q * 5 + 0), l1 = __shfl_sync(0xffffffffu, acc, q * 5 + 1);
-                float l2 = __shfl_sync(0xffffffffu, acc, q * 5 + 2), l3 = __shfl_sync(0xffffffffu, acc, q * 5 + 3);
-                float t = __shfl_sync(0xffffffffu, acc, q * 5 + 4);
-                if (tid == 0) S.sums[q] = t + ((l0 + l2) + (l1 + l3));
-            }
-        } else if (inwin) {
-            if (T.on && lk_inside<LK_JR, LK_JR>(J, jx0, jy0)) {
-                if (tid == 32) {     // previous readers / writers of jreg finished before the barrier at the top of this level
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    mbar_expect_tx(&S.mbar, LK_JR * LK_JPITCH);
-                    lk_tma_box(S.jreg, T.mj + level, jx0 & ~15, jy0, &S.mbar);
-                }
-            } else {
-                joff = lk_stage_part<LK_JR, LK_JR, LK_JPITCH>(S.jreg, J, jx0, jy0, tid - 32, LK_THREADS - 32);
-            }
+        for (int q = 0; q < 3; q++) {
+            float l0 = __shfl_sync(0xffffffffu, acc, q * 5 + 0), l1 = __shfl_sync(0xffffffffu, acc, q * 5 + 1);
+            float l2 = __shfl_sync(0xffffffffu, acc, q * 5 + 2), l3 = __shfl_sync(0xffffffffu, acc, q * 5 + 3);
+            float t = __shfl_sync(0xffffffffu, acc, q * 5 + 4);
+            sum[q] = t + ((l0 + l2) + (l1 + l3));
         }
-        if (inwin) {
-            joff = lk_stage_offset<LK_JR, LK_JR>(J, jx0, jy0, T.on);
-            if (T.on && lk_inside<LK_JR, LK_JR>(J, jx0, jy0)) lk_tma_wait(S, T);
+        if (pt == 0) {
+            const float FLT_SCALE = 1.f / (1 << 20);
+            const float A11 = sum[0] * FLT_SCALE, A12 = sum[1] * FLT_SCALE, A22 = sum[2] * FLT_SCALE;
+            const float D = A11 * A22 - A12 * A12;
+            const float minEig = (A22 + A11 - sqrtf((A11 - A22) * (A11 - A22) + 4.f * A12 * A12)) / 882.f;
+            R.A11 = A11;
+            R.A12 = A12;
+            R.A22 = A22;
+            R.ok = !(minEig < 1e-4f || D < 1.1920928955078125e-07f);
+            R.D = 1.f / D;
         }
     }
-    // this thread's share of the mismatch terms (constant over the iterations).  Its template values are read from
-    // S.tpl in every iteration rather than held in registers: the loads overlap the weight arithmetic,
-    // and the nine registers they would pin make the 80-register k_track serialise its iteration.
-    const LKUnit U1 = lk_unit(tid < LK_BT ? tid : 0);
-    const bool has2 = (tid >= 4 * LK_BCHAIN) && (LK_THREADS + tid - 4 * LK_BCHAIN < LK_BT);
-    const LKUnit U2 = lk_unit(has2 ? LK_THREADS + tid - 4 * LK_BCHAIN : 4 * LK_BCHAIN);
-    __syncthreads();
-    LKP(3);
-    float A11 = S.sums[0] * FLT_SCALE, A12 = S.sums[1] * FLT_SCALE, A22 = S.sums[2] * FLT_SCALE;
-    // the mismatch chains are 42 pair terms long: clear steps 42..83 of the SIMD chains of the two quantities they reuse
-    for (int i = tid; i < 2 * 4 * (LK_CHAIN - LK_BCHAIN); i += LK_THREADS) {
-        int q = i / (4 * (LK_CHAIN - LK_BCHAIN)), r = i - q * 4 * (LK_CHAIN - LK_BCHAIN);
-        S.terms[q * LK_Q + (LK_BCHAIN + (r >> 2)) * 5 + (r & 3)] = 0.f;
+}
+
+// Consumer role: the LK iterations of one pyramid level for one point, on the level built into buffer buf.  Run by the
+// LK_CTHREADS consumer threads (tid < LK_CTHREADS) with identical scalar arguments; each keeps identical copies of the
+// scalar state.  Warp 0 runs the sequential b chains of the fallback.
+__device__ __forceinline__ void lk_iterate(LKSmem& S, int tid, const Level& J, float2 g, float& nx, float& ny, int level,
+                                           int buf, int& status, int& iters, int& fallbacks, long long* pc, LKTma& T)
+{
+    [[maybe_unused]] long long tl = gf_clock();
+    const float FLT_SCALE = 1.f / (1 << 20);
+    uint8_t* jreg = S.jreg[level & 1];
+    int jx0, jy0;
+    bool jvalid = lk_jwin0(g, level, J, jx0, jy0);     // the window the producers staged for this level
+    int joff = jvalid ? lk_stage_offset<LK_JR, LK_JR>(J, jx0, jy0, T.on) : 0;
+    if (jvalid && T.on && lk_inside<LK_JR, LK_JR>(J, jx0, jy0)) {     // on every path: the barrier's next use needs it
+        while (!mbar_try_wait(&S.mbar_p[level & 1], (T.phase_p >> (level & 1)) & 1u)) { }
+        T.phase_p ^= 1u << (level & 1);
     }
-    float D = A11 * A22 - A12 * A12;
-    float minEig = (A22 + A11 - sqrtf((A11 - A22) * (A11 - A22) + 4.f * A12 * A12)) / 882.f;
-    if (minEig < 1e-4f || D < 1.1920928955078125e-07f) {
+    const LKLevelA R = S.lv[buf];
+    if (!R.ok) {                 // outside the image, or minEig / determinant below the thresholds
         if (level == 0) status = 0;
         return;
     }
-    D = 1.f / D;
+    const short4* tpl = S.tpl[buf];
+    // this thread's pixels (the unit map above LK_BSLOTS): pair unit tid at template index p0 and p0 + 4, then either the
+    // second pair unit (p0 + 336, p0 + 340) or tail unit tid - 40 at e0, and for 17 threads tail unit tid + 48 at e1
+    const bool pair2 = tid < LK_PAIR2, tail2 = !pair2 && tid < LK_PAIR2 + LK_TAIL2;
+    const int p0 = (tid >> 3) * LK_WIN + 8 * ((tid & 7) >> 2) + (tid & 3);
+    const int po = (tid >> 3) * LK_JPITCH + 8 * ((tid & 7) >> 2) + (tid & 3);
+    const int pslot = ((tid >> 3) * 2 + ((tid & 7) >> 2)) * 5 + (tid & 3);
+    const int v0 = tid - LK_PAIR2, v1 = tid + (LK_TAIL - LK_TAIL2 - LK_PAIR2);     // tail unit indices (used when valid)
+    const int e0 = (v0 / 5) * LK_WIN + 16 + v0 % 5, e1 = (v1 / 5) * LK_WIN + 16 + v1 % 5;
+    const int eo0 = (v0 / 5) * LK_JPITCH + 16 + v0 % 5, eo1 = (v1 / 5) * LK_JPITCH + 16 + v1 % 5;
+    constexpr int P2I = 16 * LK_WIN, P2O = 16 * LK_JPITCH, P2S = 16 * 2 * 5;        // unit + 128: 16 template rows down
 
+    float A11 = R.A11, A12 = R.A12, A22 = R.A22, D = R.D;
+    float qx = nx - 10.f, qy = ny - 10.f;
     float pdx_ = 0.f, pdy_ = 0.f;
-    LKP(4);
+    LKP(3);
     for (int j = 0; j < 30; j++) {
         int iqx = __float2int_rd(qx), iqy = __float2int_rd(qy);
         if (iqx < -LK_WIN || iqx >= J.w || iqy < -LK_WIN || iqy >= J.h) {
@@ -425,88 +466,96 @@ __device__ __forceinline__ void lk_level(LKSmem& S, int tid, const Level& I, con
         if (!(jvalid && iqx >= jx0 && iqy >= jy0 && iqx + 22 <= jx0 + LK_JR && iqy + 22 <= jy0 + LK_JR)) {
             jx0 = iqx - 9;
             jy0 = iqy - 9;
-            __syncthreads();
+            lk_bar(LK_BAR_CONS, LK_CTHREADS);     // the readers of the previous window are done
             if (T.on && lk_inside<LK_JR, LK_JR>(J, jx0, jy0)) {
                 if (tid == 0) {
                     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    mbar_expect_tx(&S.mbar, LK_JR * LK_JPITCH);
-                    lk_tma_box(S.jreg, T.mj + level, jx0 & ~15, jy0, &S.mbar);
+                    mbar_expect_tx(&S.mbar_j, LK_JR * LK_JPITCH);
+                    lk_tma_box(jreg, T.mj + level, jx0 & ~15, jy0, &S.mbar_j);
                 }
-                lk_tma_wait(S, T);     // every thread waits: the box is visible to all without a barrier
+                lk_tma_wait(&S.mbar_j, T.phase_j);     // every consumer waits: the box is visible to all without a barrier
                 joff = jx0 & 15;
             } else {
-                joff = lk_stage<LK_JR, LK_JR, LK_JPITCH>(S.jreg, J, jx0, jy0, tid);
-                __syncthreads();
+                joff = lk_stage_part<LK_JR, LK_JR, LK_JPITCH>(jreg, J, jx0, jy0, tid, LK_CTHREADS);
+                lk_bar(LK_BAR_CONS, LK_CTHREADS);
             }
             jvalid = true;
+            LKP(4);
         }
-        a = qx - (float)iqx;
-        b = qy - (float)iqy;
-        lk_weights(a, b, iw00, iw01, iw10, iw11);
-        const uint8_t* jb = S.jreg + (iqy - jy0) * LK_JPITCH + joff + (iqx - jx0);
-        // No barrier here: the window staged before the loop, the cleared terms and the A sums were published by the
-        // barrier before the loop; the previous iteration's terms and sums were consumed before its last barrier (the
-        // fast path reads neither), and its integer partials sit in the other half of S.bpart.
-        // ---- mismatch terms: 168 pmaddwd pair units (row y, k in 0..3, half h) + 105 tail pixels; this thread's unit
-        //      U1 gives (sx, sy), the second tail unit U2 of 17 threads (ex, ey) ----
-        auto unit_terms = [&](int& sx, int& sy, int& ex, int& ey) {
-            sx = sy = ex = ey = 0;
-            if (tid < LK_BT) {
-                const uint8_t* q = jb + U1.off0;
-                int jv = q[0] * iw00 + q[1] * iw01 + q[LK_JPITCH] * iw10 + q[LK_JPITCH + 1] * iw11;
-                const short4 t0 = S.tpl[U1.i0];
-                int d0 = lk_descale(jv, 9) - t0.x;
-                sx = d0 * t0.y;
-                sy = d0 * t0.z;
-                if (tid < 4 * LK_BCHAIN) {
-                    q = jb + U1.off1;
-                    jv = q[0] * iw00 + q[1] * iw01 + q[LK_JPITCH] * iw10 + q[LK_JPITCH + 1] * iw11;
-                    const short4 t1 = S.tpl[U1.i1];
-                    int d1 = lk_descale(jv, 9) - t1.x;
-                    sx += d1 * t1.y;   // pmaddwd: exact int32 pair sum, converted once
-                    sy += d1 * t1.z;
-                }
-            }
-            if (has2) {
-                const uint8_t* q = jb + U2.off0;
-                int jv = q[0] * iw00 + q[1] * iw01 + q[LK_JPITCH] * iw10 + q[LK_JPITCH + 1] * iw11;
-                const short4 t2 = S.tpl[U2.i0];
-                int d0 = lk_descale(jv, 9) - t2.x;
-                ex = d0 * t2.y;
-                ey = d0 * t2.z;
+        int iw00, iw01, iw10, iw11;
+        lk_weights(qx - (float)iqx, qy - (float)iqy, iw00, iw01, iw10, iw11);
+        const uint8_t* jb = jreg + (iqy - jy0) * LK_JPITCH + joff + (iqx - jx0);
+        // No barrier here: the window staged by the producers or in this level was published by its barrier or mbarrier, the level's template
+        // and matrix by the handoff; the previous iteration's fallback terms and sums were consumed before its last
+        // barrier (the fast path reads neither), and its integer partials sit in the other half of S.bpart.
+        // ---- mismatch terms: (d * Ix, d * Iy) of one template pixel ----
+        auto pix = [&](int i, int off, int& px, int& py) {
+            const uint8_t* q = jb + off;
+            const int jv = q[0] * iw00 + q[1] * iw01 + q[LK_JPITCH] * iw10 + q[LK_JPITCH + 1] * iw11;
+            const short4 t = tpl[i];
+            const int d = lk_descale(jv, 9) - t.x;
+            px = d * t.y;
+            py = d * t.z;
+        };
+        // units: pair unit (ux, uy) -- pmaddwd, an exact int32 pair sum converted once; second unit (vx, vy), a pair or a
+        // tail pixel; second tail pixel (wx, wy) or 0
+        auto unit_terms = [&](int& ux, int& uy, int& vx, int& vy, int& wx, int& wy) {
+            int x1, y1;
+            pix(p0, po, ux, uy);
+            pix(p0 + 4, po + 4, x1, y1);
+            ux += x1;
+            uy += y1;
+            wx = wy = 0;
+            if (pair2) {
+                pix(p0 + P2I, po + P2O, vx, vy);
+                pix(p0 + P2I + 4, po + P2O + 4, x1, y1);
+                vx += x1;
+                vy += y1;
+            } else {
+                pix(e0, eo0, vx, vy);
+                if (tail2) pix(e1, eo1, wx, wy);
             }
         };
-        int sx, sy, ex, ey;
-        unit_terms(sx, sy, ex, ey);
-        unsigned part[4] = {0u, 0u, 0u, 0u};     // this thread's x+, x-, y+, y- (all its units are of one chain)
-        lk_split(sx, part[0], part[1]);
-        lk_split(sy, part[2], part[3]);
-        lk_split(ex, part[0], part[1]);
-        lk_split(ey, part[2], part[3]);
-        lk_bpart_write(S.bpart[j & 1], tid, part);
-        __syncthreads();
+        int ux, uy, vx, vy, wx, wy;
+        unit_terms(ux, uy, vx, vy, wx, wy);
+        unsigned part[4] = {0u, 0u, 0u, 0u}, tpart[4] = {0u, 0u, 0u, 0u};     // x+, x-, y+, y- of the pair / tail chain
+        lk_split(ux, part[0], part[1]);
+        lk_split(uy, part[2], part[3]);
+        unsigned vpart[4] = {0u, 0u, 0u, 0u};
+        lk_split(vx, vpart[0], vpart[1]);
+        lk_split(vy, vpart[2], vpart[3]);
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            part[k] += pair2 ? vpart[k] : 0u;
+            tpart[k] += pair2 ? 0u : vpart[k];
+        }
+        lk_split(wx, tpart[0], tpart[1]);
+        lk_split(wy, tpart[2], tpart[3]);
+        lk_bpart_write(S.bpart[j & 1], tid, part, tpart);
+        lk_bar(LK_BAR_CONS, LK_CTHREADS);
         LKP(5);
         float s1, s2;
         if (!lk_bsum_int(S.bpart[j & 1], tid & 31, s1, s2)) {
             // Some chain may round: OpenCV's order.  The terms are computed again rather than kept in registers across
             // the barrier, stored in chain order, summed by warp 0 and broadcast.
-            unit_terms(sx, sy, ex, ey);
-            if (tid < LK_BT) {
-                S.terms[U1.slot] = (float)sx;
-                S.terms[LK_Q + U1.slot] = (float)sy;
+            unit_terms(ux, uy, vx, vy, wx, wy);
+            S.bterms[pslot] = (float)ux;
+            S.bterms[LK_Q + pslot] = (float)uy;
+            const int vslot = pair2 ? pslot + P2S : v0 * 5 + 4;
+            S.bterms[vslot] = (float)vx;
+            S.bterms[LK_Q + vslot] = (float)vy;
+            if (tail2) {
+                S.bterms[v1 * 5 + 4] = (float)wx;
+                S.bterms[LK_Q + v1 * 5 + 4] = (float)wy;
             }
-            if (has2) {
-                S.terms[U2.slot] = (float)ex;
-                S.terms[LK_Q + U2.slot] = (float)ey;
-            }
-            __syncthreads();
+            lk_bar(LK_BAR_CONS, LK_CTHREADS);
             if (tid < 32) {
-                lk_bcombine(lk_chain(S.terms, tid, 2), s1, s2);
-                if (tid == 0) { S.sums[0] = s1; S.sums[1] = s2; }
+                lk_bcombine(lk_chain(S.bterms, tid, 2), s1, s2);
+                if (tid == 0) { S.bsums[0] = s1; S.bsums[1] = s2; }
             }
-            __syncthreads();
-            s1 = S.sums[0];
-            s2 = S.sums[1];
+            lk_bar(LK_BAR_CONS, LK_CTHREADS);
+            s1 = S.bsums[0];
+            s2 = S.bsums[1];
             fallbacks++;
         }
         LKP(6);
@@ -534,19 +583,22 @@ __device__ __forceinline__ void lk_level(LKSmem& S, int tid, const Level& I, con
     }
 }
 
-// Whole pyramid for one point.  init is only read when use_init.
+// Whole pyramid for one point.  init is only read when use_init.  Every thread of the CTA calls this with identical
+// arguments and receives the same out / status; iters, fallbacks and pc are counted by the consumer threads (thread 0
+// reports them).  Level l is iterated by the consumers while the producers build level l-1; the roles meet at one
+// handoff barrier per level (and one before the first), which both pass on every path: a level that is out of the image
+// or rejected by minEig is built as "not ok" and skipped by the consumers, and the producers of level 0 build nothing.
 __device__ __forceinline__ void lk_track_point(LKSmem& S, int tid, const Pyramid& I, const Pyramid& J,
                                                float2 p, float2 init, bool use_init, int max_level,
                                                float2& out, int& status, int& iters, int& fallbacks, long long* pc, LKTma& T)
 {
     status = 1;
-    float nx = 0.f, ny = 0.f;
     [[maybe_unused]] long long tl = gf_clock();
-    __syncthreads();
-    for (int i = tid; i < 3 * LK_Q; i += LK_THREADS) S.terms[i] = 0.f;    // chain padding must read +0.0f
-    constexpr int NPAD = (LK_BSLOTS - 4 * LK_PAIR_WARPS - LK_TAIL_WARPS) * 4;      // and the unused tail partials 0
-    for (int i = tid; i < 2 * NPAD; i += LK_THREADS) (&S.bpart[i / NPAD][4 * LK_PAIR_WARPS + LK_TAIL_WARPS][0])[i % NPAD] = 0u;
+    __syncthreads();     // the previous pass's readers of every buffer are done
+    for (int i = tid; i < 3 * LK_Q; i += LK_THREADS) S.aterms[i] = 0.f;    // chain padding must read +0.0f
+    for (int i = tid; i < 2 * LK_Q; i += LK_THREADS) S.bterms[i] = 0.f;
     // the template windows of all levels depend only on p: fetch them together (one memory latency instead of one per level)
+    const float2 g = use_init ? init : p;
     int n_box = 0;
     for (int l = 0; l <= max_level; l++) {
         float ppx, ppy;
@@ -559,28 +611,46 @@ __device__ __forceinline__ void lk_track_point(LKSmem& S, int tid, const Pyramid
     if (n_box) {            // the same test again by the issuing thread: one transaction count for all boxes of this point
         if (tid == 0) {
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            mbar_expect_tx(&S.mbar, n_box * LK_IREG * LK_IPITCH);
+            mbar_expect_tx(&S.mbar_i, n_box * LK_IREG * LK_IPITCH);
             for (int l = 0; l <= max_level; l++) {
                 float ppx, ppy;
                 int ipx, ipy;
                 lk_origin(p, l, ppx, ppy, ipx, ipy);
                 if (ipx < -LK_WIN || ipx >= I.lv[l].w || ipy < -LK_WIN || ipy >= I.lv[l].h) continue;
-                if (lk_inside<LK_IREG, LK_IREG>(I.lv[l], ipx - 1, ipy - 1)) lk_tma_box(S.ireg[l], T.mi + l, (ipx - 1) & ~15, ipy - 1, &S.mbar);
+                if (lk_inside<LK_IREG, LK_IREG>(I.lv[l], ipx - 1, ipy - 1)) lk_tma_box(S.ireg[l], T.mi + l, (ipx - 1) & ~15, ipy - 1, &S.mbar_i);
             }
         }
-        lk_tma_wait(S, T);
+        lk_tma_wait(&S.mbar_i, T.phase_i);
     }
     __syncthreads();
     LKP(0);
-    for (int l = max_level; l >= 0; l--) {
-        float sc = (float)(1. / (double)(1 << l));
-        if (l == max_level) {
-            if (use_init) { nx = init.x * sc; ny = init.y * sc; }
-            else { nx = p.x * sc; ny = p.y * sc; }
-        } else { nx = nx * 2.f; ny = ny * 2.f; }
-        lk_level(S, tid, I.lv[l], J.lv[l], p, nx, ny, l, status, iters, fallbacks, pc, T);
+    if (tid >= LK_CTHREADS) {
+        const int pt = tid - LK_CTHREADS;
+        lk_build(S, pt, I.lv[max_level], J.lv[max_level], p, g, max_level, max_level & 1, T);
+        lk_bar(LK_BAR_HANDOFF, LK_THREADS);
+        for (int l = max_level; l >= 0; l--) {
+            if (l > 0) lk_build(S, pt, I.lv[l - 1], J.lv[l - 1], p, g, l - 1, (l - 1) & 1, T);    // the buffer of level l+1, free
+            lk_bar(LK_BAR_HANDOFF, LK_THREADS);
+        }
+    } else {
+        float nx = 0.f, ny = 0.f;
+        lk_bar(LK_BAR_HANDOFF, LK_THREADS);
+        LKP(1);
+        for (int l = max_level; l >= 0; l--) {
+            float sc = (float)(1. / (double)(1 << l));
+            if (l == max_level) {
+                if (use_init) { nx = init.x * sc; ny = init.y * sc; }
+                else { nx = p.x * sc; ny = p.y * sc; }
+            } else { nx = nx * 2.f; ny = ny * 2.f; }
+            lk_iterate(S, tid, J.lv[l], g, nx, ny, l, l & 1, status, iters, fallbacks, pc, T);
+            if (l == 0 && tid == 0) { S.res = make_float2(nx, ny); S.res_status = status; }
+            tl = gf_clock();
+            lk_bar(LK_BAR_HANDOFF, LK_THREADS);
+            LKP(2);
+        }
     }
-    out = make_float2(nx, ny);
+    out = S.res;
+    status = S.res_status;
 }
 
 }  // namespace gf

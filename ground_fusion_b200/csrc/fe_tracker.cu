@@ -24,6 +24,7 @@
 #include "fe_clahe.cuh"
 #include "fe_eig.cuh"
 #include "fe_lk.cuh"
+#include "fe_lk_single.cuh"
 #include "fe_select.cuh"
 
 namespace gf {
@@ -76,7 +77,7 @@ __global__ void __launch_bounds__(LK_THREADS) k_lk_stage(Pyramid I, Pyramid J, c
     const int tid = threadIdx.x, i = blockIdx.x;
     if (i >= n) return;
     lk_tma_init(sm, tid);
-    LKTma T{M.prevI, M.curJ, 0u, M.enabled != 0};
+    LKTma T{M.prevI, M.curJ, 0u, 0u, 0u, M.enabled != 0};
     float2 p = prev_pts[i], init = use_init ? next_pts[i] : p, out;
     int st, iters = 0, fallbacks = 0;
     long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -84,24 +85,38 @@ __global__ void __launch_bounds__(LK_THREADS) k_lk_stage(Pyramid I, Pyramid J, c
     if (tid == 0) { next_pts[i] = out; status[i] = (uint8_t)st; }
 }
 
+// The LK form of a tracker kernel: ROLES = the two warp roles (fe_lk.cuh), which shorten each feature's chain, when one
+// tracker has the GPU to itself; otherwise the single-role form (fe_lk_single.cuh), which measured faster when several
+// trackers share it (DESIGN.md §1.3).  Both give the same bits.
+template <bool ROLES> struct LKForm { using Smem = LKSmem; using Tma = LKTma; };
+template <> struct LKForm<false> { using Smem = lk1::LKSmem; using Tma = lk1::LKTma; };
+template <class Tma>
+__device__ __forceinline__ Tma lk_tma_of(const LKMapSet& M)
+{
+    Tma T{};                    // phases 0
+    T.mi = M.prevI; T.mj = M.curJ; T.on = M.enabled != 0;
+    return T;
+}
+
 // Prediction pass (feature_tracker.cpp:118-124): maxLevel 1 seeded with predict_pts; counts successes.  Feature blockIdx.x < n_prev.
-template <int V>
+template <int V, bool ROLES>
 __device__ __forceinline__ void lk_pred_point(const Pyramid& prev, const Pyramid& cur, TrackScalars* sc, const FeatArrays& fa, const LKMapSet& M)
 {
-    __shared__ LKSmem sm;
+    __shared__ typename LKForm<ROLES>::Smem sm;
     const int tid = threadIdx.x, i = blockIdx.x;
     lk_tma_init(sm, tid);
-    LKTma T{M.prevI, M.curJ, 0u, M.enabled != 0};
+    auto T = lk_tma_of<typename LKForm<ROLES>::Tma>(M);
     float2 out;
     int st, iters = 0, fallbacks = 0;
     long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     lk_track_point(sm, tid, prev, cur, fa.prev_pts[i], fa.pred_pts[i], true, 1, out, st, iters, fallbacks, pc, T);
     if (tid == 0) { fa.cur_pts[i] = out; fa.status[i] = (uint8_t)st; if (st) atomicAdd(&sc->pred_succ, 1); atomicAdd(&sc->lk_iters, iters); }
 }
+template <bool ROLES>
 __global__ void __launch_bounds__(LK_THREADS) k_lk_pred(Pyramid prev, Pyramid cur, TrackScalars* sc, FeatArrays fa, const __grid_constant__ LKMapSet M)
 {
     if ((int)blockIdx.x >= sc->n_prev) return;
-    lk_pred_point<0>(prev, cur, sc, fa, M);
+    lk_pred_point<0, ROLES>(prev, cur, sc, fa, M);
 }
 
 // Forward LK (3 levels) + reverse check (1 level, USE_INITIAL_FLOW) + inBorder + grey<=250
@@ -109,14 +124,14 @@ __global__ void __launch_bounds__(LK_THREADS) k_lk_pred(Pyramid prev, Pyramid cu
 #ifndef GF_TRACK_MIN_CTAS
 #define GF_TRACK_MIN_CTAS 3          // 80 registers: three features per SM when several streams share the GPU (2: 110 registers)
 #endif
-template <int V>
+template <int V, bool ROLES>
 __device__ __forceinline__ void track_point(const Pyramid& prev, const Pyramid& cur, TrackScalars* sc, const FeatArrays& fa,
                                             const FrameParams* fp, int flow_back, const LKMapSet& M)
 {
-    __shared__ LKSmem sm;
+    __shared__ typename LKForm<ROLES>::Smem sm;
     const int tid = threadIdx.x, i = blockIdx.x;
     lk_tma_init(sm, tid);
-    LKTma T{M.prevI, M.curJ, 0u, M.enabled != 0};
+    auto T = lk_tma_of<typename LKForm<ROLES>::Tma>(M);
     const float2 p = fa.prev_pts[i];
     const long long t0 = gf_clock();
     float2 q;
@@ -151,11 +166,12 @@ __device__ __forceinline__ void track_point(const Pyramid& prev, const Pyramid& 
         }
     }
 }
+template <bool ROLES>
 __global__ void __launch_bounds__(LK_THREADS, GF_TRACK_MIN_CTAS) k_track(Pyramid prev, Pyramid cur, TrackScalars* sc, FeatArrays fa,
                                                       const FrameParams* fp, int flow_back, const __grid_constant__ LKMapSet M)
 {
     if ((int)blockIdx.x >= sc->n_prev) return;
-    track_point<0>(prev, cur, sc, fa, fp, flow_back, M);
+    track_point<0, ROLES>(prev, cur, sc, fa, fp, flow_back, M);
 }
 
 // setPrediction (feature_tracker.cpp:1006-1027)
@@ -277,14 +293,14 @@ __global__ void __launch_bounds__(LK_THREADS) k_lk_pred_g(const GroupMember* __r
     const GroupMember& G = tab[blockIdx.y];
     if (!G.fp.has_pred || (int)blockIdx.x >= G.sc->n_prev) return;
     lk_maps_acquire(G.maps, threadIdx.x);
-    lk_pred_point<1>(G.prev, G.cur, G.sc, G.fa, *G.maps);
+    lk_pred_point<1, false>(G.prev, G.cur, G.sc, G.fa, *G.maps);     // a group is several cameras: the single-role form
 }
 __global__ void __launch_bounds__(LK_THREADS, GF_TRACK_MIN_CTAS) k_track_g(const GroupMember* __restrict__ tab, int flow_back)
 {
     const GroupMember& G = tab[blockIdx.y];
     if ((int)blockIdx.x >= G.sc->n_prev) return;
     lk_maps_acquire(G.maps, threadIdx.x);
-    track_point<1>(G.prev, G.cur, G.sc, G.fa, &G.fp, flow_back, *G.maps);
+    track_point<1, false>(G.prev, G.cur, G.sc, G.fa, &G.fp, flow_back, *G.maps);
 }
 __global__ void __launch_bounds__(FE_CAP) k_compact_setmask_g(const GroupMember* __restrict__ tab, int min_dist)
 {
@@ -329,8 +345,9 @@ struct gf_tracker {
     bool profiling;
     float stage_ms[GF_FE_STAGES];
     // CUDA graphs keyed by frame number mod 6 (= pyramid slot mod 3 x two-slot buffers)
-    cudaGraphExec_t g_pyr[6], g_eig[6], g_dep1[6][2], g_dep2[6];
-    int gk_pyr[6], gk_eig[6], gk_dep1[6][2], gk_dep2[6];
+    cudaGraphExec_t g_pyr[6], g_eig[6], g_dep1[6][2][2], g_dep2[6];     // g_dep1[frame][prediction][LK roles]
+    int gk_pyr[6], gk_eig[6], gk_dep1[6][2][2], gk_dep2[6];
+    bool counted;                                                          // in g_live_trackers
     bool use_graph;
     // gf_tracker_set_equalize: CLAHE of every gray frame into pyramid level 0.  Frames land in d_raw first; the copy and both
     // CLAHE kernels (a graph keyed by pyramid slot) run in order on s_up, so one raw buffer and one LUT block serve every frame
@@ -365,6 +382,17 @@ struct gf_tracker {
 };
 
 static inline int in_flight(const gf_tracker* t) { return (int)(t->n_submitted - t->n_waited); }
+
+// Trackers alive per device (gf_tracker_create .. gf_tracker_destroy).  A tracker alone on its device runs k_track in the
+// two-role LK form, which shortens the slowest feature's chain; while other trackers share the device, the throughput of
+// all of them counts and the single-role form is faster (DESIGN.md §1.3).  The choice is made per frame; each form has
+// its own captured graph.
+constexpr int GF_LIVE_DEVICES = 64;
+static std::atomic<int> g_live_trackers[GF_LIVE_DEVICES];
+static inline bool lk_roles(const gf_tracker* t)
+{
+    return t->device >= GF_LIVE_DEVICES || g_live_trackers[t->device].load() <= 1;
+}
 
 static Pyramid make_pyr(const gf_tracker* t, int slot)
 {
@@ -524,6 +552,7 @@ int gf_tracker_create(gf_tracker** out, int device, int width, int height, const
         memcpy(g_err, keep, sizeof(keep));
         return rc;
     }
+    if (device < GF_LIVE_DEVICES) { g_live_trackers[device]++; t->counted = true; }
     *out = t;
     return GF_OK;
 }
@@ -599,13 +628,14 @@ static int tracker_init(gf_tracker* t, int width, int height, const gf_tracker_c
 void gf_tracker_destroy(gf_tracker* t)
 {
     if (!t) return;
+    if (t->counted) g_live_trackers[t->device]--;
     cudaSetDevice(t->device);
     cudaDeviceSynchronize();        // (a partially built tracker may lack some of its streams)
     for (int k = 0; k < 6; k++) {
         if (t->g_pyr[k]) cudaGraphExecDestroy(t->g_pyr[k]);
         if (t->g_eig[k]) cudaGraphExecDestroy(t->g_eig[k]);
         if (t->g_dep2[k]) cudaGraphExecDestroy(t->g_dep2[k]);
-        for (int p = 0; p < 2; p++) if (t->g_dep1[k][p]) cudaGraphExecDestroy(t->g_dep1[k][p]);
+        for (int p = 0; p < 4; p++) if (t->g_dep1[k][p / 2][p % 2]) cudaGraphExecDestroy(t->g_dep1[k][p / 2][p % 2]);
     }
     for (int k = 0; k < 3; k++) if (t->g_clahe[k]) cudaGraphExecDestroy(t->g_clahe[k]);
     for (int s = 0; s < 3; s++) for (int l = 0; l < 4; l++) cudaFree(t->d_pyr[s][l]);
@@ -678,14 +708,19 @@ static int body_eig(gf_tracker* t, long long f)
     return enqueue_min_eig(t->s_eig, Pc.lv[0], t->d_eig[f % 2], t->epitch, t->d_cov, t->d_box);
 }
 
-static int body_dep1(gf_tracker* t, long long f, bool has_pred)
+static int body_dep1(gf_tracker* t, long long f, bool has_pred, bool roles)
 {
     cudaStream_t s = t->s_main;
     Pyramid Pc = make_pyr(t, (int)(f % 3)), Pp = make_pyr(t, (int)((f + 2) % 3));
     const int lk_grid = t->cfg.max_cnt;
     const LKMapSet& M = t->lk_maps[f % 3];
-    if (has_pred) { k_lk_pred<<<lk_grid, LK_THREADS, 0, s>>>(Pp, Pc, t->d_sc, t->fa, M); GF_LAUNCHED(); }
-    k_track<<<lk_grid, LK_THREADS, 0, s>>>(Pp, Pc, t->d_sc, t->fa, t->d_fp[f % 2], t->cfg.flow_back, M); GF_LAUNCHED();
+    if (roles) {
+        if (has_pred) { k_lk_pred<true><<<lk_grid, LK_THREADS, 0, s>>>(Pp, Pc, t->d_sc, t->fa, M); GF_LAUNCHED(); }
+        k_track<true><<<lk_grid, LK_THREADS, 0, s>>>(Pp, Pc, t->d_sc, t->fa, t->d_fp[f % 2], t->cfg.flow_back, M); GF_LAUNCHED();
+    } else {
+        if (has_pred) { k_lk_pred<false><<<lk_grid, LK_THREADS, 0, s>>>(Pp, Pc, t->d_sc, t->fa, M); GF_LAUNCHED(); }
+        k_track<false><<<lk_grid, LK_THREADS, 0, s>>>(Pp, Pc, t->d_sc, t->fa, t->d_fp[f % 2], t->cfg.flow_back, M); GF_LAUNCHED();
+    }
     GF_MARK(2, s);
     k_compact_setmask<<<1, FE_CAP, 0, s>>>(t->d_sc, t->fa, t->cfg.min_dist); GF_LAUNCHED();
     GF_CUDA(cudaGetLastError());
@@ -766,7 +801,8 @@ static int enqueue_frame(gf_tracker* t, long long f, double time, bool depth_val
     GF_CUDA(cudaEventRecord(t->ev_eig[es], t->s_eig));
     GF_MARK(8, t->s_eig);
     GF_CUDA(cudaStreamWaitEvent(t->s_main, t->ev_pyr[es], 0));
-    rc = run_piece(direct, t->s_main, &t->g_dep1[key][hp], &t->gk_dep1[key][hp], [&] { return body_dep1(t, f, hp != 0); });
+    const int ro = lk_roles(t) ? 1 : 0;
+    rc = run_piece(direct, t->s_main, &t->g_dep1[key][hp][ro], &t->gk_dep1[key][hp][ro], [&] { return body_dep1(t, f, hp != 0, ro != 0); });
     if (rc) return rc;
     GF_CUDA(cudaStreamWaitEvent(t->s_main, t->ev_eig[es], 0));
     rc = run_piece(direct, t->s_main, &t->g_dep2[key], &t->gk_dep2[key], [&] { return body_dep2(t, f); });
