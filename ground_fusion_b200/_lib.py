@@ -112,7 +112,7 @@ def lib():
         L.gf_stage_pyr_down.argtypes = [i, vp, i, i, vp]
         L.gf_stage_clahe.argtypes = [i, vp, sz, i, i, d, i, i, vp]
         L.gf_stage_min_eig.argtypes = [i, vp, i, i, vp, ctypes.POINTER(i)]
-        L.gf_stage_lk.argtypes = [i, vp, vp, i, i, vp, vp, i, i, i, vp]
+        L.gf_stage_lk.argtypes = [i, vp, vp, i, i, vp, vp, i, i, i, vp, i]
         L.gf_stage_gftt.argtypes = [i, vp, i, i, vp, i, i, i, vp, ctypes.POINTER(i), ctypes.POINTER(TrackInfo)]
         L.gf_stage_setmask_order.argtypes = [i, vp, i, vp]
         L.gf_dense_map_create.argtypes = [ctypes.POINTER(vp), i, ctypes.POINTER(DenseMapCfg)]

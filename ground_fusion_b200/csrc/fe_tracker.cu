@@ -70,21 +70,6 @@ __global__ void __launch_bounds__(256) k_in_boxes_stage(const float2* pts, int n
 // ------------------------------------------------------------------------------------------------
 // kernels that need the LK device code
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(LK_THREADS) k_lk_stage(Pyramid I, Pyramid J, const float2* prev_pts, float2* next_pts,
-                                                         int n, int max_level, int use_init, uint8_t* status, const __grid_constant__ LKMapSet M)
-{
-    __shared__ LKSmem sm;
-    const int tid = threadIdx.x, i = blockIdx.x;
-    if (i >= n) return;
-    lk_tma_init(sm, tid);
-    LKTma T{M.prevI, M.curJ, 0u, 0u, 0u, M.enabled != 0};
-    float2 p = prev_pts[i], init = use_init ? next_pts[i] : p, out;
-    int st, iters = 0, fallbacks = 0;
-    long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    lk_track_point(sm, tid, I, J, p, init, use_init != 0, max_level, out, st, iters, fallbacks, pc, T);
-    if (tid == 0) { next_pts[i] = out; status[i] = (uint8_t)st; }
-}
-
 // The LK form of a tracker kernel: ROLES = the two warp roles (fe_lk.cuh), which shorten each feature's chain, when one
 // tracker has the GPU to itself; otherwise the single-role form (fe_lk_single.cuh), which measured faster when several
 // trackers share it (DESIGN.md §1.3).  Both give the same bits.
@@ -96,6 +81,23 @@ __device__ __forceinline__ Tma lk_tma_of(const LKMapSet& M)
     Tma T{};                    // phases 0
     T.mi = M.prevI; T.mj = M.curJ; T.on = M.enabled != 0;
     return T;
+}
+
+// gf_stage_lk: one CTA per point, in the LK form ROLES selects (LKForm above)
+template <bool ROLES>
+__global__ void __launch_bounds__(LK_THREADS) k_lk_stage(Pyramid I, Pyramid J, const float2* prev_pts, float2* next_pts,
+                                                         int n, int max_level, int use_init, uint8_t* status, const __grid_constant__ LKMapSet M)
+{
+    __shared__ typename LKForm<ROLES>::Smem sm;
+    const int tid = threadIdx.x, i = blockIdx.x;
+    if (i >= n) return;
+    lk_tma_init(sm, tid);
+    auto T = lk_tma_of<typename LKForm<ROLES>::Tma>(M);
+    float2 p = prev_pts[i], init = use_init ? next_pts[i] : p, out;
+    int st, iters = 0, fallbacks = 0;
+    long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    lk_track_point(sm, tid, I, J, p, init, use_init != 0, max_level, out, st, iters, fallbacks, pc, T);
+    if (tid == 0) { next_pts[i] = out; status[i] = (uint8_t)st; }
 }
 
 // Prediction pass (feature_tracker.cpp:118-124): maxLevel 1 seeded with predict_pts; counts successes.  Feature blockIdx.x < n_prev.
@@ -160,9 +162,11 @@ __device__ __forceinline__ void track_point(const Pyramid& prev, const Pyramid& 
     if (tid == 0) {
         fa.cur_pts[i] = q; fa.status[i] = (uint8_t)st; atomicAdd(&sc->lk_iters, iters);
         if (fa.dbg && i < 4) for (int k = 0; k < 8; k++) fa.dbg[32 + 8 * i + k] = pc[k];
-        if (fa.dbg) {   // cycles, LK iterations, of which b sums from the integer partials / from the sequential chains
+        if (fa.dbg) {   // cycles, LK iterations, of which b sums from the integer partials / from the sequential chains,
+                        // and the LK form that ran: 2 = two warp roles, 1 = single role
             fa.dbg[64 + 8 * i] = gf_clock() - t0; fa.dbg[64 + 8 * i + 1] = iters;
             fa.dbg[64 + 8 * i + 2] = iters - fallbacks; fa.dbg[64 + 8 * i + 3] = fallbacks;
+            fa.dbg[64 + 8 * i + 4] = ROLES ? 2 : 1;
         }
     }
 }
@@ -1624,7 +1628,7 @@ int gf_stage_min_eig(int device, const uint8_t* img, int w, int h, float* eig, i
 }
 
 int gf_stage_lk(int device, const uint8_t* prev, const uint8_t* next, int w, int h, const float* prev_pts, float* next_pts, int n,
-                int max_level, int use_initial_flow, uint8_t* status)
+                int max_level, int use_initial_flow, uint8_t* status, int roles)
 {
     if (!prev || !next || !prev_pts || !next_pts || !status || n < 0 || max_level < 0 || max_level > 3) return set_err(GF_ERR_INVALID_ARG, "bad argument");
     if ((w >> max_level) < 48 || (h >> max_level) < 48) return set_err(GF_ERR_UNSUPPORTED, "coarsest pyramid level must be at least 48x48");
@@ -1652,7 +1656,9 @@ int gf_stage_lk(int device, const uint8_t* prev, const uint8_t* next, int w, int
     GF_CUDA(cudaMemcpy(dq.p, next_pts, (size_t)n * 8, cudaMemcpyHostToDevice));
     LKMapSet M;
     rc = make_lk_maps(&M, P[0], P[1], max_level + 1); if (rc) return rc;
-    k_lk_stage<<<n, LK_THREADS>>>(P[0], P[1], dp.as<float2>(), dq.as<float2>(), n, max_level, use_initial_flow, dst.as<uint8_t>(), M); GF_LAUNCHED();
+    if (roles) k_lk_stage<true><<<n, LK_THREADS>>>(P[0], P[1], dp.as<float2>(), dq.as<float2>(), n, max_level, use_initial_flow, dst.as<uint8_t>(), M);
+    else k_lk_stage<false><<<n, LK_THREADS>>>(P[0], P[1], dp.as<float2>(), dq.as<float2>(), n, max_level, use_initial_flow, dst.as<uint8_t>(), M);
+    GF_LAUNCHED();
     GF_CUDA(cudaGetLastError());
     GF_CUDA(cudaMemcpy(next_pts, dq.p, (size_t)n * 8, cudaMemcpyDeviceToHost));
     GF_CUDA(cudaMemcpy(status, dst.p, n, cudaMemcpyDeviceToHost));

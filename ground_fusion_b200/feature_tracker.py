@@ -47,14 +47,15 @@ def corner_min_eigen_val(img, device=0):
     return out, nfix.value
 
 
-def calc_optical_flow_pyr_lk(prev, nxt, prev_pts, max_level=3, init=None, device=0):
+def calc_optical_flow_pyr_lk(prev, nxt, prev_pts, max_level=3, init=None, device=0, roles=True):
+    """roles: the LK form of a tracker alone on its device (two warp roles); False: the form of several trackers."""
     prev, nxt = _u8(prev), _u8(nxt)
     h, w = prev.shape
     p = np.ascontiguousarray(prev_pts, np.float32).reshape(-1, 2)
     q = np.ascontiguousarray(init, np.float32).reshape(-1, 2).copy() if init is not None else np.zeros_like(p)
     st = np.zeros(len(p), np.uint8)
     check(_lib.lib().gf_stage_lk(device, prev.ctypes.data, nxt.ctypes.data, w, h, p.ctypes.data, q.ctypes.data,
-                                 len(p), int(max_level), int(init is not None), st.ctypes.data))
+                                 len(p), int(max_level), int(init is not None), st.ctypes.data, int(bool(roles))))
     return q, st
 
 

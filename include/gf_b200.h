@@ -228,7 +228,8 @@ int gf_tracker_set_profiling(gf_tracker* t, int enable);
 int gf_tracker_last_stage_ms(gf_tracker* t, float* ms /* GF_FE_STAGES */);
 /* Development aid: clock64 phase counters of the single-CTA kernels ([0..63]) and per-feature LK cycles/iterations
  * ([64 + 8*i], [64 + 8*i + 1]); of those iterations, the ones whose mismatch vector came from exact integer sums and
- * the ones that ran the sequential float chains ([64 + 8*i + 2], [64 + 8*i + 3]).  Rows past the frame's n_prev
+ * the ones that ran the sequential float chains ([64 + 8*i + 2], [64 + 8*i + 3]); the LK form of the frame's k_track
+ * ([64 + 8*i + 4]: 2 = two warp roles, the tracker alone on its device; 1 = single role).  Rows past the frame's n_prev
  * are stale.  n <= 64 + 8*1024. */
 int gf_tracker_debug_read(gf_tracker* t, long long* out, int n);
 
@@ -248,10 +249,12 @@ int gf_stage_in_boxes(int device, const float* pts, int n, const gf_box* boxes, 
 /* cv::cornerMinEigenVal(img, blockSize=3, ksize=3) as used by goodFeaturesToTrack. */
 int gf_stage_min_eig(int device, const uint8_t* img, int w, int h, float* eig, int* n_fixups);
 /* cv::calcOpticalFlowPyrLK(prev, next, prev_pts, next_pts, status, err, Size(21,21), max_level,
- * TermCriteria(COUNT+EPS,30,0.01), use_initial_flow ? OPTFLOW_USE_INITIAL_FLOW : 0). */
+ * TermCriteria(COUNT+EPS,30,0.01), use_initial_flow ? OPTFLOW_USE_INITIAL_FLOW : 0).  roles selects the LK form of the
+ * tracker's kernels: 1 = two warp roles (a tracker alone on its device), 0 = single role (several trackers, groups).
+ * Both give the same bits. */
 int gf_stage_lk(int device, const uint8_t* prev, const uint8_t* next, int w, int h,
                 const float* prev_pts, float* next_pts, int n, int max_level, int use_initial_flow,
-                uint8_t* status);
+                uint8_t* status, int roles);
 /* cv::goodFeaturesToTrack(img, max_corners, 0.01, min_dist, mask) where mask = 255 everywhere except
  * the integer disks d^2 <= min_dist^2 around cvRound(kept_pts[i]) (setMask, feature_tracker.cpp:56-83).
  * Returns the corners in OpenCV's output order. */

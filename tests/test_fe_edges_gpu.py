@@ -3,8 +3,8 @@
 test_fe_gpu.py checks the front end mostly at 640x480 with small motion, where every pyramid level is at least 80 px wide
 and the LK windows are staged by 2-D TMA.  This module covers the other geometries and code paths, bit-exact against
 cv2 4.13 (stage entry points) or oracle/fe_oracle.py (tracker):
-  - LK with the TMA staging on and off (GF_LK_NO_TMA, and images below 640 px wide, where it is off for the whole
-    tracker), widths that are not multiples of 16, portrait images, 1080p, large motion that restages the search window,
+  - LK in both of its forms (two warp roles, a tracker alone on its device; single role, several trackers) with the TMA
+    staging on and off (GF_LK_NO_TMA, and images below 640 px wide, where it is off for the whole tracker), widths that are not multiples of 16, portrait images, 1080p, large motion that restages the search window,
     windows on the image border at every level, flat and clipped textures, initial flow far from the truth;
   - cornerMinEigenVal at widths that are not multiples of 32;
   - goodFeaturesToTrack with more than 65536 candidates, a grown min-distance cell and an overflowing mask tile;
@@ -21,7 +21,7 @@ import numpy as np
 import pytest
 
 from conftest import make_texture_image, warp_image
-from test_fe_gpu import _padded, _run_sequence, lk_staging  # noqa: F401 (fixture)
+from test_fe_gpu import _padded, _run_sequence, lk_form, lk_staging  # noqa: F401 (fixtures)
 
 pytestmark = pytest.mark.gpu
 cv2 = pytest.importorskip("cv2")
@@ -75,20 +75,21 @@ def max_tile_apron(kept, w, h, r):
     return best
 
 
-def check_lk(gf, a, b, pts, max_level, init=None):
-    """gf_stage_lk against cv2.calcOpticalFlowPyrLK, bit for bit; returns cv2's (points, status)."""
+def check_lk(gf, a, b, pts, max_level, form, init=None):
+    """gf_stage_lk in the LK form `form` (the lk_form fixture's value) against cv2.calcOpticalFlowPyrLK, bit for bit; returns
+    cv2's (points, status)."""
     pts = np.ascontiguousarray(pts, np.float32).reshape(-1, 2)
     nxt = None if init is None else np.ascontiguousarray(init, np.float32).reshape(-1, 1, 2).copy()
     flags = 0 if init is None else cv2.OPTFLOW_USE_INITIAL_FLOW
     q_cv, st_cv, _ = cv2.calcOpticalFlowPyrLK(a, b, pts.reshape(-1, 1, 2), nxt, winSize=(21, 21), maxLevel=max_level,
                                               criteria=CRIT, flags=flags)
     q_cv, st_cv = q_cv.reshape(-1, 2), st_cv.ravel()
-    q, st = gf.calc_optical_flow_pyr_lk(a, b, pts, max_level, init=init)
+    q, st = gf.calc_optical_flow_pyr_lk(a, b, pts, max_level, init=init, roles=form == "two-role")
     bad = np.flatnonzero((st != st_cv) | np.any(bits(q) != bits(q_cv), 1))
     if len(bad):
         i = bad[0]
-        pytest.fail("%d of %d points differ; first: p=%r gpu %r/%d cv2 %r/%d" % (len(bad), len(pts), tuple(pts[i]), tuple(q[i]),
-                                                                               st[i], tuple(q_cv[i]), st_cv[i]))
+        pytest.fail("%s: %d of %d points differ; first: p=%r gpu %r/%d cv2 %r/%d" % (form, len(bad), len(pts), tuple(pts[i]),
+                                                                                   tuple(q[i]), st[i], tuple(q_cv[i]), st_cv[i]))
     return q_cv, st_cv
 
 
@@ -117,7 +118,7 @@ def boundary_points(w, h, max_level):
 # ---- A. LK ------------------------------------------------------------------------------------------------------------
 
 @pytest.mark.parametrize("w,h", LK_SHAPES)
-def test_lk_geometries_and_border_windows(gf, lk_staging, w, h):
+def test_lk_geometries_and_border_windows(gf, lk_form, lk_staging, w, h):
     """Every accepted max_level at each shape, TMA staging on and off: random points (some just outside the image) and the
     constructed border points of every level, small motion with rotation."""
     if (w, h) == (424, 400):
@@ -131,7 +132,7 @@ def test_lk_geometries_and_border_windows(gf, lk_staging, w, h):
     assert levels == [0, 1, 2, 3]
     for m in levels:
         pts = np.concatenate([rand, boundary_points(w, h, m)])
-        check_lk(gf, a, b, pts, m)
+        check_lk(gf, a, b, pts, m, lk_form)
 
 
 def _lk_iterates(a, b, pts):
@@ -182,7 +183,7 @@ def _band_points(rng, w, h, n):
 @pytest.mark.parametrize("w,h", [(640, 480), (641, 481), (424, 400), (1280, 720)])
 @pytest.mark.parametrize("max_level,dx,dy,ang", [(0, 13.4, -12.2, 0.0), (0, 24.7, 18.1, 1.0), (1, 29.3, -21.6, 1.5),
                                                  (3, 47.5, 31.2, 2.0), (3, -86.3, 44.9, -4.0)])
-def test_lk_large_motion(gf, lk_staging, w, h, max_level, dx, dy, ang):
+def test_lk_large_motion(gf, lk_form, lk_staging, w, h, max_level, dx, dy, ang):
     """Shifts of 12-30 px at max_level 0 and 1, 40-90 px with rotation at max_level 3: the search window is restaged during
     the iterations, from the interior onto the border among others.  A coarser texture widens the basin of convergence."""
     seed = 7 * w + max_level
@@ -191,7 +192,7 @@ def test_lk_large_motion(gf, lk_staging, w, h, max_level, dx, dy, ang):
     rng = np.random.default_rng(seed)
     pts = np.concatenate([np.stack([rng.uniform(0, w, 400), rng.uniform(0, h, 400)], 1).astype(np.float32),
                           _band_points(rng, w, h, 200)])
-    check_lk(gf, a, b, pts, max_level)
+    check_lk(gf, a, b, pts, max_level, lk_form)
     if max_level == 0:
         restaged, to_border = restaged_windows(a, b, pts)
         assert restaged.sum() >= 50, "only %d points restage their search window" % restaged.sum()
@@ -216,7 +217,7 @@ def _constant_windows(img, pts, max_level):
 
 
 @pytest.mark.parametrize("w,h", [(640, 480), (641, 481), (424, 400)])
-def test_lk_flat_and_clipped_texture(gf, lk_staging, w, h):
+def test_lk_flat_and_clipped_texture(gf, lk_form, lk_staging, w, h):
     """A tone curve clips a coarse texture to 0 and 255 over large areas, and a block is constant at 7: the minimum-eigenvalue
     rejection fires at coarse levels (the point continues with twice the guess) and at level 0 (status 0)."""
     t = make_texture_image(w + 3 * h, w, h, sigma=8.0, contrast=1.0).astype(np.float32)
@@ -227,7 +228,7 @@ def test_lk_flat_and_clipped_texture(gf, lk_staging, w, h):
     pts = np.concatenate([np.stack([rng.uniform(0, w, 500), rng.uniform(0, h, 500)], 1),
                           np.stack([rng.uniform(w // 4, w // 4 + 200, 60), rng.uniform(h // 3, h // 3 + 200, 60)], 1)]).astype(np.float32)
     for m in lk_levels(w, h):
-        _, st = check_lk(gf, a, b, pts, m)
+        _, st = check_lk(gf, a, b, pts, m, lk_form)
         flat = _constant_windows(a, pts, m)
         assert np.any(flat[:, 0] & (st == 0)), "no level-0 rejection"
         if m > 0:
@@ -236,13 +237,13 @@ def test_lk_flat_and_clipped_texture(gf, lk_staging, w, h):
 
 @pytest.mark.parametrize("w,h", [(641, 481), (480, 640)])
 @pytest.mark.parametrize("max_level", [1, 3])
-def test_lk_initial_flow_far_from_truth(gf, lk_staging, w, h, max_level):
+def test_lk_initial_flow_far_from_truth(gf, lk_form, lk_staging, w, h, max_level):
     a = make_texture_image(w + 2 * h, w, h, sigma=4.0, contrast=1.5)
     b = warp_image(a, 2.2, -1.6, 0.3)
     rng = np.random.default_rng(h)
     pts = np.stack([rng.uniform(-5, w + 5, 500), rng.uniform(-5, h + 5, 500)], 1).astype(np.float32)
     init = pts + np.stack([rng.uniform(-14, 14, 500), rng.uniform(-14, 14, 500)], 1).astype(np.float32)
-    check_lk(gf, a, b, pts, max_level, init=init)
+    check_lk(gf, a, b, pts, max_level, lk_form, init=init)
 
 
 # ---- B. cornerMinEigenVal and goodFeaturesToTrack ---------------------------------------------------------------------
@@ -315,41 +316,41 @@ def test_gftt_dense_kept_overflows_mask_tile(gf, w, h):
 
 # ---- C. tracker sequences ---------------------------------------------------------------------------------------------
 
-def test_track_sequence_424x400_without_tma(gf):
+def test_track_sequence_424x400_without_tma(gf, lk_form):
     assert level_sizes(424, 400)[3][0] < 80 and not lk_tma_on(424, 400, 3)
-    _run_sequence(gf, seed=3, n_frames=20, w=424, h=400, max_cnt=150, min_dist=20)
+    _run_sequence(gf, seed=3, n_frames=20, w=424, h=400, max_cnt=150, min_dist=20, form=lk_form)
 
 
-def test_track_sequence_641x481_padded_rows(gf):
-    _run_sequence(gf, seed=4, n_frames=20, w=641, h=481, max_cnt=200, min_dist=25, pad=23)
+def test_track_sequence_641x481_padded_rows(gf, lk_form):
+    _run_sequence(gf, seed=4, n_frames=20, w=641, h=481, max_cnt=200, min_dist=25, pad=23, form=lk_form)
 
 
-def test_track_sequence_480x640_portrait(gf):
+def test_track_sequence_480x640_portrait(gf, lk_form):
     """The reference reads the saturation test as at<uchar>((int)x, (int)y): row x, column y.  In a portrait image that read
     is in bounds for every point with x < 640 and y < 480, i.e. most of them.  The camera is IDC_CAM turned by 90 degrees
     (the landscape intrinsics would put the bottom rows where the radial model diverges)."""
     from oracle.fe_oracle import IDC_CAM as C, PinholeCamera
     cam = PinholeCamera(C["fy"], C["fx"], C["cy"], C["cx"], C["k1"], C["k2"], C["p2"], C["p1"])
     seen = []
-    _run_sequence(gf, seed=5, n_frames=20, w=480, h=640, max_cnt=150, min_dist=25, cam=cam,
+    _run_sequence(gf, seed=5, n_frames=20, w=480, h=640, max_cnt=150, min_dist=25, cam=cam, form=lk_form,
                   on_frame=lambda k, g, ref, got: seen.append(int(((got["v"][:, 3] < 640) & (got["v"][:, 4] < 480)).sum())))
     assert sum(seen) > 1000
 
 
-def test_track_sequence_752x480(gf):
-    _run_sequence(gf, seed=6, n_frames=20, w=752, h=480, max_cnt=150, min_dist=30)
+def test_track_sequence_752x480(gf, lk_form):
+    _run_sequence(gf, seed=6, n_frames=20, w=752, h=480, max_cnt=150, min_dist=30, form=lk_form)
 
 
-def test_track_sequence_1080p_gftt_slow_paths(gf):
+def test_track_sequence_1080p_gftt_slow_paths(gf, lk_form):
     """150 features at 1920x1080, min_dist 20: more than 65536 candidates and a grown cell grid inside the tracker."""
     assert nms_cell_size(1920, 1080, 20) > 20
     cands = []
-    _run_sequence(gf, seed=7, n_frames=10, w=1920, h=1080, max_cnt=150, min_dist=20,
+    _run_sequence(gf, seed=7, n_frames=10, w=1920, h=1080, max_cnt=150, min_dist=20, form=lk_form,
                   on_frame=lambda k, g, ref, got: cands.append(g.last_info["n_candidates"]))
     assert max(cands) > 65536, cands
 
 
-def test_track_sequence_dense_1000_features(gf):
+def test_track_sequence_dense_1000_features(gf, lk_form):
     """max_cnt 1000 at min_dist 5: setMask's std::sort replay and the disk tests near capacity."""
     aprons = []
 
@@ -358,7 +359,7 @@ def test_track_sequence_dense_1000_features(gf):
         aprons.append(max_tile_apron(ref.prev_pts[:nk], 640, 480, 5) if nk else 0)
         assert len(got) > 900
 
-    _run_sequence(gf, seed=8, n_frames=12, max_cnt=1000, min_dist=5, on_frame=on_frame)
+    _run_sequence(gf, seed=8, n_frames=12, max_cnt=1000, min_dist=5, on_frame=on_frame, form=lk_form)
     assert max(aprons) > 8
 
 

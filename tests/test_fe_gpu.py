@@ -3,6 +3,10 @@
 Every test calls the CUDA path through the C ABI (libgf_b200.so) and compares with the oracle:
 cv2 4.13.0 for the three OpenCV calls the reference makes (feature_tracker.cpp:118-153,198) and
 oracle/fe_oracle.py for FeatureTracker::trackImage as a whole.  Bar: bit-exact.
+
+LK runs in two forms that must give the same bits (DESIGN.md §1.3): two warp roles (fe_lk.cuh) while a tracker is alone on
+its device, a single role (fe_lk_single.cuh) while other trackers are live.  The lk_form fixture runs a test in each, and
+every tracker sequence asserts, from the tracker's debug slots, that each feature ran the form it expects.
 """
 import numpy as np
 import pytest
@@ -45,36 +49,38 @@ def test_min_eig_flat_and_saturated(gf):
 
 @pytest.mark.parametrize("seed,contrast", [(0, 1.0), (1, 2.5), (2, 1.7)])
 @pytest.mark.parametrize("max_level", [3, 1, 0])
-def test_lk_matches_cv2_bit_exact(gf, seed, contrast, max_level):
+def test_lk_matches_cv2_bit_exact(gf, lk_form, lk_staging, seed, contrast, max_level):
     a = make_texture_image(seed, contrast=contrast)
     b = warp_image(a, 3.3 + seed, -2.1, 0.7)
     rng = np.random.default_rng(100 + seed)
     pts = np.stack([rng.uniform(-5, 645, 500), rng.uniform(-5, 485, 500)], 1).astype(np.float32)
     q_cv, st_cv, _ = cv2.calcOpticalFlowPyrLK(a, b, pts.reshape(-1, 1, 2), None, winSize=(21, 21), maxLevel=max_level)
-    q, st = gf.calc_optical_flow_pyr_lk(a, b, pts, max_level)
+    q, st = gf.calc_optical_flow_pyr_lk(a, b, pts, max_level, roles=lk_form == "two-role")
     assert np.array_equal(st, st_cv.ravel())
     assert np.array_equal(bits(q), bits(q_cv.reshape(-1, 2)))
 
 
-def test_lk_initial_flow_reverse_pass(gf):
+def test_lk_initial_flow_reverse_pass(gf, lk_form, lk_staging):
     a = make_texture_image(5, contrast=1.5)
     b = warp_image(a, -2.6, 1.4, -0.4)
     rng = np.random.default_rng(7)
     pts = np.stack([rng.uniform(0, 640, 300), rng.uniform(0, 480, 300)], 1).astype(np.float32)
-    fwd, _ = gf.calc_optical_flow_pyr_lk(a, b, pts, 3)
+    roles = lk_form == "two-role"
+    fwd, _ = gf.calc_optical_flow_pyr_lk(a, b, pts, 3, roles=roles)
     crit = (cv2.TERM_CRITERIA_COUNT + cv2.TERM_CRITERIA_EPS, 30, 0.01)
     r_cv, st_cv, _ = cv2.calcOpticalFlowPyrLK(b, a, fwd.reshape(-1, 1, 2), pts.reshape(-1, 1, 2).copy(), winSize=(21, 21),
                                               maxLevel=1, criteria=crit, flags=cv2.OPTFLOW_USE_INITIAL_FLOW)
-    r, st = gf.calc_optical_flow_pyr_lk(b, a, fwd, 1, init=pts)
+    r, st = gf.calc_optical_flow_pyr_lk(b, a, fwd, 1, init=pts, roles=roles)
     assert np.array_equal(st, st_cv.ravel())
     assert np.array_equal(bits(r), bits(r_cv.reshape(-1, 2)))
 
 
-def test_lk_empty_and_single(gf):
+def test_lk_empty_and_single(gf, lk_form, lk_staging):
     a = make_texture_image(0)
-    q, st = gf.calc_optical_flow_pyr_lk(a, a, np.zeros((0, 2), np.float32), 3)
+    roles = lk_form == "two-role"
+    q, st = gf.calc_optical_flow_pyr_lk(a, a, np.zeros((0, 2), np.float32), 3, roles=roles)
     assert q.shape == (0, 2) and st.shape == (0,)
-    q, st = gf.calc_optical_flow_pyr_lk(a, a, np.array([[320.5, 240.25]], np.float32), 3)
+    q, st = gf.calc_optical_flow_pyr_lk(a, a, np.array([[320.5, 240.25]], np.float32), 3, roles=roles)
     q_cv, st_cv, _ = cv2.calcOpticalFlowPyrLK(a, a, np.array([[[320.5, 240.25]]], np.float32), None, winSize=(21, 21), maxLevel=3)
     assert np.array_equal(bits(q), bits(q_cv.reshape(-1, 2))) and st[0] == st_cv[0, 0]
 
@@ -115,6 +121,55 @@ def lk_staging(request, monkeypatch):
     return request.param
 
 
+LK_FORM_CODE = {"two-role": 2, "single-role": 1}       # gf_tracker_debug_read's [64 + 8*i + 4]
+
+
+@pytest.fixture(params=["two-role", "single-role"])
+def lk_form(request, gf):
+    """The LK form a test runs.  A tracker takes the two-role form while it is the only live tracker on its device and the
+    single-role form otherwise, so "single-role" keeps a small companion tracker open for the test, and "two-role" first
+    collects trackers that earlier tests left unreferenced.  Stage-level tests pass the form to gf_stage_lk instead."""
+    import gc
+    companion = None
+    if request.param == "single-role":
+        from ground_fusion_b200.synth import idc_params8
+        companion = gf.FeatureTracker(640, 480, idc_params8(), 10, 30, 1, 1)
+    else:
+        gc.collect()
+    yield request.param
+    if companion is not None:
+        companion.close()
+
+
+def lk_debug(gpu):
+    """Per-feature LK rows of the tracker's last frame (gf_tracker_debug_read [64 + 8*i + k]): k = 0 cycles, 1 iterations,
+    2 of them with b from the integer partials, 3 from the sequential chains, 4 the LK form (LK_FORM_CODE)."""
+    import ctypes
+    from ground_fusion_b200._lib import check
+    n = gpu.last_info["n_prev"]
+    buf = (ctypes.c_longlong * (64 + 8 * n))()
+    check(gpu.L.gf_tracker_debug_read(gpu._h, buf, len(buf)))
+    return np.array(buf[64:], np.int64).reshape(n, 8)
+
+
+def check_form(k, gpu, form):
+    """Every feature of the tracker's last frame ran k_track in `form`."""
+    ran = lk_debug(gpu)[:, 4]
+    hint = "is a tracker of an earlier test still alive?" if form == "two-role" else "is no other tracker alive?"
+    assert (ran == LK_FORM_CODE[form]).all(), "frame %d: %d of %d features did not run the %s LK form (%s)" % (
+        k, int((ran != LK_FORM_CODE[form]).sum()), len(ran), form, hint)
+
+
+def check_oracle(k, gpu, got, ref, want):
+    """Frame k of gpu (trackImageRaw's result got) equals the oracle's (ref after trackImage returned want), bit for bit."""
+    assert np.array_equal(gpu.last_status, ref.last_status), "frame %d: inlier mask differs" % k
+    assert list(got["id"]) == list(ref.ids), "frame %d: feature ids / order differ" % k
+    assert list(got["track_cnt"]) == list(ref.track_cnt), "frame %d" % k
+    for o in got:
+        assert np.array_equal(o["v"], want[int(o["id"])]), "frame %d id %d: %s vs %s" % (k, o["id"], o["v"], want[int(o["id"])])
+    assert gpu.last_info["n_new"] == len(ref.last_n_pts)
+
+
 def _padded(a, pad):
     """a as a view into a buffer `pad` elements wider per row; the padding holds the largest value of the type."""
     buf = np.full((a.shape[0], a.shape[1] + pad), np.iinfo(a.dtype).max, a.dtype)
@@ -122,9 +177,11 @@ def _padded(a, pad):
     return buf[:, :a.shape[1]]
 
 
-def _run_sequence(gf, seed, n_frames, w=640, h=480, max_cnt=150, min_dist=30, noise=1.0, pad=0, on_frame=None, cam=None):
+def _run_sequence(gf, seed, n_frames, w=640, h=480, max_cnt=150, min_dist=30, noise=1.0, pad=0, on_frame=None, cam=None,
+                  form="two-role"):
     """trackImage against the oracle frame by frame.  cam: the PinholeCamera (default: IDC_CAM scaled by w / 640).
-    pad > 0: gray and depth are passed as views into wider rows (row pitch > width).  on_frame(k, gpu, ref, got) runs
+    pad > 0: gray and depth are passed as views into wider rows (row pitch > width).  form: the LK form every feature must
+    report (the lk_form fixture's value; "two-role" means no other tracker may be live).  on_frame(k, gpu, ref, got) runs
     after the checks of frame k."""
     from ground_fusion_b200.synth import SyntheticStream
     from oracle.fe_oracle import IDC_CAM, FeatureTrackerOracle, PinholeCamera
@@ -142,28 +199,24 @@ def _run_sequence(gf, seed, n_frames, w=640, h=480, max_cnt=150, min_dist=30, no
             assert gray.strides[0] > w and depth.strides[0] > 2 * w
         got = gpu.trackImageRaw(t, gray, depth)
         want = ref.trackImage(t, gray, depth)
-        assert np.array_equal(gpu.last_status, ref.last_status), "frame %d: inlier mask differs" % k
-        assert list(got["id"]) == list(ref.ids), "frame %d: feature ids / order differ" % k
-        assert list(got["track_cnt"]) == list(ref.track_cnt), "frame %d" % k
-        for o in got:
-            assert np.array_equal(o["v"], want[int(o["id"])]), "frame %d id %d: %s vs %s" % (k, o["id"], o["v"], want[int(o["id"])])
-        assert gpu.last_info["n_new"] == len(ref.last_n_pts)
+        check_oracle(k, gpu, got, ref, want)
+        check_form(k, gpu, form)
         if on_frame:
             on_frame(k, gpu, ref, got)
     gpu.close()
 
 
-def test_track_sequence_c2_bit_exact(gf):
+def test_track_sequence_c2_bit_exact(gf, lk_form):
     """BASELINE config C2: 640x480, 150 features, min_dist 30."""
-    _run_sequence(gf, seed=0, n_frames=60)
+    _run_sequence(gf, seed=0, n_frames=60, form=lk_form)
 
 
-def test_track_sequence_c3_300_features(gf):
-    _run_sequence(gf, seed=1, n_frames=30, max_cnt=300, min_dist=20)
+def test_track_sequence_c3_300_features(gf, lk_form):
+    _run_sequence(gf, seed=1, n_frames=30, max_cnt=300, min_dist=20, form=lk_form)
 
 
-def test_track_sequence_c4_720p_500_features(gf):
-    _run_sequence(gf, seed=2, n_frames=12, w=1280, h=720, max_cnt=500, min_dist=25)
+def test_track_sequence_c4_720p_500_features(gf, lk_form):
+    _run_sequence(gf, seed=2, n_frames=12, w=1280, h=720, max_cnt=500, min_dist=25, form=lk_form)
 
 
 def test_two_frames_in_flight_equals_blocking_calls(gf):
@@ -264,7 +317,9 @@ def test_track_no_depth_image_quirk(gf):
     tr.close()
 
 
-def test_prediction_and_remove_outliers(gf):
+def test_prediction_and_remove_outliers(gf, lk_form):
+    """setPrediction (k_lk_pred, then k_track reusing its points; at frame 9 too few succeed and k_track runs the 3-level
+    pass) and removeOutliers, in each LK form."""
     from ground_fusion_b200.synth import SyntheticStream
     from oracle.fe_oracle import IDC_CAM, FeatureTrackerOracle, PinholeCamera
     cam = PinholeCamera(**IDC_CAM)
@@ -280,6 +335,7 @@ def test_prediction_and_remove_outliers(gf):
         assert np.array_equal(gpu.last_status, ref.last_status), "frame %d" % k
         for o in got:
             assert np.array_equal(o["v"], want[int(o["id"])])
+        check_form(k, gpu, lk_form)
         if k in (3, 6):      # feed back "BA" predictions: true ray * depth, slightly perturbed, for 2/3 of the ids
             pred = {}
             for o in got[::3] if k == 3 else got[: len(got) * 2 // 3]:

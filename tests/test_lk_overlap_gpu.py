@@ -1,23 +1,22 @@
-"""GPU tests of the paths the two LK warp roles add (run with -m gpu on an H100).
+"""GPU tests of LK's level-by-level edge cases (run with -m gpu on an H100).
 
-In k_track and the LK stage entry, consumer warps iterate pyramid level l while producer warps build level l-1
-(fe_lk.cuh).  These tests drive the hand-over between the roles through each of its cases, with the TMA staging on and
-off (GF_LK_NO_TMA), bit-exact against cv2.calcOpticalFlowPyrLK (stage entry) or oracle/fe_oracle.py (tracker):
+Each test runs in both LK forms (DESIGN.md §1.3) with the TMA staging on and off (GF_LK_NO_TMA), bit-exact against
+cv2.calcOpticalFlowPyrLK (stage entry) or oracle/fe_oracle.py (tracker).  In the two-role form (fe_lk.cuh) consumer warps
+iterate pyramid level l while producer warps build level l-1, and these cases drive the hand-over between the roles; the
+single-role form (fe_lk_single.cuh) sets up and iterates each level with all warps, and they are its level edge cases too:
   - coarse levels rejected by minEig above a valid finest level;
-  - levels that converge in one iteration, so the consumers wait for the producers at every level;
-  - the sequential-chain fallback on a coarse level, while the producers build the next one;
-  - max_level 0, where there is nothing to overlap.
+  - levels that converge in one iteration (in the two-role form the consumers wait for the producers at every level);
+  - the sequential-chain fallback on a coarse level;
+  - max_level 0, a single level.
 The host recomputes, exactly in integers, what each test needs its input to reach, and asserts it.
 """
-import ctypes
-
 import cv2
 import numpy as np
 import pytest
 
 from conftest import make_texture_image, warp_image
 from test_fe_edges_gpu import boundary_points, check_lk
-from test_fe_gpu import _run_sequence, lk_staging  # noqa: F401 (fixture)
+from test_fe_gpu import _run_sequence, lk_debug, lk_form, lk_staging  # noqa: F401 (fixtures)
 
 pytestmark = pytest.mark.gpu
 
@@ -68,7 +67,7 @@ def b_chains_exact(gx, gy, d):
     return True
 
 
-def test_coarse_levels_rejected_by_min_eig(gf, lk_staging):
+def test_coarse_levels_rejected_by_min_eig(gf, lk_form, lk_staging):
     """A texture of 2 x 2 px cells: pyrDown turns it into a one-pixel alternation at level 1, whose Scharr derivatives
     are all 0, and into near-flat grey above.  Levels 3..1 are built as rejected, level 0 is tracked."""
     yy, xx = np.mgrid[0:H, 0:W]
@@ -82,11 +81,11 @@ def test_coarse_levels_rejected_by_min_eig(gf, lk_staging):
             gx, gy, _ = window_terms(PI[l], PJ[l], x >> l, y >> l)
             me, _ = min_eig(gx, gy)
             assert (me > 2e-4) if l == 0 else (me < 5e-5), (x, y, l, me)
-    _, st = check_lk(gf, a, b, pts, 3)
+    _, st = check_lk(gf, a, b, pts, 3, lk_form)
     assert st.all()
 
 
-def test_levels_converging_in_one_iteration(gf, lk_staging):
+def test_levels_converging_in_one_iteration(gf, lk_form, lk_staging):
     """Identical images: every mismatch is 0, so each level stops after its first iteration.  The intent is a consumer
     level far shorter than the producers' build of the next one, so that the consumers wait at the hand-over; that timing
     is not observable here, only that one iteration per level gives cv2's result bit for bit."""
@@ -94,15 +93,15 @@ def test_levels_converging_in_one_iteration(gf, lk_staging):
     rng = np.random.default_rng(11)
     pts = np.stack([rng.uniform(40, W - 40, 300), rng.uniform(40, H - 40, 300)], 1).astype(np.float32)
     for m in (3, 1):
-        q_cv, st_cv = check_lk(gf, a, a.copy(), pts, m)
+        q_cv, st_cv = check_lk(gf, a, a.copy(), pts, m, lk_form)
         one, _, _ = cv2.calcOpticalFlowPyrLK(a, a.copy(), pts.reshape(-1, 1, 2), None, winSize=(21, 21), maxLevel=m,
                                              criteria=(cv2.TERM_CRITERIA_COUNT, 1, 0.0))
         assert st_cv.all() and np.array_equal(one.reshape(-1, 2), q_cv)     # one iteration per level gives the result
 
 
-def test_chain_fallback_on_a_coarse_level(gf, lk_staging):
+def test_chain_fallback_on_a_coarse_level(gf, lk_form, lk_staging):
     """A clipped, high-contrast texture under a shift: the first iteration at level 3 exceeds the integer bound of some
-    b chain and runs OpenCV's sequential chains, while the producers build level 2."""
+    b chain and runs OpenCV's sequential chains (in the two-role form while the producers build level 2)."""
     a = make_texture_image(5, W, H, contrast=5.0)
     b = warp_image(a, 6.0, -5.0, 1.0)
     PI, PJ = pyramid(a), pyramid(b)
@@ -114,34 +113,30 @@ def test_chain_fallback_on_a_coarse_level(gf, lk_staging):
         if me > 2e-4 and det > 1e-6 and not b_chains_exact(gx, gy, d):
             pts.append((x, y))
     assert len(pts) >= 200, len(pts)
-    check_lk(gf, a, b, np.array(pts[::4], np.float32), 3)
+    check_lk(gf, a, b, np.array(pts[::4], np.float32), 3, lk_form)
 
 
-def test_max_level_0(gf, lk_staging):
-    """One level: the producers build it, the consumers iterate it, no level overlaps another."""
+def test_max_level_0(gf, lk_form, lk_staging):
+    """One level: no level overlaps another (in the two-role form the producers build it, the consumers iterate it)."""
     a = make_texture_image(21, W, H, contrast=1.5)
     b = warp_image(a, 2.2, 1.7, 0.5)
     rng = np.random.default_rng(21)
     rand = np.stack([rng.uniform(-5, W + 5, 300), rng.uniform(-5, H + 5, 300)], 1).astype(np.float32)
-    check_lk(gf, a, b, np.concatenate([rand, boundary_points(W, H, 0)]), 0)
+    check_lk(gf, a, b, np.concatenate([rand, boundary_points(W, H, 0)]), 0, lk_form)
 
 
-def test_tracker_chain_fallbacks_bit_exact(gf, monkeypatch, lk_staging):
+def test_tracker_chain_fallbacks_bit_exact(gf, monkeypatch, lk_form, lk_staging):
     """k_track on the clipped high-contrast stream: both b paths run on every pass (forward levels 3..0, reverse 1..0)
     and the tracks match the oracle."""
     from ground_fusion_b200 import synth
-    from ground_fusion_b200._lib import check
     make_texture = synth.make_texture
     monkeypatch.setattr(synth, "make_texture", lambda seed: make_texture(seed, contrast=300.0))
     totals = np.zeros(2, np.int64)
 
     def on_frame(k, gpu, ref, got):
-        n = gpu.last_info["n_prev"]
-        buf = (ctypes.c_longlong * (64 + 8 * n))()
-        check(gpu.L.gf_tracker_debug_read(gpu._h, buf, len(buf)))
-        per = np.array(buf[64:], np.int64).reshape(n, 8)
+        per = lk_debug(gpu)
         assert np.array_equal(per[:, 2] + per[:, 3], per[:, 1]), "frame %d" % k
         totals[:] += per[:, 2:4].sum(0)
 
-    _run_sequence(gf, seed=4, n_frames=10, on_frame=on_frame)
+    _run_sequence(gf, seed=4, n_frames=10, on_frame=on_frame, form=lk_form)
     assert totals[0] > 0 and totals[1] > 0, totals
