@@ -15,6 +15,7 @@
 //   harness fm-bench <in> <out>  host time per frame of the FeatureManager stage from C++ alone: the calls one processImage makes
 //                           around the solve, once over a std::list on the host with the stateless gf_fm_* calls and once over
 //                           gf_fm_window, alternating; <out> is one JSON object (tools/bench_fm_window.py reads it)
+//   harness fm-group-bench <in> <out>  the same stage for K windows: through gf_fm_window_group, K windows in sequence, K threads
 #include <algorithm>
 #include <array>
 #include <chrono>
@@ -26,6 +27,7 @@
 #include <map>
 #include <memory>
 #include <set>
+#include <thread>
 #include <vector>
 
 #include "dense_map.h"
@@ -553,14 +555,152 @@ static int run_fm_bench(const char *in, const char *out)
     return 0;
 }
 
+// ---- fm-group-bench: the same stage for K windows, through gf_fm_window_group, K windows in sequence, or K threads ----
+namespace fmg {
+using namespace fmb;
+enum Arm { GROUP, SEQUENTIAL, THREADS };
+
+// the stage of one frame on window w alone, as fmb::pass runs it on the resident table
+static void single_frame(gf_fm_window *w, const std::vector<gf_obs> &obs, int fc, size_t k, const Poses &p, std::vector<gf_ba_visual_factor> &rows,
+                         std::vector<double> &para, std::vector<uint8_t> &cst, std::vector<int32_t> &ids, std::vector<double> &xyz)
+{
+    int margin = 0, nf = 0, nv = 0, n = 0; int32_t c4[4]; double par;
+    ok(gf_fm_window_add_frame(w, fc, obs.data(), (int)obs.size(), nullptr, 0.0, &margin, c4, &par), "add_frame");
+    if (fc < W) return;
+    ok(gf_fm_window_triangulate(w, fc, p.P, p.R, p.tic, p.ric), "triangulate");
+    ok(gf_fm_window_fill_problem(w, rows.data(), (int)rows.size(), &nv, para.data(), cst.data(), &nf), "fill_problem");
+    ok(gf_fm_window_set_depth(w, para.data(), nf), "set_depth");
+    ok(gf_fm_window_outliers(w, p.P, p.R, p.tic, p.ric, GF_FM_OUTLIERS_MOVING, ids.data(), &n), "outliers");
+    std::vector<int32_t> bad(ids.begin(), ids.begin() + n);
+    std::sort(bad.begin(), bad.end());
+    if (bad.size() > 3) bad.resize(3);
+    ok(gf_fm_window_remove_ids(w, bad.data(), (int)bad.size()), "remove_ids");
+    ok(gf_fm_window_predict_next(w, fc, p.P, p.R, p.tic, p.ric, ids.data(), xyz.data(), &n), "predict_next");
+    if (margin || k % 3 == 0) ok(gf_fm_window_remove_back_shift_depth(w, p.R, p.P, p.R + 9, p.P + 3), "remove_back_shift_depth");
+    else ok(gf_fm_window_remove_front(w, fc), "remove_front");
+    ok(gf_fm_window_remove_failures(w), "remove_failures");
+    ok(gf_fm_window_size(w, &n), "size");                           // the frame's work has finished on the device
+}
+
+struct Buf {
+    std::vector<gf_ba_visual_factor> rows; std::vector<double> para, xyz; std::vector<uint8_t> cst; std::vector<int32_t> ids;
+    explicit Buf(int cap) : rows((size_t)cap * 10), para(cap), xyz(3 * (size_t)cap), cst(cap), ids(cap) {}
+};
+
+// one pass of the stream on K windows; returns microseconds of host time per round (one frame of every window)
+static double pass_k(Arm arm, const std::vector<std::vector<gf_obs>> &frames, const Poses &p, std::vector<gf_fm_window *> &w, gf_fm_window_group *g,
+                     std::vector<Buf> &b, int cap)
+{
+    const int K = (int)w.size();
+    for (auto *x : w) ok(gf_fm_window_clear(x), "clear");
+    for (auto *x : w) { int n; ok(gf_fm_window_size(x, &n), "size"); }
+    const auto t0 = clk::now();
+    if (arm == THREADS) {
+        std::vector<std::thread> th;
+        for (int i = 0; i < K; i++)
+            th.emplace_back([&, i] { for (size_t k = 0; k < frames.size(); k++) single_frame(w[i], frames[k], (int)std::min<size_t>(k, W), k, p, b[i].rows, b[i].para, b[i].cst, b[i].ids, b[i].xyz); });
+        for (auto &t : th) t.join();
+        return us(t0, clk::now()) / frames.size();
+    }
+    std::vector<int32_t> fcs(K), ops(K), start(K + 1), nv(K), nf(K), n(K), c4(4 * K), margin(K), caps(K, cap * 10), ids, id_start(K + 1);
+    std::vector<double> tds(K, 0.0), par(K), shift(24 * (size_t)K), Ps(33 * (size_t)K), Rs(99 * (size_t)K), tic(3 * (size_t)K), ric(9 * (size_t)K);
+    std::vector<gf_obs> all;
+    std::vector<gf_ba_visual_factor *> vo(K); std::vector<double *> pf(K), xyz(K); std::vector<uint8_t *> cs(K); std::vector<int32_t *> io(K);
+    std::vector<const double *> x(K);
+    for (int i = 0; i < K; i++) {
+        vo[i] = b[i].rows.data(); pf[i] = b[i].para.data(); cs[i] = b[i].cst.data(); io[i] = b[i].ids.data(); xyz[i] = b[i].xyz.data(); x[i] = b[i].para.data();
+        std::copy(p.P, p.P + 33, &Ps[33 * i]); std::copy(p.R, p.R + 99, &Rs[99 * i]); std::copy(p.tic, p.tic + 3, &tic[3 * i]); std::copy(p.ric, p.ric + 9, &ric[9 * i]);
+        std::copy(p.R, p.R + 9, &shift[24 * i]); std::copy(p.P, p.P + 3, &shift[24 * i + 9]); std::copy(p.R + 9, p.R + 18, &shift[24 * i + 12]); std::copy(p.P + 3, p.P + 6, &shift[24 * i + 21]);
+    }
+    for (size_t k = 0; k < frames.size(); k++) {
+        const int fc = (int)std::min<size_t>(k, W);
+        if (arm == SEQUENTIAL) {
+            for (int i = 0; i < K; i++) single_frame(w[i], frames[k], fc, k, p, b[i].rows, b[i].para, b[i].cst, b[i].ids, b[i].xyz);
+            continue;
+        }
+        all.clear();
+        for (int i = 0; i < K; i++) { start[i] = (int)all.size(); all.insert(all.end(), frames[k].begin(), frames[k].end()); fcs[i] = fc; }
+        start[K] = (int)all.size();
+        ok(gf_fm_window_group_add_frame(g, fcs.data(), all.data(), start.data(), nullptr, tds.data(), margin.data(), c4.data(), par.data(), nullptr), "group add_frame");
+        if (fc < W) continue;
+        ok(gf_fm_window_group_triangulate(g, fcs.data(), Ps.data(), Rs.data(), tic.data(), ric.data()), "group triangulate");
+        ok(gf_fm_window_group_fill_problem(g, vo.data(), caps.data(), nv.data(), pf.data(), cs.data(), nf.data(), nullptr), "group fill_problem");
+        ok(gf_fm_window_group_set_depth(g, x.data(), nf.data()), "group set_depth");
+        ok(gf_fm_window_group_outliers(g, Ps.data(), Rs.data(), tic.data(), ric.data(), GF_FM_OUTLIERS_MOVING, io.data(), n.data()), "group outliers");
+        ids.clear(); id_start[0] = 0;
+        for (int i = 0; i < K; i++) {
+            std::vector<int32_t> bad(b[i].ids.begin(), b[i].ids.begin() + n[i]);
+            std::sort(bad.begin(), bad.end());
+            if (bad.size() > 3) bad.resize(3);
+            ids.insert(ids.end(), bad.begin(), bad.end()); id_start[i + 1] = (int)ids.size();
+        }
+        ok(gf_fm_window_group_remove_ids(g, ids.data(), id_start.data()), "group remove_ids");
+        ok(gf_fm_window_group_predict_next(g, fcs.data(), Ps.data(), Rs.data(), tic.data(), ric.data(), io.data(), xyz.data(), n.data()), "group predict_next");
+        for (int i = 0; i < K; i++) ops[i] = (margin[i] || k % 3 == 0) ? GF_FM_REMOVE_BACK_SHIFT_DEPTH : GF_FM_REMOVE_FRONT;
+        ok(gf_fm_window_group_remove(g, ops.data(), fcs.data(), shift.data()), "group remove");
+        ok(gf_fm_window_group_remove_failures(g), "group remove_failures");
+        float ms;
+        ok(gf_fm_window_group_last_device_ms(g, &ms), "group last_device_ms");     // waits for the round's work on the device
+    }
+    return us(t0, clk::now()) / frames.size();
+}
+}  // namespace fmg
+
+// input: the fm-bench input, then the number of K values and the K values.  Output: per K and arm, the host time per round
+// (one frame of all K windows) averaged over a pass, as median and [min, max] over `rounds` passes, arms alternating.
+static int run_fm_group_bench(const char *in, const char *out)
+{
+    using namespace fmb;
+    using namespace fmg;
+    FILE *f = fopen(in, "rb"), *o = fopen(out, "w");
+    if (!f || !o) return 2;
+    const int rounds = rd1<int>(f), n_frames = rd1<int>(f);
+    const double min_parallax = rd1<double>(f), depth_threshold = rd1<double>(f);
+    Poses p; rd(f, &p, sizeof(p));
+    std::vector<std::vector<gf_obs>> frames(n_frames);
+    for (auto &fr : frames) {
+        fr.resize(rd1<int>(f));
+        for (auto &ob : fr) { ob.id = rd1<int>(f); ob.track_cnt = 0; rd(f, ob.v, 64); }
+    }
+    std::vector<int> Ks(rd1<int>(f));
+    for (auto &k : Ks) k = rd1<int>(f);
+    const int cap = 2048;
+    gf_fm_window_cfg c{};
+    c.max_features = cap; c.window_size = 10; c.min_parallax = min_parallax; c.depth_threshold = depth_threshold; c.init_depth = INIT_DEPTH;
+    std::fprintf(o, "{\"window_capacity\": %d, \"unit\": \"microseconds of host time per round (one frame of every window), mean over a pass\", \"K\": {", cap);
+    for (size_t ki = 0; ki < Ks.size(); ki++) {
+        const int K = Ks[ki];
+        std::vector<gf_fm_window *> w(K);
+        std::vector<Buf> b;
+        for (int i = 0; i < K; i++) { ok(gf_fm_window_create(&w[i], 0, &c), "gf_fm_window_create"); b.emplace_back(cap); }
+        gf_fm_window_group *g = nullptr;
+        ok(gf_fm_window_group_create(&g, w.data(), K), "gf_fm_window_group_create");
+        const char *names[3] = {"group", "sequential", "threads"};
+        std::vector<double> t[3];
+        for (int a = 0; a < 3; a++) pass_k((Arm)a, frames, p, w, g, b, cap);                  // warm-up
+        for (int r = 0; r < rounds; r++) for (int a = 0; a < 3; a++) t[a].push_back(pass_k((Arm)a, frames, p, w, g, b, cap));
+        gf_fm_window_group_destroy(g);
+        for (auto *x : w) gf_fm_window_destroy(x);
+        std::fprintf(o, "%s\"%d\": {", ki ? ", " : "", K);
+        for (int a = 0; a < 3; a++)
+            std::fprintf(o, "%s\"%s\": {\"median\": %.3f, \"min\": %.3f, \"max\": %.3f}", a ? ", " : "", names[a], median(t[a]),
+                         *std::min_element(t[a].begin(), t[a].end()), *std::max_element(t[a].begin(), t[a].end()));
+        std::fprintf(o, "}");
+    }
+    std::fprintf(o, "}}\n");
+    fclose(f); fclose(o);
+    return 0;
+}
+
 int main(int argc, char **argv)
 {
-    if (argc != 4) { std::fprintf(stderr, "usage: harness fe|fe-eq|fe-box|ba|ba-multi|ba-seq|dm|gm|fm|fm-bench <in> <out>\n"); return 2; }
+    if (argc != 4) { std::fprintf(stderr, "usage: harness fe|fe-eq|fe-box|ba|ba-multi|ba-seq|dm|gm|fm|fm-bench|fm-group-bench <in> <out>\n"); return 2; }
     if (!std::strcmp(argv[1], "fe-eq")) EQUALIZE = 1;
     if (!std::strcmp(argv[1], "dm")) return run_dm(argv[2], argv[3]);
     if (!std::strcmp(argv[1], "gm")) return run_gm(argv[2], argv[3]);
     if (!std::strcmp(argv[1], "fm")) return run_fm(argv[2], argv[3]);
     if (!std::strcmp(argv[1], "fm-bench")) return run_fm_bench(argv[2], argv[3]);
+    if (!std::strcmp(argv[1], "fm-group-bench")) return run_fm_group_bench(argv[2], argv[3]);
     if (!std::strcmp(argv[1], "ba-multi") || !std::strcmp(argv[1], "ba-seq")) return run_ba_multi(argv[2], argv[3], argv[1][3] == 'm');
     return argv[1][0] == 'f' ? run_fe(argv[2], argv[3], !std::strcmp(argv[1], "fe-box")) : run_ba(argv[2], argv[3]);
 }

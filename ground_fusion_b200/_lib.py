@@ -48,6 +48,8 @@ class FmWindowCfg(ctypes.Structure):
 
 FM_WINDOW_ROWS, FM_WINDOW_ROW_DOUBLES = 11, 9
 FM_OUTLIERS_REPROJECTION, FM_OUTLIERS_MOVING = 0, 1            # gf_fm_window_outliers' `mode`
+FM_WINDOW_GROUP_MAX = 64                                       # GF_FM_WINDOW_GROUP_MAX
+FM_REMOVE_NONE, FM_REMOVE_BACK_SHIFT_DEPTH, FM_REMOVE_BACK, FM_REMOVE_FRONT = 0, 1, 2, 3   # gf_fm_window_group_remove's ops
 
 
 class Obs(ctypes.Structure):
@@ -153,6 +155,22 @@ def lib():
         L.gf_fm_window_read.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, i, ip]
         L.gf_fm_window_size.argtypes = [vp, ip]
         L.gf_fm_window_last_device_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
+        L.gf_fm_window_group_create.argtypes = [ctypes.POINTER(vp), vp, i]
+        L.gf_fm_window_group_destroy.argtypes = [vp]
+        L.gf_fm_window_group_destroy.restype = None
+        L.gf_fm_window_group_size.argtypes = [vp, ip]
+        L.gf_fm_window_group_add_frame.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+        L.gf_fm_window_group_add_frame_from_tracker_group.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
+        L.gf_fm_window_group_triangulate.argtypes = [vp, vp, vp, vp, vp, vp]
+        L.gf_fm_window_group_fill_problem.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
+        L.gf_fm_window_group_set_depth.argtypes = [vp, vp, vp]
+        L.gf_fm_window_group_remove.argtypes = [vp, vp, vp, vp]
+        L.gf_fm_window_group_remove_failures.argtypes = [vp]
+        L.gf_fm_window_group_clear_depth.argtypes = [vp]
+        L.gf_fm_window_group_remove_ids.argtypes = [vp, vp, vp]
+        L.gf_fm_window_group_outliers.argtypes = [vp, vp, vp, vp, vp, i, vp, vp]
+        L.gf_fm_window_group_predict_next.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp]
+        L.gf_fm_window_group_last_device_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
         _LIB = L
     return _LIB
 

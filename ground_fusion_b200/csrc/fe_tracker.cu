@@ -1380,6 +1380,32 @@ int gf::tracker_last_out(const gf_tracker* t, TrackerOut* o)
     return GF_OK;
 }
 
+// The step the group collected last, where the group left it on the device: member i's observations and in_box bits at
+// d_out[slot] + i * out_stride, counted as group_collect counts them.  It stays readable while the next step runs and is gone
+// once the step after that has been submitted into its slot.
+int gf::tracker_group_last_out(const gf_tracker_group* g, int n, TrackerOut* o, cudaEvent_t* downloaded)
+{
+    if (!g) return set_err(GF_ERR_INVALID_ARG, "null tracker group");
+    if (g->n != n) return set_err(GF_ERR_INVALID_ARG, "the tracker group and the window group differ in their number of members");
+    if (g->n_waited == 0) return set_err(GF_ERR_INVALID_ARG, "the tracker group has collected no step yet");
+    const long long s = g->n_waited - 1;
+    if (g->n_submitted - s > GF_PIPE)
+        return set_err(GF_ERR_INVALID_ARG, "the step the tracker group last collected is no longer on the device: a later step was submitted into its slot");
+    const int gs = (int)(s % 2);
+    for (int i = 0; i < n; i++) {
+        const gf_tracker* t = g->m[i];
+        const uint8_t* hb = g->h_out[gs] + (size_t)i * g->out_stride;
+        uint8_t* db = g->d_out[gs] + (size_t)i * g->out_stride;
+        o[i].device = g->device;
+        o[i].n = (t->cfg.depth_cam && !g->depth_valid[gs][i]) ? 0 : reinterpret_cast<const OutHeader*>(hb + offsetof(OutBlock, hdr))->n_out;
+        o[i].obs = reinterpret_cast<const gf_obs*>(db + offsetof(OutBlock, obs));
+        o[i].in_box = reinterpret_cast<const uint32_t*>(db + offsetof(OutBlock, in_box));
+        o[i].downloaded = g->ev_out[gs];
+    }
+    *downloaded = g->ev_out[gs];
+    return GF_OK;
+}
+
 // Collects the oldest step: member i's results at out + i*out_stride, in_box / status_out likewise, n_out[i*n_stride],
 // info[i*n_stride].
 static int group_collect(gf_tracker_group* g, gf_obs* out, size_t out_stride, int* n_out, size_t n_stride, uint8_t* in_box,

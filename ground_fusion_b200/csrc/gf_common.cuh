@@ -68,6 +68,8 @@ struct Pyramid {
 // (fe_tracker.cu): n observations, the in_box bits, and the event recorded after that frame's download.
 struct TrackerOut { int device, n; const gf_obs* obs; const uint32_t* in_box; cudaEvent_t downloaded; };
 int tracker_last_out(const gf_tracker* t, TrackerOut* o);
+// the n members' results of the step a tracker group collected last; *downloaded orders a reader after its download
+int tracker_group_last_out(const gf_tracker_group* g, int n, TrackerOut* o, cudaEvent_t* downloaded);
 
 // Programmatic dependent launch (PDL): a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may become
 // resident as soon as every CTA of its predecessor has executed gf_pdl_trigger (or exited); it must not touch anything the

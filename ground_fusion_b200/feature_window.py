@@ -195,3 +195,172 @@ class FeatureWindow:
         ms = ctypes.c_float(0)
         check(self.L.gf_fm_window_last_device_ms(self._h, ctypes.byref(ms)))
         return ms.value
+
+
+def _stack_poses(poses):
+    """[(Ps, Rs, tic, ric)] per member -> contiguous [K][11][3], [K][11][9], [K][3], [K][9]"""
+    p = [_poses(*x) for x in poses]
+    return tuple(np.ascontiguousarray(np.stack([q[j] for q in p])) for j in range(4))
+
+
+def _ptrs(arrays):
+    return (ctypes.c_void_p * len(arrays))(*[a.ctypes.data if a is not None else None for a in arrays])
+
+
+class FeatureWindowGroup:
+    """gf_fm_window_group: the FeatureManager calls of several FeatureWindows (one per estimator) with one set of kernel
+    launches per call.  Every method takes and returns per-member lists, and every member's results, table and Python-side
+    caches are what the same FeatureWindow method would give, so the members stay usable on their own between group calls."""
+
+    def __init__(self, windows):
+        self.members = list(windows)
+        self.L = _lib.lib()
+        self._h = ctypes.c_void_p()
+        h = (ctypes.c_void_p * len(self.members))(*[w._h for w in self.members])
+        check(self.L.gf_fm_window_group_create(ctypes.byref(self._h), h, len(self.members)))
+        self.K = len(self.members)
+        self.last_status = np.zeros(self.K, np.int32)
+
+    def close(self):
+        if self._h:
+            self.L.gf_fm_window_group_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    # ---- addFeatureCheckParallax ----
+    def _added(self, rc, margin, cnt, par, status):
+        self.last_status = status
+        for i, w in enumerate(self.members):
+            if status[i] == 0:
+                w.last_track_num, w.new_feature_num, w.long_track_num = int(cnt[i, 0]), int(cnt[i, 1]), int(cnt[i, 2])
+                w.last_average_parallax = float(par[i])
+                w._n_upper = int(cnt[i, 3])
+        check(rc)
+        return [bool(m) for m in margin]
+
+    def _out(self):
+        # status starts non-zero: an argument error returns before the library writes it, and then no member changed
+        return np.zeros(self.K, np.int32), np.zeros((self.K, 4), np.int32), np.zeros(self.K), np.ones(self.K, np.int32)
+
+    def addFrames(self, frame_counts, obs, in_box, tds):
+        """obs / in_box: per member the arrays FeatureWindow.addFrame takes (in_box None: no boxes).  Returns the keyframe flags.
+        A member that fails on the device raises after the others are applied; last_status says which."""
+        obs = [np.ascontiguousarray(o, OBS_DTYPE) for o in obs]
+        start = np.zeros(self.K + 1, np.int32); start[1:] = np.cumsum([len(o) for o in obs])
+        allo = np.ascontiguousarray(np.concatenate(obs) if start[-1] else np.zeros(1, OBS_DTYPE))
+        ib = None
+        if in_box is not None:
+            ib = np.ascontiguousarray(np.concatenate([np.zeros(len(o), np.uint8) if b is None else np.asarray(b, np.uint8)
+                                                      for o, b in zip(obs, in_box)]) if start[-1] else np.zeros(1, np.uint8))
+        fc, td = np.asarray(frame_counts, np.int32), np.asarray(tds, np.float64)
+        margin, cnt, par, st = self._out()
+        rc = self.L.gf_fm_window_group_add_frame(self._h, fc.ctypes.data, allo.ctypes.data, start.ctypes.data, ib.ctypes.data if ib is not None else None,
+                                                 td.ctypes.data, margin.ctypes.data, cnt.ctypes.data, par.ctypes.data, st.ctypes.data)
+        return self._added(rc, margin, cnt, par, st)
+
+    def addFeatureCheckParallaxes(self, frame_counts, images, tds):
+        obs = []
+        for image in images:
+            o = np.zeros(len(image), OBS_DTYPE)
+            if len(image):
+                o["id"] = list(image.keys()); o["v"] = np.asarray(list(image.values()), np.float64)[:, :8]
+            obs.append(o)
+        return self.addFrames(frame_counts, obs, None, tds)
+
+    def addFramesFromTrackerGroup(self, group, frame_counts, tds):
+        """Member i ingests member i of `group` (a TrackerGroup) from the step group.wait() returned last, on the device."""
+        fc, td = np.asarray(frame_counts, np.int32), np.asarray(tds, np.float64)
+        margin, cnt, par, st = self._out()
+        rc = self.L.gf_fm_window_group_add_frame_from_tracker_group(self._h, group._h, fc.ctypes.data, td.ctypes.data, margin.ctypes.data,
+                                                                    cnt.ctypes.data, par.ctypes.data, st.ctypes.data)
+        return self._added(rc, margin, cnt, par, st)
+
+    # ---- the solve's view ----
+    def fillProblems(self, problems):
+        """FeatureWindow.fillProblem for every member into problems[i]; returns the n_features."""
+        caps = np.array([max(w._n_upper * w.WINDOW_SIZE, 1) for w in self.members], np.int32)
+        for pb, c in zip(problems, caps):
+            pb.visual = (BaVisualFactor * int(c))()
+        vis = (ctypes.c_void_p * self.K)(*[ctypes.addressof(pb.visual) for pb in problems])
+        nv, nf, st = np.zeros(self.K, np.int32), np.zeros(self.K, np.int32), np.zeros(self.K, np.int32)
+        rc = self.L.gf_fm_window_group_fill_problem(self._h, vis, caps.ctypes.data, nv.ctypes.data, _ptrs([w._feat for w in self.members]),
+                                                    _ptrs([w._const for w in self.members]), nf.ctypes.data, st.ctypes.data)
+        self.last_status = st
+        check(rc)
+        for w, pb, n, v in zip(self.members, problems, nf, nv):
+            n = int(n)
+            pb.n_features, pb.n_visual = n, int(v)
+            pb.para_feature = np.ones(max(n, 1)); pb.para_feature[:n] = w._feat[:n]
+            pb.feature_const = np.zeros(max(n, 1), np.uint8); pb.feature_const[:n] = w._const[:n]
+        return [int(n) for n in nf]
+
+    def setDepths(self, xs):
+        xs = [np.ascontiguousarray(x, np.float64) for x in xs]
+        n = np.array([len(x) for x in xs], np.int32)
+        check(self.L.gf_fm_window_group_set_depth(self._h, _ptrs([x if len(x) else None for x in xs]), n.ctypes.data))
+
+    def triangulateAll(self, frame_counts, poses):
+        """poses: per member (Ps, Rs, tic, ric)"""
+        P, R, t, r = _stack_poses(poses)
+        fc = np.asarray(frame_counts, np.int32)
+        check(self.L.gf_fm_window_group_triangulate(self._h, fc.ctypes.data, P.ctypes.data, R.ctypes.data, t.ctypes.data, r.ctypes.data))
+
+    def clearDepth(self):
+        check(self.L.gf_fm_window_group_clear_depth(self._h))
+
+    # ---- removals ----
+    def removeFailures(self):
+        check(self.L.gf_fm_window_group_remove_failures(self._h))
+
+    def removeOutliers(self, outlier_sets):
+        ids = [np.array(sorted(s), np.int32) for s in outlier_sets]
+        start = np.zeros(self.K + 1, np.int32); start[1:] = np.cumsum([len(x) for x in ids])
+        allids = np.ascontiguousarray(np.concatenate(ids) if start[-1] else np.zeros(1, np.int32))
+        check(self.L.gf_fm_window_group_remove_ids(self._h, allids.ctypes.data, start.ctypes.data))
+
+    def remove(self, ops, frame_counts, shifts=None):
+        """ops[i]: _lib.FM_REMOVE_*; frame_counts[i]: the member's frame_count (WINDOW_SIZE for FM_REMOVE_FRONT); shifts[i]:
+        (marg_R, marg_P, new_R, new_P) for FM_REMOVE_BACK_SHIFT_DEPTH members (else None)."""
+        op, fc = np.asarray(ops, np.int32), np.asarray(frame_counts, np.int32)
+        sh = np.zeros((self.K, 24))
+        if shifts is not None:
+            for i, s in enumerate(shifts):
+                if s is not None:
+                    sh[i] = np.concatenate([np.ascontiguousarray(v, np.float64).ravel() for v in s])
+        check(self.L.gf_fm_window_group_remove(self._h, op.ctypes.data, fc.ctypes.data, sh.ctypes.data))
+
+    # ---- the loops that feed the front ends back ----
+    def _outliers(self, poses, mode):
+        P, R, t, r = _stack_poses(poses)
+        n = np.zeros(self.K, np.int32)
+        check(self.L.gf_fm_window_group_outliers(self._h, P.ctypes.data, R.ctypes.data, t.ctypes.data, r.ctypes.data, mode,
+                                                 _ptrs([w._ids for w in self.members]), n.ctypes.data))
+        out = []
+        for w, k in zip(self.members, n):
+            w.last_outlier_ids = [int(v) for v in w._ids[:k]]
+            out.append(set(w.last_outlier_ids))
+        return out
+
+    def outliersRejections(self, poses):
+        return self._outliers(poses, _lib.FM_OUTLIERS_REPROJECTION)
+
+    def movingConsistencyCheckW(self, poses):
+        return self._outliers(poses, _lib.FM_OUTLIERS_MOVING)
+
+    def predictPtsInNextFrame(self, frame_counts, poses):
+        P, R, t, r = _stack_poses(poses)
+        fc, n = np.asarray(frame_counts, np.int32), np.zeros(self.K, np.int32)
+        check(self.L.gf_fm_window_group_predict_next(self._h, fc.ctypes.data, P.ctypes.data, R.ctypes.data, t.ctypes.data, r.ctypes.data,
+                                                     _ptrs([w._ids for w in self.members]), _ptrs([w._xyz for w in self.members]),
+                                                     n.ctypes.data))
+        return [{int(w._ids[k]): w._xyz[k].copy() for k in range(m)} for w, m in zip(self.members, n)]
+
+    def last_device_ms(self):
+        ms = ctypes.c_float(0)
+        check(self.L.gf_fm_window_group_last_device_ms(self._h, ctypes.byref(ms)))
+        return ms.value

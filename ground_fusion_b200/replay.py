@@ -92,19 +92,31 @@ class WindowEstimator:
     def processImage(self, image):
         fc = self.frame_count
         self.margin_old = bool(self.fm.addFeatureCheckParallax(fc, image, self.td))
-        if not self.nonlinear:
-            if fc < WINDOW_SIZE:
-                self.frame_count += 1
-                nf = self.frame_count                    # slideWindow is not run while the window fills: the new frame starts from the last one
-                self.Ps[nf], self.Rs[nf], self.Vs[nf], self.Bas[nf], self.Bgs[nf] = self.Ps[fc].copy(), self.Rs[fc].copy(), self.Vs[fc].copy(), self.Bas[fc].copy(), self.Bgs[fc].copy()
-                return None
-            self.nonlinear = True
+        if not self.frame_added():
+            return None
         self.fm.triangulateAll(fc, self.Ps, self.Rs, self.tic, self.ric)
         removeIndex = set()
         if self.use_mcc:                                  # estimator.cpp:1104-1109
             removeIndex = self.fm.movingConsistencyCheckW(self.Ps, self.Rs, self.tic, self.ric)
             self.fm.removeOutlier(removeIndex)
         self.optimization()
+        return self.after_optimization(removeIndex)
+
+    def frame_added(self):
+        """processImage after addFeatureCheckParallax set margin_old: False while the window fills (the frame is taken and the
+        next one starts from it), True when the nonlinear branch runs."""
+        fc = self.frame_count
+        if not self.nonlinear:
+            if fc < WINDOW_SIZE:
+                self.frame_count += 1
+                nf = self.frame_count                    # slideWindow is not run while the window fills: the new frame starts from the last one
+                self.Ps[nf], self.Rs[nf], self.Vs[nf], self.Bas[nf], self.Bgs[nf] = self.Ps[fc].copy(), self.Rs[fc].copy(), self.Vs[fc].copy(), self.Bas[fc].copy(), self.Bgs[fc].copy()
+                return False
+            self.nonlinear = True
+        return True
+
+    def after_optimization(self, removeIndex):
+        """processImage after optimization(): the consistency check, the feedback to the tracker, the slide."""
         if not self.use_mcc:                              # :1123-1129 -- this set shadows the outer one: the tracker is not told about it
             self.fm.removeOutlier(self.fm.movingConsistencyCheckW(self.Ps, self.Rs, self.tic, self.ric))
         if self.tracker is not None:                      # :1131-1136 (MULTIPLE_THREAD 0)
@@ -118,6 +130,20 @@ class WindowEstimator:
 
     # estimator.cpp:2890-3636
     def optimization(self):
+        pb, n_feat = self.build_problem()
+        if n_feat is None:
+            n_feat = self.fm.fillProblem(pb)
+        R0_before, P0_before = self.Rs[0].copy(), self.Ps[0].copy()
+        self.last_summary = self.ba.optimization(pb)
+        self.fm.setDepth(self.adopt_solution(pb, n_feat, R0_before, P0_before))
+        if self.margin_old:
+            self.adopt_prior(self.ba.marginalize_old(pb))
+        else:
+            self.adopt_prior(self.ba.marginalize_second_new(pb))
+
+    def build_problem(self):
+        """vector2double, the visual factors of a host manager, the IMU factors and the prior.  Returns (problem, n_features); with
+        a FeatureWindow the visual part is left to its fillProblem (or a FeatureWindowGroup's) and n_features is None."""
         W = WINDOW_SIZE
         on_device = hasattr(self.fm, "fillProblem")      # FeatureWindow: the visual factors come from the resident table
         feats = [] if on_device else list(self.fm.iter_ba_features())
@@ -137,35 +163,50 @@ class WindowEstimator:
             for a in range(1, len(obs)):
                 pj, vj, tj = obs[a]
                 rows.append((start, start + a, k, p0, pj, v0, vj, t0, tj))
-        if on_device:
-            n_feat = self.fm.fillProblem(pb)
-        else:
+        n_feat = None
+        if not on_device:
             pb.set_visual(rows); n_feat = len(feats)
         pb.set_imu([self.pre[j].as_dict(j - 1, j) for j in range(1, W + 1) if self.pre[j] is not None and self.pre[j].sum_dt <= 10.0])
         pb.prior = self.prior
-        R0_before, P0_before = self.Rs[0].copy(), self.Ps[0].copy()
-        self.last_summary = self.ba.optimization(pb)
-        # double2vector (estimator.cpp:2440-2569)
+        return pb, n_feat
+
+    def adopt_solution(self, pb, n_feat, R0_before, P0_before):
+        """double2vector (estimator.cpp:2440-2569) of the solved problem; then the blocks are re-read for the marginalisation.
+        Returns the depth vector setDepth takes."""
+        W = WINDOW_SIZE
         from .estimator import double2vector
         Rs, Ps, Vs = double2vector(pb, R0_before, P0_before, True)
         self.Rs, self.Ps, self.Vs = Rs, Ps, Vs
         self.Bas = pb.para_speed_bias[:, 3:6].copy(); self.Bgs = pb.para_speed_bias[:, 6:9].copy()
-        self.fm.setDepth(pb.para_feature[:n_feat])
+        x = pb.para_feature[:n_feat]
         # the prior of the next window is linearised at the solved blocks as they stand (vector2double at estimator.cpp:3337 re-reads
         # the rotated state; the rotation is the identity up to the yaw fix of a window that has a prior)
         for i in range(W + 1):
             pb.para_pose[i, :3] = self.Ps[i]; pb.para_pose[i, 3:] = R_to_q(self.Rs[i])
             pb.para_speed_bias[i, :3] = self.Vs[i]
+        return x
+
+    def adopt_prior(self, prior):
+        """The marginalisation's result as margin_old says: MARGIN_OLD always replaces the prior, MARGIN_SECOND_NEW only when it
+        returned one (None: the prior stays)."""
         if self.margin_old:
-            self.prior = self.ba.marginalize_old(pb); self.n_old += 1
+            self.prior = prior; self.n_old += 1
         else:
-            new = self.ba.marginalize_second_new(pb)
-            if new is not None:
-                self.prior = new
+            if prior is not None:
+                self.prior = prior
             self.n_second_new += 1
 
     # estimator.cpp:3638-3806
     def slideWindow(self):
+        shift = self.slide_states()
+        if shift is not None:
+            self.fm.removeBackShiftDepth(*shift)                  # slideWindowOld (estimator.cpp:3808-3837)
+        else:
+            self.fm.removeFront(self.frame_count)                 # slideWindowNew (estimator.cpp:3839-3851)
+
+    def slide_states(self):
+        """slideWindow's shift of the window's states and pre-integrations.  Returns the camera poses (R0, P0, R1, P1) of
+        removeBackShiftDepth after MARGIN_OLD, None after MARGIN_SECOND_NEW (removeFront)."""
         W = WINDOW_SIZE
         if self.margin_old:
             back_R0, back_P0 = self.Rs[0].copy(), self.Ps[0].copy()
@@ -175,14 +216,14 @@ class WindowEstimator:
             self.pre[W] = Preintegration(self.acc_0, self.gyr_0, self.Bas[W], self.Bgs[W]); self.bufs[W] = []
             R0, R1 = back_R0 @ self.ric, self.Rs[0] @ self.ric
             P0, P1 = back_P0 + back_R0 @ self.tic, self.Ps[0] + self.Rs[0] @ self.tic
-            self.fm.removeBackShiftDepth(R0, P0, R1, P1)          # slideWindowOld (estimator.cpp:3808-3837)
+            return R0, P0, R1, P1
         else:
             self.Ps[W - 1], self.Rs[W - 1] = self.Ps[W].copy(), self.Rs[W].copy()
             for dt, acc, gyr in self.bufs[W]:
                 self.pre[W - 1].push_back(dt, acc, gyr); self.bufs[W - 1].append((dt, acc, gyr))
             self.Vs[W - 1], self.Bas[W - 1], self.Bgs[W - 1] = self.Vs[W].copy(), self.Bas[W].copy(), self.Bgs[W].copy()
             self.pre[W] = Preintegration(self.acc_0, self.gyr_0, self.Bas[W], self.Bgs[W]); self.bufs[W] = []
-            self.fm.removeFront(self.frame_count)                 # slideWindowNew (estimator.cpp:3839-3851)
+            return None
 
 
 def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=True, max_iter=8, feedback=False, use_mcc=False, boxes=None,
@@ -253,4 +294,99 @@ def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=Tru
         out["dense_map"] = dense_map
     if grid_map is not None:
         out["grid_map"] = grid_map
+    return out
+
+
+def replay_group(streams, trackers, windows, adjusters, n_frames, imu_per_frame=7, imu_propagate=True, max_iter=8, feedback=False):
+    """K estimators in lockstep, one per stream, each step with one call per stage for all of them: the TrackerGroup over
+    `trackers` tracks frame k of every stream, the FeatureWindowGroup over `windows` ingests the step on the device and
+    triangulates, fills the K problems, estimator.solve_multi solves them on `adjusters`, setDepth follows, then
+    estimator.marginalize_multi with each estimator's own mode, the consistency check and removal, the feedback to each member
+    tracker (feedback=True, between tracker-group steps) and the slide.  The host logic is WindowEstimator's, as in replay();
+    returns one result dict per stream in replay()'s format.  No boxes, dense map or USE_MCC."""
+    from . import _lib
+    from .estimator import marginalize_multi, solve_multi
+    from .feature_tracker import TrackerGroup
+    from .feature_window import FeatureWindowGroup
+    K = len(streams)
+    assert len(trackers) == len(windows) == len(adjusters) == K
+    tg, wg = TrackerGroup(trackers), FeatureWindowGroup(windows)
+    imus = [ImuFromStream(s) for s in streams]
+    ests = [WindowEstimator(windows[i], adjusters[i], imu_propagate=imu_propagate, max_iter=max_iter, tracker=trackers[i] if feedback else None)
+            for i in range(K)]
+    rec = [{"t": [], "P": [], "R": [], "gP": [], "gR": [], "it": []} for _ in range(K)]
+    t_prev = [None] * K
+    try:
+        for k in range(n_frames):
+            frames = [s.frame(k) for s in streams]
+            for i, (e, imu) in enumerate(zip(ests, imus)):
+                t = frames[i][0]
+                if t_prev[i] is not None:
+                    dt = (t - t_prev[i]) / imu_per_frame
+                    for s in range(1, imu_per_frame + 1):
+                        acc, gyr = imu.sample(t_prev[i] + s * dt)
+                        e.processIMU(dt, acc, gyr)
+                else:
+                    acc, gyr = imu.sample(t); e.processIMU(0.0, acc, gyr)
+            gray = [np.ascontiguousarray(f[1]) for f in frames]
+            depth = [np.ascontiguousarray(f[2]) if f[2] is not None else None for f in frames]
+            tg.submit([f[0] for f in frames], [g.ctypes.data for g in gray], [d.ctypes.data if d is not None else 0 for d in depth])
+            tg.wait()
+            for i, (e, imu) in enumerate(zip(ests, imus)):
+                if not e.nonlinear:                     # initialisation is out of scope: ground-truth states while the window fills
+                    R_wb, P = imu.pose_t(frames[i][0])
+                    e.set_state(e.frame_count, R_wb, P, imu.velocity(frames[i][0]))
+            fcs = [e.frame_count for e in ests]
+            margins = wg.addFramesFromTrackerGroup(tg, fcs, [e.td for e in ests])
+            for e, m in zip(ests, margins):
+                e.margin_old = m
+            t_prev = [f[0] for f in frames]
+            full = [e.frame_added() for e in ests]
+            assert len(set(full)) == 1, "the estimators of a group fill their windows in lockstep"
+            if not full[0]:
+                continue
+            poses = [(e.Ps, e.Rs, e.tic, e.ric) for e in ests]
+            wg.triangulateAll(fcs, poses)
+            pbs = [e.build_problem()[0] for e in ests]
+            nfs = wg.fillProblems(pbs)
+            before = [(e.Rs[0].copy(), e.Ps[0].copy()) for e in ests]
+            sums, status = solve_multi(adjusters, pbs)
+            if any(v < 0 for v in status):
+                raise _lib.GfError("solve_multi: a window's IMU covariance is singular: %s" % status)
+            xs = []
+            for e, pb, nf, (R0, P0), sm in zip(ests, pbs, nfs, before, sums):
+                e.last_summary = sm
+                xs.append(e.adopt_solution(pb, nf, R0, P0))
+            wg.setDepths(xs)
+            priors, kept = marginalize_multi(adjusters, pbs, [_lib.MARGIN_OLD if e.margin_old else _lib.MARGIN_SECOND_NEW for e in ests])
+            if any(v < 0 for v in kept):
+                raise _lib.GfError("marginalize_multi: a window's IMU covariance is singular: %s" % kept)
+            for e, pr in zip(ests, priors):
+                e.adopt_prior(pr)
+            poses = [(e.Ps, e.Rs, e.tic, e.ric) for e in ests]
+            wg.removeOutliers(wg.movingConsistencyCheckW(poses))     # as after_optimization without USE_MCC
+            if feedback:                                             # the set the tracker is told about is empty without USE_MCC
+                preds = wg.predictPtsInNextFrame([e.frame_count for e in ests], poses)
+                for e, tr, pred in zip(ests, trackers, preds):
+                    tr.removeOutliers(set())
+                    tr.setPrediction(pred)
+                    e.n_predicted += len(pred)
+            shifts = [e.slide_states() for e in ests]
+            wg.remove([_lib.FM_REMOVE_BACK_SHIFT_DEPTH if sh is not None else _lib.FM_REMOVE_FRONT for sh in shifts],
+                      [e.frame_count for e in ests], shifts)
+            wg.removeFailures()
+            for i, (e, imu) in enumerate(zip(ests, imus)):
+                R_wb, P = imu.pose_t(frames[i][0])
+                r = rec[i]
+                r["t"].append(frames[i][0]); r["P"].append(e.Ps[WINDOW_SIZE].copy()); r["R"].append(e.Rs[WINDOW_SIZE].copy())
+                r["gP"].append(P); r["gR"].append(R_wb); r["it"].append(e.last_summary["iterations"])
+    finally:
+        wg.close(); tg.close()
+    out = []
+    for e, r in zip(ests, rec):
+        P_est, P_gt = np.array(r["P"]), np.array(r["gP"])
+        ate = float(np.sqrt(np.mean(np.sum((P_est - P_gt) ** 2, axis=1)))) if len(P_est) else float("nan")
+        out.append({"t": np.array(r["t"]), "P_est": P_est, "P_gt": P_gt, "R_est": np.array(r["R"]), "R_gt": np.array(r["gR"]), "ate_m": ate,
+                    "n_margin_old": e.n_old, "n_margin_second_new": e.n_second_new, "iterations": r["it"],
+                    "n_removed": e.n_removed, "n_predicted": e.n_predicted})
     return out

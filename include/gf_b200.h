@@ -671,6 +671,70 @@ int gf_fm_window_size(gf_fm_window* w, int* n);
 /* Device time of the last call's work on the handle's stream, from CUDA events (waits for that work) */
 int gf_fm_window_last_device_ms(gf_fm_window* w, float* ms);
 
+/* A window group: n existing gf_fm_windows (members, one per estimator) whose FeatureManager calls run with ONE set of launches
+ * per call: every kernel runs once for the whole group (member = a grid dimension), so the number of launches and driver calls
+ * of a group call does not grow with n, and a call that returns something synchronises once for the group.  Member i's table,
+ * results and host-side state afterwards are exactly what the same single-window call on it would give (same kernels, same
+ * arithmetic, same bits); a single-window call is the group of one.
+ *   _create: 1 <= n <= GF_FM_WINDOW_GROUP_MAX; the windows must be distinct and bound to one device; capacities may differ.
+ *       Any violation is GF_ERR_INVALID_ARG, with gf_last_error() starting "member k: " for the member at fault.  The group
+ *       owns its stream and its ring of pinned input slots (descriptors, observations, depths, ids); it allocates nothing
+ *       after creation.  Destroy the group before its members.
+ *   State stays in the members.  Between group calls a member may be used directly, and the next group call continues from
+ *   there: work is ordered between a member's stream and the group's in both directions, with no wait while every member
+ *   stays on one of them.  A group is used from one thread at a time, and its members are not used by another thread during
+ *   a group call.
+ *   Per-member arguments are arrays of n (poses: Ps [n][11][3], Rs [n][11][9], tic [n][3], ric [n][9]; CSR lists: n + 1
+ *   offsets from 0).  Every member's arguments are checked as the single call checks them before anything is enqueued: an
+ *   argument error changes no member, and gf_last_error() starts "member k: ".
+ *   Failures found on the device are per member: status[k] (nullable) is 0 or the single call's error code for member k,
+ *   whose table and outputs are then left as they were; the other members are applied, and the call returns the code of the
+ *   first member that failed.
+ * gf_fm_window_group_last_device_ms reports the device time of the last group call. */
+typedef struct gf_fm_window_group gf_fm_window_group;
+#define GF_FM_WINDOW_GROUP_MAX 64      /* = GF_TRACKER_GROUP_MAX: a tracker group maps one to one onto a window group */
+#define GF_FM_REMOVE_NONE 0
+#define GF_FM_REMOVE_BACK_SHIFT_DEPTH 1
+#define GF_FM_REMOVE_BACK 2
+#define GF_FM_REMOVE_FRONT 3
+int gf_fm_window_group_create(gf_fm_window_group** out, gf_fm_window* const* windows, int n);
+void gf_fm_window_group_destroy(gf_fm_window_group* g);
+int gf_fm_window_group_size(gf_fm_window_group* g, int* n);
+/* add_frame for every member: member i's observations are obs[obs_start[i] .. obs_start[i + 1]), its box flags in_box at the
+ * same indices (nullable: none); margin_old [n], counters4 [n][4], last_average_parallax [n] (each nullable).  A member that does
+ * not fit (GF_ERR_CAPACITY) or would take a twelfth observation (GF_ERR_INVALID_ARG) reports it in status and is unchanged. */
+int gf_fm_window_group_add_frame(gf_fm_window_group* g, const int32_t* frame_counts, const gf_obs* obs, const int32_t* obs_start, const uint8_t* in_box,
+                                 const double* tds, int32_t* margin_old, int32_t* counters4, double* last_average_parallax, int32_t* status);
+/* The same with member i of the tracker group tg's last collected step (gf_tracker_group_wait / _track_batch), read where tg left
+ * it on the device, ordered after tg's download of that step; the count is gf_tracker_group_wait's.  tg is only read.  With
+ * two steps in flight the collected step stays readable while the next one runs (submit k + 1, wait k, ingest).
+ * GF_ERR_INVALID_ARG, every table unchanged, if tg has collected no step, has had a later step submitted into that step's
+ * slot, has another number of members, or is bound to another device. */
+int gf_fm_window_group_add_frame_from_tracker_group(gf_fm_window_group* g, const gf_tracker_group* tg, const int32_t* frame_counts, const double* tds,
+                                                    int32_t* margin_old, int32_t* counters4, double* last_average_parallax, int32_t* status);
+int gf_fm_window_group_triangulate(gf_fm_window_group* g, const int32_t* frame_counts, const double* Ps, const double* Rs, const double* tic, const double* ric);
+/* fill_problem per member: visual_out[i] holds caps[i] rows (visual_out NULL, or an entry NULL: only the feature arrays of that
+ * member); n_visual, n_features [n]; para_feature[i], feature_const[i] (nullable arrays and entries).  A member whose rows do not
+ * fit reports GF_ERR_CAPACITY in status. */
+int gf_fm_window_group_fill_problem(gf_fm_window_group* g, gf_ba_visual_factor* const* visual_out, const int32_t* caps, int32_t* n_visual,
+                                    double* const* para_feature, uint8_t* const* feature_const, int32_t* n_features, int32_t* status);
+int gf_fm_window_group_set_depth(gf_fm_window_group* g, const double* const* para_feature, const int32_t* n);
+/* One removal per member, chosen per member (members decide MARGIN_OLD or MARGIN_SECOND_NEW independently): ops[i] is
+ * GF_FM_REMOVE_NONE, _BACK_SHIFT_DEPTH (shift[i] = marg_R [9], marg_P [3], new_R [9], new_P [3], as
+ * gf_fm_window_remove_back_shift_depth; shift may be NULL when no member takes it), _BACK or _FRONT (frame_counts[i] must be
+ * WINDOW_SIZE, as gf_fm_window_remove_front requires). */
+int gf_fm_window_group_remove(gf_fm_window_group* g, const int32_t* ops, const int32_t* frame_counts, const double* shift);
+int gf_fm_window_group_remove_failures(gf_fm_window_group* g);
+int gf_fm_window_group_clear_depth(gf_fm_window_group* g);
+/* removeOutlier per member: ids[id_start[i] .. id_start[i + 1]) */
+int gf_fm_window_group_remove_ids(gf_fm_window_group* g, const int32_t* ids, const int32_t* id_start);
+/* outliers / predict_next per member: ids_out[i] (and xyz_out[i]) hold member i's max_features entries; n [n] */
+int gf_fm_window_group_outliers(gf_fm_window_group* g, const double* Ps, const double* Rs, const double* tic, const double* ric, int mode,
+                                int32_t* const* ids_out, int32_t* n);
+int gf_fm_window_group_predict_next(gf_fm_window_group* g, const int32_t* frame_counts, const double* Ps, const double* Rs, const double* tic,
+                                    const double* ric, int32_t* const* ids_out, double* const* xyz_out, int32_t* n);
+int gf_fm_window_group_last_device_ms(gf_fm_window_group* g, float* ms);
+
 /* ------------------------------------------------------------------------------------------------
  * Dense colour map (dense_map/src/pose_graph.cpp, pose_graph_node.cpp): the keyframe point sampling of the mapping node,
  * PoseGraph's voxel-density insertion (OctreePointCloudDensity, 0.01 m voxels), its RadiusOutlierRemoval (0.8 m, 10
