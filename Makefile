@@ -3,12 +3,13 @@ NVCC ?= /usr/local/cuda/bin/nvcc
 ARCH := -gencode arch=compute_90a,code=sm_90a
 CSRC := ground_fusion_b200/csrc
 OUT  := ground_fusion_b200/libgf_b200.so
+YOLO_OUT := ground_fusion_b200/libgf_yolo.so
 # -fmad=false: the front end is bit-exact with OpenCV's separately-rounded float ops (FMA only where written)
 NVFLAGS := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden -fmad=false
 SRCS := $(wildcard $(CSRC)/*.cu)
 HDRS := $(wildcard $(CSRC)/*.cuh) $(CSRC)/gm_math.h include/gf_b200.h
 
-all: $(OUT) oracle
+all: $(OUT) $(YOLO_OUT) oracle
 
 # front end: -fmad=false (bit-exact with OpenCV's separately-rounded float ops; FMA only where written)
 # back end: default FMA contraction (parity is 1e-6 m against an FP64 oracle, not bit-exactness)
@@ -28,12 +29,22 @@ $(BUILD)/dm_map.o: $(CSRC)/dm_map.cu $(HDRS)
 # occupancy grid: -fmad=false (bit-exact with oracle/gm_oracle.c's shared mode, built with -ffp-contract=off)
 $(BUILD)/gm_grid.o: $(CSRC)/gm_grid.cu $(HDRS)
 	@mkdir -p $(BUILD); $(NVCC) $(NVFLAGS) -dc -o $@ $< -Xptxas -v 2> build_ptxas_gm.log || (cat build_ptxas_gm.log; false)
-$(OUT): $(BUILD)/fe_tracker.o $(BUILD)/ba_solver.o $(BUILD)/fm_kernels.o $(BUILD)/fm_window.o $(BUILD)/dm_map.o $(BUILD)/gm_grid.o
-	$(NVCC) $(ARCH) -shared -o $@ $^
+# the detector's entry points in libgf_b200.so: host-only forwarders that open libgf_yolo.so on first use (no device code)
+$(BUILD)/yolo_forward.o: $(CSRC)/yolo_forward.cpp include/gf_b200.h
+	@mkdir -p $(BUILD); g++ -std=c++17 -O2 -fPIC -fvisibility=hidden -Wall -c -o $@ $<
+$(OUT): $(BUILD)/fe_tracker.o $(BUILD)/ba_solver.o $(BUILD)/fm_kernels.o $(BUILD)/fm_window.o $(BUILD)/dm_map.o $(BUILD)/gm_grid.o $(BUILD)/yolo_forward.o
+	$(NVCC) $(ARCH) -shared -o $@ $^ -ldl
 	@cat build_ptxas_fe.log build_ptxas_ba.log build_ptxas_dm.log build_ptxas_gm.log build_ptxas_fmw.log > build_ptxas.log
+# YOLO detector, its own library (the tracker / estimator library does not carry its device code): -fmad=false (bit-exact
+# with darknet's CPU build, compiled with -ffp-contract=off by oracle/darknet.mk)
+$(BUILD)/yolo_detector.o: $(CSRC)/yolo_detector.cu $(HDRS) $(CSRC)/yolo_cfg.cuh $(CSRC)/yolo_kernels.cuh
+	@mkdir -p $(BUILD); $(NVCC) $(NVFLAGS) -c -o $@ $< -Xptxas -v 2> build_ptxas_yolo.log || (cat build_ptxas_yolo.log; false)
+$(YOLO_OUT): $(BUILD)/yolo_detector.o
+	$(NVCC) $(ARCH) -shared -o $@ $^
 
 oracle: oracle/_build/libgf_oracle_dm.so oracle/_build/libgf_oracle_gm.so
 	$(MAKE) -C oracle
+	$(MAKE) -C oracle -f darknet.mk
 # the dense map's sequential restatement (tests and tools/bench_dense_map.py only): -O3 -ffp-contract=off as oracle/Makefile's
 # libgf_oracle_ba.so, plus -msse2 -mfpmath=sse as its libgf_oracle_fe.so
 oracle/_build/libgf_oracle_dm.so: oracle/dm_oracle.c
@@ -50,5 +61,5 @@ profile: $(SRCS) $(HDRS) $(BUILD)/fm_kernels.o $(BUILD)/fm_window.o $(BUILD)/dm_
 	$(NVCC) $(ARCH) -shared -o ground_fusion_b200/libgf_b200_prof.so $(BUILD)/fe_tracker_prof.o $(BUILD)/ba_solver_prof.o $(BUILD)/fm_kernels.o $(BUILD)/fm_window.o $(BUILD)/dm_map.o $(BUILD)/gm_grid.o
 
 clean:
-	rm -f $(OUT) build_ptxas.log; $(MAKE) -C oracle clean
+	rm -f $(OUT) $(YOLO_OUT) build_ptxas.log build_ptxas_yolo.log; $(MAKE) -C oracle clean
 .PHONY: all oracle clean profile

@@ -52,6 +52,9 @@ FM_WINDOW_GROUP_MAX = 64                                       # GF_FM_WINDOW_GR
 FM_REMOVE_NONE, FM_REMOVE_BACK_SHIFT_DEPTH, FM_REMOVE_BACK, FM_REMOVE_FRONT = 0, 1, 2, 3   # gf_fm_window_group_remove's ops
 
 
+GF_MAX_BOXES = 100                                             # darknet_ros publishes at most 100 boxes
+
+
 class Obs(ctypes.Structure):
     _fields_ = [("id", ctypes.c_int32), ("track_cnt", ctypes.c_int32), ("v", ctypes.c_double * 8)]
 
@@ -173,6 +176,40 @@ def lib():
         L.gf_fm_window_group_last_device_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
         _LIB = L
     return _LIB
+
+
+YOLO_LIB_PATH = os.path.join(_HERE, "libgf_yolo.so")
+_YOLO = None
+
+
+def yolo_lib():
+    """libgf_yolo.so: the YOLO detector's C ABI (gf_detector_*, gf_stage_letterbox), built next to libgf_b200.so."""
+    global _YOLO
+    if _YOLO is None:
+        if not os.path.exists(YOLO_LIB_PATH):
+            raise GfError("libgf_yolo.so not built (%s): run `make` or __graft_entry__.build(); "
+                          "there is no CPU fallback" % YOLO_LIB_PATH)
+        L = ctypes.CDLL(YOLO_LIB_PATH)
+        vp, i, sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t
+        ip = ctypes.POINTER(i)
+        L.gf_detector_last_error.restype = ctypes.c_char_p
+        L.gf_detector_create.argtypes = [ctypes.POINTER(vp), i, ctypes.c_char_p, ctypes.c_char_p, ctypes.c_float]
+        L.gf_detector_destroy.argtypes = [vp]
+        L.gf_detector_destroy.restype = None
+        L.gf_detector_info.argtypes = [vp, vp, ip, ip]
+        L.gf_detector_detect.argtypes = [vp, vp, sz, i, i, i, vp, vp, vp, i, ip]
+        L.gf_detector_last_device_ms.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
+        L.gf_detector_layer_shape.argtypes = [vp, i, vp]
+        L.gf_detector_layer_output.argtypes = [vp, i, vp, sz]
+        L.gf_detector_layer_times.argtypes = [vp, i, vp]
+        L.gf_stage_letterbox.argtypes = [i, vp, sz, i, i, i, i, i, vp]
+        _YOLO = L
+    return _YOLO
+
+
+def check_yolo(rc):
+    if rc != 0:
+        raise GfError("libgf_yolo error %d: %s" % (rc, yolo_lib().gf_detector_last_error().decode()))
 
 
 def check(rc):

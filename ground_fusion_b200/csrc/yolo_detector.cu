@@ -1,0 +1,568 @@
+// yolo_detector.cu -- gf_detector_* (C ABI): the use_yolo front end's detector, the darknet_ros node
+// (vins_estimator/src/YoloObjectDetector.cpp) with the vendored darknet's CPU forward pass, on the GPU and bit-exact with it.
+//   create   the cfg and .weights read on the host (yolo_cfg.cuh), every parameter in HBM once, the forward pass captured as one
+//            CUDA graph: the layers' kernels (yolo_kernels.cuh) and the copies of the [region] / [yolo] outputs to pinned memory
+//   detect   the frame to the device, k_yolo_letterbox, the graph, then on the host darknet's decoding
+//            (get_network_boxes(w, h, thresh, 0.5, 0, 1)), do_nms_obj(0.4) with libc qsort, and darknet_ros's extraction
+// DESIGN.md "YOLO detector" has the arithmetic and why there are no tensor cores here.
+// Built as its own library, libgf_yolo.so, with its own error text (gf_detector_last_error); libgf_b200.so exports the same
+// entry points as forwarders (yolo_forward.cpp) and carries none of this device code, so a tracker / estimator process that
+// never detects loads exactly what it loaded before.
+#include <algorithm>
+#include <cmath>
+#include <cstdlib>
+#include <cstring>
+#include <new>
+#include <string>
+#include <vector>
+
+#include "gf_common.cuh"
+#include "yolo_cfg.cuh"
+#include "yolo_kernels.cuh"
+
+using namespace gf;
+using namespace gfy;
+
+namespace gf {
+thread_local char g_err[512] = "";           // this library's error text (set_err, GF_CUDA)
+std::atomic<uint64_t> g_launches{0};
+}  // namespace gf
+
+namespace gfy {
+
+struct DevLayer {
+    float* out = nullptr;
+    float *w = nullptr, *bias = nullptr, *scale = nullptr, *mean = nullptr;
+    double* den = nullptr;
+    float* host_out = nullptr;           // pinned copy of a [region] / [yolo] output
+};
+
+// darknet's detection struct, field for field, so that qsort sees elements of the same size and order as the oracle's
+struct Det {
+    float x, y, w, h;
+    int classes;
+    float* prob;
+    float* mask;
+    float objectness;
+    int sort_class;
+};
+static_assert(sizeof(Det) == 48, "Det must have darknet's detection layout");
+
+}  // namespace gfy
+
+struct gf_detector {
+    int device = 0;
+    float thresh = 0.3f;
+    Net net;
+    std::vector<DevLayer> dl;
+    float* d_input = nullptr;            // [3][h][w]
+    uint8_t* d_frame = nullptr;
+    size_t frame_cap = 0;
+    cudaStream_t st = nullptr;
+    cudaGraph_t graph = nullptr;
+    cudaGraphExec_t exec = nullptr;
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    std::vector<float> prob_store;
+    bool ran = false;
+};
+
+namespace {
+
+int select_device(int device)
+{
+    int n = 0;
+    if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) return set_err(GF_ERR_NO_DEVICE, "no CUDA device visible; libgf_b200 has no CPU fallback");
+    if (device < 0 || device >= n) return set_err(GF_ERR_INVALID_ARG, "device index out of range");
+    GF_CUDA(cudaSetDevice(device));
+    return GF_OK;
+}
+
+void free_detector(gf_detector* d)
+{
+    if (!d) return;
+    if (d->exec) cudaGraphExecDestroy(d->exec);
+    if (d->graph) cudaGraphDestroy(d->graph);
+    for (DevLayer& l : d->dl) {
+        cudaFree(l.out); cudaFree(l.w); cudaFree(l.bias); cudaFree(l.scale); cudaFree(l.mean); cudaFree(l.den);
+        if (l.host_out) cudaFreeHost(l.host_out);
+    }
+    cudaFree(d->d_input);
+    cudaFree(d->d_frame);
+    if (d->ev0) cudaEventDestroy(d->ev0);
+    if (d->ev1) cudaEventDestroy(d->ev1);
+    if (d->st) cudaStreamDestroy(d->st);
+    delete d;
+}
+
+template <typename T>
+int upload(T** dst, const std::vector<T>& v)
+{
+    GF_CUDA(cudaMalloc(dst, sizeof(T) * v.size()));
+    GF_CUDA(cudaMemcpy(*dst, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice));
+    return GF_OK;
+}
+
+inline unsigned blocks(long n, int t) { return (unsigned)((n + t - 1) / t); }
+
+// darknet's letterbox geometry: the frame scaled to fit the net size, aspect kept
+void letterbox_size(int w, int h, int nw, int nh, int& new_w, int& new_h)
+{
+    if ((float)nw / w < (float)nh / h) { new_w = nw; new_h = (h * nw) / w; }
+    else { new_h = nh; new_w = (w * nh) / h; }
+}
+
+template <int BM, int BN>
+void launch_conv(const ConvArgs& a, cudaStream_t s)
+{
+    dim3 g(blocks(a.N, BN), blocks(a.M, BM));
+    k_yolo_conv<BM, BN><<<g, CONV_THREADS, 0, s>>>(a);
+    GF_LAUNCHED();
+}
+
+// layer i's kernels on stream s (captured into the graph)
+int enqueue_layer(gf_detector* d, int i, cudaStream_t s)
+{
+    const Layer& l = d->net.layers[i];
+    DevLayer& o = d->dl[i];
+    const float* in = i == 0 ? d->d_input : d->dl[i - 1].out;
+    constexpr int T = 256;
+    switch (l.type) {
+    case L_CONV: {
+        ConvArgs a{in, o.w, o.out, o.bias, o.scale, o.mean, o.den, l.c, l.h, l.w, l.n, l.c * l.size * l.size, l.ow, l.ow * l.oh,
+                   l.size, l.stride, l.pad, l.bn, l.act};
+        // 64 x 64 tiles where they fill the GPU twice over, 32 x 32 where the layer is small
+        if ((long)blocks(a.N, 64) * blocks(a.M, 64) >= 264) launch_conv<64, 64>(a, s);
+        else launch_conv<32, 32>(a, s);
+        break;
+    }
+    case L_MAXPOOL:
+        k_yolo_maxpool<<<blocks(l.outputs, T), T, 0, s>>>(in, o.out, l.w, l.h, l.c, l.ow, l.oh, l.size, l.stride, l.pad); GF_LAUNCHED();
+        break;
+    case L_ROUTE: {
+        size_t off = 0;
+        for (int k : l.in) {
+            const size_t n = (size_t)d->net.layers[k].outputs;
+            GF_CUDA(cudaMemcpyAsync(o.out + off, d->dl[k].out, 4 * n, cudaMemcpyDeviceToDevice, s));
+            off += n;
+        }
+        break;
+    }
+    case L_REORG:
+        k_yolo_reorg<<<blocks(l.outputs, T), T, 0, s>>>(in, o.out, l.w, l.h, l.c, l.stride); GF_LAUNCHED();
+        break;
+    case L_UPSAMPLE:
+        k_yolo_upsample<<<blocks(l.outputs, T), T, 0, s>>>(in, o.out, l.w, l.h, l.c, l.stride, l.scale); GF_LAUNCHED();
+        break;
+    case L_SHORTCUT:
+        k_yolo_shortcut<<<blocks(l.outputs, T), T, 0, s>>>(in, d->dl[l.in[0]].out, o.out, l.w, l.h, l.c, l.ow, l.oh, l.oc, l.alpha,
+                                                           l.beta, l.act);
+        GF_LAUNCHED();
+        break;
+    case L_REGION:
+    case L_YOLO:
+        k_yolo_head<<<blocks((long)l.ow * l.oh * l.num, 128), 128, 0, s>>>(in, o.out, l.ow * l.oh, l.num, l.classes, l.type == L_YOLO,
+                                                                           l.softmax);
+        GF_LAUNCHED();
+        GF_CUDA(cudaMemcpyAsync(o.host_out, o.out, 4 * (size_t)l.outputs, cudaMemcpyDeviceToHost, s));
+        break;
+    }
+    GF_CUDA(cudaGetLastError());
+    return GF_OK;
+}
+
+int detector_init(gf_detector* d)
+{
+    GF_CUDA(cudaStreamCreateWithFlags(&d->st, cudaStreamNonBlocking));
+    GF_CUDA(cudaEventCreate(&d->ev0));
+    GF_CUDA(cudaEventCreate(&d->ev1));
+    GF_CUDA(cudaMalloc(&d->d_input, 4 * (size_t)3 * d->net.w * d->net.h));
+    d->dl.resize(d->net.layers.size());
+    for (size_t i = 0; i < d->net.layers.size(); i++) {
+        const Layer& l = d->net.layers[i];
+        DevLayer& o = d->dl[i];
+        GF_CUDA(cudaMalloc(&o.out, 4 * (size_t)l.outputs));
+        if (l.type == L_CONV) {
+            int rc = upload(&o.w, l.weights);
+            if (!rc) rc = upload(&o.bias, l.biases);
+            if (!rc && l.bn) {
+                std::vector<double> den(l.n);
+                for (int m = 0; m < l.n; m++) den[m] = sqrt((double)l.var[m]) + (double).000001f;   // normalize_cpu's denominator
+                rc = upload(&o.scale, l.scales);
+                if (!rc) rc = upload(&o.mean, l.mean);
+                if (!rc) rc = upload(&o.den, den);
+            }
+            if (rc) return rc;
+        }
+        if (l.type == L_REGION || l.type == L_YOLO) GF_CUDA(cudaMallocHost(&o.host_out, 4 * (size_t)l.outputs));
+    }
+    GF_CUDA(cudaStreamBeginCapture(d->st, cudaStreamCaptureModeThreadLocal));
+    int rc = GF_OK;
+    for (size_t i = 0; i < d->net.layers.size() && !rc; i++) rc = enqueue_layer(d, (int)i, d->st);
+    cudaGraph_t g = nullptr;
+    const cudaError_t e = cudaStreamEndCapture(d->st, &g);
+    if (rc) { if (g) cudaGraphDestroy(g); return rc; }
+    GF_CUDA(e);
+    d->graph = g;
+    GF_CUDA(cudaGraphInstantiate(&d->exec, d->graph, 0));
+    return GF_OK;
+}
+
+// ---- host: darknet's decoding, NMS and darknet_ros's extraction ----------------------------------------------------------
+
+// correct_region_boxes / correct_yolo_boxes with relative = 1
+void correct_boxes(Det* dets, int n, int w, int h, int netw, int neth)
+{
+    int new_w = 0, new_h = 0;
+    if (((float)netw / w) < ((float)neth / h)) { new_w = netw; new_h = (h * netw) / w; }
+    else { new_h = neth; new_w = (w * neth) / h; }
+    for (int i = 0; i < n; i++) {
+        Det& b = dets[i];
+        b.x = (float)((b.x - (netw - new_w) / 2. / netw) / ((float)new_w / netw));
+        b.y = (float)((b.y - (neth - new_h) / 2. / neth) / ((float)new_h / neth));
+        b.w *= (float)netw / new_w;
+        b.h *= (float)neth / new_h;
+    }
+}
+
+// get_network_boxes(net, w, h, thresh, hier, 0, 1, &n): every layer's detections in layer order
+void network_boxes(gf_detector* d, int w, int h, std::vector<Det>& dets)
+{
+    const Net& net = d->net;
+    const float thresh = d->thresh;
+    const int classes = net.layers.back().classes;
+    size_t total = 0;
+    for (size_t li = 0; li < net.layers.size(); li++) {
+        const Layer& l = net.layers[li];
+        const int wh = l.ow * l.oh, E = l.classes + 5;
+        const float* p = d->dl[li].host_out;
+        if (l.type == L_REGION) total += (size_t)wh * l.num;
+        if (l.type == L_YOLO)
+            for (int i = 0; i < wh; i++)
+                for (int n = 0; n < l.num; n++) total += p[(size_t)n * wh * E + 4 * wh + i] > thresh;
+    }
+    dets.assign(total, Det{});
+    d->prob_store.assign(total * classes, 0.f);
+    for (size_t i = 0; i < total; i++) { dets[i].prob = d->prob_store.data() + i * classes; dets[i].mask = nullptr; }
+    size_t at = 0;
+    for (size_t li = 0; li < net.layers.size(); li++) {
+        const Layer& l = net.layers[li];
+        if (l.type != L_REGION && l.type != L_YOLO) continue;
+        const int wh = l.ow * l.oh, E = l.classes + 5;
+        const float* p = d->dl[li].host_out;
+        const size_t first = at;
+        for (int i = 0; i < wh; i++) {
+            const int row = i / l.ow, col = i % l.ow;
+            for (int n = 0; n < l.num; n++) {
+                const size_t base = (size_t)n * wh * E + i;
+                const float obj = p[base + 4 * (size_t)wh];
+                if (l.type == L_YOLO && obj <= thresh) continue;
+                // a [yolo] layer appends its detections above thresh; a [region] layer fills all of its own at n * wh + i
+                Det& b = l.type == L_YOLO ? dets[at++] : dets[first + (size_t)n * wh + i];
+                const int a = l.type == L_YOLO ? l.mask[n] : n;
+                const int bw = l.type == L_YOLO ? net.w : l.ow, bh = l.type == L_YOLO ? net.h : l.oh;
+                b.x = (col + p[base]) / l.ow;                                  // get_region_box / get_yolo_box
+                b.y = (row + p[base + wh]) / l.oh;
+                b.w = (float)(exp((double)p[base + 2 * (size_t)wh]) * l.anchors[2 * a] / bw);    // exp in double, as in C
+                b.h = (float)(exp((double)p[base + 3 * (size_t)wh]) * l.anchors[2 * a + 1] / bh);
+                if (l.type == L_YOLO) {
+                    b.objectness = obj;
+                    b.classes = l.classes;
+                } else {
+                    b.objectness = obj > thresh ? obj : 0;
+                    if (!b.objectness) continue;
+                }
+                for (int j = 0; j < l.classes; j++) {
+                    const float prob = b.objectness * p[base + (size_t)(5 + j) * wh];
+                    b.prob[j] = (prob > thresh) ? prob : 0;
+                }
+            }
+        }
+        if (l.type == L_REGION) at = first + (size_t)wh * l.num;
+        correct_boxes(dets.data() + first, (int)(at - first), w, h, net.w, net.h);
+    }
+}
+
+// darknet's nms_comparator: descending by objectness (sort_class is -1 throughout do_nms_obj)
+int nms_cmp(const void* pa, const void* pb)
+{
+    const Det* a = (const Det*)pa;
+    const Det* b = (const Det*)pb;
+    float diff = 0;
+    if (b->sort_class >= 0) diff = a->prob[b->sort_class] - b->prob[b->sort_class];
+    else diff = a->objectness - b->objectness;
+    if (diff < 0) return 1;
+    if (diff > 0) return -1;
+    return 0;
+}
+
+float overlap1(float x1, float w1, float x2, float w2)
+{
+    const float l1 = x1 - w1 / 2, l2 = x2 - w2 / 2;
+    const float left = l1 > l2 ? l1 : l2;
+    const float r1 = x1 + w1 / 2, r2 = x2 + w2 / 2;
+    const float right = r1 < r2 ? r1 : r2;
+    return right - left;
+}
+
+float iou(const Det& a, const Det& b)
+{
+    const float w = overlap1(a.x, a.w, b.x, b.w), h = overlap1(a.y, a.h, b.y, b.h);
+    const float inter = (w < 0 || h < 0) ? 0 : w * h;
+    const float uni = a.w * a.h + b.w * b.h - inter;
+    return inter / uni;
+}
+
+// do_nms_obj(dets, total, classes, 0.4): zero-objectness detections swapped to the end, qsort, greedy suppression
+void nms_obj(std::vector<Det>& dets, int classes, float thresh)
+{
+    int k = (int)dets.size() - 1;
+    for (int i = 0; i <= k; i++) {
+        if (dets[i].objectness == 0) {
+            std::swap(dets[i], dets[k]);
+            --k;
+            --i;
+        }
+    }
+    const int total = k + 1;
+    for (int i = 0; i < total; i++) dets[i].sort_class = -1;
+    qsort(dets.data(), total, sizeof(Det), nms_cmp);
+    for (int i = 0; i < total; i++) {
+        if (dets[i].objectness == 0) continue;
+        for (int j = i + 1; j < total; j++) {
+            if (dets[j].objectness == 0) continue;
+            if (iou(dets[i], dets[j]) > thresh) {
+                dets[j].objectness = 0;
+                for (int c = 0; c < classes; c++) dets[j].prob[c] = 0;
+            }
+        }
+    }
+}
+
+struct RoiBox { float x, y, w, h, prob; int cls; };
+
+// detectInThread's extraction (clamped to [0, 1], > 1 % of the frame, one entry per class with a non-zero probability) and the
+// publishing loop (count 1..100, grouped by class in class order, corners by int truncation of (centre -+ size / 2) * frame size)
+int extract(const std::vector<Det>& dets, int classes, int fw, int fh, gf_box* boxes, int* cls, float* probs, int cap)
+{
+    std::vector<RoiBox> roi;
+    for (const Det& d : dets) {
+        float xmin = (float)(d.x - d.w / 2.), xmax = (float)(d.x + d.w / 2.);
+        float ymin = (float)(d.y - d.h / 2.), ymax = (float)(d.y + d.h / 2.);
+        if (xmin < 0) xmin = 0;
+        if (ymin < 0) ymin = 0;
+        if (xmax > 1) xmax = 1;
+        if (ymax > 1) ymax = 1;
+        for (int j = 0; j < classes; j++) {
+            if (d.prob[j]) {
+                const float xc = (xmin + xmax) / 2, yc = (ymin + ymax) / 2;
+                const float bw = xmax - xmin, bh = ymax - ymin;
+                if (bw > 0.01 && bh > 0.01) roi.push_back(RoiBox{xc, yc, bw, bh, d.prob[j], j});
+            }
+        }
+    }
+    const int num = (int)roi.size();
+    if (num <= 0 || num > GF_MAX_BOXES) return 0;
+    int n = 0;
+    for (int c = 0; c < classes; c++)
+        for (const RoiBox& r : roi) {
+            if (r.cls != c) continue;
+            if (n < cap) {
+                boxes[n].xmin = (int)((r.x - r.w / 2) * fw);
+                boxes[n].ymin = (int)((r.y - r.h / 2) * fh);
+                boxes[n].xmax = (int)((r.x + r.w / 2) * fw);
+                boxes[n].ymax = (int)((r.y + r.h / 2) * fh);
+                if (cls) cls[n] = c;
+                if (probs) probs[n] = r.prob;
+            }
+            n++;
+        }
+    return n;
+}
+
+int stage_frame(gf_detector* d, const void* bgr, size_t pitch, int w, int h, int on_device, const uint8_t** src, int* src_pitch)
+{
+    if (on_device) { *src = (const uint8_t*)bgr; *src_pitch = (int)pitch; return GF_OK; }
+    const size_t need = (size_t)3 * w * h;
+    if (need > d->frame_cap) {
+        cudaFree(d->d_frame);
+        d->d_frame = nullptr; d->frame_cap = 0;
+        GF_CUDA(cudaMalloc(&d->d_frame, need));
+        d->frame_cap = need;
+    }
+    GF_CUDA(cudaMemcpy2DAsync(d->d_frame, 3 * (size_t)w, bgr, pitch, 3 * (size_t)w, h, cudaMemcpyHostToDevice, d->st));
+    *src = d->d_frame; *src_pitch = 3 * w;
+    return GF_OK;
+}
+
+int check_frame(const void* bgr, size_t pitch, int w, int h)
+{
+    if (!bgr || w < 1 || h < 1 || w > 16384 || h > 16384 || pitch < (size_t)3 * w || pitch > (1u << 30))
+        return set_err(GF_ERR_INVALID_ARG, "bad frame (BGR8, 1..16384 pixels a side, pitch >= 3 * width)");
+    return GF_OK;
+}
+
+void launch_letterbox(const uint8_t* src, int pitch, int w, int h, int nw, int nh, float* out, cudaStream_t s)
+{
+    int new_w, new_h;
+    letterbox_size(w, h, nw, nh, new_w, new_h);
+    k_yolo_letterbox<<<dim3(blocks(nw, 128), nh, 3), 128, 0, s>>>(src, pitch, w, h, nw, nh, new_w, new_h, out);
+    GF_LAUNCHED();
+}
+
+}  // namespace
+
+extern "C" {
+
+const char* gf_detector_last_error(void) { return g_err; }
+
+int gf_detector_create(gf_detector** out, int device, const char* cfg_path, const char* weights_path, float thresh)
+{
+    if (!out || !cfg_path || !weights_path) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    *out = nullptr;
+    if (!(thresh >= 0.f && thresh < 1.f)) return set_err(GF_ERR_INVALID_ARG, "thresh must lie in [0, 1)");
+    gf_detector* d = new (std::nothrow) gf_detector();
+    if (!d) return set_err(GF_ERR_CUDA, "out of host memory");
+    d->device = device;
+    d->thresh = thresh;
+    // the files first: an unsupported network is refused by name before any device is touched
+    std::string err;
+    int rc = GF_OK;
+    if (!parse_net(cfg_path, d->net, err)) rc = set_err(GF_ERR_UNSUPPORTED, "%s", err.c_str());
+    else if (!load_weights(weights_path, d->net, err)) rc = set_err(GF_ERR_INVALID_ARG, "%s", err.c_str());
+    if (rc) { delete d; return rc; }
+    rc = select_device(device);
+    if (!rc) rc = detector_init(d);
+    if (rc) {
+        char keep[sizeof(g_err)];
+        memcpy(keep, g_err, sizeof(keep));
+        free_detector(d);
+        cudaGetLastError();
+        memcpy(g_err, keep, sizeof(keep));
+        return rc;
+    }
+    *out = d;
+    return GF_OK;
+}
+
+void gf_detector_destroy(gf_detector* d)
+{
+    if (!d) return;
+    cudaSetDevice(d->device);
+    if (d->st) cudaStreamSynchronize(d->st);
+    free_detector(d);
+}
+
+int gf_detector_info(gf_detector* d, int* net_wh, int* n_layers, int* classes)
+{
+    if (!d) return set_err(GF_ERR_INVALID_ARG, "null detector");
+    if (net_wh) { net_wh[0] = d->net.w; net_wh[1] = d->net.h; }
+    if (n_layers) *n_layers = (int)d->net.layers.size();
+    if (classes) *classes = d->net.layers.back().classes;
+    return GF_OK;
+}
+
+int gf_detector_layer_shape(gf_detector* d, int layer, int* whc)
+{
+    if (!d || !whc || layer < -1 || layer >= (int)d->net.layers.size()) return set_err(GF_ERR_INVALID_ARG, "bad argument");
+    if (layer < 0) { whc[0] = d->net.w; whc[1] = d->net.h; whc[2] = 3; return GF_OK; }
+    const Layer& l = d->net.layers[layer];
+    whc[0] = l.ow; whc[1] = l.oh; whc[2] = l.oc;
+    return GF_OK;
+}
+
+int gf_detector_detect(gf_detector* d, const void* bgr, size_t pitch, int w, int h, int on_device, gf_box* boxes, int* class_ids,
+                       float* probs, int cap, int* n_out)
+{
+    if (!d || !n_out || cap < 0 || (cap > 0 && !boxes)) return set_err(GF_ERR_INVALID_ARG, "bad argument");
+    int rc = check_frame(bgr, pitch, w, h);
+    if (rc) return rc;
+    GF_CUDA(cudaSetDevice(d->device));
+    const uint8_t* src;
+    int sp;
+    rc = stage_frame(d, bgr, pitch, w, h, on_device, &src, &sp);
+    if (rc) return rc;
+    GF_CUDA(cudaEventRecord(d->ev0, d->st));
+    launch_letterbox(src, sp, w, h, d->net.w, d->net.h, d->d_input, d->st);
+    GF_CUDA(cudaGetLastError());
+    GF_CUDA(cudaGraphLaunch(d->exec, d->st));
+    GF_CUDA(cudaEventRecord(d->ev1, d->st));
+    GF_CUDA(cudaStreamSynchronize(d->st));
+    d->ran = true;
+    std::vector<Det> dets;
+    network_boxes(d, w, h, dets);
+    const int classes = d->net.layers.back().classes;
+    nms_obj(dets, classes, .4f);
+    *n_out = extract(dets, classes, w, h, boxes, class_ids, probs, cap);
+    if (*n_out > cap) return set_err(GF_ERR_CAPACITY, "more boxes than cap");
+    return GF_OK;
+}
+
+int gf_detector_last_device_ms(gf_detector* d, float* ms)
+{
+    if (!d || !ms || !d->ran) return set_err(GF_ERR_INVALID_ARG, "no detection has run");
+    GF_CUDA(cudaEventElapsedTime(ms, d->ev0, d->ev1));
+    return GF_OK;
+}
+
+int gf_detector_layer_output(gf_detector* d, int layer, float* out, size_t n)
+{
+    if (!d || !out || layer < -1 || layer >= (int)d->net.layers.size()) return set_err(GF_ERR_INVALID_ARG, "bad argument");
+    if (!d->ran) return set_err(GF_ERR_INVALID_ARG, "no detection has run");
+    const size_t need = layer < 0 ? (size_t)3 * d->net.w * d->net.h : (size_t)d->net.layers[layer].outputs;
+    if (n < need) return set_err(GF_ERR_CAPACITY, "output buffer too small");
+    GF_CUDA(cudaSetDevice(d->device));
+    GF_CUDA(cudaMemcpy(out, layer < 0 ? d->d_input : d->dl[layer].out, 4 * need, cudaMemcpyDeviceToHost));
+    return GF_OK;
+}
+
+int gf_detector_layer_times(gf_detector* d, int reps, float* ms)
+{
+    if (!d || !ms || reps < 1) return set_err(GF_ERR_INVALID_ARG, "bad argument");
+    if (!d->ran) return set_err(GF_ERR_INVALID_ARG, "no detection has run");
+    GF_CUDA(cudaSetDevice(d->device));
+    cudaEvent_t a, b;
+    GF_CUDA(cudaEventCreate(&a));
+    GF_CUDA(cudaEventCreate(&b));
+    int rc = GF_OK;
+    for (size_t i = 0; i < d->net.layers.size() && !rc; i++) {
+        cudaEventRecord(a, d->st);
+        for (int r = 0; r < reps && !rc; r++) rc = enqueue_layer(d, (int)i, d->st);
+        cudaEventRecord(b, d->st);
+        if (cudaEventSynchronize(b) != cudaSuccess || cudaEventElapsedTime(ms + i, a, b) != cudaSuccess) rc = set_err(GF_ERR_CUDA, "timing failed");
+        else ms[i] /= reps;
+    }
+    cudaEventDestroy(a);
+    cudaEventDestroy(b);
+    return rc;
+}
+
+int gf_stage_letterbox(int device, const void* bgr, size_t pitch, int w, int h, int on_device, int net_w, int net_h, float* out)
+{
+    if (!out || net_w < 1 || net_h < 1 || net_w > 8192 || net_h > 8192) return set_err(GF_ERR_INVALID_ARG, "bad argument");
+    int rc = check_frame(bgr, pitch, w, h);
+    if (rc) return rc;
+    rc = select_device(device);
+    if (rc) return rc;
+    const uint8_t* src = (const uint8_t*)bgr;
+    uint8_t* tmp = nullptr;
+    float* d_out = nullptr;
+    const size_t n = (size_t)3 * net_w * net_h;
+    if (!on_device) {
+        GF_CUDA(cudaMalloc(&tmp, (size_t)3 * w * h));
+        if (cudaMemcpy2D(tmp, 3 * (size_t)w, bgr, pitch, 3 * (size_t)w, h, cudaMemcpyHostToDevice) != cudaSuccess) {
+            cudaFree(tmp);
+            return set_err(GF_ERR_CUDA, "frame upload failed");
+        }
+        src = tmp; pitch = 3 * (size_t)w;
+    }
+    if (cudaMalloc(&d_out, 4 * n) != cudaSuccess) { cudaFree(tmp); return set_err(GF_ERR_CUDA, "cudaMalloc failed"); }
+    launch_letterbox(src, (int)pitch, w, h, net_w, net_h, d_out, 0);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpy(out, d_out, 4 * n, cudaMemcpyDeviceToHost);
+    cudaFree(d_out);
+    cudaFree(tmp);
+    if (e != cudaSuccess) return set_err(GF_ERR_CUDA, "letterbox failed: %s", cudaGetErrorString(e));
+    return GF_OK;
+}
+
+}  // extern "C"

@@ -1,0 +1,178 @@
+"""YOLO detector on the GPU: the darknet_ros node the reference's use_yolo front end takes its boxes from
+(vins_estimator/src/YoloObjectDetector.cpp), over gf_detector_* (include/gf_b200.h).
+
+    det = YoloDetector("yolov3.cfg", "yolov3.weights", thresh=0.3)
+    boxes, class_ids, probs = det.detect(bgr)          # boxes (m, 4) int64 xmin, ymin, xmax, ymax, as darknet_ros publishes them
+    tracker.trackImagebox(t, boxes, gray, depth)
+
+The network is read from the user's darknet cfg and .weights at run time; the forward pass is bit-exact with darknet's CPU build.
+parse_cfg() gives the layer shapes darknet derives from a cfg, on the host.  No CPU fallback: without a device every call raises.
+"""
+import ctypes
+
+import numpy as np
+
+from . import _lib
+
+_LAYER_TYPES = {"convolutional": "convolutional", "conv": "convolutional", "maxpool": "maxpool", "max": "maxpool",
+                "route": "route", "reorg": "reorg", "shortcut": "shortcut", "upsample": "upsample", "region": "region",
+                "yolo": "yolo"}
+
+
+def _sections(path):
+    secs = []
+    with open(path) as f:
+        for line in f:
+            s = "".join(ch for ch in line if ch not in " \t\n\r")
+            if not s or s[0] in "#;":
+                continue
+            if s[0] == "[":
+                secs.append((s[1:s.index("]")] if "]" in s else s[1:], {}))
+                continue
+            k, _, v = s.partition("=")
+            secs[-1][1][k] = v
+    return secs
+
+
+def parse_cfg(path):
+    """The layers of a darknet cfg as darknet's constructors size them: a list of dicts with `type` (darknet's name),
+    w, h, c (input), out_w, out_h, out_c and outputs, plus the parameters the weights file depends on (n, size, c and
+    batch_normalize of a convolutional layer).  Returns (net, layers) with net = dict(w, h, c).  Only the layer types the
+    detector supports are sized; another raises ValueError, as creation refuses it."""
+    secs = _sections(path)
+    if not secs or secs[0][0] not in ("net", "network"):
+        raise ValueError("cfg must start with [net]")
+    opt = secs[0][1]
+    net = {"w": int(opt.get("width", 0)), "h": int(opt.get("height", 0)), "c": int(opt.get("channels", 0))}
+    w, h, c = net["w"], net["h"], net["c"]
+    layers = []
+    for i, (name, o) in enumerate(secs[1:]):
+        t = _LAYER_TYPES.get(name)
+        if t is None:
+            raise ValueError("unsupported layer type [%s]" % name)
+        L = {"type": t, "w": w, "h": h, "c": c}
+        gi = lambda k, d: int(o.get(k, d))
+        if t == "convolutional":
+            size, stride = gi("size", 1), gi("stride", 1)
+            pad = size // 2 if gi("pad", 0) else gi("padding", 0)
+            n = gi("filters", 1)
+            L.update(n=n, size=size, stride=stride, pad=pad, batch_normalize=gi("batch_normalize", 0),
+                     out_w=(w + 2 * pad - size) // stride + 1, out_h=(h + 2 * pad - size) // stride + 1, out_c=n)
+        elif t == "maxpool":
+            stride = gi("stride", 1)
+            size = gi("size", stride)
+            pad = gi("padding", size - 1)
+            L.update(size=size, stride=stride, out_w=(w + pad - size) // stride + 1, out_h=(h + pad - size) // stride + 1, out_c=c)
+        elif t == "route":
+            idx = [int(v) for v in o["layers"].split(",")]
+            idx = [i + k if k < 0 else k for k in idx]
+            first = layers[idx[0]]
+            L.update(inputs=idx, out_w=first["out_w"], out_h=first["out_h"], out_c=sum(layers[k]["out_c"] for k in idx))
+        elif t == "reorg":
+            s = gi("stride", 1)
+            L.update(stride=s, out_w=w // s, out_h=h // s, out_c=c * s * s)
+        elif t == "shortcut":
+            k = int(o["from"])
+            k = i + k if k < 0 else k
+            L.update(index=k, out_w=w, out_h=h, out_c=c)
+        elif t == "upsample":
+            s = gi("stride", 2)
+            L.update(stride=s, out_w=w * s, out_h=h * s, out_c=c)
+        elif t == "region":
+            L.update(classes=gi("classes", 20), num=gi("num", 1), coords=gi("coords", 4), out_w=w, out_h=h, out_c=c)
+        elif t == "yolo":
+            mask = o.get("mask")
+            num = len(mask.split(",")) if mask else gi("num", 1)
+            L.update(classes=gi("classes", 20), num=num, out_w=w, out_h=h, out_c=c)
+        L["outputs"] = L["out_w"] * L["out_h"] * L["out_c"]
+        layers.append(L)
+        w, h, c = L["out_w"], L["out_h"], L["out_c"]
+    return net, layers
+
+
+def _frame(bgr):
+    """(pointer, pitch, w, h, on_device, keep-alive) of a BGR8 frame: a numpy (h, w, 3) uint8 array with contiguous rows, or a
+    CUDA torch tensor of that shape and layout."""
+    if hasattr(bgr, "is_cuda") and bgr.is_cuda:
+        if bgr.dtype.itemsize != 1 or bgr.dim() != 3 or bgr.shape[2] != 3 or bgr.stride(2) != 1 or bgr.stride(1) != 3:
+            raise ValueError("frame must be (h, w, 3) uint8 with contiguous rows")
+        return bgr.data_ptr(), bgr.stride(0), bgr.shape[1], bgr.shape[0], 1, bgr
+    a = np.asarray(bgr)
+    if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
+        raise ValueError("frame must be (h, w, 3) uint8")
+    if a.strides[2] != 1 or a.strides[1] != 3:
+        a = np.ascontiguousarray(a)
+    return a.ctypes.data, a.strides[0], a.shape[1], a.shape[0], 0, a
+
+
+class YoloDetector:
+    """darknet_ros's detector for one network on one GPU.  thresh is the node's detection threshold (its yaml's
+    threshold / value); the NMS threshold 0.4 and hier 0.5 are the node's constants."""
+
+    def __init__(self, cfg, weights, thresh=0.3, device=0):
+        L = _lib.yolo_lib()
+        self._L = L
+        self._h = ctypes.c_void_p()
+        _lib.check_yolo(L.gf_detector_create(ctypes.byref(self._h), device, str(cfg).encode(), str(weights).encode(), ctypes.c_float(thresh)))
+        wh = (ctypes.c_int * 2)()
+        nl, nc = ctypes.c_int(), ctypes.c_int()
+        _lib.check_yolo(L.gf_detector_info(self._h, wh, ctypes.byref(nl), ctypes.byref(nc)))
+        self.net_w, self.net_h, self.n_layers, self.classes = wh[0], wh[1], nl.value, nc.value
+        self.thresh = thresh
+        self._boxes = np.zeros((_lib.GF_MAX_BOXES, 4), np.int64)
+        self._cls = np.zeros(_lib.GF_MAX_BOXES, np.int32)
+        self._prob = np.zeros(_lib.GF_MAX_BOXES, np.float32)
+
+    def detect(self, bgr):
+        """boxes (m, 4) int64, class_ids (m,) int32, probs (m,) float32 of one BGR8 frame (m = 0 when the node publishes nothing)."""
+        ptr, pitch, w, h, on_dev, _keep = _frame(bgr)
+        n = ctypes.c_int()
+        _lib.check_yolo(self._L.gf_detector_detect(self._h, ptr, pitch, w, h, on_dev, self._boxes.ctypes.data, self._cls.ctypes.data,
+                                              self._prob.ctypes.data, _lib.GF_MAX_BOXES, ctypes.byref(n)))
+        m = n.value
+        return self._boxes[:m].copy(), self._cls[:m].copy(), self._prob[:m].copy()
+
+    def layer_shape(self, i):
+        whc = (ctypes.c_int * 3)()
+        _lib.check_yolo(self._L.gf_detector_layer_shape(self._h, i, whc))
+        return whc[2], whc[1], whc[0]
+
+    def layer_output(self, i):
+        """Layer i's output of the last detect as (c, h, w) float32; i = -1: the letterboxed input."""
+        shape = self.layer_shape(i)
+        out = np.empty(shape, np.float32)
+        _lib.check_yolo(self._L.gf_detector_layer_output(self._h, i, out.ctypes.data, out.size))
+        return out
+
+    def input_image(self):
+        return self.layer_output(-1)
+
+    def last_device_ms(self):
+        ms = ctypes.c_float()
+        _lib.check_yolo(self._L.gf_detector_last_device_ms(self._h, ctypes.byref(ms)))
+        return ms.value
+
+    def layer_times(self, reps=20):
+        """Mean device ms of each layer's kernels, re-run `reps` times on the last frame's data (profiling)."""
+        ms = np.zeros(self.n_layers, np.float32)
+        _lib.check_yolo(self._L.gf_detector_layer_times(self._h, reps, ms.ctypes.data))
+        return ms
+
+    def close(self):
+        if self._h:
+            self._L.gf_detector_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def letterbox(bgr, net_w, net_h, device=0):
+    """The detector's input image for a BGR8 frame, (3, net_h, net_w) float32: darknet's letterbox_image as the node calls it."""
+    ptr, pitch, w, h, on_dev, _keep = _frame(bgr)
+    out = np.empty((3, net_h, net_w), np.float32)
+    _lib.check_yolo(_lib.yolo_lib().gf_stage_letterbox(device, ptr, pitch, w, h, on_dev, net_w, net_h, out.ctypes.data))
+    return out

@@ -227,13 +227,17 @@ class WindowEstimator:
 
 
 def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=True, max_iter=8, feedback=False, use_mcc=False, boxes=None,
-           dense_map=None, grid_map=None):
+           dense_map=None, grid_map=None, detector=None):
     """Runs n_frames of `stream` through tracker -> fm -> ba.  Returns dict(t, P_est, P_gt, R_est, R_gt, keyframes, ...).
     tracker.trackImage(t, gray, depth) -> {id: v[8]};  fm / ba: see WindowEstimator.  feedback: the estimator calls the tracker's
     removeOutliers / setPrediction after every optimisation (the reference with MULTIPLE_THREAD 0).
     boxes: USE_YOLO -- the detections of frame k in boxes[k] ((m, 4) xmin, ymin, xmax, ymax).  A frame with detections goes
     through tracker.trackImagebox(t, boxes[k], gray, depth), one without through trackImage, as sync_process does
     (rosNodeTest.cpp:433-439, 519-540).
+    detector: USE_YOLO with the detector in the loop (a YoloDetector, or anything with detect(bgr) -> (boxes, class_ids, probs)):
+    frame k's boxes are detector.detect(BGR of stream.color(k)), computed before frame k is tracked, so they belong to frame k.
+    The darknet_ros node's three-slot asynchronous buffer, and the frames of latency it adds, are not reproduced.  Exclusive
+    with boxes.
     dense_map: a map with addKeyFrame(R, P, rgb, depth) (DenseMap, or the oracle's), fed as pubKeyframe feeds the mapping node
     (visualization.cpp): after every MARGIN_OLD, the pose of window frame WINDOW_SIZE - 2 with that frame's colour and depth
     images (stream.color / stream.frame), unless its position equals the previous keyframe's exactly, as the node skips it.  It is returned under "dense_map".
@@ -242,6 +246,8 @@ def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=Tru
     under "grid_map"."""
     if grid_map is not None and dense_map is None:
         raise ValueError("grid_map requires dense_map")
+    if detector is not None and boxes is not None:
+        raise ValueError("boxes and detector are exclusive")
     imu = ImuFromStream(stream)
     est = WindowEstimator(fm, ba, imu_propagate=imu_propagate, max_iter=max_iter, tracker=tracker if feedback else None, use_mcc=use_mcc)
     out_t, out_P, out_R, gt_P, gt_R, iters = [], [], [], [], [], []
@@ -258,8 +264,11 @@ def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=Tru
                 est.processIMU(dt, acc, gyr)
         else:
             acc, gyr = imu.sample(t); est.processIMU(0.0, acc, gyr)
-        if boxes is not None and len(boxes[k]) > 0:
-            image = tracker.trackImagebox(t, boxes[k], gray, depth)
+        frame_boxes = boxes[k] if boxes is not None else None
+        if detector is not None:
+            frame_boxes = detector.detect(np.ascontiguousarray(stream.color(k)[..., ::-1]))[0]
+        if frame_boxes is not None and len(frame_boxes) > 0:
+            image = tracker.trackImagebox(t, frame_boxes, gray, depth)
         else:
             image = tracker.trackImage(t, gray, depth)
         if not est.nonlinear:                           # initialisation is out of scope: ground-truth states while the window fills

@@ -822,6 +822,43 @@ int gf_grid_map_size(gf_grid_map* map, int* size_x, int* size_y, int* n_keyframe
  * (a repeated no-op update, a cell at 0 or 1) and the longest per-cell run within one chunk. */
 int gf_grid_map_stats(gf_grid_map* map, int64_t* out4);
 
+/* ---- YOLO detector (the use_yolo front end's darknet_ros node, YoloObjectDetector.cpp, on the GPU) ------------------------
+ * darknet's inference forward pass for the networks the reference ships (vins_estimator/yolo_network_config/cfg: [net],
+ * [convolutional], [maxpool], [route], [reorg], [shortcut], [upsample], [region], [yolo]; activations leaky and linear; batch 1),
+ * bit-exact with darknet's CPU build, followed by the node's decoding (get_network_boxes with hier 0.5, do_nms_obj 0.4) and box
+ * extraction.  The boxes feed gf_tracker_*_boxes / trackImagebox.
+ * The detector is implemented in its own library, libgf_yolo.so, built next to libgf_b200.so: libgf_b200.so exports these
+ * entry points as forwarders that open it on the first call, so it carries none of the detector's device code and a process
+ * that never detects never loads it.  A failing call sets gf_last_error() as usual; gf_detector_last_error() is the same
+ * text as libgf_yolo.so holds it. */
+typedef struct gf_detector gf_detector;
+/* Text of the last error raised by a gf_detector_* / gf_stage_letterbox call on the calling thread (never NULL). */
+const char* gf_detector_last_error(void);
+/* The network is read from a darknet cfg and .weights file.  A layer type, activation or key value outside the set above:
+ * GF_ERR_UNSUPPORTED with the reason in gf_last_error(); a missing or short weights file: GF_ERR_INVALID_ARG.  thresh in [0, 1)
+ * is darknet_ros's detection threshold.  Every parameter goes to device memory here, once. */
+int gf_detector_create(gf_detector** det, int device, const char* cfg_path, const char* weights_path, float thresh);
+void gf_detector_destroy(gf_detector* det);
+/* net_wh[2] = the [net] width and height; n_layers excludes [net]; classes of the last layer.  All three nullable. */
+int gf_detector_info(gf_detector* det, int* net_wh, int* n_layers, int* classes);
+/* One frame: BGR8, w x h pixels, rows `pitch` bytes apart, a host pointer or a device pointer when on_device != 0.  Writes the
+ * boxes darknet_ros would publish, grouped by class in class order, with their class ids and probabilities (both nullable), and
+ * their count in *n_out: 0 when there are none or more than GF_MAX_BOXES.  cap < *n_out: GF_ERR_CAPACITY (nothing past cap
+ * written).  Synchronous: the boxes belong to this frame. */
+int gf_detector_detect(gf_detector* det, const void* bgr, size_t pitch, int w, int h, int on_device, gf_box* boxes, int* class_ids,
+                       float* probs, int cap, int* n_out);
+/* Device time of the last detect (letterbox + network), from CUDA events. */
+int gf_detector_last_device_ms(gf_detector* det, float* ms);
+/* whc[3] = output width, height and channels of layer `layer` (0-based, [net] excluded), or of the letterboxed input for -1. */
+int gf_detector_layer_shape(gf_detector* det, int layer, int* whc);
+/* Host copy of layer `layer`'s output after the last detect, planar [c][h][w] float; -1: the letterboxed input.  n is the
+ * capacity of out in floats. */
+int gf_detector_layer_output(gf_detector* det, int layer, float* out, size_t n);
+/* Mean device time of each layer's kernels over `reps` launches on the last frame's data, into ms[n_layers] (profiling). */
+int gf_detector_layer_times(gf_detector* det, int reps, float* ms);
+/* Stage: darknet's letterbox of a BGR8 frame at net_w x net_h into out [3][net_h][net_w] (host), as gf_detector_detect does it. */
+int gf_stage_letterbox(int device, const void* bgr, size_t pitch, int w, int h, int on_device, int net_w, int net_h, float* out);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif
