@@ -45,6 +45,7 @@ $(YOLO_OUT): $(BUILD)/yolo_detector.o
 oracle: oracle/_build/libgf_oracle_dm.so oracle/_build/libgf_oracle_gm.so
 	$(MAKE) -C oracle
 	$(MAKE) -C oracle -f darknet.mk
+	$(MAKE) -C oracle -f yolo_heads.mk
 # the dense map's sequential restatement (tests and tools/bench_dense_map.py only): -O3 -ffp-contract=off as oracle/Makefile's
 # libgf_oracle_ba.so, plus -msse2 -mfpmath=sse as its libgf_oracle_fe.so
 oracle/_build/libgf_oracle_dm.so: oracle/dm_oracle.c

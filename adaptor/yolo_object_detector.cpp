@@ -12,6 +12,12 @@ YoloObjectDetector::YoloObjectDetector(const std::string& cfg, const std::string
 
 YoloObjectDetector::~YoloObjectDetector() { gf_detector_destroy(det_); }
 
+void YoloObjectDetector::setPrecision(int precision)
+{
+    if (gf_detector_set_precision(det_, precision) != GF_OK)
+        throw std::runtime_error(std::string("gf_detector_set_precision: ") + gf_detector_last_error());
+}
+
 darknet_ros_msgs::BoundingBoxes YoloObjectDetector::detect(const cv::Mat& bgr, double stamp)
 {
     gf_box boxes[GF_MAX_BOXES];

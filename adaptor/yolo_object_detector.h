@@ -23,6 +23,9 @@ public:
 
     // One frame (CV_8UC3, BGR).  Empty bounding_boxes when the node would publish nothing (no box, or more than 100).
     darknet_ros_msgs::BoundingBoxes detect(const cv::Mat& bgr, double stamp = 0);
+    // GF_DETECTOR_EXACT (the default: bit-exact with darknet's CPU build) or GF_DETECTOR_TF32 (tensor-core convolutions with
+    // TF32-rounded operands, not bit-exact).  Throws std::runtime_error on another value or a device failure.
+    void setPrecision(int precision);
 
 private:
     gf_detector* det_ = nullptr;

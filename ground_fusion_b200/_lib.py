@@ -183,7 +183,8 @@ _YOLO = None
 
 
 def yolo_lib():
-    """libgf_yolo.so: the YOLO detector's C ABI (gf_detector_*, gf_stage_letterbox), built next to libgf_b200.so."""
+    """libgf_yolo.so: the YOLO detector's C ABI (gf_detector_*, gf_stage_letterbox, gf_stage_yolo_conv), built next to
+    libgf_b200.so."""
     global _YOLO
     if _YOLO is None:
         if not os.path.exists(YOLO_LIB_PATH):
@@ -203,6 +204,9 @@ def yolo_lib():
         L.gf_detector_layer_output.argtypes = [vp, i, vp, sz]
         L.gf_detector_layer_times.argtypes = [vp, i, vp]
         L.gf_stage_letterbox.argtypes = [i, vp, sz, i, i, i, i, i, vp]
+        L.gf_detector_set_precision.argtypes = [vp, i]
+        L.gf_detector_get_precision.argtypes = [vp, ip]
+        L.gf_stage_yolo_conv.argtypes = [i, i, vp, vp, vp, vp, vp, vp, vp, vp]
         _YOLO = L
     return _YOLO
 

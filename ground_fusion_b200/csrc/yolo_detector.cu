@@ -4,7 +4,8 @@
 //            CUDA graph: the layers' kernels (yolo_kernels.cuh) and the copies of the [region] / [yolo] outputs to pinned memory
 //   detect   the frame to the device, k_yolo_letterbox, the graph, then on the host darknet's decoding
 //            (get_network_boxes(w, h, thresh, 0.5, 0, 1)), do_nms_obj(0.4) with libc qsort, and darknet_ros's extraction
-// DESIGN.md "YOLO detector" has the arithmetic and why there are no tensor cores here.
+// DESIGN.md "YOLO detector" has the arithmetic and why the default mode uses no tensor cores; gf_detector_set_precision
+// selects the TF32 tensor-core convolutions (yolo_tf32.cuh) instead, every other kernel unchanged.
 // Built as its own library, libgf_yolo.so, with its own error text (gf_detector_last_error); libgf_b200.so exports the same
 // entry points as forwarders (yolo_forward.cpp) and carries none of this device code, so a tracker / estimator process that
 // never detects loads exactly what it loaded before.
@@ -19,6 +20,7 @@
 #include "gf_common.cuh"
 #include "yolo_cfg.cuh"
 #include "yolo_kernels.cuh"
+#include "yolo_tf32.cuh"
 
 using namespace gf;
 using namespace gfy;
@@ -34,6 +36,9 @@ struct DevLayer {
     float* out = nullptr;
     float *w = nullptr, *bias = nullptr, *scale = nullptr, *mean = nullptr;
     double* den = nullptr;
+    float* w_tf32 = nullptr;             // the weights rounded to TF32, [n][kp], allocated by the first switch to TF32
+    int kp = 0;                          // K rounded up to 4
+    int* ktab = nullptr;                 // the TF32 kernel's im2col table (tf32_ktab), allocated with w_tf32
     float* host_out = nullptr;           // pinned copy of a [region] / [yolo] output
 };
 
@@ -62,6 +67,8 @@ struct gf_detector {
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    int precision = GF_DETECTOR_EXACT;
+    float* d_part = nullptr;             // the TF32 split-K partial sums, sized for the layer that needs most
     std::vector<float> prob_store;
     bool ran = false;
 };
@@ -83,10 +90,11 @@ void free_detector(gf_detector* d)
     if (d->exec) cudaGraphExecDestroy(d->exec);
     if (d->graph) cudaGraphDestroy(d->graph);
     for (DevLayer& l : d->dl) {
-        cudaFree(l.out); cudaFree(l.w); cudaFree(l.bias); cudaFree(l.scale); cudaFree(l.mean); cudaFree(l.den);
+        cudaFree(l.out); cudaFree(l.w); cudaFree(l.bias); cudaFree(l.scale); cudaFree(l.mean); cudaFree(l.den); cudaFree(l.w_tf32); cudaFree(l.ktab);
         if (l.host_out) cudaFreeHost(l.host_out);
     }
     cudaFree(d->d_input);
+    cudaFree(d->d_part);
     cudaFree(d->d_frame);
     if (d->ev0) cudaEventDestroy(d->ev0);
     if (d->ev1) cudaEventDestroy(d->ev1);
@@ -119,6 +127,86 @@ void launch_conv(const ConvArgs& a, cudaStream_t s)
     GF_LAUNCHED();
 }
 
+// a TF32 convolution's device operands: the rounded weights [M][kp], the im2col table, the split-K workspace (if it splits)
+struct Tf32Operands {
+    const float* w = nullptr;
+    int kp = 0;
+    const int* ktab = nullptr;
+    float* part = nullptr;
+};
+
+// split-K of a TF32 layer from its shape alone: enough 64 x 64 CTAs for four per SM of the H100's 132 (the kernel's occupancy),
+// each split at least 4 stages of TC_BK; splits = 1 for layers whose tiles already fill the GPU
+struct Tf32Plan { int splits, nsp; };
+Tf32Plan tf32_plan(int M, int N, int K)
+{
+    const int ns = (K + TC_BK - 1) / TC_BK;
+    const long tiles = (long)blocks(N, 64) * blocks(M, 64);
+    int want = (int)std::min<long>(std::max<long>(528 / tiles, 1), std::max(ns / 4, 1));
+    const int nsp = (ns + want - 1) / want;
+    return Tf32Plan{(ns + nsp - 1) / nsp, nsp};
+}
+
+// the im2col table of a layer (yolo_tf32.cuh): per k, c H W + ky W + kx and ky << 16 | kx; padded to whole stages with
+// entries no bounds test accepts
+std::vector<int> tf32_ktab(int C, int H, int W, int size)
+{
+    const int K = C * size * size, ns = (K + TC_BK - 1) / TC_BK;
+    std::vector<int> t(2 * (size_t)ns * TC_BK);
+    for (int k = 0; k < ns * TC_BK; k++) {
+        if (k >= K) { t[2 * k] = 0; t[2 * k + 1] = TC_KTAB_PAD << 16; continue; }
+        const int c = k / (size * size), ky = k / size % size, kx = k % size;
+        t[2 * k] = c * H * W + ky * W + kx;
+        t[2 * k + 1] = ky << 16 | kx;
+    }
+    return t;
+}
+
+size_t tf32_part_floats(int M, int N, int K)
+{
+    const Tf32Plan pl = tf32_plan(M, N, K);
+    return pl.splits > 1 ? (size_t)pl.splits * M * N : 0;
+}
+
+// the TF32 kernel's dynamic shared memory (32 KB); before any launch or capture
+int tf32_setup()
+{
+    GF_CUDA(cudaFuncSetAttribute(k_yolo_conv_tf32<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (64 + 64) * TC_BK * 8));
+    return GF_OK;
+}
+
+// one convolution at `precision`, the tile and split chosen from the layer's shape alone (the detector and gf_stage_yolo_conv
+// both come here)
+void launch_conv_layer(ConvArgs a, int precision, const Tf32Operands& t, cudaStream_t s)
+{
+    if (precision == GF_DETECTOR_TF32) {
+        a.w = t.w;
+        const Tf32Plan pl = tf32_plan(a.M, a.N, a.K);
+        float* part = pl.splits > 1 ? t.part : nullptr;
+        k_yolo_conv_tf32<64, 64><<<dim3(blocks(a.N, 64), blocks(a.M, 64), pl.splits), 128, (64 + 64) * TC_BK * 8, s>>>(
+            a, t.kp, reinterpret_cast<const int4*>(t.ktab), pl.nsp, part);
+        GF_LAUNCHED();
+        if (part) {
+            k_yolo_splitk_reduce<<<blocks((long)a.M * a.N, 256), 256, 0, s>>>(a, part, pl.splits);
+            GF_LAUNCHED();
+        }
+        return;
+    }
+    // 64 x 64 tiles where they fill the GPU twice over, 32 x 32 where the layer is small
+    if ((long)blocks(a.N, 64) * blocks(a.M, 64) >= 264) launch_conv<64, 64>(a, s);
+    else launch_conv<32, 32>(a, s);
+}
+
+// a layer's TF32 weight copy, rounded on the device by k_yolo_round_weights_tf32
+int round_weights_tf32(const float* w, int M, int K, int kp, float** out, cudaStream_t s)
+{
+    GF_CUDA(cudaMalloc(out, 4 * (size_t)M * kp));
+    k_yolo_round_weights_tf32<<<blocks((long)M * kp, 256), 256, 0, s>>>(w, M, K, kp, *out);
+    GF_LAUNCHED();
+    GF_CUDA(cudaGetLastError());
+    return GF_OK;
+}
+
 // layer i's kernels on stream s (captured into the graph)
 int enqueue_layer(gf_detector* d, int i, cudaStream_t s)
 {
@@ -130,9 +218,9 @@ int enqueue_layer(gf_detector* d, int i, cudaStream_t s)
     case L_CONV: {
         ConvArgs a{in, o.w, o.out, o.bias, o.scale, o.mean, o.den, l.c, l.h, l.w, l.n, l.c * l.size * l.size, l.ow, l.ow * l.oh,
                    l.size, l.stride, l.pad, l.bn, l.act};
-        // 64 x 64 tiles where they fill the GPU twice over, 32 x 32 where the layer is small
-        if ((long)blocks(a.N, 64) * blocks(a.M, 64) >= 264) launch_conv<64, 64>(a, s);
-        else launch_conv<32, 32>(a, s);
+        Tf32Operands t;
+        t.w = o.w_tf32; t.kp = o.kp; t.ktab = o.ktab; t.part = d->d_part;
+        launch_conv_layer(a, d->precision, t, s);
         break;
     }
     case L_MAXPOOL:
@@ -170,6 +258,8 @@ int enqueue_layer(gf_detector* d, int i, cudaStream_t s)
     return GF_OK;
 }
 
+int capture(gf_detector* d);
+
 int detector_init(gf_detector* d)
 {
     GF_CUDA(cudaStreamCreateWithFlags(&d->st, cudaStreamNonBlocking));
@@ -195,6 +285,12 @@ int detector_init(gf_detector* d)
         }
         if (l.type == L_REGION || l.type == L_YOLO) GF_CUDA(cudaMallocHost(&o.host_out, 4 * (size_t)l.outputs));
     }
+    return capture(d);
+}
+
+// the forward pass at d->precision captured as one graph; replaces the detector's graph only once the new one is instantiated
+int capture(gf_detector* d)
+{
     GF_CUDA(cudaStreamBeginCapture(d->st, cudaStreamCaptureModeThreadLocal));
     int rc = GF_OK;
     for (size_t i = 0; i < d->net.layers.size() && !rc; i++) rc = enqueue_layer(d, (int)i, d->st);
@@ -202,8 +298,15 @@ int detector_init(gf_detector* d)
     const cudaError_t e = cudaStreamEndCapture(d->st, &g);
     if (rc) { if (g) cudaGraphDestroy(g); return rc; }
     GF_CUDA(e);
+    cudaGraphExec_t x = nullptr;
+    if (cudaGraphInstantiate(&x, g, 0) != cudaSuccess) {
+        cudaGraphDestroy(g);
+        return set_err(GF_ERR_CUDA, "cudaGraphInstantiate failed");
+    }
+    if (d->exec) cudaGraphExecDestroy(d->exec);
+    if (d->graph) cudaGraphDestroy(d->graph);
     d->graph = g;
-    GF_CUDA(cudaGraphInstantiate(&d->exec, d->graph, 0));
+    d->exec = x;
     return GF_OK;
 }
 
@@ -562,6 +665,102 @@ int gf_stage_letterbox(int device, const void* bgr, size_t pitch, int w, int h, 
     cudaFree(d_out);
     cudaFree(tmp);
     if (e != cudaSuccess) return set_err(GF_ERR_CUDA, "letterbox failed: %s", cudaGetErrorString(e));
+    return GF_OK;
+}
+
+int gf_detector_set_precision(gf_detector* d, int precision)
+{
+    if (!d) return set_err(GF_ERR_INVALID_ARG, "null detector");
+    if (precision != GF_DETECTOR_EXACT && precision != GF_DETECTOR_TF32)
+        return set_err(GF_ERR_INVALID_ARG, "precision must be GF_DETECTOR_EXACT (0) or GF_DETECTOR_TF32 (1)");
+    if (precision == d->precision) return GF_OK;
+    GF_CUDA(cudaSetDevice(d->device));
+    GF_CUDA(cudaStreamSynchronize(d->st));
+    if (precision == GF_DETECTOR_TF32) {
+        int rc = tf32_setup();
+        size_t part = 0;
+        for (size_t i = 0; i < d->net.layers.size() && !rc; i++) {
+            const Layer& l = d->net.layers[i];
+            DevLayer& o = d->dl[i];
+            if (l.type != L_CONV) continue;
+            const int K = l.c * l.size * l.size;
+            part = std::max(part, tf32_part_floats(l.n, l.ow * l.oh, K));
+            if (o.w_tf32) continue;
+            o.kp = (K + 3) / 4 * 4;
+            rc = round_weights_tf32(o.w, l.n, K, o.kp, &o.w_tf32, d->st);
+            if (!rc) rc = upload(&o.ktab, tf32_ktab(l.c, l.h, l.w, l.size));
+        }
+        if (!rc && part && !d->d_part && cudaMalloc(&d->d_part, 4 * part) != cudaSuccess) rc = set_err(GF_ERR_CUDA, "cudaMalloc failed");
+        if (!rc && cudaStreamSynchronize(d->st) != cudaSuccess) rc = set_err(GF_ERR_CUDA, "rounding the weights to TF32 failed");
+        if (rc) return rc;
+    }
+    const int keep = d->precision;
+    d->precision = precision;
+    const int rc = capture(d);
+    if (rc) d->precision = keep;                 // the old graph is still in place
+    return rc;
+}
+
+int gf_detector_get_precision(gf_detector* d, int* precision)
+{
+    if (!d || !precision) return set_err(GF_ERR_INVALID_ARG, "bad argument");
+    *precision = d->precision;
+    return GF_OK;
+}
+
+int gf_stage_yolo_conv(int device, int precision, const int* shape, const float* in, const float* w, const float* bias,
+                       const float* scale, const float* mean, const float* var, float* out)
+{
+    if (!shape || !in || !w || !bias || !out) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    if (precision != GF_DETECTOR_EXACT && precision != GF_DETECTOR_TF32) return set_err(GF_ERR_INVALID_ARG, "bad precision");
+    const int C = shape[0], H = shape[1], W = shape[2], M = shape[3], size = shape[4], stride = shape[5], pad = shape[6];
+    const int bn = shape[7], act_ = shape[8];
+    if (C < 1 || H < 1 || W < 1 || M < 1 || size < 1 || stride < 1 || pad < 0 || (bn != 0 && bn != 1) || (act_ != 0 && act_ != 1) ||
+        (long)C * H * W > (1l << 28) || (long)C * size * size > (1l << 20) || (bn && (!scale || !mean || !var)))
+        return set_err(GF_ERR_INVALID_ARG, "bad shape (C H W M size stride pad bn act)");
+    const int OW = (W + 2 * pad - size) / stride + 1, OH = (H + 2 * pad - size) / stride + 1;
+    if (OW < 1 || OH < 1) return set_err(GF_ERR_INVALID_ARG, "empty output");
+    const int K = C * size * size, N = OW * OH, kp = (K + 3) / 4 * 4;
+    if ((long)M * N > (1l << 28) || (long)M * K > (1l << 28)) return set_err(GF_ERR_INVALID_ARG, "layer too large");
+    int rc = select_device(device);
+    if (!rc && precision == GF_DETECTOR_TF32) rc = tf32_setup();
+    if (rc) return rc;
+    std::vector<double> den(bn ? M : 0);
+    for (int m = 0; m < (bn ? M : 0); m++) den[m] = sqrt((double)var[m]) + (double).000001f;     // as detector_init
+    float *d_in = nullptr, *d_w = nullptr, *d_b = nullptr, *d_sc = nullptr, *d_mu = nullptr, *d_out = nullptr, *d_wt = nullptr;
+    float* d_part = nullptr;
+    int* d_ktab = nullptr;
+    double* d_den = nullptr;
+    cudaError_t e = cudaSuccess;
+    auto put = [&](auto** dst, const auto* src, size_t n) {
+        if (e == cudaSuccess) e = cudaMalloc(dst, sizeof(*src) * n);
+        if (e == cudaSuccess) e = cudaMemcpy(*dst, src, sizeof(*src) * n, cudaMemcpyHostToDevice);
+    };
+    put(&d_in, in, (size_t)C * H * W);
+    put(&d_w, w, (size_t)M * K);
+    put(&d_b, bias, (size_t)M);
+    if (bn) { put(&d_sc, scale, (size_t)M); put(&d_mu, mean, (size_t)M); put(&d_den, den.data(), (size_t)M); }
+    if (e == cudaSuccess) e = cudaMalloc(&d_out, 4 * (size_t)M * N);
+    if (e == cudaSuccess && precision == GF_DETECTOR_TF32) {
+        rc = round_weights_tf32(d_w, M, K, kp, &d_wt, 0);
+        const std::vector<int> tab = tf32_ktab(C, H, W, size);
+        if (!rc) put(&d_ktab, tab.data(), tab.size());
+        const size_t np = tf32_part_floats(M, N, K);
+        if (!rc && np && e == cudaSuccess) e = cudaMalloc(&d_part, 4 * np);
+        if (rc) e = cudaErrorUnknown;
+    }
+    if (e == cudaSuccess) {
+        const ConvArgs a{d_in, d_w, d_out, d_b, d_sc, d_mu, d_den, C, H, W, M, K, OW, N, size, stride, pad, bn, act_};
+        Tf32Operands t;
+        t.w = d_wt; t.kp = kp; t.ktab = d_ktab; t.part = d_part;
+        launch_conv_layer(a, precision, t, 0);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(out, d_out, 4 * (size_t)M * N, cudaMemcpyDeviceToHost);
+    cudaFree(d_in); cudaFree(d_w); cudaFree(d_b); cudaFree(d_sc); cudaFree(d_mu); cudaFree(d_den); cudaFree(d_out); cudaFree(d_wt);
+    cudaFree(d_part); cudaFree(d_ktab);
+    if (rc) return rc;
+    if (e != cudaSuccess) return set_err(GF_ERR_CUDA, "convolution stage failed: %s", cudaGetErrorString(e));
     return GF_OK;
 }
 

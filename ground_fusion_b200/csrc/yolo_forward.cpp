@@ -85,6 +85,11 @@ GF_FORWARD(gf_detector_layer_times, (gf_detector* det, int reps, float* ms), (de
 GF_FORWARD(gf_stage_letterbox, (int device, const void* bgr, size_t pitch, int w, int h, int on_device, int net_w, int net_h,
                                 float* out),
            (device, bgr, pitch, w, h, on_device, net_w, net_h, out))
+GF_FORWARD(gf_detector_set_precision, (gf_detector* det, int precision), (det, precision))
+GF_FORWARD(gf_detector_get_precision, (gf_detector* det, int* precision), (det, precision))
+GF_FORWARD(gf_stage_yolo_conv, (int device, int precision, const int* shape, const float* in, const float* w, const float* bias,
+                                const float* scale, const float* mean, const float* var, float* out),
+           (device, precision, shape, in, w, bias, scale, mean, var, out))
 
 void gf_detector_destroy(gf_detector* det)
 {

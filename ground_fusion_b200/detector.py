@@ -5,7 +5,9 @@
     boxes, class_ids, probs = det.detect(bgr)          # boxes (m, 4) int64 xmin, ymin, xmax, ymax, as darknet_ros publishes them
     tracker.trackImagebox(t, boxes, gray, depth)
 
-The network is read from the user's darknet cfg and .weights at run time; the forward pass is bit-exact with darknet's CPU build.
+The network is read from the user's darknet cfg and .weights at run time.  precision="exact" (the default) is bit-exact with
+darknet's CPU build; precision="tf32" runs the convolutions on the tensor cores with TF32-rounded operands (faster, not bit-exact;
+DESIGN.md has the error bound), everything else unchanged.  conv_stage() runs one convolution through the detector's kernels.
 parse_cfg() gives the layer shapes darknet derives from a cfg, on the host.  No CPU fallback: without a device every call raises.
 """
 import ctypes
@@ -13,6 +15,8 @@ import ctypes
 import numpy as np
 
 from . import _lib
+
+PRECISIONS = {"exact": 0, "tf32": 1}      # GF_DETECTOR_EXACT, GF_DETECTOR_TF32
 
 _LAYER_TYPES = {"convolutional": "convolutional", "conv": "convolutional", "maxpool": "maxpool", "max": "maxpool",
                 "route": "route", "reorg": "reorg", "shortcut": "shortcut", "upsample": "upsample", "region": "region",
@@ -107,9 +111,12 @@ def _frame(bgr):
 
 class YoloDetector:
     """darknet_ros's detector for one network on one GPU.  thresh is the node's detection threshold (its yaml's
-    threshold / value); the NMS threshold 0.4 and hier 0.5 are the node's constants."""
+    threshold / value); the NMS threshold 0.4 and hier 0.5 are the node's constants.  precision: "exact" (bit-exact with
+    darknet's CPU build) or "tf32" (tensor-core convolutions); set_precision() switches a live detector."""
 
-    def __init__(self, cfg, weights, thresh=0.3, device=0):
+    def __init__(self, cfg, weights, thresh=0.3, device=0, precision="exact"):
+        if precision not in PRECISIONS:
+            raise ValueError("precision must be one of %s" % sorted(PRECISIONS))
         L = _lib.yolo_lib()
         self._L = L
         self._h = ctypes.c_void_p()
@@ -122,6 +129,23 @@ class YoloDetector:
         self._boxes = np.zeros((_lib.GF_MAX_BOXES, 4), np.int64)
         self._cls = np.zeros(_lib.GF_MAX_BOXES, np.int32)
         self._prob = np.zeros(_lib.GF_MAX_BOXES, np.float32)
+        self.precision = "exact"
+        if precision != "exact":
+            try:
+                self.set_precision(precision)
+            except Exception:
+                self.close()
+                raise
+
+    def set_precision(self, precision):
+        """Switch every later detect to "exact" or "tf32".  The first switch to "tf32" makes a TF32-rounded copy of the weights on
+        the device (kept, so switching back and forth is cheap)."""
+        if precision not in PRECISIONS:
+            raise ValueError("precision must be one of %s" % sorted(PRECISIONS))
+        _lib.check_yolo(self._L.gf_detector_set_precision(self._h, PRECISIONS[precision]))
+        p = ctypes.c_int()
+        _lib.check_yolo(self._L.gf_detector_get_precision(self._h, ctypes.byref(p)))
+        self.precision = {v: k for k, v in PRECISIONS.items()}[p.value]
 
     def detect(self, bgr):
         """boxes (m, 4) int64, class_ids (m,) int32, probs (m,) float32 of one BGR8 frame (m = 0 when the node publishes nothing)."""
@@ -175,4 +199,30 @@ def letterbox(bgr, net_w, net_h, device=0):
     ptr, pitch, w, h, on_dev, _keep = _frame(bgr)
     out = np.empty((3, net_h, net_w), np.float32)
     _lib.check_yolo(_lib.yolo_lib().gf_stage_letterbox(device, ptr, pitch, w, h, on_dev, net_w, net_h, out.ctypes.data))
+    return out
+
+
+def conv_stage(x, w, bias, stride=1, pad=0, leaky=False, bn=None, precision="exact", device=0):
+    """One convolutional layer through the detector's kernels and tile choice for its shape: x (C, H, W), w (M, C, size, size) or
+    (M, C size size) with size given by a 4-d w, bias (M,), bn = (scale, mean, var) or None.  Returns (M, OH, OW) float32."""
+    if precision not in PRECISIONS:
+        raise ValueError("precision must be one of %s" % sorted(PRECISIONS))
+    x = np.ascontiguousarray(x, np.float32)
+    w = np.asarray(w, np.float32)
+    C, H, W = x.shape
+    M = w.shape[0]
+    size = w.shape[2] if w.ndim == 4 else int(round((w.size // (M * C)) ** 0.5))
+    if w.size != M * C * size * size:
+        raise ValueError("w must hold M x C x size x size values")
+    w = np.ascontiguousarray(w.reshape(M, C * size * size))
+    bias = np.ascontiguousarray(bias, np.float32)
+    vec = [np.ascontiguousarray(v, np.float32) for v in bn] if bn is not None else []
+    if bias.shape != (M,) or any(v.shape != (M,) for v in vec):
+        raise ValueError("bias and batch-norm vectors must have M entries")
+    OW, OH = (W + 2 * pad - size) // stride + 1, (H + 2 * pad - size) // stride + 1
+    out = np.empty((M, OH, OW), np.float32)
+    shape = (ctypes.c_int * 9)(C, H, W, M, size, stride, pad, 1 if bn is not None else 0, 1 if leaky else 0)
+    ptrs = [v.ctypes.data for v in vec] if vec else [None] * 3
+    _lib.check_yolo(_lib.yolo_lib().gf_stage_yolo_conv(device, PRECISIONS[precision], shape, x.ctypes.data, w.ctypes.data,
+                                                       bias.ctypes.data, *ptrs, out.ctypes.data))
     return out

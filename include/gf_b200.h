@@ -847,7 +847,7 @@ int gf_detector_info(gf_detector* det, int* net_wh, int* n_layers, int* classes)
  * written).  Synchronous: the boxes belong to this frame. */
 int gf_detector_detect(gf_detector* det, const void* bgr, size_t pitch, int w, int h, int on_device, gf_box* boxes, int* class_ids,
                        float* probs, int cap, int* n_out);
-/* Device time of the last detect (letterbox + network), from CUDA events. */
+/* Device time of the last detect (letterbox + network, at the precision in use), from CUDA events. */
 int gf_detector_last_device_ms(gf_detector* det, float* ms);
 /* whc[3] = output width, height and channels of layer `layer` (0-based, [net] excluded), or of the letterboxed input for -1. */
 int gf_detector_layer_shape(gf_detector* det, int layer, int* whc);
@@ -858,6 +858,25 @@ int gf_detector_layer_output(gf_detector* det, int layer, float* out, size_t n);
 int gf_detector_layer_times(gf_detector* det, int reps, float* ms);
 /* Stage: darknet's letterbox of a BGR8 frame at net_w x net_h into out [3][net_h][net_w] (host), as gf_detector_detect does it. */
 int gf_stage_letterbox(int device, const void* bgr, size_t pitch, int w, int h, int on_device, int net_w, int net_h, float* out);
+
+/* The arithmetic of the detector's convolutions, per detector.  Everything else (letterbox, pooling, route, reorg, upsample,
+ * shortcut, the heads, decoding, NMS, extraction) is the same in both.
+ *   GF_DETECTOR_EXACT  the default: bit-exact with darknet's CPU build (sequential FMUL + FADD chains, no tensor cores).
+ *   GF_DETECTOR_TF32   tensor cores (wgmma): weights and every convolution input rounded to TF32 by round-to-nearest, ties
+ *                      away from zero (10 explicit mantissa bits), products summed in FP32 in a fixed order, so the same input
+ *                      always gives the same bits.  Not equal to darknet's CPU or GPU build; DESIGN.md has the error bound. */
+#define GF_DETECTOR_EXACT 0
+#define GF_DETECTOR_TF32 1
+/* Selects the precision of every later detect.  The first switch to TF32 allocates a TF32-rounded copy of every convolution's
+ * weights beside the FP32 ones (about 250 MB for yolov3), so the handle can switch back.  Re-captures the network's graph.
+ * Another value: GF_ERR_INVALID_ARG. */
+int gf_detector_set_precision(gf_detector* det, int precision);
+int gf_detector_get_precision(gf_detector* det, int* precision);
+/* Stage: one convolutional layer at `precision` with host arrays, through the kernels and tile choice the detector uses for
+ * that shape.  shape = C H W M size stride pad bn act (act 1 = leaky, 0 = linear); in [C][H][W], w [M][C size size], bias [M],
+ * and with bn: scale, mean, var [M] (nullable without bn); out [M][OH][OW], OH = (H + 2 pad - size) / stride + 1. */
+int gf_stage_yolo_conv(int device, int precision, const int* shape, const float* in, const float* w, const float* bias,
+                       const float* scale, const float* mean, const float* var, float* out);
 
 #if defined(__GNUC__)
 #pragma GCC visibility pop
