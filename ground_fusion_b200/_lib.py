@@ -53,6 +53,7 @@ FM_REMOVE_NONE, FM_REMOVE_BACK_SHIFT_DEPTH, FM_REMOVE_BACK, FM_REMOVE_FRONT = 0,
 
 
 GF_MAX_BOXES = 100                                             # darknet_ros publishes at most 100 boxes
+GF_DETECTOR_BATCH_MAX = 64                                     # frames per gf_detector_detect_batch call
 
 
 class Obs(ctypes.Structure):
@@ -207,6 +208,9 @@ def yolo_lib():
         L.gf_detector_set_precision.argtypes = [vp, i]
         L.gf_detector_get_precision.argtypes = [vp, ip]
         L.gf_stage_yolo_conv.argtypes = [i, i, vp, vp, vp, vp, vp, vp, vp, vp]
+        L.gf_detector_set_max_batch.argtypes = [vp, i]
+        L.gf_detector_detect_batch.argtypes = [vp, i, vp, vp, vp, vp, i, vp, vp, vp, i, vp]
+        L.gf_detector_member_layer_output.argtypes = [vp, i, i, vp, sz]
         _YOLO = L
     return _YOLO
 

@@ -1,9 +1,12 @@
 // yolo_detector.cu -- gf_detector_* (C ABI): the use_yolo front end's detector, the darknet_ros node
 // (vins_estimator/src/YoloObjectDetector.cpp) with the vendored darknet's CPU forward pass, on the GPU and bit-exact with it.
-//   create   the cfg and .weights read on the host (yolo_cfg.cuh), every parameter in HBM once, the forward pass captured as one
-//            CUDA graph: the layers' kernels (yolo_kernels.cuh) and the copies of the [region] / [yolo] outputs to pinned memory
-//   detect   the frame to the device, k_yolo_letterbox, the graph, then on the host darknet's decoding
-//            (get_network_boxes(w, h, thresh, 0.5, 0, 1)), do_nms_obj(0.4) with libc qsort, and darknet_ros's extraction
+//   create   the cfg and .weights read on the host (yolo_cfg.cuh), every parameter in HBM once, the forward pass of one image
+//            captured as one CUDA graph: the layers' kernels (yolo_kernels.cuh) and the copies of the [region] / [yolo] outputs
+//            to pinned memory
+//   detect   n frames (detect is the batch of one): the frames to the device, k_yolo_letterbox, the graph of n images
+//            (captured on the first call with that n and kept), then per frame on the host darknet's decoding
+//            (get_network_boxes(w, h, thresh, 0.5, 0, 1)), do_nms_obj(0.4) with libc qsort, and darknet_ros's extraction.
+//            The per-image buffers hold gf_detector_set_max_batch images; image i's values sit at i * the per-image size.
 // DESIGN.md "YOLO detector" has the arithmetic and why the default mode uses no tensor cores; gf_detector_set_precision
 // selects the TF32 tensor-core convolutions (yolo_tf32.cuh) instead, every other kernel unchanged.
 // Built as its own library, libgf_yolo.so, with its own error text (gf_detector_last_error); libgf_b200.so exports the same
@@ -60,18 +63,21 @@ struct gf_detector {
     float thresh = 0.3f;
     Net net;
     std::vector<DevLayer> dl;
-    float* d_input = nullptr;            // [3][h][w]
-    uint8_t* d_frame = nullptr;
+    int max_batch = 1;                   // images the per-image buffers hold
+    float* d_input = nullptr;            // [max_batch][3][h][w]
+    uint8_t* d_frame = nullptr;          // the host frames of a call, staged one after another
     size_t frame_cap = 0;
     cudaStream_t st = nullptr;
-    cudaGraph_t graph = nullptr;
-    cudaGraphExec_t exec = nullptr;
+    cudaGraphExec_t exec[GF_DETECTOR_BATCH_MAX + 1] = {};     // exec[n]: the forward pass of n images, once used
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     int precision = GF_DETECTOR_EXACT;
-    float* d_part = nullptr;             // the TF32 split-K partial sums, sized for the layer that needs most
+    bool tf32_ready = false;             // the TF32 weights, tables and workspace exist
+    float* d_part = nullptr;             // the TF32 split-K partial sums, [max_batch] x the layer that needs most
     std::vector<float> prob_store;
     bool ran = false;
+    int last_n = 0;                      // frames of the last detect
 };
+static_assert(LB_MAX == GF_DETECTOR_BATCH_MAX, "one letterbox launch takes a whole batch");
 
 namespace {
 
@@ -84,11 +90,16 @@ int select_device(int device)
     return GF_OK;
 }
 
+void drop_graphs(gf_detector* d)
+{
+    for (cudaGraphExec_t& x : d->exec)
+        if (x) { cudaGraphExecDestroy(x); x = nullptr; }
+}
+
 void free_detector(gf_detector* d)
 {
     if (!d) return;
-    if (d->exec) cudaGraphExecDestroy(d->exec);
-    if (d->graph) cudaGraphDestroy(d->graph);
+    drop_graphs(d);
     for (DevLayer& l : d->dl) {
         cudaFree(l.out); cudaFree(l.w); cudaFree(l.bias); cudaFree(l.scale); cudaFree(l.mean); cudaFree(l.den); cudaFree(l.w_tf32); cudaFree(l.ktab);
         if (l.host_out) cudaFreeHost(l.host_out);
@@ -120,10 +131,11 @@ void letterbox_size(int w, int h, int nw, int nh, int& new_w, int& new_h)
 }
 
 template <int BM, int BN>
-void launch_conv(const ConvArgs& a, cudaStream_t s)
+void launch_conv(const ConvArgs& a, int n, cudaStream_t s)
 {
-    dim3 g(blocks(a.N, BN), blocks(a.M, BM));
-    k_yolo_conv<BM, BN><<<g, CONV_THREADS, 0, s>>>(a);
+    dim3 g(blocks(a.N, BN) * n, blocks(a.M, BM));
+    if (n == 1) k_yolo_conv<BM, BN><<<g, CONV_THREADS, 0, s>>>(a);
+    else k_yolo_conv_batch<BM, BN><<<g, CONV_THREADS, 0, s>>>(a);
     GF_LAUNCHED();
 }
 
@@ -136,7 +148,8 @@ struct Tf32Operands {
 };
 
 // split-K of a TF32 layer from its shape alone: enough 64 x 64 CTAs for four per SM of the H100's 132 (the kernel's occupancy),
-// each split at least 4 stages of TC_BK; splits = 1 for layers whose tiles already fill the GPU
+// each split at least 4 stages of TC_BK; splits = 1 for layers whose tiles already fill the GPU.  Per image, not per batch:
+// the split order sets the bits of every output, so a frame's result must not depend on the frames batched with it.
 struct Tf32Plan { int splits, nsp; };
 Tf32Plan tf32_plan(int M, int N, int K)
 {
@@ -168,33 +181,45 @@ size_t tf32_part_floats(int M, int N, int K)
     return pl.splits > 1 ? (size_t)pl.splits * M * N : 0;
 }
 
+// the split-K workspace one image needs: the largest of the network's layers
+size_t tf32_part_max(const Net& net)
+{
+    size_t part = 0;
+    for (const Layer& l : net.layers)
+        if (l.type == L_CONV) part = std::max(part, tf32_part_floats(l.n, l.ow * l.oh, l.c * l.size * l.size));
+    return part;
+}
+
 // the TF32 kernel's dynamic shared memory (32 KB); before any launch or capture
 int tf32_setup()
 {
     GF_CUDA(cudaFuncSetAttribute(k_yolo_conv_tf32<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (64 + 64) * TC_BK * 8));
+    GF_CUDA(cudaFuncSetAttribute(k_yolo_conv_tf32_batch<64, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (64 + 64) * TC_BK * 8));
     return GF_OK;
 }
 
-// one convolution at `precision`, the tile and split chosen from the layer's shape alone (the detector and gf_stage_yolo_conv
-// both come here)
-void launch_conv_layer(ConvArgs a, int precision, const Tf32Operands& t, cudaStream_t s)
+// one convolution of n images at `precision` (the detector and gf_stage_yolo_conv both come here).  The TF32 split comes from
+// the layer's per-image shape alone; the exact tile may look at the whole batch, since it does not change an output's sum.
+void launch_conv_layer(ConvArgs a, int precision, const Tf32Operands& t, int n, cudaStream_t s)
 {
     if (precision == GF_DETECTOR_TF32) {
         a.w = t.w;
         const Tf32Plan pl = tf32_plan(a.M, a.N, a.K);
         float* part = pl.splits > 1 ? t.part : nullptr;
-        k_yolo_conv_tf32<64, 64><<<dim3(blocks(a.N, 64), blocks(a.M, 64), pl.splits), 128, (64 + 64) * TC_BK * 8, s>>>(
-            a, t.kp, reinterpret_cast<const int4*>(t.ktab), pl.nsp, part);
+        const dim3 g(blocks(a.N, 64) * n, blocks(a.M, 64), pl.splits);
+        const int4* ktab = reinterpret_cast<const int4*>(t.ktab);
+        if (n == 1) k_yolo_conv_tf32<64, 64><<<g, 128, (64 + 64) * TC_BK * 8, s>>>(a, t.kp, ktab, pl.nsp, part);
+        else k_yolo_conv_tf32_batch<64, 64><<<g, 128, (64 + 64) * TC_BK * 8, s>>>(a, t.kp, ktab, pl.nsp, part);
         GF_LAUNCHED();
         if (part) {
-            k_yolo_splitk_reduce<<<blocks((long)a.M * a.N, 256), 256, 0, s>>>(a, part, pl.splits);
+            k_yolo_splitk_reduce<<<dim3(blocks((long)a.M * a.N, 256), n), 256, 0, s>>>(a, part, pl.splits);
             GF_LAUNCHED();
         }
         return;
     }
     // 64 x 64 tiles where they fill the GPU twice over, 32 x 32 where the layer is small
-    if ((long)blocks(a.N, 64) * blocks(a.M, 64) >= 264) launch_conv<64, 64>(a, s);
-    else launch_conv<32, 32>(a, s);
+    if ((long)blocks(a.N, 64) * blocks(a.M, 64) * n >= 264) launch_conv<64, 64>(a, n, s);
+    else launch_conv<32, 32>(a, n, s);
 }
 
 // a layer's TF32 weight copy, rounded on the device by k_yolo_round_weights_tf32
@@ -207,8 +232,8 @@ int round_weights_tf32(const float* w, int M, int K, int kp, float** out, cudaSt
     return GF_OK;
 }
 
-// layer i's kernels on stream s (captured into the graph)
-int enqueue_layer(gf_detector* d, int i, cudaStream_t s)
+// layer i's kernels for n images on stream s (captured into the graph)
+int enqueue_layer(gf_detector* d, int i, int n, cudaStream_t s)
 {
     const Layer& l = d->net.layers[i];
     DevLayer& o = d->dl[i];
@@ -220,57 +245,110 @@ int enqueue_layer(gf_detector* d, int i, cudaStream_t s)
                    l.size, l.stride, l.pad, l.bn, l.act};
         Tf32Operands t;
         t.w = o.w_tf32; t.kp = o.kp; t.ktab = o.ktab; t.part = d->d_part;
-        launch_conv_layer(a, d->precision, t, s);
+        launch_conv_layer(a, d->precision, t, n, s);
         break;
     }
     case L_MAXPOOL:
-        k_yolo_maxpool<<<blocks(l.outputs, T), T, 0, s>>>(in, o.out, l.w, l.h, l.c, l.ow, l.oh, l.size, l.stride, l.pad); GF_LAUNCHED();
+        k_yolo_maxpool<<<blocks(l.outputs * n, T), T, 0, s>>>(in, o.out, l.w, l.h, l.c * n, l.ow, l.oh, l.size, l.stride, l.pad);
+        GF_LAUNCHED();
         break;
-    case L_ROUTE: {
+    case L_ROUTE: {           // each input's n images into their rows of the concatenation
         size_t off = 0;
         for (int k : l.in) {
-            const size_t n = (size_t)d->net.layers[k].outputs;
-            GF_CUDA(cudaMemcpyAsync(o.out + off, d->dl[k].out, 4 * n, cudaMemcpyDeviceToDevice, s));
-            off += n;
+            const size_t m = (size_t)d->net.layers[k].outputs;
+            if (n == 1) GF_CUDA(cudaMemcpyAsync(o.out + off, d->dl[k].out, 4 * m, cudaMemcpyDeviceToDevice, s));
+            else GF_CUDA(cudaMemcpy2DAsync(o.out + off, 4 * (size_t)l.outputs, d->dl[k].out, 4 * m, 4 * m, n, cudaMemcpyDeviceToDevice, s));
+            off += m;
         }
         break;
     }
     case L_REORG:
-        k_yolo_reorg<<<blocks(l.outputs, T), T, 0, s>>>(in, o.out, l.w, l.h, l.c, l.stride); GF_LAUNCHED();
+        k_yolo_reorg<<<dim3(blocks(l.outputs, T), n), T, 0, s>>>(in, o.out, l.w, l.h, l.c, l.stride); GF_LAUNCHED();
         break;
     case L_UPSAMPLE:
-        k_yolo_upsample<<<blocks(l.outputs, T), T, 0, s>>>(in, o.out, l.w, l.h, l.c, l.stride, l.scale); GF_LAUNCHED();
+        k_yolo_upsample<<<blocks(l.outputs * n, T), T, 0, s>>>(in, o.out, l.w, l.h, l.c * n, l.stride, l.scale); GF_LAUNCHED();
         break;
     case L_SHORTCUT:
-        k_yolo_shortcut<<<blocks(l.outputs, T), T, 0, s>>>(in, d->dl[l.in[0]].out, o.out, l.w, l.h, l.c, l.ow, l.oh, l.oc, l.alpha,
-                                                           l.beta, l.act);
+        k_yolo_shortcut<<<dim3(blocks(l.outputs, T), n), T, 0, s>>>(in, d->dl[l.in[0]].out, o.out, l.w, l.h, l.c, l.ow, l.oh, l.oc,
+                                                                    l.alpha, l.beta, l.act);
         GF_LAUNCHED();
         break;
     case L_REGION:
     case L_YOLO:
-        k_yolo_head<<<blocks((long)l.ow * l.oh * l.num, 128), 128, 0, s>>>(in, o.out, l.ow * l.oh, l.num, l.classes, l.type == L_YOLO,
-                                                                           l.softmax);
+        k_yolo_head<<<blocks((long)l.ow * l.oh * l.num * n, 128), 128, 0, s>>>(in, o.out, l.ow * l.oh, l.num * n, l.classes,
+                                                                               l.type == L_YOLO, l.softmax);
         GF_LAUNCHED();
-        GF_CUDA(cudaMemcpyAsync(o.host_out, o.out, 4 * (size_t)l.outputs, cudaMemcpyDeviceToHost, s));
+        GF_CUDA(cudaMemcpyAsync(o.host_out, o.out, 4 * (size_t)n * l.outputs, cudaMemcpyDeviceToHost, s));
         break;
     }
     GF_CUDA(cudaGetLastError());
     return GF_OK;
 }
 
-int capture(gf_detector* d);
+// the per-image buffers of nb images: every layer's output, the heads' pinned copies, the letterboxed input and, with part > 0,
+// the TF32 split-K workspace of part floats per image
+struct BatchBufs {
+    std::vector<float*> out, host_out;
+    float* input = nullptr;
+    float* part = nullptr;
+};
+
+void free_bufs(BatchBufs& b)
+{
+    for (float* p : b.out) cudaFree(p);
+    for (float* p : b.host_out) if (p) cudaFreeHost(p);
+    cudaFree(b.input);
+    cudaFree(b.part);
+    b = BatchBufs();
+}
+
+// all or nothing: on failure every buffer allocated here is freed again
+int alloc_bufs(const gf_detector* d, int nb, size_t part, BatchBufs& b)
+{
+    const size_t nl = d->net.layers.size();
+    b.out.assign(nl, nullptr);
+    b.host_out.assign(nl, nullptr);
+    cudaError_t e = cudaMalloc(&b.input, 4 * (size_t)nb * 3 * d->net.w * d->net.h);
+    for (size_t i = 0; i < nl && e == cudaSuccess; i++) {
+        const Layer& l = d->net.layers[i];
+        e = cudaMalloc(&b.out[i], 4 * (size_t)nb * l.outputs);
+        if (e == cudaSuccess && (l.type == L_REGION || l.type == L_YOLO)) e = cudaMallocHost(&b.host_out[i], 4 * (size_t)nb * l.outputs);
+    }
+    if (e == cudaSuccess && part) e = cudaMalloc(&b.part, 4 * (size_t)nb * part);
+    if (e != cudaSuccess) {
+        free_bufs(b);
+        cudaGetLastError();
+        return set_err(GF_ERR_CUDA, "allocating the buffers of %s images failed: %s", std::to_string(nb).c_str(), cudaGetErrorString(e));
+    }
+    return GF_OK;
+}
+
+// b's buffers into the handle, the handle's previous ones into b
+void swap_bufs(gf_detector* d, BatchBufs& b)
+{
+    for (size_t i = 0; i < d->dl.size(); i++) {
+        std::swap(d->dl[i].out, b.out[i]);
+        std::swap(d->dl[i].host_out, b.host_out[i]);
+    }
+    std::swap(d->d_input, b.input);
+    std::swap(d->d_part, b.part);
+}
+
+int capture(gf_detector* d, int n, cudaGraphExec_t* out);
 
 int detector_init(gf_detector* d)
 {
     GF_CUDA(cudaStreamCreateWithFlags(&d->st, cudaStreamNonBlocking));
     GF_CUDA(cudaEventCreate(&d->ev0));
     GF_CUDA(cudaEventCreate(&d->ev1));
-    GF_CUDA(cudaMalloc(&d->d_input, 4 * (size_t)3 * d->net.w * d->net.h));
     d->dl.resize(d->net.layers.size());
+    BatchBufs b;
+    int rc = alloc_bufs(d, 1, 0, b);
+    if (rc) return rc;
+    swap_bufs(d, b);
     for (size_t i = 0; i < d->net.layers.size(); i++) {
         const Layer& l = d->net.layers[i];
         DevLayer& o = d->dl[i];
-        GF_CUDA(cudaMalloc(&o.out, 4 * (size_t)l.outputs));
         if (l.type == L_CONV) {
             int rc = upload(&o.w, l.weights);
             if (!rc) rc = upload(&o.bias, l.biases);
@@ -283,30 +361,25 @@ int detector_init(gf_detector* d)
             }
             if (rc) return rc;
         }
-        if (l.type == L_REGION || l.type == L_YOLO) GF_CUDA(cudaMallocHost(&o.host_out, 4 * (size_t)l.outputs));
     }
-    return capture(d);
+    return capture(d, 1, &d->exec[1]);
 }
 
-// the forward pass at d->precision captured as one graph; replaces the detector's graph only once the new one is instantiated
-int capture(gf_detector* d)
+// the forward pass of n images at d->precision captured as one graph and instantiated into *out (untouched on failure)
+int capture(gf_detector* d, int n, cudaGraphExec_t* out)
 {
     GF_CUDA(cudaStreamBeginCapture(d->st, cudaStreamCaptureModeThreadLocal));
     int rc = GF_OK;
-    for (size_t i = 0; i < d->net.layers.size() && !rc; i++) rc = enqueue_layer(d, (int)i, d->st);
+    for (size_t i = 0; i < d->net.layers.size() && !rc; i++) rc = enqueue_layer(d, (int)i, n, d->st);
     cudaGraph_t g = nullptr;
     const cudaError_t e = cudaStreamEndCapture(d->st, &g);
     if (rc) { if (g) cudaGraphDestroy(g); return rc; }
     GF_CUDA(e);
     cudaGraphExec_t x = nullptr;
-    if (cudaGraphInstantiate(&x, g, 0) != cudaSuccess) {
-        cudaGraphDestroy(g);
-        return set_err(GF_ERR_CUDA, "cudaGraphInstantiate failed");
-    }
-    if (d->exec) cudaGraphExecDestroy(d->exec);
-    if (d->graph) cudaGraphDestroy(d->graph);
-    d->graph = g;
-    d->exec = x;
+    const cudaError_t ei = cudaGraphInstantiate(&x, g, 0);
+    cudaGraphDestroy(g);
+    if (ei != cudaSuccess) return set_err(GF_ERR_CUDA, "cudaGraphInstantiate failed");
+    *out = x;
     return GF_OK;
 }
 
@@ -327,8 +400,8 @@ void correct_boxes(Det* dets, int n, int w, int h, int netw, int neth)
     }
 }
 
-// get_network_boxes(net, w, h, thresh, hier, 0, 1, &n): every layer's detections in layer order
-void network_boxes(gf_detector* d, int w, int h, std::vector<Det>& dets)
+// get_network_boxes(net, w, h, thresh, hier, 0, 1, &n) of image im of the last batch: every layer's detections in layer order
+void network_boxes(gf_detector* d, int im, int w, int h, std::vector<Det>& dets)
 {
     const Net& net = d->net;
     const float thresh = d->thresh;
@@ -337,7 +410,7 @@ void network_boxes(gf_detector* d, int w, int h, std::vector<Det>& dets)
     for (size_t li = 0; li < net.layers.size(); li++) {
         const Layer& l = net.layers[li];
         const int wh = l.ow * l.oh, E = l.classes + 5;
-        const float* p = d->dl[li].host_out;
+        const float* p = d->dl[li].host_out + (size_t)im * l.outputs;
         if (l.type == L_REGION) total += (size_t)wh * l.num;
         if (l.type == L_YOLO)
             for (int i = 0; i < wh; i++)
@@ -351,7 +424,7 @@ void network_boxes(gf_detector* d, int w, int h, std::vector<Det>& dets)
         const Layer& l = net.layers[li];
         if (l.type != L_REGION && l.type != L_YOLO) continue;
         const int wh = l.ow * l.oh, E = l.classes + 5;
-        const float* p = d->dl[li].host_out;
+        const float* p = d->dl[li].host_out + (size_t)im * l.outputs;
         const size_t first = at;
         for (int i = 0; i < wh; i++) {
             const int row = i / l.ow, col = i % l.ow;
@@ -482,21 +555,6 @@ int extract(const std::vector<Det>& dets, int classes, int fw, int fh, gf_box* b
     return n;
 }
 
-int stage_frame(gf_detector* d, const void* bgr, size_t pitch, int w, int h, int on_device, const uint8_t** src, int* src_pitch)
-{
-    if (on_device) { *src = (const uint8_t*)bgr; *src_pitch = (int)pitch; return GF_OK; }
-    const size_t need = (size_t)3 * w * h;
-    if (need > d->frame_cap) {
-        cudaFree(d->d_frame);
-        d->d_frame = nullptr; d->frame_cap = 0;
-        GF_CUDA(cudaMalloc(&d->d_frame, need));
-        d->frame_cap = need;
-    }
-    GF_CUDA(cudaMemcpy2DAsync(d->d_frame, 3 * (size_t)w, bgr, pitch, 3 * (size_t)w, h, cudaMemcpyHostToDevice, d->st));
-    *src = d->d_frame; *src_pitch = 3 * w;
-    return GF_OK;
-}
-
 int check_frame(const void* bgr, size_t pitch, int w, int h)
 {
     if (!bgr || w < 1 || h < 1 || w > 16384 || h > 16384 || pitch < (size_t)3 * w || pitch > (1u << 30))
@@ -504,12 +562,77 @@ int check_frame(const void* bgr, size_t pitch, int w, int h)
     return GF_OK;
 }
 
-void launch_letterbox(const uint8_t* src, int pitch, int w, int h, int nw, int nh, float* out, cudaStream_t s)
+void set_frame(LbFrames& f, int i, const uint8_t* src, int pitch, int w, int h, int nw, int nh)
 {
-    int new_w, new_h;
-    letterbox_size(w, h, nw, nh, new_w, new_h);
-    k_yolo_letterbox<<<dim3(blocks(nw, 128), nh, 3), 128, 0, s>>>(src, pitch, w, h, nw, nh, new_w, new_h, out);
+    f.bgr[i] = src; f.pitch[i] = pitch; f.w[i] = w; f.h[i] = h;
+    letterbox_size(w, h, nw, nh, f.new_w[i], f.new_h[i]);
+}
+
+void launch_letterbox(const LbFrames& f, int n, int nw, int nh, float* out, cudaStream_t s)
+{
+    k_yolo_letterbox<<<dim3(blocks(nw, 128), nh, 3 * n), 128, 0, s>>>(f, nw, nh, out);
     GF_LAUNCHED();
+}
+
+// the n frames for the letterbox: device frames in place, host frames copied one after another into the staging buffer
+int stage_frames(gf_detector* d, int n, const void* const* bgr, const size_t* pitch, const int* w, const int* h, int on_device,
+                 LbFrames& f)
+{
+    size_t need = 0;
+    for (int i = 0; i < n && !on_device; i++) need += (size_t)3 * w[i] * h[i];
+    if (need > d->frame_cap) {
+        cudaFree(d->d_frame);
+        d->d_frame = nullptr; d->frame_cap = 0;
+        GF_CUDA(cudaMalloc(&d->d_frame, need));
+        d->frame_cap = need;
+    }
+    size_t off = 0;
+    for (int i = 0; i < n; i++) {
+        const uint8_t* src = (const uint8_t*)bgr[i];
+        int sp = (int)pitch[i];
+        if (!on_device) {
+            GF_CUDA(cudaMemcpy2DAsync(d->d_frame + off, 3 * (size_t)w[i], bgr[i], pitch[i], 3 * (size_t)w[i], h[i], cudaMemcpyHostToDevice, d->st));
+            src = d->d_frame + off; sp = 3 * w[i];
+            off += (size_t)3 * w[i] * h[i];
+        }
+        set_frame(f, i, src, sp, w[i], h[i], d->net.w, d->net.h);
+    }
+    return GF_OK;
+}
+
+// the forward pass of n checked frames and the host decoding of each; frame i's boxes at box_start[i] .. box_start[i + 1],
+// nothing written at or past cap
+int detect_frames(gf_detector* d, int n, const void* const* bgr, const size_t* pitch, const int* w, const int* h, int on_device,
+                  gf_box* boxes, int* class_ids, float* probs, int cap, int* box_start)
+{
+    GF_CUDA(cudaSetDevice(d->device));
+    if (!d->exec[n]) {
+        const int rc = capture(d, n, &d->exec[n]);
+        if (rc) return rc;
+    }
+    LbFrames f;
+    const int rc = stage_frames(d, n, bgr, pitch, w, h, on_device, f);
+    if (rc) return rc;
+    GF_CUDA(cudaEventRecord(d->ev0, d->st));
+    launch_letterbox(f, n, d->net.w, d->net.h, d->d_input, d->st);
+    GF_CUDA(cudaGetLastError());
+    GF_CUDA(cudaGraphLaunch(d->exec[n], d->st));
+    GF_CUDA(cudaEventRecord(d->ev1, d->st));
+    GF_CUDA(cudaStreamSynchronize(d->st));
+    d->ran = true;
+    d->last_n = n;
+    const int classes = d->net.layers.back().classes;
+    std::vector<Det> dets;
+    box_start[0] = 0;
+    for (int i = 0; i < n; i++) {
+        network_boxes(d, i, w[i], h[i], dets);
+        nms_obj(dets, classes, .4f);
+        const int at = box_start[i], room = std::max(cap - at, 0);
+        box_start[i + 1] = at + extract(dets, classes, w[i], h[i], room ? boxes + at : nullptr,
+                                        room && class_ids ? class_ids + at : nullptr, room && probs ? probs + at : nullptr, room);
+    }
+    if (box_start[n] > cap) return set_err(GF_ERR_CAPACITY, "more boxes than cap");
+    return GF_OK;
 }
 
 }  // namespace
@@ -577,26 +700,42 @@ int gf_detector_detect(gf_detector* d, const void* bgr, size_t pitch, int w, int
                        float* probs, int cap, int* n_out)
 {
     if (!d || !n_out || cap < 0 || (cap > 0 && !boxes)) return set_err(GF_ERR_INVALID_ARG, "bad argument");
-    int rc = check_frame(bgr, pitch, w, h);
-    if (rc) return rc;
+    const int rc0 = check_frame(bgr, pitch, w, h);
+    if (rc0) return rc0;
+    int box_start[2];
+    const int rc = detect_frames(d, 1, &bgr, &pitch, &w, &h, on_device, boxes, class_ids, probs, cap, box_start);
+    if (rc == GF_OK || rc == GF_ERR_CAPACITY) *n_out = box_start[1];
+    return rc;
+}
+
+int gf_detector_detect_batch(gf_detector* d, int n, const void* const* bgr, const size_t* pitch, const int* w, const int* h,
+                             int on_device, gf_box* boxes, int* class_ids, float* probs, int cap, int* box_start)
+{
+    if (!d || !bgr || !pitch || !w || !h || !box_start || cap < 0 || (cap > 0 && !boxes) || n < 1)
+        return set_err(GF_ERR_INVALID_ARG, "bad argument");
+    for (int i = 0; i < n; i++)          // the frames before the handle: every argument error is found without touching it
+        if (check_frame(bgr[i], pitch[i], w[i], h[i]))
+            return set_err(GF_ERR_INVALID_ARG, "frame %s: bad frame (BGR8, 1..16384 pixels a side, pitch >= 3 * width)", std::to_string(i).c_str());
+    if (n > d->max_batch) return set_err(GF_ERR_CAPACITY, "%s frames exceed the handle's max_batch of %s", std::to_string(n).c_str(), std::to_string(d->max_batch).c_str());
+    return detect_frames(d, n, bgr, pitch, w, h, on_device, boxes, class_ids, probs, cap, box_start);
+}
+
+int gf_detector_set_max_batch(gf_detector* d, int max_batch)
+{
+    if (!d) return set_err(GF_ERR_INVALID_ARG, "null detector");
+    if (max_batch < 1 || max_batch > GF_DETECTOR_BATCH_MAX) return set_err(GF_ERR_INVALID_ARG, "max_batch must lie in [1, GF_DETECTOR_BATCH_MAX]");
+    if (max_batch == d->max_batch) return GF_OK;
     GF_CUDA(cudaSetDevice(d->device));
-    const uint8_t* src;
-    int sp;
-    rc = stage_frame(d, bgr, pitch, w, h, on_device, &src, &sp);
-    if (rc) return rc;
-    GF_CUDA(cudaEventRecord(d->ev0, d->st));
-    launch_letterbox(src, sp, w, h, d->net.w, d->net.h, d->d_input, d->st);
-    GF_CUDA(cudaGetLastError());
-    GF_CUDA(cudaGraphLaunch(d->exec, d->st));
-    GF_CUDA(cudaEventRecord(d->ev1, d->st));
     GF_CUDA(cudaStreamSynchronize(d->st));
-    d->ran = true;
-    std::vector<Det> dets;
-    network_boxes(d, w, h, dets);
-    const int classes = d->net.layers.back().classes;
-    nms_obj(dets, classes, .4f);
-    *n_out = extract(dets, classes, w, h, boxes, class_ids, probs, cap);
-    if (*n_out > cap) return set_err(GF_ERR_CAPACITY, "more boxes than cap");
+    BatchBufs b;
+    const int rc = alloc_bufs(d, max_batch, d->tf32_ready ? tf32_part_max(d->net) : 0, b);
+    if (rc) return rc;
+    drop_graphs(d);                      // they name the old buffers
+    swap_bufs(d, b);
+    free_bufs(b);
+    d->max_batch = max_batch;
+    d->ran = false;
+    d->last_n = 0;
     return GF_OK;
 }
 
@@ -607,15 +746,21 @@ int gf_detector_last_device_ms(gf_detector* d, float* ms)
     return GF_OK;
 }
 
-int gf_detector_layer_output(gf_detector* d, int layer, float* out, size_t n)
+int gf_detector_member_layer_output(gf_detector* d, int member, int layer, float* out, size_t n)
 {
     if (!d || !out || layer < -1 || layer >= (int)d->net.layers.size()) return set_err(GF_ERR_INVALID_ARG, "bad argument");
     if (!d->ran) return set_err(GF_ERR_INVALID_ARG, "no detection has run");
+    if (member < 0 || member >= d->last_n) return set_err(GF_ERR_INVALID_ARG, "member %s outside the last call's %s frames", std::to_string(member).c_str(), std::to_string(d->last_n).c_str());
     const size_t need = layer < 0 ? (size_t)3 * d->net.w * d->net.h : (size_t)d->net.layers[layer].outputs;
     if (n < need) return set_err(GF_ERR_CAPACITY, "output buffer too small");
     GF_CUDA(cudaSetDevice(d->device));
-    GF_CUDA(cudaMemcpy(out, layer < 0 ? d->d_input : d->dl[layer].out, 4 * need, cudaMemcpyDeviceToHost));
+    GF_CUDA(cudaMemcpy(out, (layer < 0 ? d->d_input : d->dl[layer].out) + member * need, 4 * need, cudaMemcpyDeviceToHost));
     return GF_OK;
+}
+
+int gf_detector_layer_output(gf_detector* d, int layer, float* out, size_t n)
+{
+    return gf_detector_member_layer_output(d, 0, layer, out, n);
 }
 
 int gf_detector_layer_times(gf_detector* d, int reps, float* ms)
@@ -629,7 +774,7 @@ int gf_detector_layer_times(gf_detector* d, int reps, float* ms)
     int rc = GF_OK;
     for (size_t i = 0; i < d->net.layers.size() && !rc; i++) {
         cudaEventRecord(a, d->st);
-        for (int r = 0; r < reps && !rc; r++) rc = enqueue_layer(d, (int)i, d->st);
+        for (int r = 0; r < reps && !rc; r++) rc = enqueue_layer(d, (int)i, d->last_n, d->st);
         cudaEventRecord(b, d->st);
         if (cudaEventSynchronize(b) != cudaSuccess || cudaEventElapsedTime(ms + i, a, b) != cudaSuccess) rc = set_err(GF_ERR_CUDA, "timing failed");
         else ms[i] /= reps;
@@ -659,7 +804,9 @@ int gf_stage_letterbox(int device, const void* bgr, size_t pitch, int w, int h, 
         src = tmp; pitch = 3 * (size_t)w;
     }
     if (cudaMalloc(&d_out, 4 * n) != cudaSuccess) { cudaFree(tmp); return set_err(GF_ERR_CUDA, "cudaMalloc failed"); }
-    launch_letterbox(src, (int)pitch, w, h, net_w, net_h, d_out, 0);
+    LbFrames f;
+    set_frame(f, 0, src, (int)pitch, w, h, net_w, net_h);
+    launch_letterbox(f, 1, net_w, net_h, d_out, 0);
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaMemcpy(out, d_out, 4 * n, cudaMemcpyDeviceToHost);
     cudaFree(d_out);
@@ -676,29 +823,38 @@ int gf_detector_set_precision(gf_detector* d, int precision)
     if (precision == d->precision) return GF_OK;
     GF_CUDA(cudaSetDevice(d->device));
     GF_CUDA(cudaStreamSynchronize(d->st));
-    if (precision == GF_DETECTOR_TF32) {
+    if (precision == GF_DETECTOR_TF32 && !d->tf32_ready) {
         int rc = tf32_setup();
-        size_t part = 0;
         for (size_t i = 0; i < d->net.layers.size() && !rc; i++) {
             const Layer& l = d->net.layers[i];
             DevLayer& o = d->dl[i];
-            if (l.type != L_CONV) continue;
+            if (l.type != L_CONV || o.w_tf32) continue;
             const int K = l.c * l.size * l.size;
-            part = std::max(part, tf32_part_floats(l.n, l.ow * l.oh, K));
-            if (o.w_tf32) continue;
             o.kp = (K + 3) / 4 * 4;
             rc = round_weights_tf32(o.w, l.n, K, o.kp, &o.w_tf32, d->st);
             if (!rc) rc = upload(&o.ktab, tf32_ktab(l.c, l.h, l.w, l.size));
         }
+        const size_t part = tf32_part_max(d->net) * d->max_batch;
         if (!rc && part && !d->d_part && cudaMalloc(&d->d_part, 4 * part) != cudaSuccess) rc = set_err(GF_ERR_CUDA, "cudaMalloc failed");
         if (!rc && cudaStreamSynchronize(d->st) != cudaSuccess) rc = set_err(GF_ERR_CUDA, "rounding the weights to TF32 failed");
         if (rc) return rc;
+        d->tf32_ready = true;
     }
+    // every batch size in use re-captured; the old graphs stay in place unless all succeed
     const int keep = d->precision;
     d->precision = precision;
-    const int rc = capture(d);
-    if (rc) d->precision = keep;                 // the old graph is still in place
-    return rc;
+    cudaGraphExec_t fresh[GF_DETECTOR_BATCH_MAX + 1] = {};
+    int rc = GF_OK;
+    for (int n = 1; n <= GF_DETECTOR_BATCH_MAX && !rc; n++)
+        if (d->exec[n]) rc = capture(d, n, &fresh[n]);
+    if (rc) {
+        d->precision = keep;
+        for (cudaGraphExec_t x : fresh) if (x) cudaGraphExecDestroy(x);
+        return rc;
+    }
+    drop_graphs(d);
+    std::copy(fresh, fresh + GF_DETECTOR_BATCH_MAX + 1, d->exec);
+    return GF_OK;
 }
 
 int gf_detector_get_precision(gf_detector* d, int* precision)
@@ -753,7 +909,7 @@ int gf_stage_yolo_conv(int device, int precision, const int* shape, const float*
         const ConvArgs a{d_in, d_w, d_out, d_b, d_sc, d_mu, d_den, C, H, W, M, K, OW, N, size, stride, pad, bn, act_};
         Tf32Operands t;
         t.w = d_wt; t.kp = kp; t.ktab = d_ktab; t.part = d_part;
-        launch_conv_layer(a, precision, t, 0);
+        launch_conv_layer(a, precision, t, 1, 0);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaMemcpy(out, d_out, 4 * (size_t)M * N, cudaMemcpyDeviceToHost);

@@ -87,6 +87,13 @@ GF_FORWARD(gf_stage_letterbox, (int device, const void* bgr, size_t pitch, int w
            (device, bgr, pitch, w, h, on_device, net_w, net_h, out))
 GF_FORWARD(gf_detector_set_precision, (gf_detector* det, int precision), (det, precision))
 GF_FORWARD(gf_detector_get_precision, (gf_detector* det, int* precision), (det, precision))
+GF_FORWARD(gf_detector_set_max_batch, (gf_detector* det, int max_batch), (det, max_batch))
+GF_FORWARD(gf_detector_detect_batch, (gf_detector* det, int n, const void* const* bgr, const size_t* pitch, const int* w,
+                                      const int* h, int on_device, gf_box* boxes, int* class_ids, float* probs, int cap,
+                                      int* box_start),
+           (det, n, bgr, pitch, w, h, on_device, boxes, class_ids, probs, cap, box_start))
+GF_FORWARD(gf_detector_member_layer_output, (gf_detector* det, int member, int layer, float* out, size_t n),
+           (det, member, layer, out, n))
 GF_FORWARD(gf_stage_yolo_conv, (int device, int precision, const int* shape, const float* in, const float* w, const float* bias,
                                 const float* scale, const float* mean, const float* var, float* out),
            (device, precision, shape, in, w, bias, scale, mean, var, out))

@@ -9,6 +9,10 @@
 //               sqrt(var) + 1e-6f (the denominator precomputed on the host in double), scale_bias, add_bias, activation.
 //   the rest    maxpool, reorg (darknet's forward = 0 mapping), upsample, shortcut, and the [region] / [yolo] heads'
 //               logistic / softmax with their exp in double by gm_exp (correctly rounded)
+// Every kernel runs a batch of images: image i's values sit at i * (the layer's per-image size) in each buffer.  A conv CTA's
+// pixel tile lies within one image, so each output keeps its sequential k order whatever the batch.  Maxpool, upsample and the
+// heads see the batch as more channels (anchors), which their per-channel mapping already handles; reorg and shortcut take the
+// image from blockIdx.y.
 #pragma once
 #include <cfloat>
 #include <cstdint>
@@ -23,12 +27,22 @@ __device__ __forceinline__ float act(float x, int a) { return a ? act_leaky(x) :
 // logistic_activate: 1. / (1. + exp(-x)) in double
 __device__ __forceinline__ float logistic(float x) { return __double2float_rn(__ddiv_rn(1.0, __dadd_rn(1.0, gm_exp(-(double)x)))); }
 
-// one output value of letterbox_image(mat_to_image(frame), nw, nh) per thread; out is [3][nh][nw]
-__global__ void k_yolo_letterbox(const uint8_t* __restrict__ bgr, int pitch, int w, int h, int nw, int nh, int new_w, int new_h,
-                                 float* __restrict__ out)
+constexpr int LB_MAX = 64;                 // frames per letterbox launch (GF_DETECTOR_BATCH_MAX)
+
+// per-frame geometry of one letterbox launch: the frame, its size and its letterboxed size at the net size
+struct LbFrames {
+    const uint8_t* bgr[LB_MAX];
+    int pitch[LB_MAX], w[LB_MAX], h[LB_MAX], new_w[LB_MAX], new_h[LB_MAX];
+};
+
+// one output value of letterbox_image(mat_to_image(frame), nw, nh) per thread; blockIdx.z = 3 frame + channel; out is
+// [frame][3][nh][nw]
+__global__ void k_yolo_letterbox(const __grid_constant__ LbFrames f, int nw, int nh, float* __restrict__ out)
 {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, k = blockIdx.z;
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, k = blockIdx.z % 3, im = blockIdx.z / 3;
     if (x >= nw) return;
+    const uint8_t* __restrict__ bgr = f.bgr[im];
+    const int pitch = f.pitch[im], w = f.w[im], h = f.h[im], new_w = f.new_w[im], new_h = f.new_h[im];
     const int dx = (nw - new_w) / 2, dy = (nh - new_h) / 2;
     const int c = x - dx, r = y - dy;
     float v = 0.5f;
@@ -49,13 +63,13 @@ __global__ void k_yolo_letterbox(const uint8_t* __restrict__ bgr, int pitch, int
         v = __fmul_rn(__fsub_rn(1.f, fy), part(iy));
         if (!(r == new_h - 1 || h == 1)) v = __fadd_rn(v, __fmul_rn(fy, part(iy + 1)));
     }
-    out[((size_t)k * nh + y) * nw + x] = v;
+    out[(((size_t)im * 3 + k) * nh + y) * nw + x] = v;
 }
 
 struct ConvArgs {
-    const float* in;       // [C][H][W]
+    const float* in;       // [image][C][H][W]
     const float* w;        // [M][K], K = C size^2
-    float* out;            // [M][OH][OW]
+    float* out;            // [image][M][OH][OW]
     const float* bias;
     const float* scale;    // batch norm only
     const float* mean;
@@ -65,17 +79,22 @@ struct ConvArgs {
 
 constexpr int CONV_THREADS = 256, CONV_BK = 8;
 
-// CTA tile BM filters x BN pixels, 256 threads each holding (BM / 16) x (BN / 16) sums; K staged through shared memory in chunks
-// of CONV_BK, double-buffered, the next chunk's loads issued before the current chunk's arithmetic
-template <int BM, int BN>
-__global__ void __launch_bounds__(CONV_THREADS) k_yolo_conv(ConvArgs a)
+// CTA tile BM filters x BN pixels of one image, 256 threads each holding (BM / 16) x (BN / 16) sums; K staged through shared
+// memory in chunks of CONV_BK, double-buffered, the next chunk's loads issued before the current chunk's arithmetic.
+// BATCH: blockIdx.x = image * ceil(N / BN) + pixel tile.  Without it (one image) the image terms fold away and the loop keeps
+// one image's addressing: the image offset costs the gather loop instructions, so a lone frame does not pay for it.
+template <int BM, int BN, bool BATCH>
+__device__ __forceinline__ void conv_body(const ConvArgs& a)
 {
     constexpr int TM = BM / 16, TN = BN / 16;
     constexpr int WL = BM * CONV_BK / CONV_THREADS, XL = BN * CONV_BK / CONV_THREADS;
     __shared__ float Ws[2][CONV_BK][BM];
     __shared__ float Xs[2][CONV_BK][BN];
     const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
-    const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
+    // the image's channels continue the batch's: channel ch of image im is channel im C + ch of the buffer (a.in stays the
+    // kernel parameter, so the loop's addressing is that of one image)
+    const int tiles = (a.N + BN - 1) / BN, im = BATCH ? blockIdx.x / tiles : 0, imc = im * a.C;
+    const int m0 = blockIdx.y * BM, n0 = (blockIdx.x - im * tiles) * BN;
     const int ss = a.size * a.size;
     // the pixel this thread gathers for the X tile, fixed over all chunks
     const int xp = tid % BN, xk0 = tid / BN;
@@ -100,7 +119,7 @@ __global__ void __launch_bounds__(CONV_THREADS) k_yolo_conv(ConvArgs a)
             if (pix_ok && gk < a.K) {
                 const int ch = gk / ss, rem = gk - ch * ss, ky = rem / a.size, kx = rem - ky * a.size;
                 const int iy = iy0 + ky, ix = ix0 + kx;
-                if (iy >= 0 && iy < a.H && ix >= 0 && ix < a.W) v = __ldg(a.in + ch * HW + (size_t)iy * a.W + ix);
+                if (iy >= 0 && iy < a.H && ix >= 0 && ix < a.W) v = __ldg(a.in + (imc + ch) * HW + (size_t)iy * a.W + ix);
             }
             xr[r] = v;
         }
@@ -161,10 +180,16 @@ __global__ void __launch_bounds__(CONV_THREADS) k_yolo_conv(ConvArgs a)
                 v = __fmul_rn(v, sc);
             }
             v = __fadd_rn(v, bias);
-            a.out[(size_t)m * a.N + p] = act(v, a.act);
+            a.out[((size_t)im * a.M + m) * a.N + p] = act(v, a.act);
         }
     }
 }
+
+// one image / a batch of images: the same body (so the same sums), compiled for each
+template <int BM, int BN>
+__global__ void __launch_bounds__(CONV_THREADS) k_yolo_conv(ConvArgs a) { conv_body<BM, BN, false>(a); }
+template <int BM, int BN>
+__global__ void __launch_bounds__(CONV_THREADS) k_yolo_conv_batch(ConvArgs a) { conv_body<BM, BN, true>(a); }
 
 // forward_maxpool_layer: the first strictly larger value wins, outside the input counts as -FLT_MAX
 __global__ void k_yolo_maxpool(const float* __restrict__ in, float* __restrict__ out, int W, int H, int C, int OW, int OH,
@@ -184,11 +209,14 @@ __global__ void k_yolo_maxpool(const float* __restrict__ in, float* __restrict__
     out[idx] = mx;
 }
 
-// forward_reorg_layer without reverse: reorg_cpu(in, w, h, c, stride, forward = 0), out[in_index] = in[out_index]
+// forward_reorg_layer without reverse: reorg_cpu(in, w, h, c, batch, stride, forward = 0), out[in_index] = in[out_index];
+// blockIdx.y = image (reorg_cpu's batch term is one image's w h c values)
 __global__ void k_yolo_reorg(const float* __restrict__ in, float* __restrict__ out, int w, int h, int c, int stride)
 {
     const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= (long)w * h * c) return;
+    in += (size_t)blockIdx.y * w * h * c;
+    out += (size_t)blockIdx.y * w * h * c;
     const int i = (int)(idx % w), j = (int)(idx / w % h), k = (int)(idx / ((long)w * h));
     const int out_c = c / (stride * stride);
     const int c2 = k % out_c, offset = k / out_c;
@@ -206,12 +234,16 @@ __global__ void k_yolo_upsample(const float* __restrict__ in, float* __restrict_
     out[idx] = __fmul_rn(scale, in[((size_t)k * h + y / stride) * w + x / stride]);
 }
 
-// forward_shortcut_layer: out = prev; out[mapped] = alpha out + beta add over shortcut_cpu's overlap; then the activation
+// forward_shortcut_layer: out = prev; out[mapped] = alpha out + beta add over shortcut_cpu's overlap; then the activation;
+// blockIdx.y = image
 __global__ void k_yolo_shortcut(const float* __restrict__ prev, const float* __restrict__ add, float* __restrict__ out,
                                 int w1, int h1, int c1, int w2, int h2, int c2, float alpha, float beta, int act_)
 {
     const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= (long)w2 * h2 * c2) return;
+    prev += (size_t)blockIdx.y * w2 * h2 * c2;
+    out += (size_t)blockIdx.y * w2 * h2 * c2;
+    add += (size_t)blockIdx.y * w1 * h1 * c1;
     int stride = w1 / w2, sample = w2 / w1;
     if (stride < 1) stride = 1;
     if (sample < 1) sample = 1;

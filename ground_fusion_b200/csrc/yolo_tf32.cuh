@@ -15,7 +15,8 @@
 //   im2col      a per-layer table of k -> (c H W + ky W + kx, ky, kx): two bounds tests and one load per value, no division.
 //   split-K     layers with too few tiles to fill the GPU (the 13^2 and 26^2 layers) split K over blockIdx.z; the splits'
 //               FP32 partial sums are added in split order by k_yolo_splitk_reduce.  No atomics: the order is fixed by the
-//               layer's shape, so the same input always gives the same bits.
+//               layer's per-image shape, so the same input always gives the same bits, whatever the batch around it.
+//   batch       blockIdx.x = image * ceil(N / BN) + pixel tile; each image has its own [splits][M][N] partial sums.
 //   epilogue    k_yolo_conv's, op for op (conv_epilogue_tf32 below restates it), so the modes differ only in the sums.
 #pragma once
 #include <cstdint>
@@ -77,8 +78,9 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t da, uint
     wgmma_tf32_n64(d, da, db);
 }
 
-// k_yolo_conv's epilogue for one output: normalize_cpu (double division), scale_bias, add_bias, the activation
-__device__ __forceinline__ void conv_epilogue_tf32(const ConvArgs& a, int m, int p, float v)
+// k_yolo_conv's epilogue for output (m, p) of the image whose outputs start at out: normalize_cpu (double division), scale_bias,
+// add_bias, the activation
+__device__ __forceinline__ void conv_epilogue_tf32(const ConvArgs& a, float* out, int m, int p, float v)
 {
     const float bias = a.bias[m];
     float sc = 0.f, mu = 0.f;
@@ -89,7 +91,7 @@ __device__ __forceinline__ void conv_epilogue_tf32(const ConvArgs& a, int m, int
         v = __fmul_rn(v, sc);
     }
     v = __fadd_rn(v, bias);
-    a.out[(size_t)m * a.N + p] = act(v, a.act);
+    out[(size_t)m * a.N + p] = act(v, a.act);
 }
 
 // One gather-table entry per k of the layer (host-built, tf32_ktab in yolo_detector.cu): x = c H W + ky W + kx, y = ky << 16 | kx;
@@ -104,9 +106,11 @@ constexpr int TC_KTAB_PAD = 0x7FFF;
 // a.w is the TF32 copy [M][Kp].  64 filters x 64 pixels per CTA, one warpgroup (128 threads), several CTAs per SM so that one
 // CTA's loads overlap another's tensor-core work.  Every thread stages 4 k-chunks of 4 values of A and of B per stage, and
 // gathers B for one fixed pixel.
-template <int BM, int BN>
-__global__ void __launch_bounds__(BM * 2, 4) k_yolo_conv_tf32(ConvArgs a, int Kp, const int4* __restrict__ ktab, int nsp,
-                                                             float* __restrict__ part)
+//
+// BATCH: blockIdx.x = image * ceil(N / BN) + pixel tile; without it (one image) the image terms fold away.
+template <int BM, int BN, bool BATCH>
+__device__ __forceinline__ void conv_tf32_body(const ConvArgs& a, int Kp, const int4* __restrict__ ktab, int nsp,
+                                               float* __restrict__ part)
 {
     constexpr int T = BM * 2;
     constexpr int A_BYTES = BM * TC_BK * 4, B_BYTES = BN * TC_BK * 4, STAGE = A_BYTES + B_BYTES;
@@ -116,7 +120,8 @@ __global__ void __launch_bounds__(BM * 2, 4) k_yolo_conv_tf32(ConvArgs a, int Kp
     extern __shared__ __align__(128) uint8_t smem[];
     const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(smem);
     const int tid = threadIdx.x, wg = tid / 128, lane = tid % 32, warp = (tid % 128) / 32;
-    const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
+    const int tiles = (a.N + BN - 1) / BN, im = BATCH ? blockIdx.x / tiles : 0;
+    const int m0 = blockIdx.y * BM, n0 = (blockIdx.x - im * tiles) * BN;
 
     // B: this thread's pixel and its k-chunks bj0, bj0 + T / BN, ...; a pixel past N gets a window no bounds test accepts
     const int bp = tid % BN, bj0 = tid / BN;
@@ -124,7 +129,7 @@ __global__ void __launch_bounds__(BM * 2, 4) k_yolo_conv_tf32(ConvArgs a, int Kp
     const bool pix_ok = gp < a.N;
     const int oy = pix_ok ? gp / a.OW : 0, ox = pix_ok ? gp - (gp / a.OW) * a.OW : 0;
     const int iy0 = pix_ok ? oy * a.stride - a.pad : -0x40000000, ix0 = ox * a.stride - a.pad;
-    const float* in0 = a.in + (pix_ok ? (long)iy0 * a.W + ix0 : 0l);
+    const float* in0 = a.in + (size_t)im * a.C * a.H * a.W + (pix_ok ? (long)iy0 * a.W + ix0 : 0l);
 
     float4 ar[AR], br[BR];
     // A chunk c = tid + T r: a group of 64 chunks is 8 rows x 8 k-chunks, rows fastest, so each quarter warp stores one
@@ -201,20 +206,35 @@ __global__ void __launch_bounds__(BM * 2, 4) k_yolo_conv_tf32(ConvArgs a, int Kp
         const int m = m0 + e / BN, p = n0 + e % BN;
         if (m >= a.M || p >= a.N) continue;
         const float v = tile[(e / BN) * (BN + 1) + e % BN];
-        if (part) part[((size_t)blockIdx.z * a.M + m) * a.N + p] = v;
-        else conv_epilogue_tf32(a, m, p, v);
+        if (part) part[(((size_t)im * gridDim.z + blockIdx.z) * a.M + m) * a.N + p] = v;
+        else conv_epilogue_tf32(a, a.out + (size_t)im * a.M * a.N, m, p, v);
     }
 }
 
-// the splits of a split-K layer added in split order, then k_yolo_conv's epilogue; one thread per output
+// one image / a batch of images: the same body (so the same sums), compiled for each
+template <int BM, int BN>
+__global__ void __launch_bounds__(BM * 2, 4) k_yolo_conv_tf32(ConvArgs a, int Kp, const int4* __restrict__ ktab, int nsp,
+                                                             float* __restrict__ part)
+{
+    conv_tf32_body<BM, BN, false>(a, Kp, ktab, nsp, part);
+}
+template <int BM, int BN>
+__global__ void __launch_bounds__(BM * 2, 4) k_yolo_conv_tf32_batch(ConvArgs a, int Kp, const int4* __restrict__ ktab, int nsp,
+                                                                   float* __restrict__ part)
+{
+    conv_tf32_body<BM, BN, true>(a, Kp, ktab, nsp, part);
+}
+
+// the splits of a split-K layer added in split order, then k_yolo_conv's epilogue; one thread per output, blockIdx.y = image
 __global__ void k_yolo_splitk_reduce(ConvArgs a, const float* __restrict__ part, int splits)
 {
     const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
     const long MN = (long)a.M * a.N;
     if (idx >= MN) return;
+    part += blockIdx.y * splits * MN;
     float v = part[idx];
     for (int z = 1; z < splits; z++) v = __fadd_rn(v, part[z * MN + idx]);
-    conv_epilogue_tf32(a, (int)(idx / a.N), (int)(idx % a.N), v);
+    conv_epilogue_tf32(a, a.out + blockIdx.y * MN, (int)(idx / a.N), (int)(idx % a.N), v);
 }
 
 }  // namespace gfy

@@ -5,6 +5,11 @@
     boxes, class_ids, probs = det.detect(bgr)          # boxes (m, 4) int64 xmin, ymin, xmax, ymax, as darknet_ros publishes them
     tracker.trackImagebox(t, boxes, gray, depth)
 
+Several cameras share one detector: set_max_batch(n) once, then detect_batch(frames) runs the forward pass of up to n frames
+in one graph launch, each frame's result bit-equal to detect() on it alone.  detect_batch(frames)'s per-frame boxes go to
+TrackerGroup.submit(..., boxes=[b for b, _, _ in results]); detect_batch_csr(frames) gives them as the (boxes, box_start) pair
+of the C ABI's gf_tracker_group_submit.
+
 The network is read from the user's darknet cfg and .weights at run time.  precision="exact" (the default) is bit-exact with
 darknet's CPU build; precision="tf32" runs the convolutions on the tensor cores with TF32-rounded operands (faster, not bit-exact;
 DESIGN.md has the error bound), everything else unchanged.  conv_stage() runs one convolution through the detector's kernels.
@@ -126,6 +131,7 @@ class YoloDetector:
         _lib.check_yolo(L.gf_detector_info(self._h, wh, ctypes.byref(nl), ctypes.byref(nc)))
         self.net_w, self.net_h, self.n_layers, self.classes = wh[0], wh[1], nl.value, nc.value
         self.thresh = thresh
+        self.max_batch = 1
         self._boxes = np.zeros((_lib.GF_MAX_BOXES, 4), np.int64)
         self._cls = np.zeros(_lib.GF_MAX_BOXES, np.int32)
         self._prob = np.zeros(_lib.GF_MAX_BOXES, np.float32)
@@ -156,13 +162,59 @@ class YoloDetector:
         m = n.value
         return self._boxes[:m].copy(), self._cls[:m].copy(), self._prob[:m].copy()
 
+    def set_max_batch(self, n):
+        """Size the per-image buffers for detect_batch of up to n frames (1 <= n <= 64; a detector starts at 1).  The weights
+        are shared: each further image costs only its activations (about 217 MiB of layer outputs for yolov3 at 416 x 416)."""
+        _lib.check_yolo(self._L.gf_detector_set_max_batch(self._h, int(n)))
+        self.max_batch = int(n)
+
+    def _detect_batch(self, frames):
+        if len(frames) == 0:
+            raise ValueError("detect_batch needs at least one frame")
+        fs = [_frame(f) for f in frames]
+        on_dev = {f[4] for f in fs}
+        if len(on_dev) != 1:
+            raise ValueError("the frames of one batch must be all host arrays or all CUDA tensors")
+        n = len(fs)
+        ptrs = (ctypes.c_void_p * n)(*[f[0] for f in fs])
+        pitch = (ctypes.c_size_t * n)(*[f[1] for f in fs])
+        w = (ctypes.c_int * n)(*[f[2] for f in fs])
+        h = (ctypes.c_int * n)(*[f[3] for f in fs])
+        cap = _lib.GF_MAX_BOXES * n
+        boxes, cls, prob = np.zeros((cap, 4), np.int64), np.zeros(cap, np.int32), np.zeros(cap, np.float32)
+        start = np.zeros(n + 1, np.int32)
+        _lib.check_yolo(self._L.gf_detector_detect_batch(self._h, n, ptrs, pitch, w, h, on_dev.pop(), boxes.ctypes.data,
+                                                         cls.ctypes.data, prob.ctypes.data, cap, start.ctypes.data))
+        m = start[n]
+        return boxes[:m], cls[:m], prob[:m], start
+
+    def detect_batch(self, frames):
+        """detect() of each frame in one forward pass: a list of (boxes, class_ids, probs), one per frame.  frames: a list of at
+        most max_batch BGR8 frames, all numpy arrays or all CUDA tensors, of any sizes."""
+        boxes, cls, prob, start = self._detect_batch(frames)
+        return [(boxes[a:b].copy(), cls[a:b].copy(), prob[a:b].copy()) for a, b in zip(start[:-1], start[1:])]
+
+    def detect_batch_csr(self, frames):
+        """detect_batch's boxes as (boxes (m, 4) int64, box_start (n + 1,) int32): frame i's are boxes[box_start[i]:box_start[i + 1]],
+        the layout of the C ABI's gf_tracker_group_submit (TrackerGroup.submit takes per-frame lists, as detect_batch returns)."""
+        boxes, _, _, start = self._detect_batch(frames)
+        return boxes, start
+
+    def member_layer_output(self, member, i):
+        """Layer i's output for frame `member` of the last detect / detect_batch, as layer_output."""
+        shape = self.layer_shape(i)
+        out = np.empty(shape, np.float32)
+        _lib.check_yolo(self._L.gf_detector_member_layer_output(self._h, member, i, out.ctypes.data, out.size))
+        return out
+
     def layer_shape(self, i):
         whc = (ctypes.c_int * 3)()
         _lib.check_yolo(self._L.gf_detector_layer_shape(self._h, i, whc))
         return whc[2], whc[1], whc[0]
 
     def layer_output(self, i):
-        """Layer i's output of the last detect as (c, h, w) float32; i = -1: the letterboxed input."""
+        """Layer i's output of the last detect (frame 0 of the last detect_batch) as (c, h, w) float32; i = -1: the letterboxed
+        input."""
         shape = self.layer_shape(i)
         out = np.empty(shape, np.float32)
         _lib.check_yolo(self._L.gf_detector_layer_output(self._h, i, out.ctypes.data, out.size))

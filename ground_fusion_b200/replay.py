@@ -306,19 +306,28 @@ def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=Tru
     return out
 
 
-def replay_group(streams, trackers, windows, adjusters, n_frames, imu_per_frame=7, imu_propagate=True, max_iter=8, feedback=False):
+def replay_group(streams, trackers, windows, adjusters, n_frames, imu_per_frame=7, imu_propagate=True, max_iter=8, feedback=False,
+                 boxes=None, detector=None):
     """K estimators in lockstep, one per stream, each step with one call per stage for all of them: the TrackerGroup over
     `trackers` tracks frame k of every stream, the FeatureWindowGroup over `windows` ingests the step on the device and
     triangulates, fills the K problems, estimator.solve_multi solves them on `adjusters`, setDepth follows, then
     estimator.marginalize_multi with each estimator's own mode, the consistency check and removal, the feedback to each member
     tracker (feedback=True, between tracker-group steps) and the slide.  The host logic is WindowEstimator's, as in replay();
-    returns one result dict per stream in replay()'s format.  No boxes, dense map or USE_MCC."""
+    returns one result dict per stream in replay()'s format.  No dense map or USE_MCC.
+    boxes: USE_YOLO as in replay(), per stream: boxes[i][k] are the detections of frame k of stream i.  They go into the tracker
+    group's step, and the window group takes the features inside them out on the device.
+    detector: USE_YOLO with the detector in the loop, as in replay(): step k runs one detector.detect_batch over the K streams'
+    colour frames before the tracker group's step (its max_batch is raised to K if smaller).  Exclusive with boxes."""
     from . import _lib
     from .estimator import marginalize_multi, solve_multi
     from .feature_tracker import TrackerGroup
     from .feature_window import FeatureWindowGroup
     K = len(streams)
     assert len(trackers) == len(windows) == len(adjusters) == K
+    if detector is not None and boxes is not None:
+        raise ValueError("boxes and detector are exclusive")
+    if detector is not None and detector.max_batch < K:
+        detector.set_max_batch(K)
     tg, wg = TrackerGroup(trackers), FeatureWindowGroup(windows)
     imus = [ImuFromStream(s) for s in streams]
     ests = [WindowEstimator(windows[i], adjusters[i], imu_propagate=imu_propagate, max_iter=max_iter, tracker=trackers[i] if feedback else None)
@@ -339,7 +348,11 @@ def replay_group(streams, trackers, windows, adjusters, n_frames, imu_per_frame=
                     acc, gyr = imu.sample(t); e.processIMU(0.0, acc, gyr)
             gray = [np.ascontiguousarray(f[1]) for f in frames]
             depth = [np.ascontiguousarray(f[2]) if f[2] is not None else None for f in frames]
-            tg.submit([f[0] for f in frames], [g.ctypes.data for g in gray], [d.ctypes.data if d is not None else 0 for d in depth])
+            step_boxes = [boxes[i][k] for i in range(K)] if boxes is not None else None
+            if detector is not None:
+                step_boxes = [r[0] for r in detector.detect_batch([np.ascontiguousarray(s.color(k)[..., ::-1]) for s in streams])]
+            tg.submit([f[0] for f in frames], [g.ctypes.data for g in gray], [d.ctypes.data if d is not None else 0 for d in depth],
+                      boxes=step_boxes)
             tg.wait()
             for i, (e, imu) in enumerate(zip(ests, imus)):
                 if not e.nonlinear:                     # initialisation is out of scope: ground-truth states while the window fills

@@ -824,7 +824,7 @@ int gf_grid_map_stats(gf_grid_map* map, int64_t* out4);
 
 /* ---- YOLO detector (the use_yolo front end's darknet_ros node, YoloObjectDetector.cpp, on the GPU) ------------------------
  * darknet's inference forward pass for the networks the reference ships (vins_estimator/yolo_network_config/cfg: [net],
- * [convolutional], [maxpool], [route], [reorg], [shortcut], [upsample], [region], [yolo]; activations leaky and linear; batch 1),
+ * [convolutional], [maxpool], [route], [reorg], [shortcut], [upsample], [region], [yolo]; activations leaky and linear),
  * bit-exact with darknet's CPU build, followed by the node's decoding (get_network_boxes with hier 0.5, do_nms_obj 0.4) and box
  * extraction.  The boxes feed gf_tracker_*_boxes / trackImagebox.
  * The detector is implemented in its own library, libgf_yolo.so, built next to libgf_b200.so: libgf_b200.so exports these
@@ -847,6 +847,30 @@ int gf_detector_info(gf_detector* det, int* net_wh, int* n_layers, int* classes)
  * written).  Synchronous: the boxes belong to this frame. */
 int gf_detector_detect(gf_detector* det, const void* bgr, size_t pitch, int w, int h, int on_device, gf_box* boxes, int* class_ids,
                        float* probs, int cap, int* n_out);
+/* Batches of frames: one handle runs the forward pass of up to max_batch frames (of any sizes) in one graph launch, one set of
+ * weights for all.  Each frame's result is bit-equal to gf_detector_detect on that frame alone, in both precisions: a
+ * convolution's summation order (the TF32 split-K plan included) is a function of the layer's per-image shape, never of the
+ * batch or of a frame's position in it.  gf_detector_detect is the batch of one, through the same code.
+ *   _set_max_batch  sizes the per-image buffers (every layer's output, the letterboxed inputs, the pinned head copies, the TF32
+ *       split-K workspace) for max_batch frames; a handle starts at 1.  Per image at 416 x 416, from the layer shapes: layer
+ *       outputs of about 28 MiB for yolov2-tiny, 75 MiB for yolov2 and 217 MiB for yolov3, plus 2 MiB of letterboxed input and,
+ *       once TF32 is set, 8 MiB of split-K workspace.  The weights (236 MiB FP32 for yolov3, as much again once TF32 is set)
+ *       are not per image.  max_batch outside [1, GF_DETECTOR_BATCH_MAX]:
+ *       GF_ERR_INVALID_ARG; a failed allocation: GF_ERR_CUDA with the handle unchanged.  Drops the graphs and the last call's
+ *       layer outputs.
+ *   _detect_batch  frames bgr[i] (w[i] x h[i], rows pitch[i] bytes apart; all host or all device pointers as on_device says).
+ *       Frame i's boxes, class ids and probabilities are boxes[box_start[i] .. box_start[i + 1]) (n + 1 offsets: the layout
+ *       gf_tracker_group_submit takes), each range what gf_detector_detect writes for that frame.  1 <= n <= max_batch (more:
+ *       GF_ERR_CAPACITY).  box_start[n] > cap: GF_ERR_CAPACITY with box_start filled and nothing written at or past cap.  Every
+ *       argument is checked before any work, so an argument error changes nothing.  Synchronous.  The graph of each n is captured
+ *       on its first use and kept; gf_detector_set_precision re-captures every one kept.
+ *   _member_layer_output  as gf_detector_layer_output for frame `member` of the last call; gf_detector_layer_output is member 0.
+ * gf_detector_last_device_ms and gf_detector_layer_times cover the whole last call. */
+#define GF_DETECTOR_BATCH_MAX 64      /* = GF_TRACKER_GROUP_MAX: a tracker group maps one to one onto a batch */
+int gf_detector_set_max_batch(gf_detector* det, int max_batch);
+int gf_detector_detect_batch(gf_detector* det, int n, const void* const* bgr, const size_t* pitch, const int* w, const int* h,
+                             int on_device, gf_box* boxes, int* class_ids, float* probs, int cap, int* box_start);
+int gf_detector_member_layer_output(gf_detector* det, int member, int layer, float* out, size_t n);
 /* Device time of the last detect (letterbox + network, at the precision in use), from CUDA events. */
 int gf_detector_last_device_ms(gf_detector* det, float* ms);
 /* whc[3] = output width, height and channels of layer `layer` (0-based, [net] excluded), or of the letterboxed input for -1. */

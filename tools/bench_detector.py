@@ -15,8 +15,16 @@ Prints one JSON line (and writes it to --out): per network
 With --precision exact,tf32 both precisions are timed in the same run on the same card, alternating per network in blocks of
 --frames calls (--rounds rounds; the medians over rounds are reported).  The card's name and power limit are read in the same run.
 
+With --batch 1,2,4,8,16 it times gf_detector_detect_batch instead, for each network, precision and n, on one handle sized for
+the largest n: --batch-calls calls of detect_batch over n distinct 640x480 frames, alternating in each round with the same n
+frames through n sequential detect calls on the same handle.  Per n: device ms per call (CUDA events around letterbox + graph;
+for the sequential form the sum of its n calls), host ms per call (wall time minus device time), frames per second in total,
+the per-frame gain of the batch over the sequential calls, and per layer the batch's time over n times one frame's
+(gf_detector_layer_times), which names the layers where a batch is not faster.  The handle's device memory (cudaMemGetInfo
+before and after creating it and sizing it) is reported per network and precision.
+
     python tools/bench_detector.py [--precision exact] [--frames 200] [--warmup 20] [--reps 20] [--rounds 1] [--cpu-frames 2]
-                                   [--out file.json]
+                                   [--batch 1,2,4,8,16 --batch-calls 30] [--out file.json]
 """
 import argparse
 import json
@@ -125,6 +133,78 @@ def run(name, tmp, args, frames):
     return out
 
 
+def device_free_bytes():
+    import torch
+    torch.cuda.synchronize()
+    return torch.cuda.mem_get_info()[0]
+
+
+def batch_block(det, frames, calls):
+    """calls x detect_batch(frames), then calls x (one detect per frame): per form (wall s per call, median device ms per call)."""
+    det.detect_batch(frames)
+    dev_b = []
+    t0 = time.perf_counter()
+    for _ in range(calls):
+        det.detect_batch(frames)
+        dev_b.append(det.last_device_ms())
+    wall_b = (time.perf_counter() - t0) / calls
+    for f in frames:
+        det.detect(f)
+    dev_s = []
+    t0 = time.perf_counter()
+    for _ in range(calls):
+        ms = 0.0
+        for f in frames:
+            det.detect(f)
+            ms += det.last_device_ms()
+        dev_s.append(ms)
+    wall_s = (time.perf_counter() - t0) / calls
+    return (wall_b, float(np.median(dev_b))), (wall_s, float(np.median(dev_s)))
+
+
+def run_batch(name, tmp, args, frames):
+    """One network: per precision one handle sized for the largest n, every n timed in alternating batch / sequential blocks."""
+    cfg = yolo_ref.cfg_path(name)
+    w = yolo_ref.write_weights(cfg, os.path.join(tmp, name + ".weights"), seed=1)
+    _, layers = conv_flops(cfg)
+    ns = [int(v) for v in args.batch.split(",")]
+    out = {"net": name, "net_size": [416, 416], "frame": [640, 480], "precisions": []}
+    for p in args.precision.split(","):
+        free0 = device_free_bytes()
+        det = YoloDetector(cfg, w, thresh=0.3, precision=p)
+        free1 = device_free_bytes()
+        det.set_max_batch(max(ns))
+        free2 = device_free_bytes()
+        res = {"precision": p, "handle_mib_at_max_batch_1": (free0 - free1) / 2 ** 20,
+               "handle_mib_at_max_batch_%d" % max(ns): (free0 - free2) / 2 ** 20, "batches": []}
+        try:
+            blocks = {n: [] for n in ns}
+            for _ in range(args.rounds):
+                for n in ns:
+                    blocks[n].append(batch_block(det, frames[:n], args.batch_calls))
+            for n in ns:
+                (wb, db), (ws, ds) = [(float(np.median([b[k][0] for b in blocks[n]])), float(np.median([b[k][1] for b in blocks[n]])))
+                                      for k in (0, 1)]
+                det.detect(frames[0])
+                one = det.layer_times(args.reps)
+                det.detect_batch(frames[:n])
+                many = det.layer_times(args.reps)
+                ratio = many / np.maximum(n * one, 1e-9)
+                slow = [{"i": int(i), "type": layers[i]["type"], "out": [layers[i]["out_c"], layers[i]["out_h"], layers[i]["out_w"]],
+                         "batch_ms": round(float(many[i]), 5), "n_x_single_ms": round(float(n * one[i]), 5),
+                         "ratio": round(float(ratio[i]), 3)} for i in np.argsort(-ratio)[:5]]
+                res["batches"].append({
+                    "n": n, "batch_device_ms": db, "batch_host_ms": wb * 1e3 - db, "batch_fps": n / wb,
+                    "sequential_device_ms": ds, "sequential_host_ms": ws * 1e3 - ds, "sequential_fps": n / ws,
+                    "device_gain_per_frame": ds / db, "wall_gain_per_frame": ws / wb,
+                    "layers_ms_batch": float(many.sum()), "layers_ms_n_x_single": float(n * one.sum()),
+                    "layers_least_gain": slow})
+        finally:
+            det.close()
+        out["precisions"].append(res)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=200)
@@ -134,16 +214,23 @@ def main():
     ap.add_argument("--nets", default="yolov2-tiny,yolov3")
     ap.add_argument("--precision", default="exact", help="comma-separated: exact, tf32")
     ap.add_argument("--rounds", type=int, default=1)
+    ap.add_argument("--batch", default=None, help="comma-separated batch sizes: time detect_batch against sequential detect")
+    ap.add_argument("--batch-calls", type=int, default=30)
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     from ground_fusion_b200.synth import SyntheticStream
     st = SyntheticStream(seed=0)
-    frames = [np.ascontiguousarray(st.color(k)[..., ::-1]) for k in range(8)]
+    n_frames = max([8] + [int(v) for v in args.batch.split(",")] if args.batch else [8])
+    frames = [np.ascontiguousarray(st.color(k)[..., ::-1]) for k in range(n_frames)]
     gpu = gpu_name_and_power_limit()
     with tempfile.TemporaryDirectory() as tmp:
-        res = {"gpu": gpu, "nets": [run(n, tmp, args, frames) for n in args.nets.split(",")]}
-        if args.precision == "exact":
-            res["bound"] = BOUNDS["exact"][0]
+        if args.batch:
+            res = {"gpu": gpu, "rounds": args.rounds, "calls_per_block": args.batch_calls,
+                   "nets": [run_batch(n, tmp, args, frames) for n in args.nets.split(",")]}
+        else:
+            res = {"gpu": gpu, "nets": [run(n, tmp, args, frames) for n in args.nets.split(",")]}
+            if args.precision == "exact":
+                res["bound"] = BOUNDS["exact"][0]
     line = json.dumps(res)
     print(line)
     if args.out:
