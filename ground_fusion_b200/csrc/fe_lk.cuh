@@ -118,9 +118,12 @@ __device__ __forceinline__ void lk_tma_wait(unsigned long long* bar, unsigned& p
     while (!mbar_try_wait(bar, phase)) { }
     phase ^= 1u;
 }
-// once per kernel, before the first lk_track_point
+// once per kernel, before the first lk_track_point.  Also zeroes the chain padding, which must read +0.0f: no pass writes a
+// padding slot, and every pass rewrites each real slot before the chains read it.
 __device__ __forceinline__ void lk_tma_init(LKSmem& S, int tid)
 {
+    for (int i = tid; i < 3 * LK_Q; i += LK_THREADS) S.aterms[i] = 0.f;
+    for (int i = tid; i < 2 * LK_Q; i += LK_THREADS) S.bterms[i] = 0.f;
     if (tid == 0) {
         mbar_init(&S.mbar_i, 1);
         mbar_init(&S.mbar_p[0], 1);
@@ -595,8 +598,6 @@ __device__ __forceinline__ void lk_track_point(LKSmem& S, int tid, const Pyramid
     status = 1;
     [[maybe_unused]] long long tl = gf_clock();
     __syncthreads();     // the previous pass's readers of every buffer are done
-    for (int i = tid; i < 3 * LK_Q; i += LK_THREADS) S.aterms[i] = 0.f;    // chain padding must read +0.0f
-    for (int i = tid; i < 2 * LK_Q; i += LK_THREADS) S.bterms[i] = 0.f;
     // the template windows of all levels depend only on p: fetch them together (one memory latency instead of one per level)
     const float2 g = use_init ? init : p;
     int n_box = 0;

@@ -85,7 +85,7 @@ __device__ __forceinline__ Tma lk_tma_of(const LKMapSet& M)
 
 // gf_stage_lk: one CTA per point, in the LK form ROLES selects (LKForm above)
 template <bool ROLES>
-__global__ void __launch_bounds__(LK_THREADS) k_lk_stage(Pyramid I, Pyramid J, const float2* prev_pts, float2* next_pts,
+__global__ void __launch_bounds__(LK_THREADS) k_lk_stage(const __grid_constant__ Pyramid I, const __grid_constant__ Pyramid J, const float2* prev_pts, float2* next_pts,
                                                          int n, int max_level, int use_init, uint8_t* status, const __grid_constant__ LKMapSet M)
 {
     __shared__ typename LKForm<ROLES>::Smem sm;
@@ -115,7 +115,7 @@ __device__ __forceinline__ void lk_pred_point(const Pyramid& prev, const Pyramid
     if (tid == 0) { fa.cur_pts[i] = out; fa.status[i] = (uint8_t)st; if (st) atomicAdd(&sc->pred_succ, 1); atomicAdd(&sc->lk_iters, iters); }
 }
 template <bool ROLES>
-__global__ void __launch_bounds__(LK_THREADS) k_lk_pred(Pyramid prev, Pyramid cur, TrackScalars* sc, FeatArrays fa, const __grid_constant__ LKMapSet M)
+__global__ void __launch_bounds__(LK_THREADS) k_lk_pred(const __grid_constant__ Pyramid prev, const __grid_constant__ Pyramid cur, TrackScalars* sc, FeatArrays fa, const __grid_constant__ LKMapSet M)
 {
     if ((int)blockIdx.x >= sc->n_prev) return;
     lk_pred_point<0, ROLES>(prev, cur, sc, fa, M);
@@ -171,8 +171,8 @@ __device__ __forceinline__ void track_point(const Pyramid& prev, const Pyramid& 
     }
 }
 template <bool ROLES>
-__global__ void __launch_bounds__(LK_THREADS, GF_TRACK_MIN_CTAS) k_track(Pyramid prev, Pyramid cur, TrackScalars* sc, FeatArrays fa,
-                                                      const FrameParams* fp, int flow_back, const __grid_constant__ LKMapSet M)
+__global__ void __launch_bounds__(LK_THREADS, GF_TRACK_MIN_CTAS) k_track(const __grid_constant__ Pyramid prev, const __grid_constant__ Pyramid cur,
+                                                      TrackScalars* sc, FeatArrays fa, const FrameParams* fp, int flow_back, const __grid_constant__ LKMapSet M)
 {
     if ((int)blockIdx.x >= sc->n_prev) return;
     track_point<0, ROLES>(prev, cur, sc, fa, fp, flow_back, M);
