@@ -66,7 +66,8 @@ std::map<int, std::vector<std::pair<int, Eigen::Matrix<double, 8, 1>>>> FeatureT
     start(_cur_time, _img);
     int n = 0;
     const uint16_t *depth = _img1.empty() ? nullptr : _img1.ptr<uint16_t>();
-    if (gf_tracker_track(gf_, _cur_time, _img.data, _img.step, depth, _img1.empty() ? 0 : _img1.step, out_.data(), &n, nullptr, nullptr))
+    if (gf_tracker_track(gf_, _cur_time, _img.data, _img.step, depth, _img1.empty() ? 0 : _img1.step, 0, nullptr, 0, out_.data(), &n, nullptr,
+                         nullptr, nullptr))
         gf_fatal("gf_tracker_track");
     return publish(n, nullptr);
 }
@@ -79,9 +80,9 @@ std::map<int, std::vector<std::pair<int, Eigen::Matrix<double, 8, 1>>>> FeatureT
     for (const darknet_ros_msgs::BoundingBox &b : _boxes->bounding_boxes) boxes_.push_back(gf_box{b.xmin, b.ymin, b.xmax, b.ymax});
     int n = 0;
     const uint16_t *depth = _img1.empty() ? nullptr : _img1.ptr<uint16_t>();
-    if (gf_tracker_track_boxes(gf_, _cur_time, _img.data, _img.step, depth, _img1.empty() ? 0 : _img1.step, 0, boxes_.data(), (int)boxes_.size(),
-                               out_.data(), &n, in_box_.data(), nullptr, nullptr))
-        gf_fatal("gf_tracker_track_boxes");
+    if (gf_tracker_track(gf_, _cur_time, _img.data, _img.step, depth, _img1.empty() ? 0 : _img1.step, 0, boxes_.data(), (int)boxes_.size(),
+                         out_.data(), &n, in_box_.data(), nullptr, nullptr))
+        gf_fatal("gf_tracker_track");
     return publish(n, in_box_.data());
 }
 

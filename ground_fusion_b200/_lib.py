@@ -87,20 +87,13 @@ def lib():
         L.gf_tracker_destroy.argtypes = [vp]
         L.gf_tracker_destroy.restype = None
         L.gf_tracker_host_buffers.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
-        L.gf_tracker_track.argtypes = [vp, d, vp, sz, vp, sz, vp, ctypes.POINTER(i), vp, ctypes.POINTER(TrackInfo)]
-        L.gf_tracker_submit.argtypes = [vp, d, vp, sz, vp, sz]
-        L.gf_tracker_submit_device.argtypes = [vp, d, vp, vp]
+        L.gf_tracker_track.argtypes = [vp, d, vp, sz, vp, sz, i, vp, i, vp, ctypes.POINTER(i), vp, vp, ctypes.POINTER(TrackInfo)]
+        L.gf_tracker_submit.argtypes = [vp, d, vp, sz, vp, sz, i, vp, i]
+        L.gf_tracker_wait.argtypes = [vp, vp, ctypes.POINTER(i), vp, vp, ctypes.POINTER(TrackInfo)]
+        L.gf_tracker_track_batch.argtypes = [vp, i, vp, vp, sz, vp, sz, i, vp, vp, vp, vp, vp, vp, vp]
+        L.gf_tracker_track_batch_multi.argtypes = [vp, i, i, vp, vp, sz, vp, sz, i, vp, vp, vp, vp, vp, vp, vp]
         L.gf_tracker_timer_start.argtypes = [vp]
         L.gf_tracker_timer_stop.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
-        L.gf_tracker_wait.argtypes = [vp, vp, ctypes.POINTER(i), vp, ctypes.POINTER(TrackInfo)]
-        L.gf_tracker_track_device.argtypes = [vp, d, vp, vp, vp, ctypes.POINTER(i), vp, ctypes.POINTER(TrackInfo)]
-        L.gf_tracker_track_batch.argtypes = [vp, i, vp, vp, sz, vp, sz, i, vp, vp, vp, vp]
-        L.gf_tracker_track_batch_multi.argtypes = [vp, i, i, vp, vp, sz, vp, sz, i, vp, vp, vp, vp]
-        L.gf_tracker_submit_boxes.argtypes = [vp, d, vp, sz, vp, sz, i, vp, i]
-        L.gf_tracker_wait_boxes.argtypes = [vp, vp, ctypes.POINTER(i), vp, vp, ctypes.POINTER(TrackInfo)]
-        L.gf_tracker_track_boxes.argtypes = [vp, d, vp, sz, vp, sz, i, vp, i, vp, ctypes.POINTER(i), vp, vp, ctypes.POINTER(TrackInfo)]
-        L.gf_tracker_track_batch_boxes.argtypes = [vp, i, vp, vp, sz, vp, sz, i, vp, vp, vp, vp, vp, vp, vp]
-        L.gf_tracker_track_batch_multi_boxes.argtypes = [vp, i, i, vp, vp, sz, vp, sz, i, vp, vp, vp, vp, vp, vp, vp]
         L.gf_tracker_group_create.argtypes = [ctypes.POINTER(vp), vp, i]
         L.gf_tracker_group_destroy.argtypes = [vp]
         L.gf_tracker_group_destroy.restype = None

@@ -55,6 +55,25 @@ static int check_boxes(const gf_box* b, int n)
     if (n > GF_MAX_BOXES) return set_err(GF_ERR_CAPACITY, "more than GF_MAX_BOXES boxes in one frame");
     return GF_OK;
 }
+// The box lists boxes[box_start[k] .. box_start[k + 1]) of frames k < count; *bad is the first bad frame.
+static int check_box_lists(const gf_box* boxes, const int* box_start, long long count, long long* bad)
+{
+    for (long long k = 0; k < count; k++) {
+        *bad = k;
+        if (box_start[k] < 0) return set_err(GF_ERR_INVALID_ARG, "bad box offsets");
+        int rc = check_boxes(boxes ? boxes + box_start[k] : nullptr, box_start[k + 1] - box_start[k]);
+        if (rc) return rc;
+    }
+    return GF_OK;
+}
+// Host frames may have row pitches larger than the row; device frames are tightly packed (their pitches are ignored).
+static int check_pitches(int w, bool on_device, size_t gray_pitch, bool has_depth, size_t depth_pitch)
+{
+    if (on_device) return GF_OK;
+    if (gray_pitch < (size_t)w) return set_err(GF_ERR_INVALID_ARG, "gray_pitch smaller than width");
+    if (has_depth && depth_pitch < (size_t)w * 2) return set_err(GF_ERR_INVALID_ARG, "depth_pitch smaller than width*2");
+    return GF_OK;
+}
 
 // gf_stage_in_boxes: the test k_select_finalize applies to its outputs, on its own
 __global__ void __launch_bounds__(256) k_in_boxes_stage(const float2* pts, int n, const BoxSet* boxes, uint8_t* in_box)
@@ -381,11 +400,34 @@ struct gf_tracker {
     double prev_time;
     bool has_pred, depth_valid[2];
     float last_ms;
-    long long out_frame1;                // 1 + the index of the frame gf_tracker_wait* last returned (its results are in slot index % 2 until
+    long long out_frame1;                // 1 + the index of the frame gf_tracker_wait last returned (its results are in slot index % 2 until
                                          // frame index + GF_PIPE is submitted); 0: none, or a group step
 };
 
 static inline int in_flight(const gf_tracker* t) { return (int)(t->n_submitted - t->n_waited); }
+
+// The number of features a result block returns.  Reference quirk: depth_cam with an empty depth image produces an empty
+// featureFrame (feature_tracker.cpp:342).
+static int out_count(const gf_tracker* t, const OutBlock* ob, bool depth_valid)
+{
+    return (t->cfg.depth_cam && !depth_valid) ? 0 : ob->hdr.n_out;
+}
+
+// Copies the host copy of a result block (an OutBlock prefix up to obs[max_cnt]) into the caller's arrays, each nullable.
+static void decode_out(const gf_tracker* t, const OutBlock* ob, bool depth_valid, gf_obs* out, int* n_out, uint8_t* in_box,
+                       uint8_t* status_out, gf_track_info* info)
+{
+    const OutHeader& hd = ob->hdr;
+    const int n = out_count(t, ob, depth_valid);
+    if (n_out) *n_out = n;
+    if (out && n > 0) memcpy(out, ob->obs, (size_t)n * sizeof(gf_obs));
+    if (in_box) for (int i = 0; i < n; i++) in_box[i] = (uint8_t)((ob->in_box[i >> 5] >> (i & 31)) & 1u);
+    if (status_out && hd.n_prev > 0) memcpy(status_out, ob->status, hd.n_prev);
+    if (info) {
+        info->n_prev = hd.n_prev; info->n_tracked = hd.n_tracked; info->n_kept = hd.n_kept; info->n_new = hd.n_new;
+        info->n_candidates = hd.n_cand; info->nms_rounds = hd.nms_rounds; info->eig_fixups = hd.eig_fixups; info->lk_iterations = hd.lk_iters;
+    }
+}
 
 // Trackers alive per device (gf_tracker_create .. gf_tracker_destroy).  A tracker alone on its device runs k_track in the
 // two-role LK form, which shortens the slowest feature's chain; while other trackers share the device, the throughput of
@@ -774,16 +816,47 @@ static int run_piece(bool direct, cudaStream_t s, cudaGraphExec_t* exec, int* nk
     return GF_OK;
 }
 
+// Enqueues on s the copies of tracker t's next frame: gray into d_raw (equalisation) or pyramid level 0, depth (nullable)
+// into the frame's depth slot.
+static int enqueue_upload(cudaStream_t s, const gf_tracker* t, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch,
+                          bool on_device)
+{
+    const long long f = t->n_submitted;
+    const int w = t->w, h = t->h;
+    if (on_device) { gray_pitch = w; depth_pitch = (size_t)w * 2; }
+    const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    if (t->equalize) GF_CUDA(cudaMemcpy2DAsync(t->d_raw, t->raw_pitch, gray, gray_pitch, w, h, kind, s));
+    else GF_CUDA(cudaMemcpy2DAsync(t->d_pyr[f % 3][0], t->lp[0], gray, gray_pitch, w, h, kind, s));
+    if (depth)
+        GF_CUDA(cudaMemcpy2DAsync(t->d_depth[f % 2], (size_t)t->depth_pitch_el * 2, depth, depth_pitch, (size_t)w * 2, h, kind, s));
+    return GF_OK;
+}
+
+// The parameters of tracker t's next frame, taken at `time`.
+static void frame_params(FrameParams* fp, const gf_tracker* t, double time, bool depth_valid, const gf_box* boxes, int n_boxes)
+{
+    fp->dt = time - t->prev_time;
+    fp->has_pred = t->has_pred ? 1 : 0;
+    fp->depth_valid = depth_valid ? 1 : 0;
+    put_boxes(fp->boxes, boxes, n_boxes);
+}
+
+// Advances tracker t's host state past its next frame, once that frame has been enqueued.
+static void frame_enqueued(gf_tracker* t, double time, bool depth_valid)
+{
+    t->prev_time = time;
+    t->has_pred = false;
+    t->depth_valid[t->n_submitted % 2] = depth_valid;
+    t->n_submitted++;
+}
+
 // Everything after the H2D (or D2D) copies of frame f have been enqueued on s_up.  With equalisation the gray frame is in
 // d_raw and CLAHE writes pyramid level 0 on s_up, ahead of ev_up (profiling: part of stage 1).
 static int enqueue_frame(gf_tracker* t, long long f, double time, bool depth_valid, const gf_box* boxes, int n_boxes)
 {
     const int es = (int)(f % 2), key = (int)(f % 6), hp = t->has_pred ? 1 : 0;
     const bool direct = !t->use_graph || t->profiling;
-    t->h_fp[es]->dt = time - t->prev_time;
-    t->h_fp[es]->has_pred = hp;
-    t->h_fp[es]->depth_valid = depth_valid ? 1 : 0;
-    put_boxes(t->h_fp[es]->boxes, boxes, n_boxes);
+    frame_params(t->h_fp[es], t, time, depth_valid, boxes, n_boxes);
     GF_MARK(0, t->s_up);   // end of upload
     if (t->equalize) {
         const int slot = (int)(f % 3);
@@ -816,10 +889,7 @@ static int enqueue_frame(gf_tracker* t, long long f, double time, bool depth_val
     GF_CUDA(cudaMemcpyAsync(t->h_out[es], t->d_out[es], offsetof(OutBlock, obs) + (size_t)t->cfg.max_cnt * sizeof(gf_obs),
                             cudaMemcpyDeviceToHost, t->s_out));
     GF_CUDA(cudaEventRecord(t->ev_out[es], t->s_out));
-    t->prev_time = time;
-    t->has_pred = false;
-    t->depth_valid[es] = depth_valid;
-    t->n_submitted = f + 1;
+    frame_enqueued(t, time, depth_valid);
     return GF_OK;
 }
 
@@ -834,54 +904,25 @@ static int check_submit(gf_tracker* t)
     return GF_OK;
 }
 
-// Frame intake.  Host frames may have row pitches larger than the row; the caller's buffers are read by the copy engine
-// directly: truly asynchronous when they are pinned (gf_tracker_host_buffers or any cudaHostAlloc/cudaHostRegister memory:
-// keep them unchanged until the frame has been collected); for pageable memory CUDA stages the data before cudaMemcpy2DAsync
-// returns.  Device frames are tightly packed (the pitches are ignored).
-static int submit(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch, bool on_device,
-                  const gf_box* boxes, int n_boxes)
-{
-    if (!t || !gray) return set_err(GF_ERR_INVALID_ARG, "null argument");
-    int rc = check_submit(t);
-    if (rc) return rc;
-    GF_CUDA(cudaSetDevice(t->device));
-    const int w = t->w, h = t->h;
-    if (on_device) {
-        gray_pitch = w; depth_pitch = (size_t)w * 2;
-    } else {
-        if (gray_pitch < (size_t)w) return set_err(GF_ERR_INVALID_ARG, "gray_pitch smaller than width");
-        if (depth && depth_pitch < (size_t)w * 2) return set_err(GF_ERR_INVALID_ARG, "depth_pitch smaller than width*2");
-    }
-    const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    const long long f = t->n_submitted;
-    cudaStream_t s = t->s_up;
-    GF_CUDA(cudaEventRecord(t->ev_t0[f % 2], s));
-    if (t->equalize) GF_CUDA(cudaMemcpy2DAsync(t->d_raw, t->raw_pitch, gray, gray_pitch, w, h, kind, s));
-    else GF_CUDA(cudaMemcpy2DAsync(t->d_pyr[f % 3][0], t->lp[0], gray, gray_pitch, w, h, kind, s));
-    if (depth)
-        GF_CUDA(cudaMemcpy2DAsync(t->d_depth[f % 2], (size_t)t->depth_pitch_el * 2, depth, depth_pitch, (size_t)w * 2, h, kind, s));
-    return enqueue_frame(t, f, time, depth != nullptr, boxes, n_boxes);
-}
-
-int gf_tracker_submit(gf_tracker* t, double time, const uint8_t* gray, size_t gray_pitch, const uint16_t* depth, size_t depth_pitch)
-{
-    return submit(t, time, gray, gray_pitch, depth, depth_pitch, false, nullptr, 0);
-}
-
-int gf_tracker_submit_device(gf_tracker* t, double time, const void* d_gray, const void* d_depth)
-{
-    return submit(t, time, d_gray, 0, d_depth, 0, true, nullptr, 0);
-}
-
-int gf_tracker_submit_boxes(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch,
-                            int on_device, const gf_box* boxes, int n_boxes)
+// Frame intake.  The caller's host buffers are read by the copy engine directly: truly asynchronous when they are pinned
+// (gf_tracker_host_buffers or any cudaHostAlloc/cudaHostRegister memory: keep them unchanged until the frame has been
+// collected); for pageable memory CUDA stages the data before cudaMemcpy2DAsync returns.
+int gf_tracker_submit(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch, int on_device,
+                      const gf_box* boxes, int n_boxes)
 {
     int rc = check_boxes(boxes, n_boxes);
     if (rc) return rc;
-    return submit(t, time, gray, gray_pitch, depth, depth_pitch, on_device != 0, boxes, n_boxes);
+    if (!t || !gray) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    if ((rc = check_submit(t))) return rc;
+    GF_CUDA(cudaSetDevice(t->device));
+    if ((rc = check_pitches(t->w, on_device != 0, gray_pitch, depth != nullptr, depth_pitch))) return rc;
+    const long long f = t->n_submitted;
+    GF_CUDA(cudaEventRecord(t->ev_t0[f % 2], t->s_up));
+    if ((rc = enqueue_upload(t->s_up, t, gray, gray_pitch, depth, depth_pitch, on_device != 0))) return rc;
+    return enqueue_frame(t, f, time, depth != nullptr, boxes, n_boxes);
 }
 
-int gf_tracker_wait_boxes(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info)
+int gf_tracker_wait(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info)
 {
     if (!t) return set_err(GF_ERR_INVALID_ARG, "null tracker");
     if (in_flight(t) == 0) return set_err(GF_ERR_INVALID_ARG, "no frame in flight");
@@ -897,51 +938,17 @@ int gf_tracker_wait_boxes(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* in_bo
         for (int i = 0; i < 7; i++) GF_CUDA(cudaEventElapsedTime(&t->stage_ms[i], b[i], b[i + 1]));
         GF_CUDA(cudaEventElapsedTime(&t->stage_ms[7], t->ev_st[7], t->ev_st[8]));
     }
-    const OutBlock& ob = *t->h_out[es];
-    const OutHeader& hd = ob.hdr;
-    int n = hd.n_out;
-    if (t->cfg.depth_cam && !t->depth_valid[es]) n = 0;   // see body_dep2
-    if (n_out) *n_out = n;
-    if (out && n > 0) memcpy(out, ob.obs, (size_t)n * sizeof(gf_obs));
-    if (in_box) for (int i = 0; i < n; i++) in_box[i] = (uint8_t)((ob.in_box[i >> 5] >> (i & 31)) & 1u);
-    if (status_out && hd.n_prev > 0) memcpy(status_out, ob.status, hd.n_prev);
-    if (info) {
-        info->n_prev = hd.n_prev; info->n_tracked = hd.n_tracked; info->n_kept = hd.n_kept; info->n_new = hd.n_new;
-        info->n_candidates = hd.n_cand; info->nms_rounds = hd.nms_rounds; info->eig_fixups = hd.eig_fixups; info->lk_iterations = hd.lk_iters;
-    }
+    decode_out(t, t->h_out[es], t->depth_valid[es], out, n_out, in_box, status_out, info);
     return GF_OK;
 }
 
-int gf_tracker_wait(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* status_out, gf_track_info* info)
-{
-    return gf_tracker_wait_boxes(t, out, n_out, nullptr, status_out, info);
-}
-
-int gf_tracker_track(gf_tracker* t, double time, const uint8_t* gray, size_t gray_pitch, const uint16_t* depth, size_t depth_pitch,
-                     gf_obs* out, int* n_out, uint8_t* status_out, gf_track_info* info)
+int gf_tracker_track(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch, int on_device,
+                     const gf_box* boxes, int n_boxes, gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info)
 {
     if (t && in_flight(t) > 0) return set_err(GF_ERR_INVALID_ARG, "previous frame not collected: call gf_tracker_wait first");
-    int rc = gf_tracker_submit(t, time, gray, gray_pitch, depth, depth_pitch);
+    int rc = gf_tracker_submit(t, time, gray, gray_pitch, depth, depth_pitch, on_device, boxes, n_boxes);
     if (rc) return rc;
-    return gf_tracker_wait(t, out, n_out, status_out, info);
-}
-
-int gf_tracker_track_device(gf_tracker* t, double time, const void* d_gray, const void* d_depth, gf_obs* out, int* n_out,
-                            uint8_t* status_out, gf_track_info* info)
-{
-    if (t && in_flight(t) > 0) return set_err(GF_ERR_INVALID_ARG, "previous frame not collected");
-    int rc = gf_tracker_submit_device(t, time, d_gray, d_depth);
-    if (rc) return rc;
-    return gf_tracker_wait(t, out, n_out, status_out, info);
-}
-
-int gf_tracker_track_boxes(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch, int on_device,
-                           const gf_box* boxes, int n_boxes, gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info)
-{
-    if (t && in_flight(t) > 0) return set_err(GF_ERR_INVALID_ARG, "previous frame not collected: call gf_tracker_wait first");
-    int rc = gf_tracker_submit_boxes(t, time, gray, gray_pitch, depth, depth_pitch, on_device, boxes, n_boxes);
-    if (rc) return rc;
-    return gf_tracker_wait_boxes(t, out, n_out, in_box, status_out, info);
+    return gf_tracker_wait(t, out, n_out, in_box, status_out, info);
 }
 
 // One camera stream of a batch call: its frames, where its results go, and how far it has got.
@@ -959,24 +966,21 @@ static int lane_collect(BatchLane& L)
 {
     const int k = L.collected++;
     const size_t cap = (size_t)L.t->cfg.max_cnt;
-    return gf_tracker_wait_boxes(L.t, L.out ? L.out + (size_t)k * cap : nullptr, L.n_out ? L.n_out + k : nullptr,
-                                 L.in_box ? L.in_box + (size_t)k * cap : nullptr, L.status_out ? L.status_out + (size_t)k * cap : nullptr,
-                                 L.info ? L.info + k : nullptr);
+    return gf_tracker_wait(L.t, L.out ? L.out + (size_t)k * cap : nullptr, L.n_out ? L.n_out + k : nullptr,
+                           L.in_box ? L.in_box + (size_t)k * cap : nullptr, L.status_out ? L.status_out + (size_t)k * cap : nullptr,
+                           L.info ? L.info + k : nullptr);
 }
 
-int gf_tracker_track_batch_multi_boxes(gf_tracker* const* trackers, int n_trackers, int n, const double* times, const void* const* gray,
-                                       size_t gray_pitch, const void* const* depth, size_t depth_pitch, int on_device,
-                                       const gf_box* boxes, const int* box_start, gf_obs* out, int* n_out, uint8_t* in_box,
-                                       uint8_t* status_out, gf_track_info* info)
+int gf_tracker_track_batch_multi(gf_tracker* const* trackers, int n_trackers, int n, const double* times, const void* const* gray,
+                                 size_t gray_pitch, const void* const* depth, size_t depth_pitch, int on_device,
+                                 const gf_box* boxes, const int* box_start, gf_obs* out, int* n_out, uint8_t* in_box,
+                                 uint8_t* status_out, gf_track_info* info)
 {
     if (!trackers || n_trackers < 1 || n < 0 || (n > 0 && (!times || !gray))) return set_err(GF_ERR_INVALID_ARG, "null argument");
-    if (box_start && n > 0) {            // every frame's list is checked before the first frame is submitted
-        for (long long k = 0; k < (long long)n_trackers * n; k++) {
-            if (box_start[k] < 0) return set_err(GF_ERR_INVALID_ARG, "bad box offsets");
-            int rc = check_boxes(boxes ? boxes + box_start[k] : nullptr, box_start[k + 1] - box_start[k]);
-            if (rc) return rc;
-        }
-    }
+    int rc;
+    long long bad;
+    // every frame's list is checked before the first frame is submitted
+    if (box_start && (rc = check_box_lists(boxes, box_start, (long long)n_trackers * n, &bad))) return rc;
     std::vector<BatchLane> lanes((size_t)n_trackers);
     for (int i = 0; i < n_trackers; i++) {
         gf_tracker* t = trackers[i];
@@ -984,10 +988,7 @@ int gf_tracker_track_batch_multi_boxes(gf_tracker* const* trackers, int n_tracke
         for (int j = 0; j < i; j++) if (trackers[j] == t) return set_err(GF_ERR_INVALID_ARG, "the same tracker listed twice");
         if (in_flight(t) > 0) return set_err(GF_ERR_INVALID_ARG, "previous frame not collected");
         if (t->profiling) return set_err(GF_ERR_INVALID_ARG, "profiling mode runs one frame at a time");
-        if (!on_device) {
-            if (gray_pitch < (size_t)t->w) return set_err(GF_ERR_INVALID_ARG, "gray_pitch smaller than width");
-            if (depth && depth_pitch < (size_t)t->w * 2) return set_err(GF_ERR_INVALID_ARG, "depth_pitch smaller than width*2");
-        }
+        if ((rc = check_pitches(t->w, on_device != 0, gray_pitch, depth != nullptr, depth_pitch))) return rc;
         const size_t cap = (size_t)t->cfg.max_cnt, o = (size_t)i * n;
         BatchLane& L = lanes[i];
         L.t = t; L.times = times + o; L.gray = gray + o; L.depth = depth ? depth + o : nullptr;
@@ -998,13 +999,12 @@ int gf_tracker_track_batch_multi_boxes(gf_tracker* const* trackers, int n_tracke
         for (int k = 0; k < n; k++) if (!L.gray[k]) return set_err(GF_ERR_INVALID_ARG, "null frame pointer");
     }
     if (n == 0) return GF_OK;
-    int rc;
     // Every lane goes frame by frame through the five-stream submit / wait pipeline of gf_tracker_submit, lanes interleaved:
     // one host thread keeps up to two frames in flight on each tracker.
     for (int k = 0; k < n; k++) {
         for (BatchLane& L : lanes) {
-            rc = submit(L.t, L.times[k], L.gray[k], gray_pitch, L.depth ? L.depth[k] : nullptr, depth_pitch, on_device != 0,
-                        L.frame_boxes(k), L.n_boxes(k));
+            rc = gf_tracker_submit(L.t, L.times[k], L.gray[k], gray_pitch, L.depth ? L.depth[k] : nullptr, depth_pitch, on_device,
+                                   L.frame_boxes(k), L.n_boxes(k));
             if (rc) return rc;
         }
         for (BatchLane& L : lanes) if (in_flight(L.t) == GF_PIPE && (rc = lane_collect(L))) return rc;
@@ -1013,27 +1013,12 @@ int gf_tracker_track_batch_multi_boxes(gf_tracker* const* trackers, int n_tracke
     return GF_OK;
 }
 
-int gf_tracker_track_batch_multi(gf_tracker* const* trackers, int n_trackers, int n, const double* times, const void* const* gray, size_t gray_pitch,
-                                 const void* const* depth, size_t depth_pitch, int on_device,
-                                 gf_obs* out, int* n_out, uint8_t* status_out, gf_track_info* info)
-{
-    return gf_tracker_track_batch_multi_boxes(trackers, n_trackers, n, times, gray, gray_pitch, depth, depth_pitch, on_device, nullptr, nullptr,
-                                              out, n_out, nullptr, status_out, info);
-}
-
 int gf_tracker_track_batch(gf_tracker* t, int n, const double* times, const void* const* gray, size_t gray_pitch,
-                           const void* const* depth, size_t depth_pitch, int on_device,
-                           gf_obs* out, int* n_out, uint8_t* status_out, gf_track_info* info)
+                           const void* const* depth, size_t depth_pitch, int on_device, const gf_box* boxes, const int* box_start,
+                           gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info)
 {
-    return gf_tracker_track_batch_multi(&t, 1, n, times, gray, gray_pitch, depth, depth_pitch, on_device, out, n_out, status_out, info);
-}
-
-int gf_tracker_track_batch_boxes(gf_tracker* t, int n, const double* times, const void* const* gray, size_t gray_pitch,
-                                 const void* const* depth, size_t depth_pitch, int on_device, const gf_box* boxes, const int* box_start,
-                                 gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info)
-{
-    return gf_tracker_track_batch_multi_boxes(&t, 1, n, times, gray, gray_pitch, depth, depth_pitch, on_device, boxes, box_start,
-                                              out, n_out, in_box, status_out, info);
+    return gf_tracker_track_batch_multi(&t, 1, n, times, gray, gray_pitch, depth, depth_pitch, on_device, boxes, box_start,
+                                        out, n_out, in_box, status_out, info);
 }
 
 int gf_tracker_set_prediction(gf_tracker* t, const int32_t* ids, const double* xyz, int n)
@@ -1150,6 +1135,11 @@ struct gf_tracker_group {
 };
 
 static inline int group_in_flight(const gf_tracker_group* g) { return (int)(g->n_submitted - g->n_waited); }
+// Member i's result block in a step's d_out or h_out
+static inline OutBlock* group_block(uint8_t* out, const gf_tracker_group* g, int i)
+{
+    return reinterpret_cast<OutBlock*>(out + (size_t)i * g->out_stride);
+}
 
 static int member_err(int code, int k, const char* what)
 {
@@ -1279,14 +1269,8 @@ static int group_submit(gf_tracker_group* g, const double* times, const void* co
                         size_t depth_pitch, bool on_device, const gf_box* const* bx, const int* nb)
 {
     if (group_in_flight(g) >= GF_PIPE) return set_err(GF_ERR_INVALID_ARG, "two steps in flight: call gf_tracker_group_wait first");
-    const gf_tracker* a = g->m[0];
-    const int w = a->w, h = a->h;
-    if (on_device) {
-        gray_pitch = w; depth_pitch = (size_t)w * 2;
-    } else {
-        if (gray_pitch < (size_t)w) return set_err(GF_ERR_INVALID_ARG, "gray_pitch smaller than width");
-        if (depth && depth_pitch < (size_t)w * 2) return set_err(GF_ERR_INVALID_ARG, "depth_pitch smaller than width*2");
-    }
+    int rc = check_pitches(g->m[0]->w, on_device, gray_pitch, depth != nullptr, depth_pitch);
+    if (rc) return rc;
     for (int i = 0; i < g->n; i++) {
         const gf_tracker* t = g->m[i];
         if (!gray[i]) return member_err(GF_ERR_INVALID_ARG, i, "null frame pointer");
@@ -1310,30 +1294,18 @@ static int group_submit(gf_tracker_group* g, const double* times, const void* co
         G.sc = t->d_sc; G.fa = t->fa; G.grid = t->grid; G.cam = t->cam;
         G.eig = t->d_eig[es]; G.cov = t->d_cov; G.box = t->d_box;
         G.depth = t->d_depth[es]; G.raw = t->d_raw; G.lut = t->d_lut;
-        uint8_t* ob = g->d_out[gs] + (size_t)i * g->out_stride;
-        G.hdr = reinterpret_cast<OutHeader*>(ob + offsetof(OutBlock, hdr)); G.obs = reinterpret_cast<gf_obs*>(ob + offsetof(OutBlock, obs));
-        G.status = ob + offsetof(OutBlock, status); G.in_box = reinterpret_cast<uint32_t*>(ob + offsetof(OutBlock, in_box));
-        G.fp.dt = times[i] - t->prev_time;
-        G.fp.has_pred = t->has_pred ? 1 : 0;
-        G.fp.depth_valid = (depth && depth[i]) ? 1 : 0;
-        put_boxes(G.fp.boxes, bx ? bx[i] : nullptr, nb ? nb[i] : 0);
+        OutBlock* ob = group_block(g->d_out[gs], g, i);
+        G.hdr = &ob->hdr; G.obs = ob->obs; G.status = ob->status; G.in_box = ob->in_box;
+        frame_params(&G.fp, t, times[i], depth && depth[i], bx[i], nb[i]);
         any_pred |= t->has_pred;
     }
-    const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     cudaStream_t s = g->s_up;
     GF_CUDA(cudaEventRecord(g->ev_t0[gs], s));
     GF_CUDA(cudaMemcpyAsync(g->d_tab[gs], g->h_tab[gs], (size_t)g->n * sizeof(GroupMember), cudaMemcpyHostToDevice, s));
-    for (int i = 0; i < g->n; i++) {
-        const gf_tracker* t = g->m[i];
-        const int es = (int)(t->n_submitted % 2);
-        if (g->equalize) GF_CUDA(cudaMemcpy2DAsync(t->d_raw, t->raw_pitch, gray[i], gray_pitch, w, h, kind, s));
-        else GF_CUDA(cudaMemcpy2DAsync(t->d_pyr[t->n_submitted % 3][0], t->lp[0], gray[i], gray_pitch, w, h, kind, s));
-        if (depth && depth[i])
-            GF_CUDA(cudaMemcpy2DAsync(t->d_depth[es], (size_t)t->depth_pitch_el * 2, depth[i], depth_pitch, (size_t)w * 2, h, kind, s));
-    }
+    for (int i = 0; i < g->n; i++)
+        if ((rc = enqueue_upload(s, g->m[i], gray[i], gray_pitch, depth ? depth[i] : nullptr, depth_pitch, on_device))) return rc;
     const bool direct = !g->use_graph;
     const int hp = any_pred ? 1 : 0;
-    int rc;
     if (g->equalize && (rc = run_piece(direct, s, &g->g_clahe[gs], &g->gk_clahe[gs], [&] { return group_body_clahe(g, gs); }))) return rc;
     GF_CUDA(cudaEventRecord(g->ev_up[gs], s));
     GF_CUDA(cudaStreamWaitEvent(g->s_pyr, g->ev_up[gs], 0));
@@ -1350,14 +1322,10 @@ static int group_submit(gf_tracker_group* g, const double* times, const void* co
     GF_CUDA(cudaStreamWaitEvent(g->s_out, g->ev_dep[gs], 0));
     GF_CUDA(cudaMemcpyAsync(g->h_out[gs], g->d_out[gs], (size_t)g->n * g->out_stride, cudaMemcpyDeviceToHost, g->s_out));
     GF_CUDA(cudaEventRecord(g->ev_out[gs], g->s_out));
-    for (int i = 0; i < g->n; i++) {          // the members' host-side state advances as enqueue_frame advances it
-        gf_tracker* t = g->m[i];
+    for (int i = 0; i < g->n; i++) {
         const bool dv = depth && depth[i];
-        t->prev_time = times[i];
-        t->has_pred = false;
-        t->depth_valid[t->n_submitted % 2] = dv;
-        t->n_submitted++;
-        t->group_steps++;
+        frame_enqueued(g->m[i], times[i], dv);
+        g->m[i]->group_steps++;
         g->depth_valid[gs][i] = dv ? 1 : 0;
     }
     g->n_submitted++;
@@ -1374,7 +1342,7 @@ int gf::tracker_last_out(const gf_tracker* t, TrackerOut* o)
         return set_err(GF_ERR_INVALID_ARG, "the frame the tracker last returned is no longer on the device: a later frame was submitted into its result slot");
     const int es = (int)(f % GF_PIPE);
     o->device = t->device;
-    o->n = (t->cfg.depth_cam && !t->depth_valid[es]) ? 0 : t->h_out[es]->hdr.n_out;   // as gf_tracker_wait_boxes
+    o->n = out_count(t, t->h_out[es], t->depth_valid[es]);
     o->obs = t->d_out[es]->obs; o->in_box = t->d_out[es]->in_box;
     o->downloaded = t->ev_out[es];
     return GF_OK;
@@ -1393,13 +1361,11 @@ int gf::tracker_group_last_out(const gf_tracker_group* g, int n, TrackerOut* o, 
         return set_err(GF_ERR_INVALID_ARG, "the step the tracker group last collected is no longer on the device: a later step was submitted into its slot");
     const int gs = (int)(s % 2);
     for (int i = 0; i < n; i++) {
-        const gf_tracker* t = g->m[i];
-        const uint8_t* hb = g->h_out[gs] + (size_t)i * g->out_stride;
-        uint8_t* db = g->d_out[gs] + (size_t)i * g->out_stride;
+        const OutBlock* db = group_block(g->d_out[gs], g, i);
         o[i].device = g->device;
-        o[i].n = (t->cfg.depth_cam && !g->depth_valid[gs][i]) ? 0 : reinterpret_cast<const OutHeader*>(hb + offsetof(OutBlock, hdr))->n_out;
-        o[i].obs = reinterpret_cast<const gf_obs*>(db + offsetof(OutBlock, obs));
-        o[i].in_box = reinterpret_cast<const uint32_t*>(db + offsetof(OutBlock, in_box));
+        o[i].n = out_count(g->m[i], group_block(g->h_out[gs], g, i), g->depth_valid[gs][i]);
+        o[i].obs = db->obs;
+        o[i].in_box = db->in_box;
         o[i].downloaded = g->ev_out[gs];
     }
     *downloaded = g->ev_out[gs];
@@ -1424,21 +1390,9 @@ static int group_collect(gf_tracker_group* g, gf_obs* out, size_t out_stride, in
         t->group_steps--;
         t->out_frame1 = 0;
         t->last_ms = ms;
-        const uint8_t* ob = g->h_out[gs] + (size_t)i * g->out_stride;
-        const OutHeader& hd = *reinterpret_cast<const OutHeader*>(ob + offsetof(OutBlock, hdr));
-        const uint32_t* bits = reinterpret_cast<const uint32_t*>(ob + offsetof(OutBlock, in_box));
-        int n = hd.n_out;
-        if (t->cfg.depth_cam && !g->depth_valid[gs][i]) n = 0;   // see body_dep2
         const size_t o = (size_t)i * out_stride, q = (size_t)i * n_stride;
-        if (n_out) n_out[q] = n;
-        if (out && n > 0) memcpy(out + o, ob + offsetof(OutBlock, obs), (size_t)n * sizeof(gf_obs));
-        if (in_box) for (int k = 0; k < n; k++) in_box[o + k] = (uint8_t)((bits[k >> 5] >> (k & 31)) & 1u);
-        if (status_out && hd.n_prev > 0) memcpy(status_out + o, ob + offsetof(OutBlock, status), hd.n_prev);
-        if (info) {
-            gf_track_info& r = info[q];
-            r.n_prev = hd.n_prev; r.n_tracked = hd.n_tracked; r.n_kept = hd.n_kept; r.n_new = hd.n_new;
-            r.n_candidates = hd.n_cand; r.nms_rounds = hd.nms_rounds; r.eig_fixups = hd.eig_fixups; r.lk_iterations = hd.lk_iters;
-        }
+        decode_out(t, group_block(g->h_out[gs], g, i), g->depth_valid[gs][i], out ? out + o : nullptr, n_out ? n_out + q : nullptr,
+                   in_box ? in_box + o : nullptr, status_out ? status_out + o : nullptr, info ? info + q : nullptr);
     }
     return GF_OK;
 }
@@ -1500,17 +1454,12 @@ int gf_tracker_group_submit(gf_tracker_group* g, const double* times, const void
                             const void* const* depth, size_t depth_pitch, int on_device, const gf_box* boxes, const int* box_start)
 {
     if (!g || !times || !gray) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    long long bad;
+    int rc = box_start ? check_box_lists(boxes, box_start, g->n, &bad) : GF_OK;
+    if (rc) return member_prefix(rc, (int)bad);
     std::vector<const gf_box*> bx((size_t)g->n, nullptr);
     std::vector<int> nb((size_t)g->n, 0);
-    if (box_start) {
-        for (int i = 0; i < g->n; i++) {
-            if (box_start[i] < 0) return member_err(GF_ERR_INVALID_ARG, i, "bad box offsets");
-            bx[i] = boxes ? boxes + box_start[i] : nullptr;
-            nb[i] = box_start[i + 1] - box_start[i];
-            int rc = check_boxes(bx[i], nb[i]);
-            if (rc) return member_prefix(rc, i);
-        }
-    }
+    for (int i = 0; box_start && i < g->n; i++) { bx[i] = boxes ? boxes + box_start[i] : nullptr; nb[i] = box_start[i + 1] - box_start[i]; }
     return group_submit(g, times, gray, gray_pitch, depth, depth_pitch, on_device != 0, bx.data(), nb.data());
 }
 
@@ -1527,22 +1476,18 @@ int gf_tracker_group_track_batch(gf_tracker_group* g, int n_steps, const double*
     if (!g || n_steps < 0 || (n_steps > 0 && (!times || !gray))) return set_err(GF_ERR_INVALID_ARG, "null argument");
     if (group_in_flight(g) > 0) return set_err(GF_ERR_INVALID_ARG, "a step in flight: call gf_tracker_group_wait first");
     const int K = g->n, n = n_steps;
-    for (int i = 0; i < K; i++)             // every frame pointer and box list is checked before the first step is submitted
-        for (int k = 0; k < n; k++) {
-            const size_t j = (size_t)i * n + k;
-            if (!gray[j]) return member_err(GF_ERR_INVALID_ARG, i, "null frame pointer");
-            if (box_start) {
-                if (box_start[j] < 0) return member_err(GF_ERR_INVALID_ARG, i, "bad box offsets");
-                int rc = check_boxes(boxes ? boxes + box_start[j] : nullptr, box_start[j + 1] - box_start[j]);
-                if (rc) return member_prefix(rc, i);
-            }
-        }
+    // every box list and frame pointer is checked before the first step is submitted
+    long long bad;
+    int rc = box_start ? check_box_lists(boxes, box_start, (long long)K * n, &bad) : GF_OK;
+    if (rc) return member_prefix(rc, (int)(bad / n));
+    for (long long j = 0; j < (long long)K * n; j++)
+        if (!gray[j]) return member_err(GF_ERR_INVALID_ARG, (int)(j / n), "null frame pointer");
     std::vector<double> ts((size_t)K);
     std::vector<const void*> gp((size_t)K), dp((size_t)K);
     std::vector<const gf_box*> bx((size_t)K, nullptr);
     std::vector<int> nb((size_t)K, 0);
     const size_t cap = (size_t)g->m[0]->cfg.max_cnt;
-    int collected = 0, rc;
+    int collected = 0;
     auto collect = [&]() {
         const size_t j = (size_t)collected++;
         return group_collect(g, out ? out + j * cap : nullptr, (size_t)n * cap, n_out ? n_out + j : nullptr, (size_t)n,

@@ -64,7 +64,7 @@ struct Pyramid {
 };
 
 
-// Where the frame a tracker last returned through gf_tracker_wait* lies on the device, for gf_fm_window_add_frame_from_tracker
+// Where the frame a tracker last returned through gf_tracker_wait lies on the device, for gf_fm_window_add_frame_from_tracker
 // (fe_tracker.cu): n observations, the in_box bits, and the event recorded after that frame's download.
 struct TrackerOut { int device, n; const gf_obs* obs; const uint32_t* in_box; cudaEvent_t downloaded; };
 int tracker_last_out(const gf_tracker* t, TrackerOut* o);

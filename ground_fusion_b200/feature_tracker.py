@@ -157,19 +157,30 @@ class FeatureTracker:
             return a
         return np.ascontiguousarray(a, dtype)
 
+    def _track(self, cur_time, img, depth, on_device=False, boxes=None):
+        """One blocking gf_tracker_track call: host frames are arrays, device frames integer addresses of tightly packed frames.
+        boxes: None for trackImage (returns obs), else an (m, 4) gf_box array for trackImagebox (returns (obs, in_box))."""
+        if on_device:
+            frame = (img, 0, depth, 0)
+        else:
+            img = self._rows(img, np.uint8)
+            assert img.shape == (self.height, self.width)
+            if depth is not None:
+                depth = self._rows(depth, np.uint16)
+            frame = (img.ctypes.data, img.strides[0], None if depth is None else depth.ctypes.data, 0 if depth is None else depth.strides[0])
+        nb = 0 if boxes is None else len(boxes)
+        in_box = None if boxes is None else np.zeros(self.max_cnt, np.uint8)
+        n, info = ctypes.c_int(0), TrackInfo()
+        check(self.L.gf_tracker_track(self._h, float(cur_time), *frame, int(bool(on_device)), boxes.ctypes.data if nb else None, nb,
+                                      self._obs.ctypes.data, ctypes.byref(n), None if in_box is None else in_box.ctypes.data,
+                                      self._status.ctypes.data, ctypes.byref(info)))
+        obs = self._collect(n, info)
+        return obs if in_box is None else (obs, in_box[:n.value].view(np.bool_))
+
     def trackImageRaw(self, cur_time, img, depth=None):
         """Returns the structured array of gf_obs in the tracker's internal (cur_pts) order.  Row-padded views are passed
         with their row pitch, as a cv::Mat with a larger step is in the reference."""
-        img = self._rows(img, np.uint8)
-        assert img.shape == (self.height, self.width)
-        dp, dpitch = None, 0
-        if depth is not None:
-            depth = self._rows(depth, np.uint16)
-            dp, dpitch = depth.ctypes.data, depth.strides[0]
-        n, info = ctypes.c_int(0), TrackInfo()
-        check(self.L.gf_tracker_track(self._h, float(cur_time), img.ctypes.data, img.strides[0], dp, dpitch,
-                                      self._obs.ctypes.data, ctypes.byref(n), self._status.ctypes.data, ctypes.byref(info)))
-        return self._collect(n, info)
+        return self._track(cur_time, img, depth)
 
     def trackImage(self, cur_time, img, depth=None):
         """map<int, vector<pair<int, Matrix<double,8,1>>>> as {id: v[8]} (camera id is always 0)."""
@@ -180,19 +191,7 @@ class FeatureTracker:
         """trackImagebox (feature_tracker.cpp:374-678): (obs, in_box).  obs is exactly what trackImageRaw returns for the frame;
         in_box[i] marks the features that trackImagebox leaves out of featureFrame because they lie strictly inside one of the
         boxes ((m, 4) xmin, ymin, xmax, ymax).  Those features stay in the tracker and are tracked on the next frame."""
-        img = self._rows(img, np.uint8)
-        assert img.shape == (self.height, self.width)
-        dp, dpitch = None, 0
-        if depth is not None:
-            depth = self._rows(depth, np.uint16)
-            dp, dpitch = depth.ctypes.data, depth.strides[0]
-        b = box_array(boxes)
-        n, info = ctypes.c_int(0), TrackInfo()
-        in_box = np.zeros(self.max_cnt, np.uint8)
-        check(self.L.gf_tracker_track_boxes(self._h, float(cur_time), img.ctypes.data, img.strides[0], dp, dpitch, 0,
-                                            b.ctypes.data if len(b) else None, len(b), self._obs.ctypes.data, ctypes.byref(n),
-                                            in_box.ctypes.data, self._status.ctypes.data, ctypes.byref(info)))
-        return self._collect(n, info), in_box[:n.value].view(np.bool_)
+        return self._track(cur_time, img, depth, boxes=box_array(boxes))
 
     def trackImagebox(self, cur_time, boxes, img, depth=None):
         """{id: v[8]} of trackImage without the features strictly inside a box (Estimator::inputImagebox's front end)."""
@@ -200,10 +199,7 @@ class FeatureTracker:
         return {int(o["id"]): o["v"].copy() for o in obs[~in_box]}
 
     def trackDevice(self, cur_time, d_gray_ptr, d_depth_ptr=None):
-        n, info = ctypes.c_int(0), TrackInfo()
-        check(self.L.gf_tracker_track_device(self._h, float(cur_time), d_gray_ptr, d_depth_ptr, self._obs.ctypes.data,
-                                             ctypes.byref(n), self._status.ctypes.data, ctypes.byref(info)))
-        return self._collect(n, info)
+        return self._track(cur_time, d_gray_ptr, d_depth_ptr, on_device=True)
 
     @staticmethod
     def _frame(img, dtype, shape):
@@ -218,87 +214,34 @@ class FeatureTracker:
         if depth is not None:
             depth = self._frame(depth, np.uint16, (self.height, self.width))
         dp, dpitch = (depth.ctypes.data, depth.strides[0]) if depth is not None else (None, 0)
-        check(self.L.gf_tracker_submit(self._h, float(cur_time), img.ctypes.data, img.strides[0], dp, dpitch))
+        check(self.L.gf_tracker_submit(self._h, float(cur_time), img.ctypes.data, img.strides[0], dp, dpitch, 0, None, 0))
 
     def trackBatch(self, times, gray_ptrs, depth_ptrs=None, on_device=False, gray_pitch=None, depth_pitch=None, want=True, boxes=None):
         """n consecutive trackImage calls in ONE library call (gf_tracker_track_batch: two frames in flight inside the
         library).  gray_ptrs / depth_ptrs: integer addresses of the frames (host, ideally pinned, or device).  Returns a
         list of (obs, status, info) per frame when `want`, else None (bench loops that only need the work done).
-        boxes: one (m, 4) box list per frame (empty: trackImage); the frames then go through trackImagebox
-        (gf_tracker_track_batch_boxes) and every result gains in_box: (obs, status, info, in_box)."""
-        if boxes is not None:
-            r = FeatureTracker.trackBatchMulti([self], [times], [gray_ptrs], None if depth_ptrs is None else [depth_ptrs], on_device,
-                                               gray_pitch, depth_pitch, want, boxes=[boxes])
-            return r[0] if want else None
-        n = len(times)
-        t = np.ascontiguousarray(times, np.float64)
-        g = (ctypes.c_void_p * n)(*[int(a) for a in gray_ptrs])
-        d = (ctypes.c_void_p * n)(*[(int(a) if a else None) for a in depth_ptrs]) if depth_ptrs is not None else None
-        obs = np.zeros((n, self.max_cnt), OBS_DTYPE) if want else None
-        st = np.zeros((n, self.max_cnt), np.uint8) if want else None
-        cnt = np.zeros(n, np.int32)
-        info = (TrackInfo * n)()
-        check(self.L.gf_tracker_track_batch(self._h, n, t.ctypes.data, g, int(gray_pitch or self.width), d,
-                                            int(depth_pitch or 2 * self.width), int(bool(on_device)),
-                                            obs.ctypes.data if want else None, cnt.ctypes.data, st.ctypes.data if want else None, info))
-        self.last_info = info[n - 1].as_dict() if n else {}
-        self.batch_infos = [info[k].as_dict() for k in range(n)]
-        if not want:
-            return None
-        return [(obs[k, :cnt[k]].copy(), st[k, :info[k].n_prev].copy(), info[k].as_dict()) for k in range(n)]
+        boxes: one (m, 4) box list per frame (empty: trackImage); the frames then go through trackImagebox and every result
+        gains in_box: (obs, status, info, in_box)."""
+        r = _track_streams(lambda *a: self.L.gf_tracker_track_batch(self._h, *a), [self], [times], [gray_ptrs],
+                           None if depth_ptrs is None else [depth_ptrs], on_device, gray_pitch, depth_pitch, want,
+                           None if boxes is None else [boxes])
+        return r[0] if want else None
 
     @staticmethod
     def trackBatchMulti(trackers, times, gray_ptrs, depth_ptrs=None, on_device=False, gray_pitch=None, depth_pitch=None, want=True, boxes=None):
         """gf_tracker_track_batch_multi: n frames on each of S independent trackers in one call, fed by one host thread.
         times / gray_ptrs / depth_ptrs: per tracker lists of n entries.  Returns per tracker what trackBatch returns.
-        boxes: per tracker lists of n box lists (gf_tracker_track_batch_multi_boxes; results gain in_box as in trackBatch)."""
-        S, n = len(trackers), len(times[0])
-        a = trackers[0]
-        assert all(len(x) == n for x in times) and all(tr.max_cnt == a.max_cnt and tr.width == a.width for tr in trackers)
-        t = np.ascontiguousarray(times, np.float64).reshape(S * n)
-        g = (ctypes.c_void_p * (S * n))(*[int(p) for row in gray_ptrs for p in row])
-        d = (ctypes.c_void_p * (S * n))(*[(int(p) if p else None) for row in depth_ptrs for p in row]) if depth_ptrs is not None else None
-        h = (ctypes.c_void_p * S)(*[tr._h for tr in trackers])
-        obs = np.zeros((S, n, a.max_cnt), OBS_DTYPE) if want else None
-        st = np.zeros((S, n, a.max_cnt), np.uint8) if want else None
-        cnt = np.zeros((S, n), np.int32)
-        info = (TrackInfo * (S * n))()
-        ib = None
-        if boxes is None:
-            check(a.L.gf_tracker_track_batch_multi(h, S, n, t.ctypes.data, g, int(gray_pitch or a.width), d, int(depth_pitch or 2 * a.width),
-                                                   int(bool(on_device)), obs.ctypes.data if want else None, cnt.ctypes.data,
-                                                   st.ctypes.data if want else None, info))
-        else:
-            assert len(boxes) == S and all(len(x) == n for x in boxes)
-            bx, start = _box_csr([b for row in boxes for b in row])
-            ib = np.zeros((S, n, a.max_cnt), np.uint8) if want else None
-            check(a.L.gf_tracker_track_batch_multi_boxes(h, S, n, t.ctypes.data, g, int(gray_pitch or a.width), d, int(depth_pitch or 2 * a.width),
-                                                         int(bool(on_device)), bx.ctypes.data if len(bx) else None, start.ctypes.data,
-                                                         obs.ctypes.data if want else None, cnt.ctypes.data, ib.ctypes.data if want else None,
-                                                         st.ctypes.data if want else None, info))
-        return FeatureTracker._results(trackers, n, obs, st, cnt, info, ib)
-
-    @staticmethod
-    def _results(trackers, n, obs, st, cnt, info, ib):
-        """Per tracker lists of n (obs, status, info[, in_box]) from the (S, n, max_cnt) result arrays of a multi-stream call;
-        updates every tracker's batch_infos / last_info."""
-        for i, tr in enumerate(trackers):
-            tr.batch_infos = [info[i * n + k].as_dict() for k in range(n)]
-            tr.last_info = tr.batch_infos[-1] if n else {}
-        if obs is None:
-            return None
-        if ib is not None:
-            return [[(obs[i, k, :cnt[i, k]].copy(), st[i, k, :info[i * n + k].n_prev].copy(), info[i * n + k].as_dict(),
-                      ib[i, k, :cnt[i, k]].view(np.bool_).copy()) for k in range(n)] for i in range(len(trackers))]
-        return [[(obs[i, k, :cnt[i, k]].copy(), st[i, k, :info[i * n + k].n_prev].copy(), info[i * n + k].as_dict()) for k in range(n)]
-                for i in range(len(trackers))]
+        boxes: per tracker lists of n box lists (results gain in_box as in trackBatch)."""
+        h = (ctypes.c_void_p * len(trackers))(*[tr._h for tr in trackers])
+        return _track_streams(lambda *a: trackers[0].L.gf_tracker_track_batch_multi(h, len(trackers), *a), trackers, times, gray_ptrs,
+                              depth_ptrs, on_device, gray_pitch, depth_pitch, want, boxes)
 
     def submitDevice(self, cur_time, d_gray_ptr, d_depth_ptr=None):
-        check(self.L.gf_tracker_submit_device(self._h, float(cur_time), d_gray_ptr, d_depth_ptr))
+        check(self.L.gf_tracker_submit(self._h, float(cur_time), d_gray_ptr, 0, d_depth_ptr, 0, 1, None, 0))
 
     def wait(self):
         n, info = ctypes.c_int(0), TrackInfo()
-        check(self.L.gf_tracker_wait(self._h, self._obs.ctypes.data, ctypes.byref(n), self._status.ctypes.data, ctypes.byref(info)))
+        check(self.L.gf_tracker_wait(self._h, self._obs.ctypes.data, ctypes.byref(n), None, self._status.ctypes.data, ctypes.byref(info)))
         return self._collect(n, info)
 
     def timer_start(self):
@@ -401,24 +344,37 @@ class TrackerGroup:
     def trackBatch(self, times, gray_ptrs, depth_ptrs=None, on_device=False, gray_pitch=None, depth_pitch=None, want=True, boxes=None):
         """n steps in one call (gf_tracker_group_track_batch, two steps in flight).  times / gray_ptrs / depth_ptrs / boxes: per
         member lists of n entries, and the return value, as FeatureTracker.trackBatchMulti on the members."""
-        S, n = len(self.members), len(times[0])
-        assert len(times) == S and all(len(x) == n for x in times)
-        w = self.members[0].width
-        t = np.ascontiguousarray(times, np.float64).reshape(S * n)
-        g = (ctypes.c_void_p * (S * n))(*[int(p) for row in gray_ptrs for p in row])
-        d = (ctypes.c_void_p * (S * n))(*[(int(p) if p else None) for row in depth_ptrs for p in row]) if depth_ptrs is not None else None
-        obs = np.zeros((S, n, self.max_cnt), OBS_DTYPE) if want else None
-        st = np.zeros((S, n, self.max_cnt), np.uint8) if want else None
-        cnt = np.zeros((S, n), np.int32)
-        info = (TrackInfo * (S * n))()
-        bx, start, ib = np.zeros((0, 4), np.int64), None, None
-        if boxes is not None:
-            assert len(boxes) == S and all(len(x) == n for x in boxes)
-            bx, start = _box_csr([b for row in boxes for b in row])
-            ib = np.zeros((S, n, self.max_cnt), np.uint8) if want else None
-        check(self.L.gf_tracker_group_track_batch(self._h, n, t.ctypes.data, g, int(gray_pitch or w), d, int(depth_pitch or 2 * w),
-                                                  int(bool(on_device)), bx.ctypes.data if len(bx) else None,
-                                                  start.ctypes.data if start is not None else None, obs.ctypes.data if want else None,
-                                                  cnt.ctypes.data, ib.ctypes.data if ib is not None else None,
-                                                  st.ctypes.data if want else None, info))
-        return FeatureTracker._results(self.members, n, obs, st, cnt, info, ib)
+        return _track_streams(lambda *a: self.L.gf_tracker_group_track_batch(self._h, *a), self.members, times, gray_ptrs, depth_ptrs,
+                              on_device, gray_pitch, depth_pitch, want, boxes)
+
+
+def _track_streams(call, trackers, times, gray_ptrs, depth_ptrs, on_device, gray_pitch, depth_pitch, want, boxes):
+    """n frames on each of the S streams `trackers` in one library call: call(n, times, gray, ...) takes the arguments of
+    gf_tracker_track_batch from n on, with stream i's frame k at i*n + k.  Returns per stream a list of n (obs, status, info)
+    (with boxes: (obs, status, info, in_box)) when `want`, else None; updates every tracker's batch_infos / last_info."""
+    S, n = len(trackers), len(times[0])
+    a = trackers[0]
+    assert len(times) == S and all(len(x) == n for x in times)
+    assert all(tr.max_cnt == a.max_cnt and tr.width == a.width for tr in trackers)
+    t = np.ascontiguousarray(times, np.float64).reshape(S * n)
+    g = (ctypes.c_void_p * (S * n))(*[int(p) for row in gray_ptrs for p in row])
+    d = (ctypes.c_void_p * (S * n))(*[(int(p) if p else None) for row in depth_ptrs for p in row]) if depth_ptrs is not None else None
+    obs = np.zeros((S, n, a.max_cnt), OBS_DTYPE) if want else None
+    st = np.zeros((S, n, a.max_cnt), np.uint8) if want else None
+    cnt = np.zeros((S, n), np.int32)
+    info = (TrackInfo * (S * n))()
+    bx, start, ib = np.zeros((0, 4), np.int64), None, None
+    if boxes is not None:
+        assert len(boxes) == S and all(len(x) == n for x in boxes)
+        bx, start = _box_csr([b for row in boxes for b in row])
+        ib = np.zeros((S, n, a.max_cnt), np.uint8) if want else None
+    check(call(n, t.ctypes.data, g, int(gray_pitch or a.width), d, int(depth_pitch or 2 * a.width), int(bool(on_device)),
+               bx.ctypes.data if len(bx) else None, None if start is None else start.ctypes.data, None if obs is None else obs.ctypes.data,
+               cnt.ctypes.data, None if ib is None else ib.ctypes.data, None if st is None else st.ctypes.data, info))
+    for i, tr in enumerate(trackers):
+        tr.batch_infos = [info[i * n + k].as_dict() for k in range(n)]
+        tr.last_info = tr.batch_infos[-1] if n else {}
+    if obs is None:
+        return None
+    return [[(obs[i, k, :cnt[i, k]].copy(), st[i, k, :info[i * n + k].n_prev].copy(), info[i * n + k].as_dict())
+             + (() if ib is None else (ib[i, k, :cnt[i, k]].view(np.bool_).copy(),)) for k in range(n)] for i in range(S)]

@@ -75,101 +75,84 @@ typedef struct gf_track_info {
 int gf_tracker_create(gf_tracker** out, int device, int width, int height, const gf_tracker_cfg* cfg);
 void gf_tracker_destroy(gf_tracker* t);
 
-/* Pinned host staging buffers owned by the tracker (width*height u8, width*height u16).  A caller
- * that renders/decodes straight into them avoids one host memcpy; any other pointer is also accepted
- * by gf_tracker_track and is copied into these buffers first. */
+/* Pinned host staging buffers owned by the tracker (width*height u8, width*height u16).  A caller that renders/decodes
+ * straight into them and submits them gets truly asynchronous uploads; any other host pointer is also accepted (see
+ * gf_tracker_submit). */
 int gf_tracker_host_buffers(gf_tracker* t, uint8_t** gray, uint16_t** depth);
-
-/* FeatureTracker::trackImage(t, img, depth) (feature_tracker.cpp:103-372).
- *   gray: H x W u8, row pitch gray_pitch bytes; only read during the call (as cv::Mat in the reference)
- *   depth: H x W u16 millimetres or NULL (then v[7] = -2.4 as feature_tracker.cpp:338)
- *   out: caller-allocated, capacity >= cfg.max_cnt; entries are in the tracker's internal order
- *        (the reference's std::map iterates by id: sort by id on the caller side if needed)
- *   status_out (nullable, capacity >= max_cnt): combined status of the n_prev points that entered LK
- *        (LK status & reverse check & inBorder & grey<=250), i.e. the reference's `status` vector at
- *        feature_tracker.cpp:170 */
-int gf_tracker_track(gf_tracker* t, double time, const uint8_t* gray, size_t gray_pitch,
-                     const uint16_t* depth, size_t depth_pitch, gf_obs* out, int* n_out,
-                     uint8_t* status_out, gf_track_info* info);
-
-/* Asynchronous split of gf_tracker_track.  _submit enqueues the copies and kernels of one frame and returns;
- * _wait blocks for the result of the OLDEST frame not yet collected.  Up to two frames may be in flight
- * (submit t, submit t+1, wait t, submit t+2, wait t+1, ...): the upload, pyramid and min-eig map of frame t+1 then
- * overlap the tracking of frame t, which is how a recorded sequence (rosbag replay) or a camera with one frame of
- * buffering is processed at the rate of the dependent chain alone.  Results are identical to the blocking call.
- * Pinned caller buffers passed to _submit must stay unchanged until that frame has been collected.
- * gf_tracker_set_prediction / gf_tracker_remove_ids act on the state after the last collected frame and are
- * therefore only accepted with no frame in flight, exactly as the reference calls them between trackImage calls. */
-int gf_tracker_submit(gf_tracker* t, double time, const uint8_t* gray, size_t gray_pitch,
-                      const uint16_t* depth, size_t depth_pitch);
-int gf_tracker_wait(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* status_out, gf_track_info* info);
-
-/* Device-resident variant used by bench.py's kernel-only `value`: the frame is already in HBM
- * (device pointers, tightly packed W x H), nothing is copied from the host. */
-int gf_tracker_track_device(gf_tracker* t, double time, const void* d_gray, const void* d_depth,
-                            gf_obs* out, int* n_out, uint8_t* status_out, gf_track_info* info);
-/* Asynchronous form of gf_tracker_track_device (collect with gf_tracker_wait; same two-frame rule as _submit). */
-int gf_tracker_submit_device(gf_tracker* t, double time, const void* d_gray, const void* d_depth);
-
-/* A recorded run of n consecutive frames (rosbag replay, one call per batch): the same submit / wait pipeline as above,
- * two frames in flight, driven from inside the library so that the host costs one call per batch instead of ~10 driver
- * calls per frame.  Frame k = (times[k], gray[k], depth[k] or NULL / depth == NULL); on_device != 0: the pointers are
- * device pointers to tightly packed frames (pitches ignored), else host pointers with the given row pitches (pinned
- * buffers make the uploads asynchronous).  Results of frame k land at out + k*max_cnt, n_out[k],
- * status_out + k*max_cnt, info[k] (each nullable).  Identical to n calls of gf_tracker_track. */
-int gf_tracker_track_batch(gf_tracker* t, int n, const double* times, const void* const* gray, size_t gray_pitch,
-                           const void* const* depth, size_t depth_pitch, int on_device,
-                           gf_obs* out, int* n_out, uint8_t* status_out, gf_track_info* info);
-/* The same for several independent camera streams at once (a multi-camera rig, several robots served by one GPU): stream i
- * is trackers[i] with frames times / gray / depth [i*n + k] and results at out + (i*n + k)*max_cnt, n_out / info [i*n + k],
- * status_out + (i*n + k)*max_cnt.  One host thread feeds all streams round-robin (frame k of every stream is enqueued before
- * frame k-1 of any stream is collected), so a server does not need one thread per camera: measured on one H100 SXM at 700 W,
- * 8 streams reach 26.6-27.0 k frames/s this way and 20.6-26.9 k with 8 threads calling gf_tracker_track_batch.  Results are identical to calling
- * gf_tracker_track_batch per stream. */
-int gf_tracker_track_batch_multi(gf_tracker* const* trackers, int n_trackers, int n, const double* times, const void* const* gray,
-                                 size_t gray_pitch, const void* const* depth, size_t depth_pitch, int on_device,
-                                 gf_obs* out, int* n_out, uint8_t* status_out, gf_track_info* info);
-
-/* The config key `equalize` (parameters.h:33): cv::createCLAHE(clip_limit, Size(tiles_x, tiles_y))->apply on every gray frame
- * before it is tracked, as getImageFromMsg does (rosNodeTest.cpp:256-261; the reference's call is createCLAHE() with its
- * defaults, clip_limit 40 and an 8 x 8 grid).  LK on both pyramids, goodFeaturesToTrack and the grey > 250 test then all see
- * the equalised image, bit-exact with OpenCV 4.13.  Off by default; tiles_x = 0 turns it off.  1 <= tiles_x, tiles_y <= 16;
- * clip_limit <= 0: no clipping.  Accepted only before the first frame is submitted (GF_ERR_INVALID_ARG afterwards).
- * Covers every intake path: _track / _submit, _track_device / _submit_device and the batch calls. */
-int gf_tracker_set_equalize(gf_tracker* t, double clip_limit, int tiles_x, int tiles_y);
 
 /* The config key `use_yolo` (parameters.cpp:159): FeatureTracker::trackImagebox (feature_tracker.cpp:374-678), which
  * Estimator::inputImagebox (estimator.cpp:244-273) calls on every frame whose detection message has the frame's timestamp.  It is
  * trackImage with one difference: a feature strictly inside a detected box, pointPolygonTest(contour of the box, pt, true) > 0, is
  * left out of featureFrame.  It stays in the tracker (cur_pts / ids / track_cnt / velocity history): it is tracked on the next
  * frame and counts against max_cnt.  The boxes are the fields of darknet_ros_msgs/BoundingBox; the reference copies them into
- * `int`, and so does the library (a modular wrap of values outside int32).
- *   _submit_boxes: gf_tracker_submit / gf_tracker_submit_device (on_device != 0: tightly packed device frames, pitches ignored)
- *       with the frame's n_boxes boxes.  n_boxes == 0 is trackImage.  n_boxes > GF_MAX_BOXES (darknet_ros publishes at most 100,
- *       YoloObjectDetector.cpp:559): GF_ERR_CAPACITY; n_boxes < 0 or boxes == NULL with n_boxes > 0: GF_ERR_INVALID_ARG; in both
- *       cases no frame is consumed.  The boxes are copied before the call returns.
- *   _wait_boxes: gf_tracker_wait plus in_box (nullable, capacity >= max_cnt): in_box[i] = 1 for the entries of out that
- *       trackImagebox leaves out of featureFrame, 0 otherwise (all 0 for a frame submitted without boxes).  out / n_out /
- *       status_out / info are exactly what trackImage returns for the frame.  Collects any frame.
- *   _track_batch_boxes / _track_batch_multi_boxes: the batch calls with per-frame boxes: frame j (j = i*n + k for stream i) has
- *       boxes[box_start[j] .. box_start[j + 1]) (box_start: n + 1, resp. n_trackers*n + 1 offsets; NULL: no boxes) and its flags at
- *       in_box + j*max_cnt.  Every list is checked before the first frame is submitted.
- * The box test runs on the device, inside the last kernel of the frame; the other entry points run the same kernels without boxes. */
+ * `int`, and so does the library (a modular wrap of values outside int32).  darknet_ros publishes at most GF_MAX_BOXES boxes
+ * per frame (YoloObjectDetector.cpp:559). */
 #define GF_MAX_BOXES 100
 typedef struct gf_box { int64_t xmin, ymin, xmax, ymax; } gf_box;
-int gf_tracker_submit_boxes(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch,
-                            int on_device, const gf_box* boxes, int n_boxes);
-int gf_tracker_wait_boxes(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info);
-/* Blocking form of _submit_boxes + _wait_boxes, the call trackImagebox makes (no frame may be in flight, as for gf_tracker_track). */
-int gf_tracker_track_boxes(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch, int on_device,
-                           const gf_box* boxes, int n_boxes, gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info);
-int gf_tracker_track_batch_boxes(gf_tracker* t, int n, const double* times, const void* const* gray, size_t gray_pitch,
-                                 const void* const* depth, size_t depth_pitch, int on_device, const gf_box* boxes, const int* box_start,
-                                 gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info);
-int gf_tracker_track_batch_multi_boxes(gf_tracker* const* trackers, int n_trackers, int n, const double* times, const void* const* gray,
-                                       size_t gray_pitch, const void* const* depth, size_t depth_pitch, int on_device,
-                                       const gf_box* boxes, const int* box_start, gf_obs* out, int* n_out, uint8_t* in_box,
-                                       uint8_t* status_out, gf_track_info* info);
+
+/* FeatureTracker::trackImage(t, img, depth) (feature_tracker.cpp:103-372), and trackImagebox(t, img, depth, boxes) when
+ * n_boxes > 0.  Blocking: gf_tracker_submit followed by gf_tracker_wait; no frame may be in flight.
+ *   gray: H x W u8; depth: H x W u16 millimetres or NULL (then v[7] = -2.4 as feature_tracker.cpp:338).  on_device == 0: host
+ *        pointers with row pitches gray_pitch / depth_pitch bytes, only read during the call (as cv::Mat in the reference).
+ *        on_device != 0: device pointers to tightly packed frames already in HBM, nothing is copied from the host (the pitches
+ *        are ignored); bench.py's kernel-only `value` runs this way.
+ *   boxes: the frame's n_boxes detections; boxes == NULL, n_boxes == 0 is trackImage.  n_boxes > GF_MAX_BOXES: GF_ERR_CAPACITY;
+ *        n_boxes < 0 or boxes == NULL with n_boxes > 0: GF_ERR_INVALID_ARG; in both cases no frame is consumed.
+ *   out: caller-allocated, capacity >= cfg.max_cnt; entries are in the tracker's internal order
+ *        (the reference's std::map iterates by id: sort by id on the caller side if needed)
+ *   in_box (nullable, capacity >= max_cnt): in_box[i] = 1 for the entries of out that trackImagebox leaves out of featureFrame,
+ *        0 otherwise (all 0 for a frame without boxes).  out / n_out / status_out / info are exactly what trackImage returns.
+ *   status_out (nullable, capacity >= max_cnt): combined status of the n_prev points that entered LK
+ *        (LK status & reverse check & inBorder & grey<=250), i.e. the reference's `status` vector at
+ *        feature_tracker.cpp:170
+ * The box test runs on the device, inside the last kernel of the frame; without boxes the same kernels run. */
+int gf_tracker_track(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch,
+                     int on_device, const gf_box* boxes, int n_boxes, gf_obs* out, int* n_out, uint8_t* in_box,
+                     uint8_t* status_out, gf_track_info* info);
+
+/* Asynchronous split of gf_tracker_track, with its arguments.  _submit enqueues the copies and kernels of one frame and
+ * returns (the boxes are copied before it returns); _wait blocks for the result of the OLDEST frame not yet collected, whatever
+ * intake it came through.  Up to two frames may be in flight (submit t, submit t+1, wait t, submit t+2, wait t+1, ...): the
+ * upload, pyramid and min-eig map of frame t+1 then overlap the tracking of frame t, which is how a recorded sequence (rosbag
+ * replay) or a camera with one frame of buffering is processed at the rate of the dependent chain alone.  Results are
+ * identical to the blocking call.  _submit reads host frames with the copy engine after it returns: truly asynchronous from
+ * pinned memory (gf_tracker_host_buffers, cudaHostAlloc, cudaHostRegister), which must stay unchanged until that frame has
+ * been collected; pageable memory is staged by CUDA before the call returns.
+ * gf_tracker_set_prediction / gf_tracker_remove_ids act on the state after the last collected frame and are
+ * therefore only accepted with no frame in flight, exactly as the reference calls them between trackImage calls. */
+int gf_tracker_submit(gf_tracker* t, double time, const void* gray, size_t gray_pitch, const void* depth, size_t depth_pitch,
+                      int on_device, const gf_box* boxes, int n_boxes);
+int gf_tracker_wait(gf_tracker* t, gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info);
+
+/* A recorded run of n consecutive frames (rosbag replay, one call per batch): the same submit / wait pipeline as above,
+ * two frames in flight, driven from inside the library so that the host costs one call per batch instead of ~10 driver
+ * calls per frame.  Frame k = (times[k], gray[k], depth[k] or NULL / depth == NULL), on_device and the pitches as for
+ * gf_tracker_track (pinned host buffers make the uploads asynchronous); its boxes are boxes[box_start[k] .. box_start[k + 1])
+ * (n + 1 offsets; box_start NULL: no boxes).  Every box list is checked before the first frame is submitted.  Results of
+ * frame k land at out + k*max_cnt, n_out[k], in_box + k*max_cnt, status_out + k*max_cnt, info[k] (each nullable).
+ * Identical to n calls of gf_tracker_track. */
+int gf_tracker_track_batch(gf_tracker* t, int n, const double* times, const void* const* gray, size_t gray_pitch,
+                           const void* const* depth, size_t depth_pitch, int on_device, const gf_box* boxes, const int* box_start,
+                           gf_obs* out, int* n_out, uint8_t* in_box, uint8_t* status_out, gf_track_info* info);
+/* The same for several independent camera streams at once (a multi-camera rig, several robots served by one GPU): stream i
+ * is trackers[i] with frame j = i*n + k at times / gray / depth [j], boxes[box_start[j] .. box_start[j + 1]) (n_trackers*n + 1
+ * offsets) and results at out + j*max_cnt, n_out[j], in_box + j*max_cnt, status_out + j*max_cnt, info[j].  One host thread
+ * feeds all streams round-robin (frame k of every stream is enqueued before frame k-1 of any stream is collected), so a server
+ * does not need one thread per camera: measured on one H100 SXM at 700 W, 8 streams reach 26.6-27.0 k frames/s this way and
+ * 20.6-26.9 k with 8 threads calling gf_tracker_track_batch.  Results are identical to calling gf_tracker_track_batch per
+ * stream. */
+int gf_tracker_track_batch_multi(gf_tracker* const* trackers, int n_trackers, int n, const double* times, const void* const* gray,
+                                 size_t gray_pitch, const void* const* depth, size_t depth_pitch, int on_device,
+                                 const gf_box* boxes, const int* box_start, gf_obs* out, int* n_out, uint8_t* in_box,
+                                 uint8_t* status_out, gf_track_info* info);
+
+/* The config key `equalize` (parameters.h:33): cv::createCLAHE(clip_limit, Size(tiles_x, tiles_y))->apply on every gray frame
+ * before it is tracked, as getImageFromMsg does (rosNodeTest.cpp:256-261; the reference's call is createCLAHE() with its
+ * defaults, clip_limit 40 and an 8 x 8 grid).  LK on both pyramids, goodFeaturesToTrack and the grey > 250 test then all see
+ * the equalised image, bit-exact with OpenCV 4.13.  Off by default; tiles_x = 0 turns it off.  1 <= tiles_x, tiles_y <= 16;
+ * clip_limit <= 0: no clipping.  Accepted only before the first frame is submitted (GF_ERR_INVALID_ARG afterwards).
+ * Covers every intake path: host and device frames, _track / _submit and the batch calls. */
+int gf_tracker_set_equalize(gf_tracker* t, double clip_limit, int tiles_x, int tiles_y);
 
 /* A tracker group: n existing trackers (members) that track frame k of their streams in lockstep, one step at a time, with
  * ONE set of launches per step: every kernel of the frame runs once for the whole group (member = a grid dimension), so the
@@ -189,13 +172,13 @@ int gf_tracker_track_batch_multi_boxes(gf_tracker* const* trackers, int n_tracke
  *   _destroy: the members stay usable (a step still in flight is completed and dropped).  Destroying a member that belongs to
  *       a live group is a caller error.
  *   _submit: one step, two steps in flight at most (as gf_tracker_submit): member i tracks times[i], gray[i], depth[i] (depth
- *       nullable, and NULL entries: no depth image); on_device and the pitches as gf_tracker_submit_boxes; boxes / box_start:
+ *       nullable, and NULL entries: no depth image); on_device and the pitches as gf_tracker_submit; boxes / box_start:
  *       member i's detections are boxes[box_start[i] .. box_start[i + 1]) (n + 1 offsets; box_start NULL: no boxes).  Every
  *       member's pointers and box list are checked before anything is enqueued: an argument error consumes no frame.
  *   _wait: collects the oldest step: member i's results at out + i*max_cnt, n_out[i], in_box + i*max_cnt,
- *       status_out + i*max_cnt, info[i] (each nullable), as gf_tracker_wait_boxes returns them.
+ *       status_out + i*max_cnt, info[i] (each nullable), as gf_tracker_wait returns them.
  *   _track_batch: n_steps steps in one call, two in flight, with the arguments and layout of
- *       gf_tracker_track_batch_multi_boxes (member i = stream i: frame k at [i*n_steps + k]).
+ *       gf_tracker_track_batch_multi (member i = stream i: frame k at [i*n_steps + k]).
  * gf_tracker_last_device_ms of a member reports the device time of the last collected step. */
 typedef struct gf_tracker_group gf_tracker_group;
 #define GF_TRACKER_GROUP_MAX 64
@@ -243,7 +226,7 @@ int gf_stage_pyr_down(int device, const uint8_t* src, int w, int h, uint8_t* dst
  * src rows are src_pitch bytes apart; dst is w x h, tightly packed.  Same limits as the tracker's image and tile grid. */
 int gf_stage_clahe(int device, const uint8_t* src, size_t src_pitch, int w, int h, double clip_limit, int tiles_x, int tiles_y,
                    uint8_t* dst);
-/* trackImagebox's box test on its own (the device function of gf_tracker_submit_boxes): in_box[i] = 1 when point i
+/* trackImagebox's box test on its own (the device function of gf_tracker_submit with boxes): in_box[i] = 1 when point i
  * (pts: n x,y float pairs) lies strictly inside one of the n_boxes boxes, as pointPolygonTest(contour, pt, true) > 0 decides. */
 int gf_stage_in_boxes(int device, const float* pts, int n, const gf_box* boxes, int n_boxes, uint8_t* in_box);
 /* cv::cornerMinEigenVal(img, blockSize=3, ksize=3) as used by goodFeaturesToTrack. */
@@ -622,7 +605,7 @@ int gf_fm_window_clear(gf_fm_window* w);
  * WINDOW_SIZE added a second time without a slide in between) is GF_ERR_INVALID_ARG; the reference's list would grow. */
 int gf_fm_window_add_frame(gf_fm_window* w, int frame_count, const gf_obs* obs, int n, const uint8_t* in_box, double td, int* margin_old,
                            int32_t* counters4, double* last_average_parallax);
-/* The same with the frame `tracker` last returned through gf_tracker_wait* / gf_tracker_track*, read where the tracker left it
+/* The same with the frame `tracker` last returned through gf_tracker_wait (or a call built on it), read where the tracker left it
  * on the device (its observations and its in_box flags), ordered after the tracker's download of that frame.  The tracker is
  * only read.  With the pipelined calls the tracker has two result slots: the returned frame k stays on the device while frame
  * k + 1 is in flight (submit k + 1, wait k, add_frame_from_tracker is fine), and is gone once frame k + 2 has been submitted.
@@ -826,7 +809,7 @@ int gf_grid_map_stats(gf_grid_map* map, int64_t* out4);
  * darknet's inference forward pass for the networks the reference ships (vins_estimator/yolo_network_config/cfg: [net],
  * [convolutional], [maxpool], [route], [reorg], [shortcut], [upsample], [region], [yolo]; activations leaky and linear),
  * bit-exact with darknet's CPU build, followed by the node's decoding (get_network_boxes with hier 0.5, do_nms_obj 0.4) and box
- * extraction.  The boxes feed gf_tracker_*_boxes / trackImagebox.
+ * extraction.  The boxes feed the tracker's boxes argument (trackImagebox).
  * The detector is implemented in its own library, libgf_yolo.so, built next to libgf_b200.so: libgf_b200.so exports these
  * entry points as forwarders that open it on the first call, so it carries none of the detector's device code and a process
  * that never detects never loads it.  A failing call sets gf_last_error() as usual; gf_detector_last_error() is the same

@@ -149,20 +149,20 @@ def test_boxes_change_in_box_only(gf):
 def _submit_boxes(tr, t, g, d, boxes):
     from ground_fusion_b200._lib import check
     bx = np.ascontiguousarray(boxes, np.int64).reshape(-1, 4)
-    check(tr.L.gf_tracker_submit_boxes(tr._h, float(t), g.ctypes.data, g.strides[0], d.ctypes.data if d is not None else None,
-                                       d.strides[0] if d is not None else 0, 0, bx.ctypes.data if len(bx) else None, len(bx)))
+    check(tr.L.gf_tracker_submit(tr._h, float(t), g.ctypes.data, g.strides[0], d.ctypes.data if d is not None else None,
+                                 d.strides[0] if d is not None else 0, 0, bx.ctypes.data if len(bx) else None, len(bx)))
 
 
 def _wait_boxes(tr):
     from ground_fusion_b200._lib import TrackInfo, check
     n, info, ib = ctypes.c_int(0), TrackInfo(), np.zeros(tr.max_cnt, np.uint8)
-    check(tr.L.gf_tracker_wait_boxes(tr._h, tr._obs.ctypes.data, ctypes.byref(n), ib.ctypes.data, tr._status.ctypes.data, ctypes.byref(info)))
+    check(tr.L.gf_tracker_wait(tr._h, tr._obs.ctypes.data, ctypes.byref(n), ib.ctypes.data, tr._status.ctypes.data, ctypes.byref(info)))
     return tr._collect(n, info), ib[:n.value].view(np.bool_)
 
 
 def test_two_frames_in_flight(gf):
-    """submit_boxes t+1 before wait_boxes t: the parameter block with the boxes rotates with the frame; frames with and without
-    depth and with and without boxes interleave, and gf_tracker_wait collects a boxed frame as trackImage's result."""
+    """submit t+1 with boxes before wait t: the parameter block with the boxes rotates with the frame; frames with and without
+    depth and with and without boxes interleave, and gf_tracker_wait without in_box collects a boxed frame as trackImage's result."""
     frames = dynamic_frames(9, 640, 480, 17)
     frames = [(t, np.ascontiguousarray(g), (np.ascontiguousarray(d) if k % 5 != 2 else None), b) for k, (t, g, d, b) in enumerate(frames)]
     want = _oracle(frames, 640)
@@ -278,7 +278,7 @@ def test_argument_errors_consume_no_frame(gf):
         tr.trackImageboxRaw(t, np.zeros((101, 4), np.int64), g, d)
     for nb, ptr in ((-1, None), (3, None)):
         with pytest.raises(GfError, match="-1"):
-            check(tr.L.gf_tracker_submit_boxes(tr._h, t, g.ctypes.data, 640, d.ctypes.data, 1280, 0, ptr, nb))
+            check(tr.L.gf_tracker_submit(tr._h, t, g.ctypes.data, 640, d.ctypes.data, 1280, 0, ptr, nb))
     bad = [b, np.zeros((101, 4), np.int64)]
     with pytest.raises(GfError, match="-4"):
         tr.trackBatch([f[0] for f in frames[:2]], [f[1].ctypes.data for f in frames[:2]], [f[2].ctypes.data for f in frames[:2]], boxes=bad)

@@ -98,6 +98,22 @@ def test_obs_struct_layout():
     assert ctypes.sizeof(Obs) == 72 and OBS_DTYPE.fields["v"][1] == 8
 
 
+def test_ctypes_argtypes_match_header_arity():
+    """Every function _lib.lib() declares argtypes for takes as many arguments as its prototype in include/gf_b200.h: ctypes
+    passes a call with the wrong count without complaint, and the C side then reads garbage."""
+    from ground_fusion_b200 import _lib
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "gf_b200.h")).read(), flags=re.S)
+    arity = {}
+    for name, params in re.findall(r"\b(gf_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", src):
+        params = params.strip()
+        arity[name] = 0 if params in ("", "void") else params.count(",") + 1
+    declared = {n: f.argtypes for n, f in vars(_lib.lib()).items() if isinstance(f, ctypes._CFuncPtr) and f.argtypes is not None}
+    assert len(declared) >= 50 and "gf_tracker_track" in declared
+    for name, argtypes in sorted(declared.items()):
+        assert name in arity, "%s has argtypes but no prototype in gf_b200.h" % name
+        assert len(argtypes) == arity[name], (name, len(argtypes), arity[name])
+
+
 def test_double2vector_matches_numpy_restatement():
     """Estimator::double2vector (estimator.cpp:2440-2494): host-only entry point of the library against oracle/ba_glue.py,
     including the Euler-singularity branch (pitch within 1 degree of +-90)."""

@@ -6,7 +6,7 @@ alternately in one process, frames resident in HBM (value) and in pinned host me
 gives medians and ranges in frames/s summed over the K cameras, and the device time of one step (CUDA events from its first copy
 to its result copy: the latency each camera sees, which for a lockstep group ends with its slowest member).  Also in the same run:
   host_us_per_frame: host time inside the submit calls, K = 8, frames in HBM (a host clock around each call, ctypes included;
-      ctypes_call_us is the cost of an empty call for comparison), for gf_tracker_submit_device as gf_tracker_track_batch_multi
+      ctypes_call_us is the cost of an empty call for comparison), for gf_tracker_submit of a device frame as gf_tracker_track_batch_multi
       issues it and for gf_tracker_group_submit divided by K;
   kernels_k8: per-kernel device times of one K = 8 run of each path (torch.profiler);
   gpu: the card's name and power limit.
@@ -90,7 +90,7 @@ def host_cost(ring, wl, K=8, frames=400):
         for i, t in enumerate(rig.tr):
             j = bench.tri(rig.k[i] + k, ring.n)
             t0 = time.perf_counter_ns()
-            _lib.check(L.gf_tracker_submit_device(t._h, (rig.k[i] + k) / 30.0, g[j], d[j]))
+            _lib.check(L.gf_tracker_submit(t._h, (rig.k[i] + k) / 30.0, g[j], 0, d[j], 0, 1, None, 0))
             ns_multi += time.perf_counter_ns() - t0
         if k >= 1:
             for t in rig.tr:
