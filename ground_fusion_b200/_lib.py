@@ -29,6 +29,7 @@ class DenseMapCfg(ctypes.Structure):
 
 
 DENSE_MAP_CLOUD, DENSE_MAP_FILTERED = 0, 1      # gf_dense_map_read's `which`
+MAP_GROUP_MAX = 64                              # GF_DENSE_MAP_GROUP_MAX = GF_GRID_MAP_GROUP_MAX
 
 
 class GridMapCfg(ctypes.Structure):
@@ -131,6 +132,17 @@ def lib():
         L.gf_grid_map_read.argtypes = [vp, i, vp]
         L.gf_grid_map_size.argtypes = [vp] + [ctypes.POINTER(i)] * 4
         L.gf_grid_map_stats.argtypes = [vp, vp]
+        L.gf_dense_map_group_create.argtypes = [ctypes.POINTER(vp), vp, i]
+        L.gf_dense_map_group_destroy.argtypes = [vp]
+        L.gf_dense_map_group_destroy.restype = None
+        L.gf_dense_map_group_size.argtypes = [vp, ctypes.POINTER(i)]
+        L.gf_dense_map_group_add_keyframes.argtypes = [vp, vp, i, vp, vp, vp, vp, vp, vp, i, vp, vp]
+        L.gf_grid_map_group_create.argtypes = [ctypes.POINTER(vp), vp, i]
+        L.gf_grid_map_group_destroy.argtypes = [vp]
+        L.gf_grid_map_group_destroy.restype = None
+        L.gf_grid_map_group_size.argtypes = [vp, ctypes.POINTER(i)]
+        L.gf_grid_map_group_add_keyframes.argtypes = [vp, vp, i, vp, vp, vp, vp, vp, i, vp]
+        L.gf_grid_map_group_add_dense_keyframes.argtypes = [vp, vp, vp, i, vp, vp, vp]
         ip, dp = ctypes.POINTER(i), ctypes.POINTER(d)
         L.gf_fm_window_create.argtypes = [ctypes.POINTER(vp), i, ctypes.POINTER(FmWindowCfg)]
         L.gf_fm_window_destroy.argtypes = [vp]

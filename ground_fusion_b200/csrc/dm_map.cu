@@ -86,13 +86,12 @@ __device__ __forceinline__ uint32_t hinsert(uint64_t* keys, uint32_t mask, uint6
     }
 }
 
-// one thread per sample: lift, depth / colour tests, local point, world point, z band, voxel key
-__global__ void k_dm_sample(CamParams cam, int su, int n, int B, int D, const uint8_t* __restrict__ rgb, size_t rgb_pitch,
-                            const uint16_t* __restrict__ depth, size_t depth_pitch, Ext e, Pose T, Anchor A, uint64_t* __restrict__ key,
-                            uint32_t* __restrict__ idx, float* __restrict__ loc, uchar4* __restrict__ col, float* __restrict__ wxyz, int* bad)
+// sample s: lift, depth / colour tests, local point, world point, z band, voxel key
+__device__ __forceinline__ void dm_sample(int s, const CamParams& cam, int su, int B, int D, const uint8_t* __restrict__ rgb, size_t rgb_pitch,
+                                          const uint16_t* __restrict__ depth, size_t depth_pitch, const Ext& e, const Pose& T, const Anchor& A,
+                                          uint64_t* __restrict__ key, uint32_t* __restrict__ idx, float* __restrict__ loc, uchar4* __restrict__ col,
+                                          float* __restrict__ wxyz, int* bad)
 {
-    const int s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= n) return;
     idx[s] = s;
     key[s] = INVALID;
     const int u = B + (s % su) * D, v = B + (s / su) * D;
@@ -113,6 +112,15 @@ __global__ void k_dm_sample(CamParams cam, int su, int n, int B, int D, const ui
     col[s] = make_uchar4(r, g, b, 0);
     key[s] = dm_voxel_key(A, f, bad);
 }
+// one thread per sample
+__global__ void k_dm_sample(CamParams cam, int su, int n, int B, int D, const uint8_t* __restrict__ rgb, size_t rgb_pitch,
+                            const uint16_t* __restrict__ depth, size_t depth_pitch, Ext e, Pose T, Anchor A, uint64_t* __restrict__ key,
+                            uint32_t* __restrict__ idx, float* __restrict__ loc, uchar4* __restrict__ col, float* __restrict__ wxyz, int* bad)
+{
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    dm_sample(s, cam, su, B, D, rgb, rgb_pitch, depth, depth_pitch, e, T, A, key, idx, loc, col, wxyz, bad);
+}
 
 // one thread per kept keyframe point: its world point under the keyframe's current pose (updatePath: no z band)
 __global__ void k_dm_rebuild_xform(int n, const float* __restrict__ kf_xyz, const int* __restrict__ kf_id, const Pose* __restrict__ poses, Ext e,
@@ -131,11 +139,10 @@ __global__ void k_dm_rebuild_xform(int n, const float* __restrict__ kf_xyz, cons
 // Over the (key, index) pairs sorted stably by key: the first thread of each voxel's run reads the voxel's count c and accepts
 // the run's j-th point iff c + j < cap -- the sequential rule, since the run lists the voxel's points in input order.
 // add[i] = the number accepted (at the run's first position, 0 elsewhere).
-__global__ void k_dm_gate(int n, const uint64_t* __restrict__ skey, const uint32_t* __restrict__ sidx, const uint64_t* __restrict__ vkeys,
-                          const int* __restrict__ vcnt, uint32_t vmask, int cap, int* __restrict__ flag, int* __restrict__ add)
+__device__ __forceinline__ void dm_gate_run(int i, int n, const uint64_t* __restrict__ skey, const uint32_t* __restrict__ sidx,
+                                            const uint64_t* __restrict__ vkeys, const int* __restrict__ vcnt, uint32_t vmask, int cap,
+                                            int* __restrict__ flag, int* __restrict__ add)
 {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
     const uint64_t k = skey[i];
     add[i] = 0;
     if (k == INVALID) { flag[sidx[i]] = 0; return; }
@@ -150,28 +157,42 @@ __global__ void k_dm_gate(int n, const uint64_t* __restrict__ skey, const uint32
     }
     add[i] = a;
 }
+__global__ void k_dm_gate(int n, const uint64_t* __restrict__ skey, const uint32_t* __restrict__ sidx, const uint64_t* __restrict__ vkeys,
+                          const int* __restrict__ vcnt, uint32_t vmask, int cap, int* __restrict__ flag, int* __restrict__ add)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    dm_gate_run(i, n, skey, sidx, vkeys, vcnt, vmask, cap, flag, add);
+}
 __global__ void k_dm_hash_add(int n, const uint64_t* __restrict__ skey, const int* __restrict__ add, uint64_t* vkeys, int* vcnt, uint32_t vmask)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n || add[i] == 0) return;
     atomicAdd(&vcnt[hinsert(vkeys, vmask, skey[i])], add[i]);
 }
-// stable compaction of the accepted points: cloud at c0 (+ the keyframe's kept local points at k0 when loc != nullptr)
+// point i, accepted at position p of the compaction: cloud at c0 (+ the keyframe's kept local points at k0 when loc != nullptr)
+__device__ __forceinline__ void dm_scatter_one(int i, int p, const float* __restrict__ wxyz, const uchar4* __restrict__ col, float* __restrict__ cxyz,
+                                               uchar4* __restrict__ ccol, int c0, const float* __restrict__ loc, float* __restrict__ kxyz,
+                                               uchar4* __restrict__ kcol, int* __restrict__ kid, int k0, int kf)
+{
+    const size_t c = (size_t)c0 + p;
+    for (int k = 0; k < 3; k++) cxyz[3 * c + k] = wxyz[3 * (size_t)i + k];
+    ccol[c] = col[i];
+    if (loc) {
+        const size_t q = (size_t)k0 + p;
+        for (int k = 0; k < 3; k++) kxyz[3 * q + k] = loc[3 * (size_t)i + k];
+        kcol[q] = col[i];
+        kid[q] = kf;
+    }
+}
+// stable compaction of the accepted points
 __global__ void k_dm_scatter(int n, const int* __restrict__ flag, const int* __restrict__ pos, const float* __restrict__ wxyz, const uchar4* __restrict__ col,
                              float* __restrict__ cxyz, uchar4* __restrict__ ccol, int c0, const float* __restrict__ loc, float* __restrict__ kxyz,
                              uchar4* __restrict__ kcol, int* __restrict__ kid, int k0, int kf)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n || !flag[i]) return;
-    const size_t c = (size_t)c0 + pos[i];
-    for (int k = 0; k < 3; k++) cxyz[3 * c + k] = wxyz[3 * (size_t)i + k];
-    ccol[c] = col[i];
-    if (loc) {
-        const size_t q = (size_t)k0 + pos[i];
-        for (int k = 0; k < 3; k++) kxyz[3 * q + k] = loc[3 * (size_t)i + k];
-        kcol[q] = col[i];
-        kid[q] = kf;
-    }
+    dm_scatter_one(i, pos[i], wxyz, col, cxyz, ccol, c0, loc, kxyz, kcol, kid, k0, kf);
 }
 
 // ---- radius filter over a cell index: cells of side >= radius (slightly larger, so that rounding of the cell coordinate
@@ -213,20 +234,14 @@ __global__ void k_dm_mark_dirty(int n, int from, const float* __restrict__ xyz, 
 // returns more than min_pts points, itself and duplicates included; FLANN's L2_Simple distance ((dx*dx) + dy*dy) + dz*dz in
 // float, compared strictly with float(radius^2).  A kept point stays kept (its count can only grow until the next rebuild), so
 // only points not yet kept whose stencil touches a dirty cell are counted.
-__global__ void k_dm_count(int n, const float* __restrict__ xyz, double inv_cell, const uint64_t* __restrict__ hkeys, const int2* __restrict__ hrange,
-                           const uint8_t* __restrict__ dirty, uint32_t hmask, const float4* __restrict__ sxyz, float r2, int min_pts, uint8_t* __restrict__ kept)
+// the count of a query point over its 27-cell stencil (slots: each cell's hash slot, -1 when empty): 1 / 0 = kept or not,
+// -1 when no cell of the stencil is dirty (the point cannot have gained a neighbour)
+__device__ __forceinline__ int dm_stencil_count(float qx, float qy, float qz, const int* slots, const int2* __restrict__ hrange,
+                                                const uint8_t* __restrict__ dirty, const float4* __restrict__ sxyz, float r2, int min_pts)
 {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n || kept[i]) return;
-    const float qx = xyz[3 * (size_t)i], qy = xyz[3 * (size_t)i + 1], qz = xyz[3 * (size_t)i + 2];
-    const int cx = cell_of(qx, inv_cell), cy = cell_of(qy, inv_cell), cz = cell_of(qz, inv_cell);
-    int slots[27];
     bool any = false;
-    for (int t = 0; t < 27; t++) {
-        slots[t] = hfind(hkeys, hmask, cell_key(cx + t % 3 - 1, cy + (t / 3) % 3 - 1, cz + t / 9 - 1));
-        if (slots[t] >= 0 && dirty[slots[t]]) any = true;
-    }
-    if (!any) return;
+    for (int t = 0; t < 27; t++) if (slots[t] >= 0 && dirty[slots[t]]) any = true;
+    if (!any) return -1;
     int cnt = 0;
     for (int t = 0; t < 27 && cnt <= min_pts; t++) {
         if (slots[t] < 0) continue;
@@ -238,7 +253,19 @@ __global__ void k_dm_count(int n, const float* __restrict__ xyz, double inv_cell
             if (dist < r2 && ++cnt > min_pts) break;
         }
     }
-    kept[i] = cnt > min_pts;
+    return cnt > min_pts;
+}
+__global__ void k_dm_count(int n, const float* __restrict__ xyz, double inv_cell, const uint64_t* __restrict__ hkeys, const int2* __restrict__ hrange,
+                           const uint8_t* __restrict__ dirty, uint32_t hmask, const float4* __restrict__ sxyz, float r2, int min_pts, uint8_t* __restrict__ kept)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || kept[i]) return;
+    const float qx = xyz[3 * (size_t)i], qy = xyz[3 * (size_t)i + 1], qz = xyz[3 * (size_t)i + 2];
+    const int cx = cell_of(qx, inv_cell), cy = cell_of(qy, inv_cell), cz = cell_of(qz, inv_cell);
+    int slots[27];
+    for (int t = 0; t < 27; t++) slots[t] = hfind(hkeys, hmask, cell_key(cx + t % 3 - 1, cy + (t / 3) % 3 - 1, cz + t / 9 - 1));
+    const int r = dm_stencil_count(qx, qy, qz, slots, hrange, dirty, sxyz, r2, min_pts);
+    if (r >= 0) kept[i] = r;
 }
 
 // scratch of the radius filter over up to cap points
@@ -326,6 +353,7 @@ struct gf_dense_map {
     uint32_t vmask = 0;
     // host state
     int n_cloud = 0, n_filtered = 0, n_kf_points = 0;
+    bool nf_stale = false;                           // a group call filtered the cloud: n_filtered is in nsel on the device
     std::vector<Pose> poses;                         // pose each keyframe was last inserted with
     std::vector<int> kf_off{0};                      // keyframe k's kept points are [kf_off[k], kf_off[k+1])
     // device
@@ -389,6 +417,18 @@ static int dm_filter(gf_dense_map* m, int from)
     if (rc) return rc;
     GF_CUDA(cudaMemcpyAsync(&m->n_filtered, m->nsel, 4, cudaMemcpyDeviceToHost, m->st));
     GF_CUDA(cudaStreamSynchronize(m->st));
+    m->nf_stale = false;
+    return GF_OK;
+}
+
+// n_filtered after a group call, read on the map's stream (which waits for the group's work)
+static int dm_fetch_n_filtered(gf_dense_map* m)
+{
+    if (!m->nf_stale) return GF_OK;
+    GF_CUDA(cudaSetDevice(m->device));
+    GF_CUDA(cudaMemcpyAsync(&m->n_filtered, m->nsel, 4, cudaMemcpyDeviceToHost, m->st));
+    GF_CUDA(cudaStreamSynchronize(m->st));
+    m->nf_stale = false;
     return GF_OK;
 }
 
@@ -544,6 +584,8 @@ int gf_dense_map_update_poses(gf_dense_map* m, int n_keyframes, const double* R,
 int gf_dense_map_size(gf_dense_map* m, int* n_cloud, int* n_filtered, int* n_keyframes)
 {
     if (!m) return set_err(GF_ERR_INVALID_ARG, "bad argument");
+    int rc = dm_fetch_n_filtered(m);
+    if (rc) return rc;
     if (n_cloud) *n_cloud = m->n_cloud;
     if (n_filtered) *n_filtered = m->n_filtered;
     if (n_keyframes) *n_keyframes = (int)m->poses.size();
@@ -553,6 +595,8 @@ int gf_dense_map_size(gf_dense_map* m, int* n_cloud, int* n_filtered, int* n_key
 int gf_dense_map_read(gf_dense_map* m, int which, float* xyz, uint8_t* rgb, int32_t* idx)
 {
     if (!m || (which != GF_DENSE_MAP_CLOUD && which != GF_DENSE_MAP_FILTERED)) return set_err(GF_ERR_INVALID_ARG, "bad argument");
+    int rc = dm_fetch_n_filtered(m);
+    if (rc) return rc;
     GF_CUDA(cudaSetDevice(m->device));
     const int n = m->n_cloud;
     std::vector<float> cx(3 * (size_t)n);
@@ -622,3 +666,450 @@ int gf_stage_radius_filter(int device, const float* xyz, int n, double radius, i
 }
 
 }  // extern "C"
+
+// ---- gf_dense_map_group: one keyframe for each of several maps with one launch chain ----
+// Gate: every member has the same ns samples, so the samples of a call form equal segments; a segmented sort orders each
+// member's (voxel key, sample) pairs as the single map's sort does (the 63-bit voxel key leaves no bits for a member index).
+// Filter: the cloud points lie inside the octree's box (|coordinate| < 15000 m, < 2^18 filter cells), so a cell key of 3 x 19
+// bits leaves the top bits for the member, and one device-wide sort keeps every member's cells apart.
+namespace gfdm {
+
+constexpr int GROUP_MAX = 64;
+constexpr int GCELL_OFF = 1 << 18;
+
+struct DmMember {                                     // one member of a group call
+    CamParams cam; Ext ext; Pose T; Anchor A;
+    const uint8_t* rgb; const uint16_t* depth; size_t rgb_pitch, depth_pitch;
+    uint64_t* vkeys; int* vcnt; uint32_t vmask;
+    float *cxyz, *kxyz; uchar4 *ccol, *kcol; int* kid;
+    int c0, k0, kf;
+};
+struct DmFilt {                                       // one member of the group's radius filter: points [from, n) are new
+    const float* xyz; uint8_t* kept; int* fidx; int* nsel;
+    int n, from;
+};
+
+// the segment a of bases[0..F] (increasing, bases[0] = 0) holding i
+__device__ __forceinline__ int dm_seg(const int* __restrict__ base, int F, int i)
+{
+    int lo = 0, hi = F;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (base[mid] <= i) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+__device__ __forceinline__ uint64_t gcell_key(int a, int cx, int cy, int cz)
+{
+    return ((uint64_t)a << 57) | ((uint64_t)(unsigned)(cx + GCELL_OFF) << 38) | ((uint64_t)(unsigned)(cy + GCELL_OFF) << 19) | (uint64_t)(unsigned)(cz + GCELL_OFF);
+}
+
+// grid (samples, members): member a's samples are [a n, (a + 1) n) of every scratch array
+__global__ void k_dmg_sample(const DmMember* __restrict__ mb, int su, int n, int B, int D, uint64_t* __restrict__ key, uint32_t* __restrict__ idx,
+                             float* __restrict__ loc, uchar4* __restrict__ col, float* __restrict__ wxyz, int* bad)
+{
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    const DmMember& M = mb[blockIdx.y];
+    const size_t o = (size_t)blockIdx.y * n;
+    dm_sample(s, M.cam, su, B, D, M.rgb, M.rgb_pitch, M.depth, M.depth_pitch, M.ext, M.T, M.A, key + o, idx + o, loc + 3 * o, col + o, wxyz + 3 * o,
+              bad + blockIdx.y);
+}
+__global__ void k_dmg_gate(const DmMember* __restrict__ mb, int n, const uint64_t* __restrict__ skey, const uint32_t* __restrict__ sidx, int cap,
+                           int* __restrict__ flag, int* __restrict__ add)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const DmMember& M = mb[blockIdx.y];
+    const size_t o = (size_t)blockIdx.y * n;
+    dm_gate_run(i, n, skey + o, sidx + o, M.vkeys, M.vcnt, M.vmask, cap, flag + o, add + o);
+}
+// res[2 a] = member a's accepted points, res[2 a + 1] = its out-of-box flag
+__global__ void k_dmg_counts(int A, int n, const int* __restrict__ flag, const int* __restrict__ pos, const int* __restrict__ bad, int* __restrict__ res)
+{
+    const int a = threadIdx.x;
+    if (a >= A) return;
+    const size_t o = (size_t)a * n;
+    res[2 * a] = pos[o + n - 1] - pos[o] + flag[o + n - 1];
+    res[2 * a + 1] = bad[a];
+}
+// commit of the members whose bit is set in ok
+__global__ void k_dmg_hash_add(const DmMember* __restrict__ mb, int n, uint64_t ok, const uint64_t* __restrict__ skey, const int* __restrict__ add)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || !((ok >> blockIdx.y) & 1)) return;
+    const size_t o = (size_t)blockIdx.y * n;
+    if (add[o + i] == 0) return;
+    const DmMember& M = mb[blockIdx.y];
+    atomicAdd(&M.vcnt[hinsert(M.vkeys, M.vmask, skey[o + i])], add[o + i]);
+}
+__global__ void k_dmg_scatter(const DmMember* __restrict__ mb, int n, uint64_t ok, const int* __restrict__ flag, const int* __restrict__ pos,
+                              const float* __restrict__ wxyz, const uchar4* __restrict__ col, const float* __restrict__ loc)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || !((ok >> blockIdx.y) & 1)) return;
+    const size_t o = (size_t)blockIdx.y * n;
+    if (!flag[o + i]) return;
+    const DmMember& M = mb[blockIdx.y];
+    dm_scatter_one(i, pos[o + i] - pos[o], wxyz + 3 * o, col + o, M.cxyz, M.ccol, M.c0, loc + 3 * o, M.kxyz, M.kcol, M.kid, M.k0, M.kf);
+}
+
+// the radius filter over the clouds of F members, concatenated: member a's points are [fb[a], fb[a + 1]), its new ones
+// [nb[a], nb[a + 1]) of the new points' concatenation
+__global__ void k_dmg_cell_keys(int N, const DmFilt* __restrict__ f, const int* __restrict__ fb, int F, double inv_cell, uint64_t* __restrict__ key,
+                                uint32_t* __restrict__ idx)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    const int a = dm_seg(fb, F, i);
+    const float* x = f[a].xyz + 3 * (size_t)(i - fb[a]);
+    key[i] = gcell_key(a, cell_of(x[0], inv_cell), cell_of(x[1], inv_cell), cell_of(x[2], inv_cell));
+    idx[i] = i;
+}
+__global__ void k_dmg_cell_build(int N, const uint64_t* __restrict__ skey, const uint32_t* __restrict__ sidx, const DmFilt* __restrict__ f,
+                                 const int* __restrict__ fb, int F, uint64_t* hkeys, int2* hrange, uint32_t hmask, float4* __restrict__ sxyz)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    const int p = sidx[i], a = dm_seg(fb, F, p);
+    const float* x = f[a].xyz + 3 * (size_t)(p - fb[a]);
+    sxyz[i] = make_float4(x[0], x[1], x[2], 0.f);
+    const uint64_t k = skey[i];
+    if (i == 0 || skey[i - 1] != k) hrange[hinsert(hkeys, hmask, k)].x = i;
+    if (i == N - 1 || skey[i + 1] != k) hrange[hinsert(hkeys, hmask, k)].y = i + 1;
+}
+// a new point: not kept yet, and its cell is dirty
+__global__ void k_dmg_mark_dirty(int Nn, const DmFilt* __restrict__ f, const int* __restrict__ nb, int F, double inv_cell,
+                                 const uint64_t* __restrict__ hkeys, uint32_t hmask, uint8_t* __restrict__ dirty)
+{
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= Nn) return;
+    const int a = dm_seg(nb, F, t);
+    const size_t l = (size_t)f[a].from + (t - nb[a]);
+    f[a].kept[l] = 0;
+    const float* x = f[a].xyz + 3 * l;
+    dirty[hfind(hkeys, hmask, gcell_key(a, cell_of(x[0], inv_cell), cell_of(x[1], inv_cell), cell_of(x[2], inv_cell)))] = 1;
+}
+__global__ void k_dmg_count(int N, const DmFilt* __restrict__ f, const int* __restrict__ fb, int F, double inv_cell, const uint64_t* __restrict__ hkeys,
+                            const int2* __restrict__ hrange, const uint8_t* __restrict__ dirty, uint32_t hmask, const float4* __restrict__ sxyz, float r2,
+                            int min_pts)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    const int a = dm_seg(fb, F, i);
+    const size_t l = (size_t)(i - fb[a]);
+    uint8_t* kept = f[a].kept;
+    if (kept[l]) return;
+    const float* x = f[a].xyz + 3 * l;
+    const float qx = x[0], qy = x[1], qz = x[2];
+    const int cx = cell_of(qx, inv_cell), cy = cell_of(qy, inv_cell), cz = cell_of(qz, inv_cell);
+    int slots[27];
+    for (int t = 0; t < 27; t++) slots[t] = hfind(hkeys, hmask, gcell_key(a, cx + t % 3 - 1, cy + (t / 3) % 3 - 1, cz + t / 9 - 1));
+    const int r = dm_stencil_count(qx, qy, qz, slots, hrange, dirty, sxyz, r2, min_pts);
+    if (r >= 0) kept[l] = r;
+}
+__global__ void k_dmg_flags(int N, const DmFilt* __restrict__ f, const int* __restrict__ fb, int F, int* __restrict__ flg)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    const int a = dm_seg(fb, F, i);
+    flg[i] = f[a].kept[i - fb[a]];
+}
+// each member's kept indices in order, and their number
+__global__ void k_dmg_select(int N, const DmFilt* __restrict__ f, const int* __restrict__ fb, int F, const int* __restrict__ flg, const int* __restrict__ pos)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    const int a = dm_seg(fb, F, i), p0 = pos[fb[a]];
+    if (flg[i]) f[a].fidx[pos[i] - p0] = i - fb[a];
+    if (i == fb[a + 1] - 1) *f[a].nsel = pos[i] + flg[i] - p0;
+}
+
+}  // namespace gfdm
+
+struct DmCall {                                       // a call's descriptors, uploaded to the device
+    DmMember mb[GROUP_MAX];
+    DmFilt fl[GROUP_MAX];
+    int fb[GROUP_MAX + 1], nb[GROUP_MAX + 1];
+};
+
+struct gf_dense_map_group {
+    int device = 0, n = 0, ns = 0, gcap = 0, fcap = 0;
+    std::vector<gf_dense_map*> m;
+    cudaStream_t st = nullptr;
+    cudaEvent_t ev = nullptr;                         // orders the members' streams and the group's
+    DmCall* h = nullptr;                              // host copy of the descriptors (pageable: reusable once its upload returns)
+    DmCall* d = nullptr;
+    // gate scratch, n * ns entries
+    uint64_t *key = nullptr, *skey = nullptr;
+    uint32_t *idx = nullptr, *sidx = nullptr;
+    int *flag = nullptr, *pos = nullptr, *add = nullptr, *bad = nullptr, *res = nullptr, *seg = nullptr;
+    float *loc = nullptr, *wxyz = nullptr;
+    uchar4* col = nullptr;
+    // filter scratch over the members' capacities together
+    uint64_t *fkey = nullptr, *fskey = nullptr, *hkeys = nullptr;
+    uint32_t *fidx = nullptr, *fsidx = nullptr, hmask = 0;
+    int *flg = nullptr, *fpos = nullptr;
+    int2* hrange = nullptr;
+    uint8_t* dirty = nullptr;
+    float4* sxyz = nullptr;
+    void* tmp = nullptr; size_t tmp_bytes = 0;
+    int* h_res = nullptr;                             // pinned: accepted, out-of-box flag per member
+};
+
+static int dm_member_err(int rc, int k)
+{
+    char keep[sizeof(g_err)];
+    memcpy(keep, g_err, sizeof(keep));
+    snprintf(g_err, sizeof(g_err), "member %d: %s", k, keep);
+    return rc;
+}
+
+static void dmg_free(gf_dense_map_group* g)
+{
+    for (void* p : {(void*)g->d, (void*)g->key, (void*)g->skey, (void*)g->idx, (void*)g->sidx, (void*)g->flag, (void*)g->pos, (void*)g->add, (void*)g->bad,
+                    (void*)g->res, (void*)g->seg, (void*)g->loc, (void*)g->wxyz, (void*)g->col, (void*)g->fkey, (void*)g->fskey, (void*)g->hkeys,
+                    (void*)g->fidx, (void*)g->fsidx, (void*)g->flg, (void*)g->fpos, (void*)g->hrange, (void*)g->dirty, (void*)g->sxyz, g->tmp})
+        if (p) cudaFree(p);
+    if (g->h_res) cudaFreeHost(g->h_res);
+    if (g->ev) cudaEventDestroy(g->ev);
+    if (g->st) cudaStreamDestroy(g->st);
+    delete g->h;
+    delete g;
+}
+
+// the group's filter over the members listed in g->h->fl[0, F), fb / nb filled; N points, Nn of them new
+static int dmg_filter(gf_dense_map_group* g, int F, int N, int Nn)
+{
+    const double inv_cell = 1.0 / (RADIUS * (65.0 / 64.0));
+    const float r2 = (float)(RADIUS * RADIUS);
+    const DmFilt* fl = g->d->fl;
+    const int *fb = g->d->fb, *nb = g->d->nb;
+    uint32_t hm = 63;
+    while (hm < g->hmask && (size_t)hm + 1 < 2 * (size_t)N) hm = (hm << 1) | 1;
+    const int blocks = (N + 255) / 256;
+    k_dmg_cell_keys<<<blocks, 256, 0, g->st>>>(N, fl, fb, F, inv_cell, g->fkey, g->fidx);
+    GF_LAUNCHED();
+    size_t b = g->tmp_bytes;
+    GF_CUDA(cub::DeviceRadixSort::SortPairs(g->tmp, b, g->fkey, g->fskey, g->fidx, g->fsidx, N, 0, 63, g->st));
+    GF_CUDA(cudaMemsetAsync(g->hkeys, 0xff, 8 * ((size_t)hm + 1), g->st));
+    GF_CUDA(cudaMemsetAsync(g->dirty, 0, (size_t)hm + 1, g->st));
+    k_dmg_cell_build<<<blocks, 256, 0, g->st>>>(N, g->fskey, g->fsidx, fl, fb, F, g->hkeys, g->hrange, hm, g->sxyz);
+    GF_LAUNCHED();
+    k_dmg_mark_dirty<<<(Nn + 255) / 256, 256, 0, g->st>>>(Nn, fl, nb, F, inv_cell, g->hkeys, hm, g->dirty);
+    GF_LAUNCHED();
+    k_dmg_count<<<(N + 127) / 128, 128, 0, g->st>>>(N, fl, fb, F, inv_cell, g->hkeys, g->hrange, g->dirty, hm, g->sxyz, r2, MIN_PTS);
+    GF_LAUNCHED();
+    k_dmg_flags<<<blocks, 256, 0, g->st>>>(N, fl, fb, F, g->flg);
+    GF_LAUNCHED();
+    b = g->tmp_bytes;
+    GF_CUDA(cub::DeviceScan::ExclusiveSum(g->tmp, b, g->flg, g->fpos, N, g->st));
+    k_dmg_select<<<blocks, 256, 0, g->st>>>(N, fl, fb, F, g->flg, g->fpos);
+    GF_LAUNCHED();
+    return GF_OK;
+}
+
+extern "C" {
+
+int gf_dense_map_group_create(gf_dense_map_group** out, gf_dense_map* const* maps, int n)
+{
+    if (!out || !maps) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    *out = nullptr;
+    if (n < 1) return set_err(GF_ERR_INVALID_ARG, "a group has at least one map");
+    if (n > GROUP_MAX) return set_err(GF_ERR_INVALID_ARG, "a group has at most GF_DENSE_MAP_GROUP_MAX (64) maps");
+    long long fcap = 0;
+    for (int k = 0; k < n; k++) {
+        if (!maps[k]) return dm_member_err(set_err(GF_ERR_INVALID_ARG, "null map"), k);
+        for (int j = 0; j < k; j++) if (maps[j] == maps[k]) return dm_member_err(set_err(GF_ERR_INVALID_ARG, "the map is listed twice"), k);
+        const gf_dense_map_cfg &a = maps[0]->cfg, &c = maps[k]->cfg;
+        if (maps[k]->device != maps[0]->device) return dm_member_err(set_err(GF_ERR_INVALID_ARG, "bound to another device than member 0"), k);
+        if (c.width != a.width || c.height != a.height || c.depth_dist != a.depth_dist || c.depth_boundary != a.depth_boundary)
+            return dm_member_err(set_err(GF_ERR_INVALID_ARG, "width, height, depth_dist or depth_boundary differ from member 0's"), k);
+        fcap += c.max_points;
+    }
+    if (fcap > (1ll << 30)) return set_err(GF_ERR_CAPACITY, "the members' max_points add up to more than 2^30");
+    GF_CUDA(cudaSetDevice(maps[0]->device));
+    gf_dense_map_group* g = new gf_dense_map_group();
+    g->device = maps[0]->device; g->n = n; g->ns = maps[0]->ns;
+    g->m.assign(maps, maps + n);
+    g->h = new DmCall();
+    g->gcap = n * g->ns;
+    g->fcap = (int)fcap;
+    const size_t G = (size_t)g->gcap, C = (size_t)g->fcap;
+    uint32_t hc = 64;
+    while (hc < 2u * (uint32_t)C) hc <<= 1;
+    g->hmask = hc - 1;
+#define DMG_ALLOC(p, bytes) do { if (cudaMalloc(&(p), (bytes)) != cudaSuccess) { cudaGetLastError(); dmg_free(g); return set_err(GF_ERR_CUDA, "cudaMalloc failed (dense map group)"); } } while (0)
+    if (cudaStreamCreateWithFlags(&g->st, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&g->ev, cudaEventDisableTiming) != cudaSuccess) {
+        cudaGetLastError(); dmg_free(g); return set_err(GF_ERR_CUDA, "stream creation failed");
+    }
+    DMG_ALLOC(g->d, sizeof(DmCall));
+    DMG_ALLOC(g->key, 8 * G); DMG_ALLOC(g->skey, 8 * G); DMG_ALLOC(g->idx, 4 * G); DMG_ALLOC(g->sidx, 4 * G);
+    DMG_ALLOC(g->flag, 4 * G); DMG_ALLOC(g->pos, 4 * G); DMG_ALLOC(g->add, 4 * G);
+    DMG_ALLOC(g->loc, 12 * G); DMG_ALLOC(g->wxyz, 12 * G); DMG_ALLOC(g->col, 4 * G);
+    DMG_ALLOC(g->bad, 4 * GROUP_MAX); DMG_ALLOC(g->res, 8 * GROUP_MAX); DMG_ALLOC(g->seg, 4 * (GROUP_MAX + 1));
+    DMG_ALLOC(g->fkey, 8 * C); DMG_ALLOC(g->fskey, 8 * C); DMG_ALLOC(g->fidx, 4 * C); DMG_ALLOC(g->fsidx, 4 * C);
+    DMG_ALLOC(g->flg, 4 * C); DMG_ALLOC(g->fpos, 4 * C); DMG_ALLOC(g->sxyz, 16 * C);
+    DMG_ALLOC(g->hkeys, 8 * (size_t)hc); DMG_ALLOC(g->hrange, 8 * (size_t)hc); DMG_ALLOC(g->dirty, hc);
+#undef DMG_ALLOC
+    size_t b[4] = {0, 0, 0, 0};
+    if (cub::DeviceSegmentedRadixSort::SortPairs(nullptr, b[0], g->key, g->skey, g->idx, g->sidx, g->gcap, n, g->seg, g->seg + 1, 0, 64) != cudaSuccess ||
+        cub::DeviceScan::ExclusiveSum(nullptr, b[1], g->flag, g->pos, g->gcap) != cudaSuccess ||
+        cub::DeviceRadixSort::SortPairs(nullptr, b[2], g->fkey, g->fskey, g->fidx, g->fsidx, g->fcap, 0, 63) != cudaSuccess ||
+        cub::DeviceScan::ExclusiveSum(nullptr, b[3], g->flg, g->fpos, g->fcap) != cudaSuccess) {
+        dmg_free(g); return set_err(GF_ERR_CUDA, "cub sizing failed");
+    }
+    g->tmp_bytes = *std::max_element(b, b + 4);
+    std::vector<int> seg(GROUP_MAX + 1);
+    for (int a = 0; a <= GROUP_MAX; a++) seg[a] = a * g->ns;
+    if (cudaMalloc(&g->tmp, g->tmp_bytes) != cudaSuccess || cudaMallocHost(&g->h_res, 8 * GROUP_MAX) != cudaSuccess ||
+        cudaMemcpy(g->seg, seg.data(), 4 * seg.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
+        cudaGetLastError(); dmg_free(g); return set_err(GF_ERR_CUDA, "allocation failed (dense map group)");
+    }
+    *out = g;
+    return GF_OK;
+}
+
+void gf_dense_map_group_destroy(gf_dense_map_group* g)
+{
+    if (!g) return;
+    cudaSetDevice(g->device);
+    cudaStreamSynchronize(g->st);
+    dmg_free(g);
+}
+
+int gf_dense_map_group_size(gf_dense_map_group* g, int* n)
+{
+    if (!g || !n) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    *n = g->n;
+    return GF_OK;
+}
+
+int gf_dense_map_group_add_keyframes(gf_dense_map_group* g, const int32_t* members, int m, const double* R, const double* P,
+                                     const uint8_t* const* rgb, const size_t* rgb_pitch, const uint16_t* const* depth, const size_t* depth_pitch,
+                                     int on_device, int32_t* n_inserted, int32_t* status)
+{
+    if (!g || !members || !R || !P || !rgb || !rgb_pitch || !depth || !depth_pitch) return set_err(GF_ERR_INVALID_ARG, "null argument");
+    if (m < 1 || m > g->n) return set_err(GF_ERR_INVALID_ARG, "m must lie in [1, group size]");
+    const int w = g->m[0]->cfg.width, h = g->m[0]->cfg.height, ns = g->ns;
+    uint64_t seen = 0;
+    for (int j = 0; j < m; j++) {
+        const int k = members[j];
+        if (k < 0 || k >= g->n) return dm_member_err(set_err(GF_ERR_INVALID_ARG, "member index out of range"), j);
+        if ((seen >> k) & 1) return dm_member_err(set_err(GF_ERR_INVALID_ARG, "the member is listed twice"), j);
+        seen |= 1ull << k;
+        if (!rgb[j] || !depth[j]) return dm_member_err(set_err(GF_ERR_INVALID_ARG, "null frame"), j);
+        if (rgb_pitch[j] < 3 * (size_t)w || depth_pitch[j] < 2 * (size_t)w) return dm_member_err(set_err(GF_ERR_INVALID_ARG, "row pitch below the row width"), j);
+        if ((depth_pitch[j] | (size_t)(uintptr_t)depth[j]) & 1) return dm_member_err(set_err(GF_ERR_INVALID_ARG, "depth rows must start at even addresses (uint16)"), j);
+    }
+    GF_CUDA(cudaSetDevice(g->device));
+    std::vector<int> st(m, GF_OK), act;                 // act: the call's j of each active member
+    for (int j = 0; j < m; j++) {
+        if (n_inserted) n_inserted[j] = 0;
+        gf_dense_map* dm = g->m[members[j]];
+        if ((int)dm->poses.size() >= dm->cfg.max_keyframes) st[j] = dm_member_err(set_err(GF_ERR_CAPACITY, "max_keyframes reached"), j);
+        else act.push_back(j);
+    }
+    const int A = (int)act.size();
+    int first = GF_OK;
+    char first_err[sizeof(g_err)] = "";
+    auto note = [&](int j) { if (first == GF_OK && st[j] != GF_OK) { first = st[j]; memcpy(first_err, g_err, sizeof(first_err)); } };
+    for (int j = 0; j < m; j++) note(j);
+    if (A > 0) {
+        DmCall& c = *g->h;
+        for (int a = 0; a < A; a++) {
+            const int j = act[a];
+            gf_dense_map* dm = g->m[members[j]];
+            GF_CUDA(cudaEventRecord(g->ev, dm->st));
+            GF_CUDA(cudaStreamWaitEvent(g->st, g->ev, 0));
+            DmMember& M = c.mb[a];
+            M.cam = dm->cam; M.ext = dm->ext; M.A = dm->anchor;
+            memcpy(M.T.R, R + 9 * (size_t)j, sizeof(M.T.R)); memcpy(M.T.P, P + 3 * (size_t)j, sizeof(M.T.P));
+            M.rgb = rgb[j]; M.depth = depth[j]; M.rgb_pitch = rgb_pitch[j]; M.depth_pitch = depth_pitch[j];
+            if (!on_device) {
+                GF_CUDA(cudaMemcpy2DAsync(dm->rgb, 3 * (size_t)w, rgb[j], rgb_pitch[j], 3 * (size_t)w, h, cudaMemcpyHostToDevice, g->st));
+                GF_CUDA(cudaMemcpy2DAsync(dm->depth, 2 * (size_t)w, depth[j], depth_pitch[j], 2 * (size_t)w, h, cudaMemcpyHostToDevice, g->st));
+                M.rgb = dm->rgb; M.depth = dm->depth; M.rgb_pitch = 3 * (size_t)w; M.depth_pitch = 2 * (size_t)w;
+            }
+            M.vkeys = dm->vkeys; M.vcnt = dm->vcnt; M.vmask = dm->vmask;
+            M.cxyz = dm->cxyz; M.ccol = dm->ccol; M.kxyz = dm->kxyz; M.kcol = dm->kcol; M.kid = dm->kid;
+            M.c0 = dm->n_cloud; M.k0 = dm->n_kf_points; M.kf = (int)dm->poses.size();
+        }
+        GF_CUDA(cudaMemcpyAsync(g->d->mb, c.mb, sizeof(DmMember) * A, cudaMemcpyHostToDevice, g->st));
+        GF_CUDA(cudaMemsetAsync(g->bad, 0, 4 * A, g->st));
+        const dim3 g128((ns + 127) / 128, A), g256((ns + 255) / 256, A);
+        const gf_dense_map_cfg& cf = g->m[0]->cfg;
+        k_dmg_sample<<<g128, 128, 0, g->st>>>(g->d->mb, g->m[0]->su, ns, cf.depth_boundary, cf.depth_dist, g->key, g->idx, g->loc, g->col, g->wxyz, g->bad);
+        GF_LAUNCHED();
+        size_t b = g->tmp_bytes;
+        GF_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(g->tmp, b, g->key, g->skey, g->idx, g->sidx, A * ns, A, g->seg, g->seg + 1, 0, 64, g->st));
+        k_dmg_gate<<<g256, 256, 0, g->st>>>(g->d->mb, ns, g->skey, g->sidx, GATE_ADD, g->flag, g->add);
+        GF_LAUNCHED();
+        b = g->tmp_bytes;
+        GF_CUDA(cub::DeviceScan::ExclusiveSum(g->tmp, b, g->flag, g->pos, A * ns, g->st));
+        k_dmg_counts<<<1, GROUP_MAX, 0, g->st>>>(A, ns, g->flag, g->pos, g->bad, g->res);
+        GF_LAUNCHED();
+        GF_CUDA(cudaMemcpyAsync(g->h_res, g->res, 8 * (size_t)A, cudaMemcpyDeviceToHost, g->st));
+        GF_CUDA(cudaStreamSynchronize(g->st));           // the call's one wait: every member's accepted count and box flag
+        uint64_t ok = 0;
+        int F = 0, N = 0, Nn = 0;
+        c.fb[0] = c.nb[0] = 0;
+        for (int a = 0; a < A; a++) {
+            const int j = act[a], acc = g->h_res[2 * a];
+            gf_dense_map* dm = g->m[members[j]];
+            if (g->h_res[2 * a + 1]) st[j] = dm_member_err(set_err(GF_ERR_INVALID_ARG, "a point of the keyframe falls outside the octree's bounding box"), j);
+            else if (dm->n_kf_points + acc > dm->max_points) st[j] = dm_member_err(set_err(GF_ERR_CAPACITY, "max_points reached"), j);
+            note(j);
+            if (st[j] != GF_OK) continue;
+            ok |= 1ull << a;
+            if (n_inserted) n_inserted[j] = acc;
+            const int from = dm->n_cloud;
+            dm->n_cloud += acc;
+            dm->n_kf_points += acc;
+            dm->kf_off.push_back(dm->n_kf_points);
+            dm->poses.push_back(c.mb[a].T);
+            if (acc > 0) {                              // no new point: the filter's result stands
+                c.fl[F] = DmFilt{dm->cxyz, dm->kept, dm->fidx, dm->nsel, dm->n_cloud, from};
+                N += dm->n_cloud; Nn += acc;
+                c.fb[F + 1] = N; c.nb[F + 1] = Nn;
+                F++;
+                dm->nf_stale = true;
+            }
+        }
+        if (ok) {
+            k_dmg_hash_add<<<g256, 256, 0, g->st>>>(g->d->mb, ns, ok, g->skey, g->add);
+            GF_LAUNCHED();
+            k_dmg_scatter<<<g256, 256, 0, g->st>>>(g->d->mb, ns, ok, g->flag, g->pos, g->wxyz, g->col, g->loc);
+            GF_LAUNCHED();
+        }
+        if (F > 0) {
+            GF_CUDA(cudaMemcpyAsync(g->d->fl, c.fl, sizeof(DmFilt) * F, cudaMemcpyHostToDevice, g->st));
+            GF_CUDA(cudaMemcpyAsync(g->d->fb, c.fb, 4 * (size_t)(F + 1), cudaMemcpyHostToDevice, g->st));
+            GF_CUDA(cudaMemcpyAsync(g->d->nb, c.nb, 4 * (size_t)(F + 1), cudaMemcpyHostToDevice, g->st));
+            int rc = dmg_filter(g, F, N, Nn);
+            if (rc) return rc;
+        }
+        GF_CUDA(cudaGetLastError());
+        GF_CUDA(cudaEventRecord(g->ev, g->st));           // the members' later work follows the group's
+        for (int a = 0; a < A; a++) GF_CUDA(cudaStreamWaitEvent(g->m[members[act[a]]]->st, g->ev, 0));
+    }
+    if (status) for (int j = 0; j < m; j++) status[j] = st[j];
+    if (first != GF_OK) memcpy(g_err, first_err, sizeof(first_err));
+    return first;
+}
+
+}  // extern "C"
+
+// For gf_grid_map_group_add_dense_keyframes (gm_grid.cu; not exported): member k of a group, and the device points (packed
+// float3) of the keyframe a map added last, with the stream their writes are ordered on.
+gf_dense_map* gf_dense_map_group_member(gf_dense_map_group* g, int k) { return k >= 0 && k < g->n ? g->m[k] : nullptr; }
+int gf_dense_map_last_keyframe_device(gf_dense_map* m, const float** xyz, int* n, cudaStream_t* st, int* device)
+{
+    const int k = (int)m->poses.size() - 1;
+    if (k < 0) return set_err(GF_ERR_INVALID_ARG, "the dense map has no keyframe");
+    *xyz = m->kxyz + 3 * (size_t)m->kf_off[k];
+    *n = m->kf_off[k + 1] - m->kf_off[k];
+    *st = m->st;
+    *device = m->device;
+    return GF_OK;
+}

@@ -40,12 +40,8 @@ class DenseMap:
         except Exception:
             pass
 
-    def addKeyFrame(self, R, P, rgb, depth):
-        """One keyframe with body pose (R, P): rgb (H, W, 3) uint8 and depth (H, W) uint16 millimetres, numpy arrays (rows may be
-        padded) or CUDA tensors.  Returns the number of points inserted."""
-        R = np.ascontiguousarray(R, np.float64).reshape(9)
-        P = np.ascontiguousarray(P, np.float64).reshape(3)
-        n = ctypes.c_int()
+    def _frame(self, rgb, depth):
+        """(rgb pointer, rgb pitch, depth pointer, depth pitch, on_device) of a frame addKeyFrame takes."""
         h, w = self.height, self.width
         if tuple(rgb.shape) != (h, w, 3) or tuple(depth.shape) != (h, w):
             raise ValueError("rgb must be (%d, %d, 3) and depth (%d, %d)" % (h, w, h, w))
@@ -55,13 +51,20 @@ class DenseMap:
                 raise ValueError("CUDA frames: rgb uint8, depth int16 / uint16 (the millimetres' bits), both on the device")
             if rgb.stride(2) != 1 or rgb.stride(1) != 3 or depth.stride(1) != 1:
                 raise ValueError("rows must be packed pixels")
-            args = (ctypes.c_void_p(rgb.data_ptr()), rgb.stride(0), ctypes.c_void_p(depth.data_ptr()), depth.stride(0) * 2, 1)
-        else:
-            if rgb.dtype != np.uint8 or depth.dtype != np.uint16:
-                raise ValueError("rgb must be uint8 and depth uint16")
-            if rgb.strides[1:] != (3, 1) or depth.strides[1] != 2:
-                raise ValueError("rows must be packed pixels")
-            args = (_p(rgb), rgb.strides[0], _p(depth), depth.strides[0], 0)
+            return ctypes.c_void_p(rgb.data_ptr()), rgb.stride(0), ctypes.c_void_p(depth.data_ptr()), depth.stride(0) * 2, 1
+        if rgb.dtype != np.uint8 or depth.dtype != np.uint16:
+            raise ValueError("rgb must be uint8 and depth uint16")
+        if rgb.strides[1:] != (3, 1) or depth.strides[1] != 2:
+            raise ValueError("rows must be packed pixels")
+        return _p(rgb), rgb.strides[0], _p(depth), depth.strides[0], 0
+
+    def addKeyFrame(self, R, P, rgb, depth):
+        """One keyframe with body pose (R, P): rgb (H, W, 3) uint8 and depth (H, W) uint16 millimetres, numpy arrays (rows may be
+        padded) or CUDA tensors.  Returns the number of points inserted."""
+        R = np.ascontiguousarray(R, np.float64).reshape(9)
+        P = np.ascontiguousarray(P, np.float64).reshape(3)
+        n = ctypes.c_int()
+        args = self._frame(rgb, depth)
         _lib.check(_lib.lib().gf_dense_map_add_keyframe(self._m, _p(R), _p(P), *args, ctypes.byref(n)))
         return n.value
 
@@ -100,6 +103,71 @@ class DenseMap:
         out = np.zeros((n.value, 6), np.float32)
         _lib.check(_lib.lib().gf_dense_map_keyframe_points(self._m, k, _p(out), ctypes.byref(n)))
         return out
+
+
+def _members(members, K):
+    """members as int32, checked on the host: distinct indices in [0, K), at least one."""
+    mb = np.ascontiguousarray(members, np.int32).reshape(-1)
+    if len(mb) == 0:
+        raise ValueError("no member given")
+    if mb.min() < 0 or mb.max() >= K:
+        raise ValueError("member index out of range [0, %d)" % K)
+    if len(np.unique(mb)) != len(mb):
+        raise ValueError("a member is listed twice")
+    return mb
+
+
+def _poses(Rs, Ps, m):
+    Rs = np.ascontiguousarray(Rs, np.float64).reshape(-1, 9)
+    Ps = np.ascontiguousarray(Ps, np.float64).reshape(-1, 3)
+    if len(Rs) != m or len(Ps) != m:
+        raise ValueError("one pose per member: Rs (m, 3, 3), Ps (m, 3)")
+    return Rs, Ps
+
+
+class DenseMapGroup:
+    """gf_dense_map_group: one keyframe for each of several DenseMaps (one per estimator) with one launch chain and one host
+    synchronisation per call.  Every member's map afterwards is bit-equal to the same DenseMap.addKeyFrame on it alone; the maps
+    stay usable on their own between group calls.  The maps must share width, height, depth_dist and depth_boundary."""
+
+    def __init__(self, maps):
+        self.members = list(maps)
+        self.K = len(self.members)
+        self._h = ctypes.c_void_p()
+        h = (ctypes.c_void_p * self.K)(*[m._m for m in self.members])
+        _lib.check(_lib.lib().gf_dense_map_group_create(ctypes.byref(self._h), h, self.K))
+
+    def close(self):
+        if self._h:
+            _lib.lib().gf_dense_map_group_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def addKeyFrames(self, members, Rs, Ps, rgbs, depths):
+        """Member members[j] takes pose (Rs[j], Ps[j]) and frame (rgbs[j], depths[j]), as DenseMap.addKeyFrame takes them (all
+        numpy or all CUDA).  Returns (points inserted, status) per entry: status[j] is 0 or the error code the single call
+        would have raised for that member, which is then unchanged.  Argument errors raise and change nothing."""
+        mb = _members(members, self.K)
+        m = len(mb)
+        Rs, Ps = _poses(Rs, Ps, m)
+        if len(rgbs) != m or len(depths) != m:
+            raise ValueError("one frame per member")
+        fr = [self.members[k]._frame(r, d) for k, r, d in zip(mb, rgbs, depths)]
+        if len({f[4] for f in fr}) != 1:
+            raise ValueError("frames must be all host arrays or all CUDA tensors")
+        vp = ctypes.c_void_p * m
+        rgb, dep = vp(*[f[0] for f in fr]), vp(*[f[2] for f in fr])
+        rp, dp = np.array([f[1] for f in fr], np.uint64), np.array([f[3] for f in fr], np.uint64)
+        n, st = np.zeros(m, np.int32), np.zeros(m, np.int32)
+        rc = _lib.lib().gf_dense_map_group_add_keyframes(self._h, _p(mb), m, _p(Rs), _p(Ps), rgb, _p(rp), dep, _p(dp), fr[0][4], _p(n), _p(st))
+        if rc != 0 and not st.any():                  # per-member failures are reported in st; anything else changed nothing
+            _lib.check(rc)
+        return n, st
 
 
 def radius_filter(xyz, radius=0.8, min_pts=10, device=0):

@@ -13,6 +13,21 @@ def _p(a):
     return a.ctypes.data_as(ctypes.c_void_p)
 
 
+def _points(points):
+    """(pointer, n, stride in floats, on_device, the array kept alive) of the points addKeyFrame takes."""
+    if hasattr(points, "is_cuda") and points.is_cuda:
+        import torch
+        if points.dtype != torch.float32 or points.dim() != 2 or points.shape[1] < 3 or (len(points) and points.stride(1) != 1):
+            raise ValueError("points must be float32 (n, >= 3) with packed rows")
+        n, stride = points.shape[0], (points.stride(0) if len(points) > 1 else points.shape[1])
+        return ctypes.c_void_p(points.data_ptr()), n, stride, 1, points
+    points = np.asarray(points)
+    if points.dtype != np.float32 or points.ndim != 2 or points.shape[1] < 3:
+        raise ValueError("points must be float32 (n, >= 3)")
+    points = np.ascontiguousarray(points)
+    return _p(points), len(points), points.shape[1], 0, points
+
+
 class GridMap:
     """ric (3x3), tic (3): camera to body.  The grid has size_x x size_y cells of cell_size metres, world (0, 0) in cell
     (init_x, init_y); p_occ / p_free / p_prior: the inverse sensor model.  Defaults are the tool's.  max_points bounds the points
@@ -46,18 +61,8 @@ class GridMap:
         they are -- a numpy array or a CUDA tensor."""
         R = np.ascontiguousarray(R, np.float64).reshape(9)
         P = np.ascontiguousarray(P, np.float64).reshape(3)
-        if hasattr(points, "is_cuda") and points.is_cuda:
-            import torch
-            if points.dtype != torch.float32 or points.dim() != 2 or points.shape[1] < 3 or (len(points) and points.stride(1) != 1):
-                raise ValueError("points must be float32 (n, >= 3) with packed rows")
-            n, stride = points.shape[0], (points.stride(0) if len(points) > 1 else points.shape[1])
-            _lib.check(_lib.lib().gf_grid_map_add_keyframe(self._m, _p(R), _p(P), ctypes.c_void_p(points.data_ptr()), n, stride, 1))
-            return
-        points = np.asarray(points)
-        if points.dtype != np.float32 or points.ndim != 2 or points.shape[1] < 3:
-            raise ValueError("points must be float32 (n, >= 3)")
-        points = np.ascontiguousarray(points)
-        _lib.check(_lib.lib().gf_grid_map_add_keyframe(self._m, _p(R), _p(P), _p(points), len(points), points.shape[1], 0))
+        ptr, n, stride, on_device, _ = _points(points)
+        _lib.check(_lib.lib().gf_grid_map_add_keyframe(self._m, _p(R), _p(P), ptr, n, stride, on_device))
 
     def updatePath(self, Rs, Ps):
         """The rebuild after a pose correction: Rs (n, 3, 3), Ps (n, 3), one pose per keyframe added."""
@@ -98,3 +103,61 @@ class GridMap:
         out = np.zeros(4, np.int64)
         _lib.check(_lib.lib().gf_grid_map_stats(self._m, _p(out)))
         return dict(zip(("records", "applied", "skipped", "longest_run"), (int(v) for v in out)))
+
+
+class GridMapGroup:
+    """gf_grid_map_group: one keyframe for each of several GridMaps with one launch chain per call.  Every member's grid afterwards
+    is bit-equal to the same GridMap.addKeyFrame on it alone; the grids stay usable on their own between group calls."""
+
+    def __init__(self, grids):
+        self.members = list(grids)
+        self.K = len(self.members)
+        self._h = ctypes.c_void_p()
+        h = (ctypes.c_void_p * self.K)(*[g._m for g in self.members])
+        _lib.check(_lib.lib().gf_grid_map_group_create(ctypes.byref(self._h), h, self.K))
+
+    def close(self):
+        if self._h:
+            _lib.lib().gf_grid_map_group_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @staticmethod
+    def _done(rc, st):
+        if rc != 0 and not st.any():                  # per-member failures are reported in st; anything else changed nothing
+            _lib.check(rc)
+        return st
+
+    def addKeyFrames(self, members, Rs, Ps, points):
+        """Member members[j] takes pose (Rs[j], Ps[j]) and points[j] as GridMap.addKeyFrame takes them (all numpy or all CUDA).
+        Returns the status per entry: 0, or the error code the single call would have raised (the member is then unchanged)."""
+        from .dense_map import _members, _poses
+        mb = _members(members, self.K)
+        m = len(mb)
+        Rs, Ps = _poses(Rs, Ps, m)
+        if len(points) != m:
+            raise ValueError("one point set per member")
+        pp = [_points(x) for x in points]
+        if len({x[3] for x in pp}) != 1:
+            raise ValueError("points must be all host arrays or all CUDA tensors")
+        ptrs = (ctypes.c_void_p * m)(*[x[0] for x in pp])
+        n, stride = np.array([x[1] for x in pp], np.int32), np.array([x[2] for x in pp], np.int32)
+        st = np.zeros(m, np.int32)
+        rc = _lib.lib().gf_grid_map_group_add_keyframes(self._h, _p(mb), m, _p(Rs), _p(Ps), ptrs, _p(n), _p(stride), pp[0][3], _p(st))
+        return self._done(rc, st)
+
+    def addDenseKeyFrames(self, dense_group, members, Rs, Ps):
+        """Member k takes the keyframe that member k of dense_group (a DenseMapGroup) added last, read on the device, with pose
+        (Rs[j], Ps[j]) for k = members[j].  Returns the status per entry, as addKeyFrames."""
+        from .dense_map import _members, _poses
+        mb = _members(members, self.K)
+        m = len(mb)
+        Rs, Ps = _poses(Rs, Ps, m)
+        st = np.zeros(m, np.int32)
+        rc = _lib.lib().gf_grid_map_group_add_dense_keyframes(self._h, dense_group._h, _p(mb), m, _p(Rs), _p(Ps), _p(st))
+        return self._done(rc, st)

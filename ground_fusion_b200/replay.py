@@ -306,18 +306,38 @@ def replay(stream, tracker, fm, ba, n_frames, imu_per_frame=7, imu_propagate=Tru
     return out
 
 
+def slide_slots(slot, margin_old):
+    """slideWindow's shift of the stream frames held by the window slots (Headers[]), in place."""
+    if margin_old:
+        slot[:WINDOW_SIZE] = slot[1:]
+    else:
+        slot[WINDOW_SIZE - 1] = slot[WINDOW_SIZE]
+
+
+def keyframe_members(ests, last_P):
+    """The estimators that add a map keyframe after this step's slide, as replay() decides it for one: MARGIN_OLD, and the pose
+    of window frame WINDOW_SIZE - 2 not at the previous keyframe's position exactly (last_P[i]: None before the first)."""
+    return [i for i, e in enumerate(ests) if e.margin_old and not np.array_equal(e.Ps[WINDOW_SIZE - 2], last_P[i])]
+
+
 def replay_group(streams, trackers, windows, adjusters, n_frames, imu_per_frame=7, imu_propagate=True, max_iter=8, feedback=False,
-                 boxes=None, detector=None):
+                 boxes=None, detector=None, dense_maps=None, grid_maps=None, use_mcc=False):
     """K estimators in lockstep, one per stream, each step with one call per stage for all of them: the TrackerGroup over
     `trackers` tracks frame k of every stream, the FeatureWindowGroup over `windows` ingests the step on the device and
     triangulates, fills the K problems, estimator.solve_multi solves them on `adjusters`, setDepth follows, then
     estimator.marginalize_multi with each estimator's own mode, the consistency check and removal, the feedback to each member
     tracker (feedback=True, between tracker-group steps) and the slide.  The host logic is WindowEstimator's, as in replay();
-    returns one result dict per stream in replay()'s format.  No dense map or USE_MCC.
+    returns one result dict per stream in replay()'s format.
     boxes: USE_YOLO as in replay(), per stream: boxes[i][k] are the detections of frame k of stream i.  They go into the tracker
     group's step, and the window group takes the features inside them out on the device.
     detector: USE_YOLO with the detector in the loop, as in replay(): step k runs one detector.detect_batch over the K streams'
-    colour frames before the tracker group's step (its max_batch is raised to K if smaller).  Exclusive with boxes."""
+    colour frames before the tracker group's step (its max_batch is raised to K if smaller).  Exclusive with boxes.
+    dense_maps: one DenseMap per stream (sharing the frame geometry), fed as replay() feeds its dense_map, with one
+    DenseMapGroup call per step for the members that add a keyframe; grid_maps: one GridMap per stream (requires dense_maps),
+    each fed on the device with the keyframe its stream's dense map just added (GridMapGroup.addDenseKeyFrames).  They are
+    returned under "dense_map" / "grid_map" of each stream's dict.
+    use_mcc: USE_MCC as in replay(): the moving-consistency check and removal before the solve, none after it; with feedback the
+    removed ids reach each member's tracker."""
     from . import _lib
     from .estimator import marginalize_multi, solve_multi
     from .feature_tracker import TrackerGroup
@@ -326,15 +346,28 @@ def replay_group(streams, trackers, windows, adjusters, n_frames, imu_per_frame=
     assert len(trackers) == len(windows) == len(adjusters) == K
     if detector is not None and boxes is not None:
         raise ValueError("boxes and detector are exclusive")
+    if grid_maps is not None and dense_maps is None:
+        raise ValueError("grid_maps requires dense_maps")
+    if (dense_maps is not None and len(dense_maps) != K) or (grid_maps is not None and len(grid_maps) != K):
+        raise ValueError("one dense map and one grid map per stream")
     if detector is not None and detector.max_batch < K:
         detector.set_max_batch(K)
     tg, wg = TrackerGroup(trackers), FeatureWindowGroup(windows)
+    dg = gg = None
     imus = [ImuFromStream(s) for s in streams]
-    ests = [WindowEstimator(windows[i], adjusters[i], imu_propagate=imu_propagate, max_iter=max_iter, tracker=trackers[i] if feedback else None)
-            for i in range(K)]
+    ests = [WindowEstimator(windows[i], adjusters[i], imu_propagate=imu_propagate, max_iter=max_iter, tracker=trackers[i] if feedback else None,
+                            use_mcc=use_mcc) for i in range(K)]
     rec = [{"t": [], "P": [], "R": [], "gP": [], "gR": [], "it": []} for _ in range(K)]
     t_prev = [None] * K
+    slots = [[0] * (WINDOW_SIZE + 1) for _ in range(K)]  # stream frame held by each window slot, per stream
+    last_P = [None] * K                                 # position of the last keyframe fed to each dense map
     try:
+        if dense_maps is not None:
+            from .dense_map import DenseMapGroup
+            dg = DenseMapGroup(dense_maps)
+        if grid_maps is not None:
+            from .grid_map import GridMapGroup
+            gg = GridMapGroup(grid_maps)
         for k in range(n_frames):
             frames = [s.frame(k) for s in streams]
             for i, (e, imu) in enumerate(zip(ests, imus)):
@@ -359,6 +392,8 @@ def replay_group(streams, trackers, windows, adjusters, n_frames, imu_per_frame=
                     R_wb, P = imu.pose_t(frames[i][0])
                     e.set_state(e.frame_count, R_wb, P, imu.velocity(frames[i][0]))
             fcs = [e.frame_count for e in ests]
+            for sl, fc in zip(slots, fcs):
+                sl[fc] = k
             margins = wg.addFramesFromTrackerGroup(tg, fcs, [e.td for e in ests])
             for e, m in zip(ests, margins):
                 e.margin_old = m
@@ -369,6 +404,10 @@ def replay_group(streams, trackers, windows, adjusters, n_frames, imu_per_frame=
                 continue
             poses = [(e.Ps, e.Rs, e.tic, e.ric) for e in ests]
             wg.triangulateAll(fcs, poses)
+            removed = [set() for _ in ests]
+            if use_mcc:                                              # as processImage with USE_MCC
+                removed = wg.movingConsistencyCheckW(poses)
+                wg.removeOutliers(removed)
             pbs = [e.build_problem()[0] for e in ests]
             nfs = wg.fillProblems(pbs)
             before = [(e.Rs[0].copy(), e.Ps[0].copy()) for e in ests]
@@ -386,29 +425,65 @@ def replay_group(streams, trackers, windows, adjusters, n_frames, imu_per_frame=
             for e, pr in zip(ests, priors):
                 e.adopt_prior(pr)
             poses = [(e.Ps, e.Rs, e.tic, e.ric) for e in ests]
-            wg.removeOutliers(wg.movingConsistencyCheckW(poses))     # as after_optimization without USE_MCC
+            if not use_mcc:                                          # as after_optimization without USE_MCC
+                wg.removeOutliers(wg.movingConsistencyCheckW(poses))
             if feedback:                                             # the set the tracker is told about is empty without USE_MCC
                 preds = wg.predictPtsInNextFrame([e.frame_count for e in ests], poses)
-                for e, tr, pred in zip(ests, trackers, preds):
-                    tr.removeOutliers(set())
+                for e, tr, pred, rm in zip(ests, trackers, preds, removed):
+                    tr.removeOutliers(rm)
                     tr.setPrediction(pred)
-                    e.n_predicted += len(pred)
+                    e.n_removed += len(rm); e.n_predicted += len(pred)
             shifts = [e.slide_states() for e in ests]
             wg.remove([_lib.FM_REMOVE_BACK_SHIFT_DEPTH if sh is not None else _lib.FM_REMOVE_FRONT for sh in shifts],
                       [e.frame_count for e in ests], shifts)
             wg.removeFailures()
+            for sl, e in zip(slots, ests):
+                slide_slots(sl, e.margin_old)
+            if dg is not None:
+                add_group_keyframes(dg, gg, streams, ests, slots, last_P)
             for i, (e, imu) in enumerate(zip(ests, imus)):
                 R_wb, P = imu.pose_t(frames[i][0])
                 r = rec[i]
                 r["t"].append(frames[i][0]); r["P"].append(e.Ps[WINDOW_SIZE].copy()); r["R"].append(e.Rs[WINDOW_SIZE].copy())
                 r["gP"].append(P); r["gR"].append(R_wb); r["it"].append(e.last_summary["iterations"])
     finally:
-        wg.close(); tg.close()
+        for grp in (gg, dg, wg, tg):
+            if grp is not None:
+                grp.close()
     out = []
-    for e, r in zip(ests, rec):
+    for i, (e, r) in enumerate(zip(ests, rec)):
         P_est, P_gt = np.array(r["P"]), np.array(r["gP"])
         ate = float(np.sqrt(np.mean(np.sum((P_est - P_gt) ** 2, axis=1)))) if len(P_est) else float("nan")
         out.append({"t": np.array(r["t"]), "P_est": P_est, "P_gt": P_gt, "R_est": np.array(r["R"]), "R_gt": np.array(r["gR"]), "ate_m": ate,
                     "n_margin_old": e.n_old, "n_margin_second_new": e.n_second_new, "iterations": r["it"],
                     "n_removed": e.n_removed, "n_predicted": e.n_predicted})
+        if dense_maps is not None:
+            out[-1]["dense_map"] = dense_maps[i]
+        if grid_maps is not None:
+            out[-1]["grid_map"] = grid_maps[i]
     return out
+
+
+def add_group_keyframes(dg, gg, streams, ests, slots, last_P):
+    """The keyframes of one replay_group step: one dense-map group call for the members keyframe_members picks, each with the
+    pose of window frame WINDOW_SIZE - 2 and the colour and depth of the stream frame in that slot; then, with a grid group gg,
+    one call feeding each of those grids its dense map's new keyframe on the device.  A member's failure raises, as replay()'s
+    single call does.  Returns the members fed."""
+    from . import _lib
+    req = keyframe_members(ests, last_P)
+    if not req:
+        return req
+    W2 = WINDOW_SIZE - 2
+    Rs = [ests[i].Rs[W2].copy() for i in req]
+    Ps = [ests[i].Ps[W2].copy() for i in req]
+    for i, P in zip(req, Ps):
+        last_P[i] = P
+    fr = [slots[i][W2] for i in req]
+    _, st = dg.addKeyFrames(req, Rs, Ps, [streams[i].color(j) for i, j in zip(req, fr)], [streams[i].frame(j)[2] for i, j in zip(req, fr)])
+    if np.any(st):
+        raise _lib.GfError("dense map group: member status %s" % dict(zip(req, (int(v) for v in st))))
+    if gg is not None:
+        st = gg.addDenseKeyFrames(dg, req, Rs, Ps)
+        if np.any(st):
+            raise _lib.GfError("grid map group: member status %s" % dict(zip(req, (int(v) for v in st))))
+    return req

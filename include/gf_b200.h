@@ -762,6 +762,31 @@ int gf_dense_map_keyframe_points(gf_dense_map* map, int k, float* out6, int* n);
  * distance < float(radius^2). */
 int gf_stage_radius_filter(int device, const float* xyz, int n, double radius, int min_pts, uint8_t* keep);
 
+/* A dense-map group: n existing gf_dense_maps (members, e.g. one per estimator) that take one keyframe each with ONE launch chain
+ * per call and ONE host synchronisation, where n single calls make ten launches and two synchronisations each.  Member k's
+ * cloud, keyframe lists, voxel counts, filter result and n_filtered afterwards are bit-equal to what
+ * gf_dense_map_add_keyframe on it alone would give.  DESIGN.md "Groups of maps" has the layout and the order argument.
+ *   _create: 1 <= n <= GF_DENSE_MAP_GROUP_MAX; the maps must be distinct, bound to one device and share width, height,
+ *       depth_dist and depth_boundary (so the samples per keyframe); capacities, intrinsics and extrinsics may differ.  Any
+ *       violation is GF_ERR_INVALID_ARG with gf_last_error() starting "member k: ".  The group borrows the maps (destroy it
+ *       first) and allocates its scratch once: about 100 bytes per point of the members' max_points together.
+ *   Between group calls a member may be used directly (add_keyframe, update_poses, read, keyframe_points): work is ordered
+ *   between a member's stream and the group's in both directions.  A group is used from one thread at a time.
+ * _add_keyframes: one keyframe for each of m distinct members, members[j] in [0, n) any subset; member members[j] takes pose
+ * R [j][9], P [j][3] and the frame rgb[j] (rows of rgb_pitch[j] bytes), depth[j] (rows of depth_pitch[j] bytes), all HOST
+ * pointers or all device pointers (on_device).  Argument errors (a member listed twice or out of range, a null frame, a pitch)
+ * change nothing; gf_last_error() starts "member j: " for entry j.  A member that would fail the single call (max_keyframes,
+ * max_points, a point outside the octree's box) reports that code in status[j] (nullable) and stays unchanged; the others are
+ * applied, and the call returns the first failing entry's code.  n_inserted [m] (nullable): points added. */
+typedef struct gf_dense_map_group gf_dense_map_group;
+#define GF_DENSE_MAP_GROUP_MAX 64
+int gf_dense_map_group_create(gf_dense_map_group** out, gf_dense_map* const* maps, int n);
+void gf_dense_map_group_destroy(gf_dense_map_group* g);
+int gf_dense_map_group_size(gf_dense_map_group* g, int* n);
+int gf_dense_map_group_add_keyframes(gf_dense_map_group* g, const int32_t* members, int m, const double* R, const double* P,
+                                     const uint8_t* const* rgb, const size_t* rgb_pitch, const uint16_t* const* depth, const size_t* depth_pitch,
+                                     int on_device, int32_t* n_inserted, int32_t* status);
+
 /* ------------------------------------------------------------------------------------------------
  * Occupancy grid (support_files/grid_mapping: main.cpp, grid_mapper.cpp, grid_map.cpp): the 2-D log-odds grid the reference
  * builds offline from every keyframe's point_rgbd and corrected pose, here built online.  Keyframe points whose world height
@@ -804,6 +829,28 @@ int gf_grid_map_size(gf_grid_map* map, int* size_x, int* size_y, int* n_keyframe
 /* Of the last add_keyframe / update_poses: out4 = ray steps (records), updates applied, updates the exact shortcuts skipped
  * (a repeated no-op update, a cell at 0 or 1) and the longest per-cell run within one chunk. */
 int gf_grid_map_stats(gf_grid_map* map, int64_t* out4);
+
+/* A grid group: n existing gf_grid_maps whose keyframes are applied with one launch chain per call (count, scan, emit, sort and
+ * apply run once over every member's rays).  Member k's bel (so its image and occupancy) afterwards is bit-equal to what
+ * gf_grid_map_add_keyframe on it alone would give; its stats are those of its own records.
+ *   _create: 1 <= n <= GF_GRID_MAP_GROUP_MAX grids, distinct and bound to one device; sizes, sensor models and capacities may
+ *       differ.  The group sorts at most min(max_records) of its members' records at once (more are chunked, in order) and
+ *       allocates 16 bytes per point of the members' max_points together and 16 per record.  Member use between group calls
+ *       and errors are as for the dense-map group.
+ * _add_keyframes: member members[j] takes pose R [j][9], P [j][3] and n_pts[j] points, rows of stride_floats[j] floats at
+ * pts[j], all host or all device pointers (on_device).  Per-member failures (a non-finite pose or point, max_keyframes,
+ * max_points, a ray of more than 2^24 steps) go to status[j] with the member unchanged.
+ * _add_dense_keyframes: the same, each grid member's points being, read on the device, the keyframe that member of the dense-map
+ * group dg with the SAME index added last (grid member k pairs with dense member k); no host copy. */
+typedef struct gf_grid_map_group gf_grid_map_group;
+#define GF_GRID_MAP_GROUP_MAX 64
+int gf_grid_map_group_create(gf_grid_map_group** out, gf_grid_map* const* grids, int n);
+void gf_grid_map_group_destroy(gf_grid_map_group* g);
+int gf_grid_map_group_size(gf_grid_map_group* g, int* n);
+int gf_grid_map_group_add_keyframes(gf_grid_map_group* g, const int32_t* members, int m, const double* R, const double* P, const float* const* pts,
+                                    const int32_t* n_pts, const int32_t* stride_floats, int on_device, int32_t* status);
+int gf_grid_map_group_add_dense_keyframes(gf_grid_map_group* g, gf_dense_map_group* dg, const int32_t* members, int m, const double* R,
+                                          const double* P, int32_t* status);
 
 /* ---- YOLO detector (the use_yolo front end's darknet_ros node, YoloObjectDetector.cpp, on the GPU) ------------------------
  * darknet's inference forward pass for the networks the reference ships (vins_estimator/yolo_network_config/cfg: [net],
