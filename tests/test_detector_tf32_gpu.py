@@ -13,12 +13,10 @@ import ctypes
 import numpy as np
 import pytest
 
-from tf32_ref import conv_shapes, detect_from_heads, heads_oracle_available, im2col, rna_tf32
-from yolo_ref import CFGS, cfg_at, conv_params_expected, oracle_available, write_weights
+from tf32_ref import check_dyadic_operands, conv_shapes, detect_from_heads, heads_oracle_available, layer_bound_check, rna_tf32
+from yolo_ref import CFGS, cfg_at, oracle_available, write_weights
 
 pytestmark = pytest.mark.gpu
-
-U = 2.0 ** -24           # FP32 unit roundoff
 
 
 def synth_bgr(k=0):
@@ -57,35 +55,9 @@ def _shapes():
 SHAPES = _shapes()
 
 
-def _dyadic(rng, n):
-    return (rng.integers(-8, 9, n) / 8.0).astype(np.float32)
-
-
 @pytest.mark.parametrize("shape", SHAPES, ids=["C%d_H%d_W%d_M%d_s%d_st%d_p%d" % s for s in SHAPES])
 def test_dyadic_operands_give_the_exact_modes_bits(shape):
-    from ground_fusion_b200.detector import conv_stage
-    C, H, W, M, size, stride, pad = shape
-    rng = np.random.default_rng(hash(shape) % (1 << 32))
-    x = _dyadic(rng, C * H * W).reshape(C, H, W)
-    w = _dyadic(rng, M * C * size * size).reshape(M, C, size, size)
-    zero = np.zeros(M, np.float32)
-    # the sums alone: both modes and float64 agree bit for bit
-    t = conv_stage(x, w, zero, stride, pad, precision="tf32")
-    e = conv_stage(x, w, zero, stride, pad, precision="exact")
-    cols, OH, OW = im2col(x.astype(np.float64), size, stride, pad)
-    ref = (w.reshape(M, -1).astype(np.float64) @ cols).astype(np.float32).reshape(M, OH, OW)
-    assert t.shape == ref.shape
-    assert np.array_equal(e.view(np.uint32), ref.view(np.uint32))
-    bad = np.flatnonzero(t.view(np.uint32) != ref.view(np.uint32))
-    assert bad.size == 0, "%d of %d differ, first at %d: %r vs %r" % (bad.size, t.size, bad[0], t.flat[bad[0]], ref.flat[bad[0]])
-    # the epilogue: bias, batch norm and leaky give the same bits in both modes
-    bias = rng.standard_normal(M).astype(np.float32)
-    bn = (rng.uniform(0.5, 1.5, M).astype(np.float32), rng.standard_normal(M).astype(np.float32),
-          rng.uniform(0.2, 2.0, M).astype(np.float32))
-    for kw in (dict(leaky=True), dict(bn=bn), dict(bn=bn, leaky=True)):
-        t = conv_stage(x, w, bias, stride, pad, precision="tf32", **kw)
-        e = conv_stage(x, w, bias, stride, pad, precision="exact", **kw)
-        assert np.array_equal(t.view(np.uint32), e.view(np.uint32)), kw
+    check_dyadic_operands(shape)
 
 
 def test_operands_are_rounded_to_nearest_ties_away():
@@ -114,61 +86,6 @@ def test_operands_are_rounded_to_nearest_ties_away():
             assert not np.array_equal(got.reshape(M, -1), trunc.astype(np.float32))
 
 
-def _layer_bound_check(det, cfg, weights):
-    """For every convolution: |o_gpu - o_ref| <= L K 2^-22 S + E_epi elementwise, and mean(|o_gpu - o_ref| / (L S)) <= 2^-20.
-    Returns the largest error / bound ratio.
-
-    o_ref is the layer in float64 from the GPU's own input: s = sum_k w~ x~ (w~, x~ the TF32-rounded operands), then
-    normalize_cpu, scale, bias and leaky without rounding.  S = sum_k |w~| |x~|, and L = |scale| / den with batch norm, 1
-    without.  K 2^-22 S is twice the first-order bound on truncated FP32 additions in any order, propagated through the
-    epilogue's gain L (leaky's slope is <= 1).
-    E_epi: the epilogue's own roundings, each at most U = 2^-24 of its result: the subtraction of the mean (U L |s - mu|
-    once carried through den and scale), the rounding of the double division (U L |s - mu|), the product with scale
-    (U L |s - mu|), the bias addition and leaky's product (U |y| each, |y| <= L |s - mu| + |b|).  That is at most
-    5 U L |s - mu| + 2 U |b| to first order; E_epi = 8 U (L |s - mu| + |b|) covers it with the second-order terms and the
-    difference between the GPU's sum and s (both far smaller)."""
-    from ground_fusion_b200.detector import parse_cfg
-    _, layers = parse_cfg(cfg)
-    params = conv_params_expected(cfg, weights)
-    worst = 0.0
-    for k, L_ in enumerate(layers):
-        if L_["type"] != "convolutional":
-            continue
-        p = params[k]
-        x = det.layer_output(k - 1) if k > 0 else det.input_image()
-        size, M = L_["size"], L_["n"]
-        cols, OH, OW = im2col(rna_tf32(x).astype(np.float64), size, L_["stride"], L_["pad"])
-        wt = rna_tf32(p["weights"]).reshape(M, -1).astype(np.float64)
-        s = wt @ cols
-        S = np.abs(wt) @ np.abs(cols)
-        K = wt.shape[1]
-        b = p["biases"].astype(np.float64)[:, None]
-        if L_["batch_normalize"]:
-            mu = p["mean"].astype(np.float64)[:, None]
-            den = np.sqrt(p["var"].astype(np.float64)) + float(np.float32(1e-6))
-            gain = (np.abs(p["scales"].astype(np.float64)) / den)[:, None]
-            y = (s - mu) / den[:, None] * p["scales"].astype(np.float64)[:, None] + b
-        else:
-            mu, gain = 0.0, np.ones((M, 1))
-            y = s + b
-        act = det.layer_output(k).reshape(M, -1).astype(np.float64)
-        ref = np.where(y > 0, y, 0.1 * y) if _is_leaky(cfg, k) else y
-        err = np.abs(act - ref)
-        bound = gain * K * 2.0 ** -22 * S + 8 * U * (gain * np.abs(s - mu) + np.abs(b)) + 1e-30
-        ratio = float((err / bound).max())
-        assert ratio <= 1.0, "layer %d: error %g exceeds its bound by %.3f" % (k, float(err.max()), ratio)
-        mean_rel = float(np.mean(err / np.maximum(gain * S, 1e-30)))
-        assert mean_rel <= 2.0 ** -20, "layer %d: mean relative error %g" % (k, mean_rel)
-        worst = max(worst, ratio)
-    return worst
-
-
-def _is_leaky(cfg, k):
-    from ground_fusion_b200.detector import _sections
-    secs = [s for s in _sections(cfg)[1:]]
-    return secs[k][1].get("activation", "logistic") == "leaky"
-
-
 @pytest.mark.parametrize("name", CFGS)
 def test_every_convolution_within_the_error_bound_at_160(name, files):
     from ground_fusion_b200.detector import YoloDetector
@@ -176,7 +93,7 @@ def test_every_convolution_within_the_error_bound_at_160(name, files):
     det = YoloDetector(cfg, w, thresh=0.3, precision="tf32")
     try:
         det.detect(synth_bgr(0))
-        worst = _layer_bound_check(det, cfg, w)
+        worst = layer_bound_check(det, cfg, w)
     finally:
         det.close()
     print("%s at 160: largest error / bound %.4f" % (name, worst))
@@ -188,7 +105,7 @@ def test_yolov3_at_416_within_the_error_bound(files):
     det = YoloDetector(cfg, w, thresh=0.3, precision="tf32")
     try:
         det.detect(synth_bgr(3))
-        worst = _layer_bound_check(det, cfg, w)
+        worst = layer_bound_check(det, cfg, w)
     finally:
         det.close()
     print("yolov3 at 416: largest error / bound %.4f" % worst)
